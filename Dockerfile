@@ -8,6 +8,6 @@ ENV DEBIAN_FRONTEND=noninteractive HOROVOD_LOG_LEVEL=warning
 RUN apt-get update && apt-get install -y --no-install-recommends openssh-client openssh-server && rm -rf /var/lib/apt/lists/*
 WORKDIR /workspace/horovod_b200
 COPY . .
-# sm_100a only: nvcc cross-compiles without a GPU present
+# sm_90a only: nvcc cross-compiles without a GPU present
 RUN python -m pip install --no-build-isolation -e . && python -c "import horovod_b200.torch as hvd; print('p2p built:', hvd.p2p_built())"
 CMD ["python", "-m", "pytest", "tests", "-q", "-m", "not gpu"]

@@ -44,6 +44,9 @@ def parse():
     p.add_argument('--no-extras', action='store_true', help='skip extra.bert_large / extra.allreduce_busbw / extra.checks')
     p.add_argument('--sizes', default=None, help='allreduce sweep: comma separated byte sizes')
     p.add_argument('--dtype', default='fp32', help='allreduce sweep dtype: fp32|bf16|fp16')
+    p.add_argument('--dump-outputs', metavar='DIR', default=None,
+                   help='after the timed steps, write the loss of the last step and a fixed sample of the updated parameters '
+                        'as DIR/<name>.npy (float32), to compare two builds output for output')
     return p.parse_args()
 
 
@@ -189,11 +192,27 @@ def build_model(args, torch):
     return model, make_batch, step_fn, bs, seq, 'samples/sec'
 
 
-def _time_train(args, model_name, steps, warmup, hvd, torch, sample_clocks):
+DUMP_PARAM_SAMPLE = 1 << 22  # parameters written by --dump-outputs: 16 MiB of float32
+
+
+def _dump_outputs(dump_dir, loss, model, torch):
+    """What a caller of the timed step holds after its last step: the loss it returned and the parameters it updated
+    (a sample drawn with a fixed seed, so two runs with the same arguments write the same positions)."""
+    import numpy as np
+    os.makedirs(dump_dir, exist_ok=True)
+    flat = torch.cat([p.detach().float().reshape(-1) for p in model.parameters()])
+    gen = torch.Generator(device='cpu').manual_seed(0)
+    idx = torch.randint(0, flat.numel(), (min(flat.numel(), DUMP_PARAM_SAMPLE),), generator=gen).sort().values
+    np.save(os.path.join(dump_dir, 'loss.npy'), loss.detach().float().reshape(1).cpu().numpy())
+    np.save(os.path.join(dump_dir, 'params_sample.npy'), flat[idx.to(flat.device)].cpu().numpy())
+
+
+def _time_train(args, model_name, steps, warmup, hvd, torch, sample_clocks, dump_dir=None):
     """One training configuration: device-timed arm (inputs resident) and end-to-end arm (per-step pinned H2D input copy +
     D2H loss read).  Returns a dict; frees the model before returning."""
     from horovod_b200.data import DevicePrefetcher
     rank, size, local_rank = hvd.rank(), hvd.size(), hvd.local_rank()
+    torch.manual_seed(0)  # same weights and synthetic batch on every run with the same arguments
     margs = argparse.Namespace(**vars(args))
     margs.model = model_name
     if model_name != args.model:
@@ -286,8 +305,10 @@ def _time_train(args, model_name, steps, warmup, hvd, torch, sample_clocks):
     sampler = ClockSampler(local_rank) if (rank == 0 and sample_clocks) else None
     if sampler:
         sampler.start()
-    ms, launches, _ = timed(steps, e2e=False)
+    ms, launches, last = timed(steps, e2e=False)
     clocks = sampler.stop() if sampler else None
+    if dump_dir and rank == 0:
+        _dump_outputs(dump_dir, last, model, torch)
     for _ in range(2):
         graphed(*tuple(t.cuda(non_blocking=True) for t in host_batch))
     e2e_ms, _, last_loss = timed(steps, e2e=True)
@@ -384,7 +405,7 @@ def _busbw_extra(args, hvd, torch):
         rows.append(row)
         del x
     return {'dtype': 'fp32', 'tensors': 'plain cudaMalloc (unregistered), in place, blocking loop', 'rows': rows,
-            'roofline_gbs_per_direction': 900}
+            'roofline_gbs_per_direction': 450}
 
 
 def _checks_extra(hvd, torch):
@@ -445,12 +466,15 @@ def train_bench(args):
     hvd.init()
     rank, size = hvd.rank(), hvd.size()
     torch.cuda.set_device(hvd.local_rank())
-    torch.backends.cudnn.benchmark = True
+    # cuDNN's heuristic algorithm choice, not its autotuner: the autotuner picks convolution algorithms by timing, so two
+    # runs could compute the same step with different algorithms (and round differently); on an H100 the heuristic choice
+    # is as fast for ResNet-50
+    torch.backends.cudnn.benchmark = False
     torch.backends.cuda.matmul.allow_tf32 = not args.parity
     torch.backends.cudnn.allow_tf32 = not args.parity
     if args.parity:
         args.fp32 = True  # the stock reference benchmark: fp32, eager hooks, unfused optimizer, batch 64
-    main = _time_train(args, args.model, args.steps, args.warmup, hvd, torch, sample_clocks=True)
+    main = _time_train(args, args.model, args.steps, args.warmup, hvd, torch, sample_clocks=True, dump_dir=args.dump_outputs)
     extra = {}
     if not args.no_extras:
         try:
@@ -484,7 +508,7 @@ def train_bench(args):
                        'bucket_wire_dtype': args.bucket_wire_dtype or 'fp32', 'bucket_cap_mb': args.bucket_cap_mb,
                        'parity_mode': bool(args.parity), 'cuda_graph': main['cuda_graph'], 'cuda_graph_fallback': main['cuda_graph_fallback'],
                        'allreduce_in_graph': main['allreduce_in_graph'], 'gradient_buckets': main['gradient_buckets'],
-                       'l2': 'per-step working set (activations + 100+ MB of gradients) exceeds the 126 MB L2; no explicit flush',
+                       'l2': 'per-step working set (activations + 100+ MB of gradients) exceeds the 50 MB L2 of an H100; no explicit flush',
                        'gpu_backend': hvd.gpu_backend_info(), 'tunables': hvd.tunable_params()},
             'clocks': main['clocks'],
             'e2e': {'value': main['e2e_value'], 'unit': main['unit'], 'ms_per_step': main['e2e_ms_per_step'],
@@ -538,7 +562,7 @@ def allreduce_bench(args):
         print(json.dumps({'metric': 'allreduce bus bandwidth sweep', 'value': best, 'unit': 'GB/s (peak busBW)', 'n_gpus': size,
                           'higher_is_better': True, 'dtype': args.dtype, 'impl': 'ours', 'rows': rows,
                           'config': {'gpu_backend': hvd.gpu_backend_info(), 'tunables': hvd.tunable_params(),
-                                     'roofline_gbs_per_dir': 900, 'measured_peer_copy_gbs': 770}}), flush=True)
+                                     'roofline_gbs_per_dir': 450}}), flush=True)
     hvd.shutdown()
     return 0
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Bandwidth sweep of the non-allreduce collectives: allgather, broadcast, alltoall, reducescatter.
 
-    torchrun --nproc-per-node 8 bench/collective_sweep.py --out gpurun_out/collectives8.json
+    torchrun --nproc-per-node 8 bench/collective_sweep.py --out collectives8.json
     HVD_EXCHANGE_TMA=1 torchrun ... bench/collective_sweep.py --ops allgather,broadcast --tag tma
 
 Every op is timed on the device (CUDA events around `iters` back-to-back calls after warm-up, max over ranks) through

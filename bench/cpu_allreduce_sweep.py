@@ -2,7 +2,7 @@
 """Host-memory allreduce: this runtime's CPU data plane (shared-memory / TCP ring, `csrc/ops/cpu_ops.cc`) next to
 torch.distributed's Gloo backend (the reference's CPU data plane is Gloo as well) on the same tensors.
 
-    hvdrun -np 4 python bench/cpu_allreduce_sweep.py --out profiles/cpu_allreduce_np4.json
+    hvdrun -np 4 python bench/cpu_allreduce_sweep.py --out cpu_allreduce_np4.json
 
 Wall-clock timing (there is no device): `iters` back-to-back calls after warm-up between barriers, max over ranks.
 busBW = 2 (N-1)/N * bytes / time.

@@ -2,7 +2,7 @@
 """Host-memory allgather / broadcast / reducescatter / alltoall: this runtime's CPU data plane next to torch.distributed's Gloo
 backend (the reference's CPU ops run on Gloo or MPI) on the same tensors.
 
-    hvdrun -np 4 python bench/cpu_collective_sweep.py --out profiles/cpu_collectives_np4_vs_gloo.json
+    hvdrun -np 4 python bench/cpu_collective_sweep.py --out cpu_collectives_np4_vs_gloo.json
     HVD_TEST_FAKE_HOSTS=2 hvdrun -np 4 python bench/cpu_collective_sweep.py        # ranks presented as 2 hosts: TCP between them
 
 `bytes` is the size of the RESULT on one rank (allgather: N x input; reducescatter: input / N).  Wall-clock timing, `iters`

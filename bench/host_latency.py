@@ -2,7 +2,7 @@
 """Host path of a blocking small collective, split with the runtime's own probes (`hvd.metrics()['latency']`: queue = enqueue ->
 negotiation start, negotiate = negotiation, execute = data path, total = enqueue -> completion callback).
 
-    hvdrun -np 4 python bench/host_latency.py --out profiles/host_latency_np4.json
+    hvdrun -np 4 python bench/host_latency.py --out host_latency_np4.json
     HVD_TEST_FAKE_HOSTS=2 hvdrun -np 4 python bench/host_latency.py          # 2 "hosts": two-level control plane, TCP between them
 
 Cases: a cached allreduce (same name every call), an allreduce under a NEW name every call (coordinator round), allgather,

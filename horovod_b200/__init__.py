@@ -1,4 +1,4 @@
-"""horovod_b200 — a Blackwell-native data-parallel collective library with Horovod's capabilities.
+"""horovod_b200 — a Hopper-native (H100) data-parallel collective library with Horovod's capabilities.
 
 `import horovod_b200.torch as hvd` gives the reference's PyTorch API
 (horovod/torch/__init__.py): init/rank/size, async named collectives,

@@ -4,7 +4,7 @@ the buffer protocol for host arrays — instead of compiling one C++ adapter per
 
 The reference builds a separate native extension per framework (tensorflow/mpi_ops.cc ~1900 lines, mxnet/mpi_ops.cc +
 adapter.cc/tensor_util.cc ~1300 lines, torch/mpi_ops_v2.cc ~1200 lines), each re-implementing the same
-Tensor/OpContext/ReadyEvent adapters (common/common.h:265-330).  On a B200 every framework that matters exports
+Tensor/OpContext/ReadyEvent adapters (common/common.h:265-330).  On an H100 every framework that matters exports
 DLPack capsules that alias its device memory, so one adapter is enough: the kernels read and write the framework's own
 HBM allocation, and stream ordering is handled by the framework's DLPack stream contract (the producer stream is
 synchronised with the consumer's current stream when the capsule is imported).

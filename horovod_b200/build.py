@@ -1,12 +1,12 @@
 """In-tree native build: `python -m horovod_b200.build [--force] [--no-torch]`.
 
-Produces (next to this file, git-ignored but shipped by gpurun):
-  lib/libhvd_core.so   C++ runtime + sm_100a CUDA kernels (g++ / nvcc, no torch headers: compiles in seconds)
+Produces (next to this file, git-ignored):
+  lib/libhvd_core.so   C++ runtime + sm_90a CUDA kernels (g++ / nvcc, no torch headers: compiles in seconds)
   lib/_hvd_torch.so    pybind11/ATen binding linked against libhvd_core.so
 
 Role parity: the reference's CMakeLists.txt + setup.py CMake driver
 (horovod/CMakeLists.txt, cmake/build_utils.py:93-118 for the -gencode list).
-Here the only device target is sm_100a.
+Here the only device target is sm_90a (H100).
 """
 import hashlib
 import os
@@ -22,7 +22,7 @@ OUT = os.path.join(ROOT, "lib")
 OBJ = os.path.join(ROOT, "build", "obj")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 CORE_DIRS = ["common", "common/optim", "transport", "ops", "symm", "kernels"]
 
@@ -161,7 +161,7 @@ def clean():
 def build_tsan_selftest(force=False, sanitizer="thread"):
     """ThreadSanitizer build of the C++ runtime + its native self-test (N engines in one process over the loopback
     transport: controller, response cache, fusion, CPU ops, process sets, join, error paths) as a stand-alone executable.
-    The sm_100a kernel objects are linked as they are (device code is not instrumented).  The reference has no sanitizer
+    The sm_90a kernel objects are linked as they are (device code is not instrumented).  The reference has no sanitizer
     build at all (SURVEY.md 5.2).  `sanitizer="address,undefined"` builds the AddressSanitizer + UBSan flavour of the same binary."""
     build_core()
     tag = "tsan" if sanitizer == "thread" else "san_" + "".join(c if c.isalnum() else "_" for c in sanitizer)

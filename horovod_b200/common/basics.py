@@ -281,7 +281,7 @@ class HorovodBasics(object):
         return bool(self.lib.hvd_ccl_built())
 
     def cuda_built(self):
-        """True when the native library was built with the sm_100a kernels."""
+        """True when the native library was built with the sm_90a kernels."""
         return bool(self.lib.hvd_cuda_built())
 
     def rocm_built(self):
@@ -289,7 +289,7 @@ class HorovodBasics(object):
         return bool(self.lib.hvd_rocm_built())
 
     def p2p_built(self):
-        """True: the sm_100a NVLink peer-to-peer kernels are compiled in (new capability)."""
+        """True: the sm_90a NVLink peer-to-peer kernels are compiled in (new capability)."""
         return bool(self.lib.hvd_p2p_built())
 
     # ---- timeline -------------------------------------------------------------

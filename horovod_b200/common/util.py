@@ -88,7 +88,7 @@ def extension_available(ext_base_name, verbose=False):
 
 
 def gpu_available(ext_base_name='torch', verbose=False):
-    """True when the native runtime sees at least one CUDA device (the P2P kernels are sm_100a only)."""
+    """True when the native runtime sees at least one CUDA device (the P2P kernels are sm_90a only)."""
     if not extension_available(ext_base_name, verbose):
         return False
     try:

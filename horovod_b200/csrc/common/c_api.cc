@@ -65,7 +65,7 @@ int hvd_ddl_built() { return 0; }
 int hvd_ccl_built() { return 0; }
 int hvd_cuda_built() { return 1; }
 int hvd_rocm_built() { return 0; }
-int hvd_p2p_built() { return 1; }     // sm_100a NVLink kernels
+int hvd_p2p_built() { return 1; }     // sm_90a NVLink kernels
 int hvd_cuda_available() { return GpuContext::Get().Available() ? 1 : 0; }
 
 int hvd_add_process_set(const int* ranks, int n) {

@@ -147,7 +147,7 @@ struct TensorTableEntry {
 };
 
 // ---- environment knobs (names kept where the reference meaning carries over,
-// operations.cc:460-650; HVD_* are new B200-specific knobs) -----------------
+// operations.cc:460-650; HVD_* are new knobs of this library) -----------------
 #define HOROVOD_FUSION_THRESHOLD "HOROVOD_FUSION_THRESHOLD"
 #define HOROVOD_CYCLE_TIME "HOROVOD_CYCLE_TIME"
 #define HOROVOD_CACHE_CAPACITY "HOROVOD_CACHE_CAPACITY"

@@ -352,7 +352,7 @@ void Engine::BackgroundThread() {
 //   * when the oldest queued tensor is HVD_BATCH_DELAY_MS old
 //   * every cycle_time when idle, so this rank still takes part in rounds other ranks start.
 // Each fused response costs one kernel launch whose CTAs rendezvous with the peer GPUs; fewer, larger responses keep
-// SMs for the overlapping backward pass (49 launches per ResNet-50 step doubled the step time; see profiles/).
+// SMs for the overlapping backward pass (49 launches per ResNet-50 step doubled the step time).
 bool Engine::RunLoopOnce() {
   static const int64_t batch_bytes = EnvInt("HVD_BATCH_BYTES", 16ll << 20);
   static const double batch_delay_ms = EnvDouble("HVD_BATCH_DELAY_MS", 2.0);

@@ -2,7 +2,7 @@
 // allocations on one device and N concurrently launched kernels on N streams.
 // The cross-"GPU" flag protocol, chunk ownership and descriptor walking are
 // exactly what runs across NVLink; only the address mapping differs.  Lets the
-// kernels be validated (and run under compute-sanitizer) on one B200.
+// kernels be validated (and run under compute-sanitizer) on one GPU.
 #include <cuda_runtime.h>
 #include <cstdlib>
 #include <cstring>

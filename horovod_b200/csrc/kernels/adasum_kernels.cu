@@ -1,4 +1,4 @@
-// Adasum (adaptive summation) on GPUs over peer-mapped symmetric buffers, sm_100a.
+// Adasum (adaptive summation) on GPUs over peer-mapped symmetric buffers, sm_90a.
 //
 // The reference only has a CPU implementation of the pairwise Adasum reduction
 // (ops/adasum/adasum.h:195-435, vector-halving distance-doubling over MPI); its

@@ -1,4 +1,4 @@
-// Fused allreduce / reducescatter over peer-mapped symmetric buffers (sm_100a).
+// Fused allreduce / reducescatter over peer-mapped symmetric buffers (sm_90a).
 //
 // One launch per fused response:
 //   pack     every tensor -> my symmetric buffer   (prescale, cast T -> wire W)
@@ -453,7 +453,7 @@ inplace_allreduce_kernel(const __grid_constant__ CommParams cp, const __grid_con
 // HVD_PIPELINED_ALLREDUCE=1; variant kPipelined).
 //
 // The three-phase kernel above runs pack, reduce and unpack back to back: NVLink idles while HBM is busy and vice versa
-// (ncu + sweeps: 451 GB/s busBW at 1 GiB vs 834 GB/s for the zero-copy kernel).  Here the message is cut into chunks that
+// (it trails the zero-copy kernel at 1 GiB).  Here the message is cut into chunks that
 // travel through a ring of slots in the symmetric buffer, and the CTAs are specialised by blockIdx & 3:
 //     0     pack    chunk c   : tensors -> my slot (prescale, cast)
 //     1, 2  reduce  chunk c-1 : my 1/N slice of the slot on ALL ranks: multimem.ld_reduce + multimem.st (or P2P loads /
@@ -782,7 +782,7 @@ namespace {
 template <typename T, typename W> cudaError_t launch_scale(const void* in, void* out, int64_t n, double scale, cudaStream_t s) {
   int64_t per = (int64_t)kThreads * (16 / sizeof(T));
   int64_t blocks = (n + per - 1) / per;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks < 1) blocks = 1;
   scale_kernel<T><<<(int)blocks, kThreads, 0, s>>>((const T*)in, (T*)out, n, scale);
   CountKernelLaunch();

@@ -1,5 +1,5 @@
 // "pack -> flag barrier -> pull" byte-moving kernel behind allgather(v),
-// broadcast and alltoall(v) on peer-mapped symmetric buffers (sm_100a).
+// broadcast and alltoall(v) on peer-mapped symmetric buffers (sm_90a).
 //
 // Every rank copies what it sends into its own symmetric buffer (send descs),
 // the CTAs rendezvous with the same-index CTAs of all peers, then every rank
@@ -123,7 +123,7 @@ exchange_kernel(const __grid_constant__ CommParams cp, const __grid_constant__ E
 // asynchronous copies (cp.async.bulk, SASS UBLKCP) through a ring of shared-memory stages driven by ONE thread per CTA:
 // global (local HBM or a peer over NVLink) -> smem stage -> global.  No registers or LSU slots are spent on the payload
 // and (kTmaStages - 1) x 16 KiB per CTA are in flight regardless of occupancy, which is what a pure copy collective
-// (allgather / broadcast / alltoall) wants on a B200.
+// (allgather / broadcast / alltoall) wants on an H100.
 constexpr int kTmaStages = 3;  // 3 x 32 KiB: two CTAs per SM still fit in 227 KB of shared memory
 constexpr int kTmaStageBytes = kXChunk;
 

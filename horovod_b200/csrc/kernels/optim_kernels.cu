@@ -1,4 +1,4 @@
-// Multi-tensor fused optimizer updates (SGD+momentum, Adam/AdamW) for sm_100a.
+// Multi-tensor fused optimizer updates (SGD+momentum, Adam/AdamW) for sm_90a.
 // One launch updates every parameter of the model: blockIdx.y selects the
 // tensor from a device table, blockIdx.x strides over it with 16 B vectors.
 // The reference leaves the optimizer to the framework (one or several kernels

@@ -1,4 +1,4 @@
-// Host-side interface of the sm_100a peer-to-peer collective kernels.
+// Host-side interface of the sm_90a peer-to-peer collective kernels.
 //
 // These kernels replace the reference's three-launch GPU data path
 // (batched_scaled_memcpy_k -> ncclAllReduce -> batched_scaled_memcpy_k,
@@ -19,7 +19,7 @@ namespace kern {
 unsigned long long KernelLaunchCount();
 void CountKernelLaunch();
 
-constexpr int kMaxPeers = 8;          // one NVSwitch domain of the HGX B200 box
+constexpr int kMaxPeers = 8;          // one NVSwitch domain of an HGX H100 box
 constexpr int kMaxCtas = 256;         // flag slots per team
 // 256-thread CTAs capped at 128 registers: two fit on an SM and one fits NEXT TO resident compute CTAs of an
 // overlapping backward pass, so a communication kernel does not have to wait for whole SMs to drain

@@ -2,7 +2,7 @@
 // by local_size (ops/adasum_gpu_operations.cc:169-275, operations.cc:1459-1466);
 // the real pairwise reduction only runs on the CPU across nodes.  Here the true
 // VHDD Adasum runs for GPU tensors as well: on a peer-mapped team through the
-// sm_100a kernels in kernels/adasum_kernels.cu, otherwise staged through the
+// sm_90a kernels in kernels/adasum_kernels.cu, otherwise staged through the
 // host implementation (cpu::AdasumAllreduce, the numerical oracle).
 #include <cstring>
 #include "../common/logging.h"

@@ -337,7 +337,7 @@ Status GpuOps::HierarchicalAllreduce(ProcessSet& ps, Entries& es, const Response
   const auto* dtab = (const kern::TensorDesc*)ctx.Stage(device, descs.data(), descs.size() * sizeof(kern::TensorDesc), s);
   if (!dtab) return Status::UnknownError("descriptor table too large");
   if (env_.timeline && env_.timeline->Initialized()) env_.timeline->ActivityStartAll(es, HVD_ACT_HIER_ALLREDUCE);
-  HVD_CUDA(kern::LaunchPackUnpack(F, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.prescale, 0, 148, s));
+  HVD_CUDA(kern::LaunchPackUnpack(F, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.prescale, 0, 132, s));
   // ---- 1. intra-host reduce-scatter: local GPU q ends up with block q of the host-local reduction ----
   const int64_t cap = (int64_t)team.buffer_bytes();
   const int64_t win = std::min<int64_t>(B, cap / L / 128 * 128);
@@ -380,7 +380,7 @@ Status GpuOps::HierarchicalAllreduce(ProcessSet& ps, Entries& es, const Response
     st = RunExchange(team, ctx, device, s, sends, recvs, env_.params->comm_ctas, b);
     if (!st.ok()) return st;
   }
-  HVD_CUDA(kern::LaunchPackUnpack(F, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.postscale, 1, 148, s));
+  HVD_CUDA(kern::LaunchPackUnpack(F, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.postscale, 1, 132, s));
   return Status::OK();
 }
 
@@ -438,7 +438,7 @@ int GpuOps::CtasFor(int variant, int64_t seg_bytes, int n) const {
   const TunableParams& tp = *env_.params;
   const int64_t per = variant == kern::kOneShot ? 8192 : (int64_t)4096 * n;  // >= 2 rows (one-shot) or one row per rank (two-shot) per CTA
   const int64_t big_ctas = env_.large_msg_ctas;
-  // (2 x B200: a 1 MiB one-shot took 22 us on 16 CTAs — four dependent NVLink trips per CTA — against NCCL's 14 us)
+  // (a one-shot CTA makes four dependent NVLink trips, so a 1 MiB message wants more than 16 CTAs)
   const int64_t cap_ctas = seg_bytes <= (256 << 10) ? std::min<int64_t>(tp.comm_ctas, 16)
                          : seg_bytes <= (16 << 20) ? std::min<int64_t>(tp.comm_ctas, 64)
                          : seg_bytes < (64 << 20) ? tp.comm_ctas : std::max<int64_t>(tp.comm_ctas, big_ctas);
@@ -654,11 +654,10 @@ Status GpuOps::Allreduce(ProcessSet& ps, Entries& es, const Response& r, int dev
       if (lat_lane) cap = lat_area / 128 * 128;
       const TunableParams& tp = *env_.params;
       // ---- large fused messages of plain tensors: TWO LANES.  The three-phase kernel is pack (HBM) -> NVLink phase -> unpack
-      // (HBM) back to back, so the links idle while it packs and HBM idles while it reduces (8 x B200, 1 GiB: 2.98 ms vs
-      // 2.24 ms for the pure NVLink phase of the zero-copy kernel).  The message is cut into segments that alternate
+      // (HBM) back to back, so the links idle while it packs and HBM idles while it reduces.  The message is cut into segments that alternate
       // between two streams — lane 0 = the hvd stream on channel 0 / buffer slot 0, lane 1 = an auxiliary stream on its
       // own barrier channel / slot 1 — so one lane's pack and unpack run under the other lane's NVLink phase.  No
-      // fine-grained hand-offs: the overlap comes from two ordinary kernels being resident together (2 x 128 CTAs <= 296
+      // fine-grained hand-offs: the overlap comes from two ordinary kernels being resident together (2 x 128 CTAs <= 264
       // slots).  Only the two-barrier variants (two-shot / NVLS) may reuse a slot back to back: after barrier 2 nobody reads
       // a peer's buffer any more.
       int64_t fused_total = 0;
@@ -705,8 +704,8 @@ Status GpuOps::Allreduce(ProcessSet& ps, Entries& es, const Response& r, int dev
         // opt-in: software-pipelined pack / NVLS / unpack for large segments of plain tensors (docs/roadmap.md B1)
         const bool pipelined_on = env_.pipelined;
         const int64_t pipe_chunk = env_.pipe_chunk_bytes, pipe_min = env_.pipe_min_bytes;
-        // (measured at N = 2, where the reduce stage is plain P2P: 195 GB/s pipelined vs 476 GB/s for the three-phase kernel
-        // at 1 GiB — the pipeline only pays when the reduce stage is the in-switch multimem one)
+        // (at N = 2, where the reduce stage is plain P2P, the pipeline lost to the three-phase kernel at 1 GiB — it only pays
+        // when the reduce stage is the in-switch multimem one)
         if (pipelined_on && env_.variant == "auto" && nvls_ok && n >= 4 && seg_bytes >= pipe_min && cap / pipe_chunk >= 2) {
           variant = kern::kPipelined;
           a.pipe_chunk_bytes = pipe_chunk;
@@ -807,10 +806,10 @@ Status GpuOps::NcclAllreduce(ProcessSet& ps, Entries& es, const Response& r, int
   if (!fusion) return Status::UnknownError("out of device memory for the NCCL fusion buffer");
   const auto* dtab = (const kern::TensorDesc*)ctx.Stage(device, descs.data(), descs.size() * sizeof(kern::TensorDesc), s);
   if (!dtab) return Status::UnknownError("descriptor table too large");
-  HVD_CUDA(kern::LaunchPackUnpack(fusion, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.prescale, 0, 148, s));
+  HVD_CUDA(kern::LaunchPackUnpack(fusion, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.prescale, 0, 132, s));
   st = NcclAllReduceCall(*ps.nccl, fusion, fusion, total / (int64_t)esz, r.dtype, r.reduce_op, s);
   if (!st.ok()) return st;
-  HVD_CUDA(kern::LaunchPackUnpack(fusion, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.postscale, 1, 148, s));
+  HVD_CUDA(kern::LaunchPackUnpack(fusion, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.postscale, 1, 132, s));
   return Status::OK();
 }
 

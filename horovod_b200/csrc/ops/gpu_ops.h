@@ -83,7 +83,7 @@ struct GpuOpEnv {
   size_t symm_buffer_bytes = 128ull << 20;
   bool want_multicast = true;
   // software-pipelined allreduce of large plain (unregistered) tensors: pack / reduce / unpack CTAs on a chunk ring
-  bool pipelined = false;  // opt-in: measured 8 x B200: 328 GB/s (4 MiB chunks) .. 455 GB/s (16 MiB) vs 630 GB/s for the three-phase kernel
+  bool pipelined = false;  // opt-in: slower than the three-phase kernel where it was measured (8 GPUs)
   int64_t pipe_chunk_bytes = 4 << 20, pipe_min_bytes = 32 << 20, pipe_rblock_bytes = 16384;
   int64_t large_msg_ctas = 256;   // CTAs for >= 64 MiB fused messages (two per SM)
   bool broadcast_multicast = true;
@@ -93,12 +93,12 @@ struct GpuOpEnv {
   // buffer tail) instead of queueing behind large ones on the main stream; 0 = off
   int64_t latency_lane_bytes = 256 << 10;
   bool adasum_persistent = true;   // single-launch Adasum (grid barriers inside the kernel) instead of 2 + 2 log2(N) launches
-  bool dual_lane = false;  // opt-in: measured on 8 x B200 it does not pay (64 MiB: 393 vs 597 GB/s, 1 GiB: 618 vs 619): each lane's
+  bool dual_lane = false;  // opt-in: where it was measured (8 GPUs) it did not pay: each lane's
                            // pack / unpack runs at half the CTAs and the two NVLink phases contend
   int64_t dual_lane_min_bytes = 64 << 20;
   // teams of up to this many ranks reduce IPC-registered plain tensors in place with the P2P two-shot kernel; larger
   // teams keep the fused pack + NVLS + unpack kernel for sums and use IPC only for MIN / MAX / PRODUCT
-  int ipc_max_ranks = 4;  // measured: 4 x B200, 1 GiB: 655 GB/s zero-copy P2P vs 534 GB/s three-phase NVLS vs 629 GB/s NCCL; at 8 GPUs the two tie
+  int ipc_max_ranks = 4;  // at 4 GPUs zero-copy P2P beat the three-phase NVLS kernel where it was measured; at 8 GPUs the two tied
   // Kernel-variant crossovers measured on this box when the global set's team is created (cached per topology under
   // HVD_CACHE_DIR): the engine applies them to the tunable parameters unless the environment pinned those.
   int64_t zero_copy_nvls_min_bytes = 1 << 20;  // registered tensors: multimem from this size (two-shot P2P below)

@@ -455,7 +455,7 @@ void CapturedAllreduce(at::Tensor tensor, int reduce_op, double prescale, double
                                                postscale, process_set_id, max_ctas, (void*)stream));
 }
 
-// ---- fused optimizer kernels (B200-native extra; see kernels/optim_kernels.cu) --------------
+// ---- fused optimizer kernels (an extra of this library; see kernels/optim_kernels.cu) --------------
 void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momenta, double lr,
                   double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step) {
   TORCH_CHECK(params.size() == grads.size(), "fused_sgd: list sizes differ");

@@ -1,7 +1,7 @@
 """Pinned-memory, side-stream host→device prefetcher for the training input pipeline.
 
 The reference leaves host→device staging to the framework's DataLoader (its synthetic benchmarks create the batch on
-the device once: examples/pytorch/pytorch_synthetic_benchmark.py:79-86).  On a B200 a ResNet-50 step is ~17 ms, so a
+the device once: examples/pytorch/pytorch_synthetic_benchmark.py:79-86).  A ResNet-50 step takes tens of milliseconds, so a
 38 MB batch copied synchronously from pageable memory is a visible bubble.  ``DevicePrefetcher`` wraps any iterable of
 (nested) CPU tensors: batch *i+1* is copied into a ring of pinned staging buffers and sent over a dedicated copy
 stream while batch *i* is being consumed; the consumer stream only waits on an event.

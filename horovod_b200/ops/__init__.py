@@ -1,4 +1,4 @@
-"""Python access to the native sm_100a operations that are not collectives of the `hvd.*` API:
+"""Python access to the native sm_90a operations that are not collectives of the `hvd.*` API:
 
 * `fused_sgd_step`, `fused_adam_step` — multi-tensor optimizer kernels (`csrc/kernels/optim_kernels.cu`);
 * `symm_empty`, `symm_available` — registered symmetric memory for the zero-copy allreduce path;

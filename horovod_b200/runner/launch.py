@@ -79,7 +79,7 @@ def check_build(verbose):
         [{gloo}] Native mesh (TCP + shared memory; fills Gloo's role)
 
     Available Tensor Operations:
-        [{p2p}] NVLink P2P (sm_100a one-shot / two-shot / NVLS kernels)
+        [{p2p}] NVLink P2P (sm_90a one-shot / two-shot / NVLS kernels)
         [{nccl_ops}] NCCL (baseline)
         [{ddl_ops}] DDL
         [{ccl_ops}] CCL

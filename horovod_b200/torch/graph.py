@@ -1,9 +1,9 @@
 """CUDA-graph training step: forward + backward captured once, replayed every step; gradients are reduced and the
 (fused) optimizer applied right after the replay.
 
-Why (B200-first; nothing like it exists in the reference): a ResNet-50 / BERT step in eager PyTorch issues 1–3 thousand
-kernel launches, and on a B200 the GPU finishes them faster than one Python thread can issue them — the measured step
-time is the host's launch time, identical at 1 and 8 GPUs.  Replaying the step as ONE graph launch removes that bound.
+Why (nothing like it exists in the reference): a ResNet-50 / BERT step in eager PyTorch issues 1–3 thousand
+kernel launches, and a GPU such as the H100 can finish them faster than one Python thread issues them — the step
+time then is the host's launch time.  Replaying the step as ONE graph launch removes that bound.
 On several GPUs the gradient allreduce is PART of the graph: while the step is being captured, the hook of the last
 gradient of every zero-copy bucket records that bucket's `hvd.captured_allreduce_` kernel (multimem / P2P in-place
 reduction on peer-mapped memory, flag barrier inside the kernel) on a forked high-priority stream, so on replay the

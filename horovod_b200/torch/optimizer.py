@@ -6,7 +6,7 @@ _DistributedOptimizer, _DistributedAdasumOptimizer).  Mechanism differences:
 hooks use `register_post_accumulate_grad_hook` (fires right after AccumulateGrad
 with no autograd-graph surgery), completion is event-chained (no host sync per
 tensor), and `fused=True` replaces the wrapped SGD/Adam(W) math by one
-multi-tensor sm_100a kernel (csrc/kernels/optim_kernels.cu).
+multi-tensor sm_90a kernel (csrc/kernels/optim_kernels.cu).
 """
 import os
 import warnings
@@ -158,7 +158,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                     self._requires_update.add(p)
                     self._grad_accs.append(p.register_post_accumulate_grad_hook(self._make_hook(p)))
 
-    # ---- zero-copy gradient buckets (B200-first: the reference allreduces per-parameter tensors through a fusion buffer) ----
+    # ---- zero-copy gradient buckets (new here: the reference allreduces per-parameter tensors through a fusion buffer) ----
     def _setup_buckets(self, cap_bytes):
         """Lays the gradients of all dense CUDA parameters out in a few flat buffers of registered symmetric memory
         (p.grad becomes a view, like DDP's gradient_as_bucket_view). A bucket is allreduced IN PLACE as one tensor by the
@@ -336,8 +336,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             return False
         lo_pri, hi_pri = torch.cuda.Stream.priority_range() if hasattr(torch.cuda.Stream, 'priority_range') else (0, -1)
         self._graph_capture = {'comm': torch.cuda.Stream(priority=hi_pri), 'launched': set(),
-                               # few CTAs while backward still needs the SMs (8 x B200, BERT-large: 16 CTAs 30.64 ms/step, 32: 30.73,
-                               # 64: 31.82), all of them for the tail bucket(s) that nothing overlaps any more
+                               # few CTAs while backward still needs the SMs, all of them for the tail bucket(s) that nothing overlaps any more
                                # (without NVLS — teams of 2 — the P2P two-shot kernel needs more CTAs to keep up with backward)
                                'ctas': int(os.environ.get('HVD_GRAPH_COMM_CTAS', '16' if '+mc' in mpi_ops.gpu_backend_info() and self.process_set.size() >= 4 else '32')),
                                'tail_ctas': int(os.environ.get('HVD_GRAPH_COMM_TAIL_CTAS', '128')), 'tail': False,

@@ -1,5 +1,5 @@
 """pip / setuptools entry point.  `pip install -e .` (or `python setup.py build_ext --inplace`) compiles the native
-runtime IN-TREE for sm_100a through horovod_b200/build.py (g++ + nvcc, no CMake needed; a CMakeLists.txt for the core
+runtime IN-TREE for sm_90a through horovod_b200/build.py (g++ + nvcc, no CMake needed; a CMakeLists.txt for the core
 library is provided as well).  Role parity: the reference's setup.py (CMake extension driver)."""
 import os
 import sys
@@ -53,7 +53,7 @@ class native_selftest(Command):
 setup(
     name='horovod_b200',
     version='0.1.0',
-    description='Blackwell-native data-parallel collective library with the capabilities of Horovod',
+    description='Hopper-native (H100) data-parallel collective library with the capabilities of Horovod',
     packages=find_packages(include=['horovod_b200', 'horovod_b200.*', 'horovod']),
     package_data={'horovod_b200': ['lib/*.so', 'csrc/**/*']},
     scripts=['bin/hvdrun', 'bin/horovodrun'],

@@ -10,7 +10,7 @@ if REPO not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (run on the B200 box with `pytest -m gpu`)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (run on an H100 with `pytest -m gpu`)")
 
 
 def run_parallel(script, np=2, args=(), timeout=180, env=None, expect_fail=False, launcher_args=()):

@@ -1,5 +1,5 @@
 """Multi-GPU runs of the op matrix over the NVLink P2P kernels (and the NCCL baseline). Needs >= 2 GPUs:
-`gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu`."""
+`python -m pytest tests/test_gpu_multi.py -m gpu` on a machine with several GPUs."""
 import pytest
 import torch
 
