@@ -1015,6 +1015,27 @@ Status Engine::CapturedAllreduce(void* ptr, int64_t bytes, DataType dtype, Reduc
   return gpu_ops_->CapturedAllreduce(*ps, ptr, bytes, dtype, op, prescale, postscale, max_ctas, (cudaStream_t)stream);
 }
 
+Status Engine::CapturedReducescatter(void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale, double postscale,
+                                     int32_t psid, int max_ctas, void* stream) {
+  std::shared_ptr<ProcessSet> ps;
+  Status st = CheckSet(psid, &ps);
+  if (!st.ok()) return st;
+  if (op == ReduceOp::ADASUM) return Status::InvalidArgument("captured reducescatter does not support Adasum");
+  if (op == ReduceOp::AVERAGE) { op = ReduceOp::SUM; postscale /= (double)ps->set_size(); }
+  if (ps->set_size() == 1) return Status::OK();
+  captured_launches_.fetch_add(1, std::memory_order_relaxed);
+  return gpu_ops_->CapturedReducescatter(*ps, ptr, bytes, dtype, op, prescale, postscale, max_ctas, (cudaStream_t)stream);
+}
+
+Status Engine::CapturedAllgather(void* ptr, int64_t bytes, int32_t psid, int max_ctas, void* stream) {
+  std::shared_ptr<ProcessSet> ps;
+  Status st = CheckSet(psid, &ps);
+  if (!st.ok()) return st;
+  if (ps->set_size() == 1) return Status::OK();
+  captured_launches_.fetch_add(1, std::memory_order_relaxed);
+  return gpu_ops_->CapturedAllgather(*ps, ptr, bytes, max_ctas, (cudaStream_t)stream);
+}
+
 Status Engine::StartTimeline(const std::string& file, bool mark_cycles) {
   if (!initialized_.load()) return Status::PreconditionError(NOT_INITIALIZED_ERROR_MSG);
   std::lock_guard<std::mutex> l(tl_mu_);

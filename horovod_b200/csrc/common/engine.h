@@ -84,6 +84,10 @@ class Engine {
   // `stream` is a cudaStream_t.  See GpuOps::CapturedAllreduce.
   Status CapturedAllreduce(void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale, double postscale,
                            int32_t process_set_id, int max_ctas, void* stream);
+  // The two halves of a sharded optimizer step, same contract (see GpuOps::CapturedReducescatter / CapturedAllgather).
+  Status CapturedReducescatter(void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale, double postscale,
+                               int32_t process_set_id, int max_ctas, void* stream);
+  Status CapturedAllgather(void* ptr, int64_t bytes, int32_t process_set_id, int max_ctas, void* stream);
 
   // ---- timeline ----
   Status StartTimeline(const std::string& file, bool mark_cycles);

@@ -218,6 +218,38 @@ int hvd_sim_inplace(int nranks, int device, int64_t bytes, const uint64_t* ptrs,
   return Finish(nranks, e);
 }
 
+// The two halves of a sharded optimizer step over N simulated ranks: ptrs[r] = rank r's registered range (plain device
+// memory here), rank r owns the contiguous slice [r * bytes / n, (r + 1) * bytes / n).  `reducescatter` != 0 runs the
+// in-place reduce-scatter (dtype, op, scale as hvd_sim_inplace), else the in-place allgather (bytes only).
+static int hvd_sim_inplace_sharded(int nranks, int device, int64_t bytes, const uint64_t* ptrs, int dtype, int op, int ctas, double scale,
+                            int repeats, int reducescatter) {
+  if (cudaSetDevice(device) != cudaSuccess) return -1;
+  Sim* sim = GetSim(nranks, device, 1 << 20);
+  if (!sim) return -1;
+  cudaDeviceSynchronize();
+  for (int it = 0; it < repeats; ++it) {
+    for (int r = 0; r < nranks; ++r) {
+      kern::InplaceArgs a {};
+      for (int p = 0; p < nranks; ++p) a.ptr[p] = (void*)ptrs[p];
+      a.mc = nullptr; a.bytes = bytes; a.scale = scale; a.op = op; a.dtype = dtype; a.use_multicast = 0; a.ctas = ctas;
+      kern::CommParams cp = sim->teams[r]->Params(sim->teams[r]->NextSlot());
+      cudaError_t e = reducescatter ? kern::LaunchInplaceReducescatter(cp, a, sim->streams[r])
+                                    : kern::LaunchInplaceAllgather(cp, a, sim->streams[r]);
+      if (e != cudaSuccess) return (int)e;
+    }
+  }
+  return Finish(nranks, cudaDeviceSynchronize());
+}
+
+int hvd_sim_inplace_reducescatter(int nranks, int device, int64_t bytes, const uint64_t* ptrs, int dtype, int op, int ctas,
+                                  double scale, int repeats) {
+  return hvd_sim_inplace_sharded(nranks, device, bytes, ptrs, dtype, op, ctas, scale, repeats, 1);
+}
+
+int hvd_sim_inplace_allgather(int nranks, int device, int64_t bytes, const uint64_t* ptrs, int ctas, int repeats) {
+  return hvd_sim_inplace_sharded(nranks, device, bytes, ptrs, 0, 1, ctas, 1.0, repeats, 0);
+}
+
 void hvd_sim_reset() {
   for (auto& kv : g_sims) for (auto st : kv.second.streams) cudaStreamDestroy(st);
   g_sims.clear();

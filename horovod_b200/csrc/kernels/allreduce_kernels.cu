@@ -447,6 +447,144 @@ inplace_allreduce_kernel(const __grid_constant__ CommParams cp, const __grid_con
   if (threadIdx.x == 0) cp.epochs[cta] = epoch;
 }
 
+// ---------------------------------------------------------------------------
+// Zero-copy reduce-scatter / allgather on REGISTERED tensors, the two halves of a sharded optimizer step (ZeRO-1).
+// Contiguous ownership, not the interleaved chunks of the allreduce above: for a range of `bytes` (a multiple of
+// 16 * nranks) rank r owns [r*S, (r+1)*S) with S = bytes / nranks, so that its shard is one slice it can update.
+// CTA b of every rank covers the same chunks of every shard and only synchronises with CTA b of its peers; a launch on
+// rank q completes only after all of its CTAs passed barrier B, i.e. after every CTA of every peer did its last access.
+
+// In-switch reduction of [lo, hi) stored to `dst` only (a plain local store instead of multimem.st).
+template <typename W, int UN>
+__device__ __forceinline__ void nvls_reduce_rows(const char* mc, char* dst, int64_t lo, int64_t hi,
+                                                 typename ScaleOf<typename Traits<W>::Acc>::type scale) {
+  using A = typename Traits<W>::Acc;
+  using S = typename ScaleOf<A>::type;
+  constexpr int NW = 16 / (int)sizeof(W);
+  for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)UN * kRowBytes) {
+    uint4 v[UN];
+#pragma unroll
+    for (int j = 0; j < UN; ++j) { const int64_t o = o0 + (int64_t)j * kRowBytes; if (o < hi) v[j] = Nvls<W>::ld_reduce(mc + o); }
+#pragma unroll
+    for (int j = 0; j < UN; ++j) {
+      const int64_t o = o0 + (int64_t)j * kRowBytes;
+      if (o < hi) {
+        if (scale != (S)1) {
+          A acc[NW];
+          unpack_vec<W, NW>(v[j], acc);
+#pragma unroll
+          for (int i = 0; i < NW; ++i) acc[i] = apply_scale<A>(acc[i], scale);
+          v[j] = pack_vec<W, NW>(acc);
+        }
+        st_stream(dst + o, v[j]);
+      }
+    }
+  }
+}
+
+//   barrier A   every rank's gradients are final
+//   reduce      rank r loads its shard out of all N tensors (or one multimem.ld_reduce), combines, scales and stores the
+//               result into ITS OWN tensor only; bytes outside the shard are neither reduced nor written
+//   barrier B   no peer may overwrite its gradients (next zero_grad / backward) while a reader still loads them
+template <typename W, int NR>
+__global__ void __launch_bounds__(kThreads, 2)
+inplace_reducescatter_kernel(const __grid_constant__ CommParams cp, const __grid_constant__ InplaceArgs a) {
+  using A = typename Traits<W>::Acc;
+  using S = typename ScaleOf<A>::type;
+  constexpr int NW = 16 / (int)sizeof(W);
+  constexpr int U = 8 / NR;
+  const int cta = blockIdx.x, grid = gridDim.x;
+  uint32_t epoch = cp.epochs[cta];
+  const int64_t shard = a.bytes / cp.nranks, base = shard * cp.rank;
+  const int chunk_bytes = a.chunk_bytes;
+  const int64_t nchunks = (shard + chunk_bytes - 1) / chunk_bytes;
+  const S scale = (S)a.scale;
+  char* mine = reinterpret_cast<char*>(a.ptr[cp.rank]);
+  bool alive = peer_barrier(cp, epoch, cta);
+  for (int64_t c = cta; c < nchunks && alive; c += grid) {
+    const int64_t lo = base + c * chunk_bytes;
+    const int64_t hi = lo + chunk_bytes < base + shard ? lo + chunk_bytes : base + shard;
+    if (a.use_multicast) {
+      if constexpr (Nvls<W>::ok) {
+        const char* mc = reinterpret_cast<const char*>(a.mc);
+        if (a.nvls_unroll == 8) nvls_reduce_rows<W, 8>(mc, mine, lo, hi, scale);
+        else nvls_reduce_rows<W, 4>(mc, mine, lo, hi, scale);
+      }
+    } else {
+      for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)U * kRowBytes) {
+        uint4 v[U][NR];
+#pragma unroll
+        for (int j = 0; j < U; ++j) {
+          const int64_t o = o0 + (int64_t)j * kRowBytes;
+          if (o < hi) {
+#pragma unroll
+            for (int p = 0; p < NR; ++p) {
+              int q = cp.rank + p; if (q >= cp.nranks) q -= cp.nranks;
+              if (p < cp.nranks) v[j][p] = ld_stream(reinterpret_cast<const char*>(a.ptr[q]) + o);
+            }
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < U; ++j) {
+          const int64_t o = o0 + (int64_t)j * kRowBytes;
+          if (o < hi) {
+            A acc[NW];
+            peer_combine<W, NR>(cp, v[j], a.op, acc);
+#pragma unroll
+            for (int i = 0; i < NW; ++i) acc[i] = apply_scale<A>(acc[i], scale);
+            st_stream(mine + o, pack_vec<W, NW>(acc));
+          }
+        }
+      }
+    }
+  }
+  if (alive) peer_barrier(cp, epoch, cta);
+  if (threadIdx.x == 0) cp.epochs[cta] = epoch;
+}
+
+//   barrier A   every owner's update of its shard is final and every peer finished reading its own copy (backward)
+//   store       the owner reads its shard locally and writes it into every peer's copy (16 B stores per peer, or one
+//               multimem.st through the multicast alias); bytes only, the dtype does not matter
+//   barrier B   every shard landed before any rank's launch completes
+template <int NR>
+__global__ void __launch_bounds__(kThreads, 2)
+inplace_allgather_kernel(const __grid_constant__ CommParams cp, const __grid_constant__ InplaceArgs a) {
+  constexpr int U = 8;
+  const int cta = blockIdx.x, grid = gridDim.x;
+  uint32_t epoch = cp.epochs[cta];
+  const int64_t shard = a.bytes / cp.nranks, base = shard * cp.rank;
+  const int chunk_bytes = a.chunk_bytes;
+  const int64_t nchunks = (shard + chunk_bytes - 1) / chunk_bytes;
+  const char* mine = reinterpret_cast<const char*>(a.ptr[cp.rank]);
+  bool alive = peer_barrier(cp, epoch, cta);
+  for (int64_t c = cta; c < nchunks && alive; c += grid) {
+    const int64_t lo = base + c * chunk_bytes;
+    const int64_t hi = lo + chunk_bytes < base + shard ? lo + chunk_bytes : base + shard;
+    for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)U * kRowBytes) {
+      uint4 v[U];
+#pragma unroll
+      for (int j = 0; j < U; ++j) { const int64_t o = o0 + (int64_t)j * kRowBytes; if (o < hi) v[j] = ld_stream(mine + o); }
+#pragma unroll
+      for (int j = 0; j < U; ++j) {
+        const int64_t o = o0 + (int64_t)j * kRowBytes;
+        if (o < hi) {
+          if (a.use_multicast) {
+            multimem_st(reinterpret_cast<char*>(a.mc) + o, v[j]);
+          } else {
+#pragma unroll
+            for (int p = 1; p < NR; ++p) {  // p = 0 is my own copy, which already holds the shard
+              int q = cp.rank + p; if (q >= cp.nranks) q -= cp.nranks;
+              if (p < cp.nranks) st_stream(reinterpret_cast<char*>(a.ptr[q]) + o, v[j]);
+            }
+          }
+        }
+      }
+    }
+  }
+  if (alive) peer_barrier(cp, epoch, cta);
+  if (threadIdx.x == 0) cp.epochs[cta] = epoch;
+}
+
 
 // ---------------------------------------------------------------------------
 // Software-pipelined allreduce for LARGE fused responses of ordinary (unregistered) tensors (opt-in,
@@ -640,6 +778,31 @@ cudaError_t launch_inplace(const CommParams& cp, const InplaceArgs& a, cudaStrea
   return cudaGetLastError();
 }
 
+template <typename W>
+cudaError_t launch_reducescatter(const CommParams& cp, const InplaceArgs& a, cudaStream_t s) {
+  if (cp.nranks <= 2) inplace_reducescatter_kernel<W, 2><<<a.ctas, kThreads, 0, s>>>(cp, a);
+  else if (cp.nranks <= 4) inplace_reducescatter_kernel<W, 4><<<a.ctas, kThreads, 0, s>>>(cp, a);
+  else inplace_reducescatter_kernel<W, 8><<<a.ctas, kThreads, 0, s>>>(cp, a);
+  CountKernelLaunch();
+  return cudaGetLastError();
+}
+
+// Checks shared by the sharded launchers and the chunk size / NVLS unroll they pick (as LaunchInplaceAllreduce does).
+bool prepare_sharded(const CommParams& cp, InplaceArgs* a) {
+  if (a->ctas < 1 || a->ctas > kMaxCtas || cp.nranks < 1 || cp.nranks > kMaxPeers || a->bytes <= 0 ||
+      a->bytes % (16 * (int64_t)cp.nranks))
+    return false;
+  int64_t want = a->bytes / ((int64_t)a->ctas * cp.nranks);
+  int chunk = (int)((want / kRowBytes) * kRowBytes);
+  if (chunk < kRowBytes) chunk = kRowBytes;
+  const int max_chunk = [] { const char* e = getenv("HVD_INPLACE_CHUNK_BYTES"); int v = e ? atoi(e) : kChunkBytes;
+                                    return v < kRowBytes ? kRowBytes : (v / kRowBytes) * kRowBytes; }();
+  if (chunk > max_chunk) chunk = max_chunk;
+  a->chunk_bytes = chunk;
+  a->nvls_unroll = [] { const char* e = getenv("HVD_NVLS_UNROLL"); return e && atoi(e) == 8 ? 8 : 4; }();
+  return true;
+}
+
 // Stand-alone pack / unpack (NCCL baseline path): whole grid strides over rows.
 template <typename T, typename W>
 __global__ void __launch_bounds__(kThreads)
@@ -770,6 +933,33 @@ cudaError_t LaunchInplaceAllreduce(const CommParams& cp, const InplaceArgs& args
     case 5: if (a.use_multicast) return cudaErrorInvalidValue; return launch_inplace<int64_t>(cp, a, stream);
     default: return cudaErrorInvalidValue;
   }
+}
+
+cudaError_t LaunchInplaceReducescatter(const CommParams& cp, const InplaceArgs& args, cudaStream_t stream) {
+  InplaceArgs a = args;
+  if (!prepare_sharded(cp, &a)) return cudaErrorInvalidValue;
+  const bool sum_like = a.op == 1;
+  if (a.use_multicast && (!sum_like || a.mc == nullptr)) return cudaErrorInvalidValue;
+  switch (a.dtype) {
+    case 7: return launch_reducescatter<float>(cp, a, stream);
+    case 6: return launch_reducescatter<__half>(cp, a, stream);
+    case 10: return launch_reducescatter<__nv_bfloat16>(cp, a, stream);
+    case 8: if (a.use_multicast) return cudaErrorInvalidValue; return launch_reducescatter<double>(cp, a, stream);
+    case 4: if (a.use_multicast) return cudaErrorInvalidValue; return launch_reducescatter<int32_t>(cp, a, stream);
+    case 5: if (a.use_multicast) return cudaErrorInvalidValue; return launch_reducescatter<int64_t>(cp, a, stream);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+cudaError_t LaunchInplaceAllgather(const CommParams& cp, const InplaceArgs& args, cudaStream_t stream) {
+  InplaceArgs a = args;
+  if (!prepare_sharded(cp, &a)) return cudaErrorInvalidValue;
+  if (a.use_multicast && a.mc == nullptr) return cudaErrorInvalidValue;
+  if (cp.nranks <= 2) inplace_allgather_kernel<2><<<a.ctas, kThreads, 0, stream>>>(cp, a);
+  else if (cp.nranks <= 4) inplace_allgather_kernel<4><<<a.ctas, kThreads, 0, stream>>>(cp, a);
+  else inplace_allgather_kernel<8><<<a.ctas, kThreads, 0, stream>>>(cp, a);
+  CountKernelLaunch();
+  return cudaGetLastError();
 }
 
 cudaError_t LaunchPackUnpack(void* buffer, const TensorDesc* descs, int ndesc, int64_t total_bytes, int dtype,

@@ -118,6 +118,14 @@ struct InplaceArgs {
   int nvls_unroll;    // filled in by the launcher (4 | 8 multimem.ld_reduce in flight per thread)
 };
 cudaError_t LaunchInplaceAllreduce(const CommParams& cp, const InplaceArgs& args, cudaStream_t stream);
+// The two halves of a sharded optimizer step on a registered range, with contiguous shards: rank r owns
+// [r*S, (r+1)*S), S = bytes / nranks; bytes must be a multiple of 16 * nranks (cudaErrorInvalidValue otherwise).
+// Reduce-scatter: rank r's shard of its own tensor receives the reduction (scaled by `scale`); nothing else is written.
+// Multicast for SUM-like ops on fp32 / fp16 / bf16 only.
+cudaError_t LaunchInplaceReducescatter(const CommParams& cp, const InplaceArgs& args, cudaStream_t stream);
+// Allgather: rank r's shard of its own tensor is copied into every peer's tensor.  Bytes only: `dtype`, `op` and `scale`
+// are ignored.
+cudaError_t LaunchInplaceAllgather(const CommParams& cp, const InplaceArgs& args, cudaStream_t stream);
 
 // Generic "pack -> barrier -> pull" used by allgather / broadcast / alltoall.
 // send: local src -> local symmetric buffer offset; recv: peer buffer offset -> local dst.

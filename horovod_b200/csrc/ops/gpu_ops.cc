@@ -431,6 +431,43 @@ Status GpuOps::CapturedAllreduce(ProcessSet& ps, void* ptr, int64_t bytes, DataT
   return Status::OK();
 }
 
+// The two halves of a sharded optimizer step, launched exactly like CapturedAllreduce (caller's stream, graph channel, no
+// negotiation).  Rank r owns the contiguous slice [r*S, (r+1)*S), S = bytes / n, of the registered range.
+Status GpuOps::CapturedReducescatter(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
+                                     double postscale, int max_ctas, cudaStream_t stream) {
+  std::shared_ptr<SymmTeam> team;
+  { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
+  if (!team) return Status::PreconditionError("captured reducescatter: the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
+  if (team->abort_state() != 0) return Status::Aborted("captured reducescatter: the team was aborted");
+  if (bytes % (16 * (int64_t)team->nranks()) != 0)
+    return Status::InvalidArgument("captured reducescatter: the byte size must be a multiple of 16 * the process set size");
+  kern::InplaceArgs ia {};
+  if (max_ctas <= 0) max_ctas = env_.params->comm_ctas;
+  if (!BuildInplaceArgs(*team, ptr, bytes, dtype, op, prescale, postscale, -1, std::min(max_ctas, kern::kMaxCtas), &ia))
+    return Status::InvalidArgument("captured reducescatter: tensor is not (entirely) inside registered symmetric memory, is not 16 B "
+                                   "aligned, or combines MIN/MAX/PRODUCT with scale factors");
+  cudaError_t ce = kern::LaunchInplaceReducescatter(team->Params(0, kern::kGraphChannel), ia, stream);
+  if (ce != cudaSuccess) return Status::UnknownError(std::string("captured reducescatter launch failed: ") + cudaGetErrorString(ce));
+  return Status::OK();
+}
+
+Status GpuOps::CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int max_ctas, cudaStream_t stream) {
+  std::shared_ptr<SymmTeam> team;
+  { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
+  if (!team) return Status::PreconditionError("captured allgather: the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
+  if (team->abort_state() != 0) return Status::Aborted("captured allgather: the team was aborted");
+  if (bytes % (16 * (int64_t)team->nranks()) != 0)
+    return Status::InvalidArgument("captured allgather: the byte size must be a multiple of 16 * the process set size");
+  kern::InplaceArgs ia {};
+  if (max_ctas <= 0) max_ctas = env_.params->comm_ctas;
+  // a byte copy: described as an fp32 SUM so that the multicast store follows the same policy as the reductions
+  if (!BuildInplaceArgs(*team, ptr, bytes, DataType::FLOAT32, ReduceOp::SUM, 1.0, 1.0, -1, std::min(max_ctas, kern::kMaxCtas), &ia))
+    return Status::InvalidArgument("captured allgather: tensor is not (entirely) inside registered symmetric memory or is not 16 B aligned");
+  cudaError_t ce = kern::LaunchInplaceAllgather(team->Params(0, kern::kGraphChannel), ia, stream);
+  if (ce != cudaSuccess) return Status::UnknownError(std::string("captured allgather launch failed: ") + cudaGetErrorString(ce));
+  return Status::OK();
+}
+
 // CTAs of a fused allreduce launch.  Small messages are latency bound (few CTAs = cheap flag barrier, SMs left to compute);
 // >= 64 MiB of plain tensors are bound by the local pack / unpack phases, which need two CTAs per SM (ncu: 12.5 % warps
 // active at one).

@@ -125,6 +125,12 @@ class GpuOps {
   // graph channel, with no negotiation: callable from framework threads.
   Status CapturedAllreduce(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                            double postscale, int max_ctas, cudaStream_t stream);
+  // Sharded optimizer step (ZeRO-1), same launch contract as CapturedAllreduce: rank r owns [r*S, (r+1)*S), S = bytes / n,
+  // and bytes must be a multiple of 16 * n.  Reduce-scatter: rank r's shard of its own tensor receives the reduction.
+  // Allgather: every owner's shard is copied into every peer's tensor.
+  Status CapturedReducescatter(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
+                               double postscale, int max_ctas, cudaStream_t stream);
+  Status CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int max_ctas, cudaStream_t stream);
   bool BuildInplaceArgs(SymmTeam& team, const void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                         double postscale, int64_t expect_off, int max_ctas, kern::InplaceArgs* out);
 

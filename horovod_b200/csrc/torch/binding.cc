@@ -455,6 +455,27 @@ void CapturedAllreduce(at::Tensor tensor, int reduce_op, double prescale, double
                                                postscale, process_set_id, max_ctas, (void*)stream));
 }
 
+// The two halves of a sharded optimizer step on a registered tensor, launched like CapturedAllreduce.  Rank r owns the
+// contiguous slice [r*S, (r+1)*S) of the tensor's bytes, S = bytes / set size.
+void CapturedReducescatter(at::Tensor tensor, int reduce_op, double prescale, double postscale, int process_set_id, int max_ctas) {
+  TORCH_CHECK(tensor.is_cuda(), "captured_reducescatter_: CUDA tensor expected");
+  TORCH_CHECK(tensor.is_non_overlapping_and_dense(), "captured_reducescatter_: tensor must be dense");
+  c10::cuda::CUDAGuard guard(tensor.device());
+  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(tensor.get_device());
+  const int64_t bytes = (int64_t)tensor.numel() * (int64_t)tensor.element_size();
+  ThrowIfError(Engine::Get().CapturedReducescatter(tensor.data_ptr(), bytes, MapDtype(tensor.scalar_type()), (ReduceOp)reduce_op,
+                                                   prescale, postscale, process_set_id, max_ctas, (void*)stream));
+}
+
+void CapturedAllgather(at::Tensor tensor, int process_set_id, int max_ctas) {
+  TORCH_CHECK(tensor.is_cuda(), "captured_allgather_: CUDA tensor expected");
+  TORCH_CHECK(tensor.is_non_overlapping_and_dense(), "captured_allgather_: tensor must be dense");
+  c10::cuda::CUDAGuard guard(tensor.device());
+  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(tensor.get_device());
+  const int64_t bytes = (int64_t)tensor.numel() * (int64_t)tensor.element_size();
+  ThrowIfError(Engine::Get().CapturedAllgather(tensor.data_ptr(), bytes, process_set_id, max_ctas, (void*)stream));
+}
+
 // ---- fused optimizer kernels (an extra of this library; see kernels/optim_kernels.cu) --------------
 void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momenta, double lr,
                   double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step) {
@@ -528,6 +549,8 @@ PYBIND11_MODULE(_hvd_torch, m) {
   m.def("reset_noname_counters", &ResetNonameCounters);
   m.def("symm_empty", &SymmEmpty);
   m.def("captured_allreduce_", &CapturedAllreduce);
+  m.def("captured_reducescatter_", &CapturedReducescatter);
+  m.def("captured_allgather_", &CapturedAllgather);
   m.def("fused_sgd_step", &FusedSgdStep);
   m.def("fused_adam_step", &FusedAdamStep);
 }

@@ -29,6 +29,9 @@ def lib():
                                      ctypes.c_double]
         L.hvd_sim_inplace.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int64, u64p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                       ctypes.c_double, ctypes.c_int, f32p]
+        L.hvd_sim_inplace_reducescatter.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int64, u64p, ctypes.c_int, ctypes.c_int,
+                                                    ctypes.c_int, ctypes.c_double, ctypes.c_int]
+        L.hvd_sim_inplace_allgather.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int64, u64p, ctypes.c_int, ctypes.c_int]
         _lib = L
     return _lib
 
@@ -63,6 +66,25 @@ def inplace_allreduce(tensors, op=SUM, ctas=8, scale=1.0, repeats=1, device=0):
     _check(lib().hvd_sim_inplace(n, device, nbytes, ptrs, DTYPE_CODE[tensors[0].dtype], op, ctas, scale, repeats, ctypes.byref(ms)),
            'sim in-place allreduce')
     return ms.value / max(repeats, 1)
+
+
+def inplace_reducescatter(tensors, op=SUM, ctas=8, scale=1.0, repeats=1, device=0):
+    """tensors: one tensor per simulated rank; rank r's contiguous 1/n slice of its own tensor receives the reduction
+    (scaled by `scale`), nothing else is written.  The byte size must be a multiple of 16 * n."""
+    n = len(tensors)
+    ptrs = (ctypes.c_uint64 * n)(*[t.data_ptr() for t in tensors])
+    nbytes = tensors[0].numel() * tensors[0].element_size()
+    _check(lib().hvd_sim_inplace_reducescatter(n, device, nbytes, ptrs, DTYPE_CODE[tensors[0].dtype], op, ctas, scale, repeats),
+           'sim in-place reduce-scatter')
+
+
+def inplace_allgather(tensors, ctas=8, repeats=1, device=0):
+    """tensors: one tensor per simulated rank; rank r's contiguous 1/n slice of its own tensor is copied into every other
+    rank's tensor.  The byte size must be a multiple of 16 * n."""
+    n = len(tensors)
+    ptrs = (ctypes.c_uint64 * n)(*[t.data_ptr() for t in tensors])
+    nbytes = tensors[0].numel() * tensors[0].element_size()
+    _check(lib().hvd_sim_inplace_allgather(n, device, nbytes, ptrs, ctas, repeats), 'sim in-place allgather')
 
 
 def allgather(ins, outs, ctas=8, device=0):

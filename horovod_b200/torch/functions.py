@@ -79,6 +79,11 @@ def broadcast_optimizer_state(optimizer, root_rank, model=None, process_set=glob
     """Broadcasts optimizer state (tensors by collective, scalars/hyper-parameters as one pickled object)."""
     if isinstance(optimizer, torch.optim.LBFGS):
         raise ValueError('cannot broadcast torch.optim.LBFGS state')
+    from horovod_b200.torch.sharded_optimizer import _ShardedDistributedOptimizer
+    if isinstance(optimizer, _ShardedDistributedOptimizer):
+        # every shard of the state has one owner: only hyper-parameters and step counts travel, no zero-gradient step
+        optimizer._broadcast_state(root_rank)
+        return
     state_dict = optimizer.state_dict()
     # Newly created optimizers have no state: materialise it with a zero-gradient step so every rank has the same keys
     created = []

@@ -703,6 +703,44 @@ def captured_allreduce_(tensor, op=Average, prescale_factor=1.0, postscale_facto
     return tensor
 
 
+def _shard_view(tensor, process_set):
+    n = process_set.size() or 1
+    flat = tensor.view(-1)
+    shard = flat.numel() // n
+    r = process_set.rank() if n > 1 else 0
+    return flat[r * shard:(r + 1) * shard]
+
+
+def captured_reducescatter_(tensor, op=Average, prescale_factor=1.0, postscale_factor=1.0, process_set=global_process_set,
+                            max_ctas=0):
+    """In-place reduce-scatter of a contiguous tensor allocated with `hvd.symm_empty` (or a view of one taken identically on
+    every rank), issued like `captured_allreduce_`: ONE kernel on the current CUDA stream, no handle, no negotiation, so
+    it can be captured into a CUDA graph.  Every rank issues the same sequence of captured collectives.
+
+    Rank r owns the contiguous slice [r*S, (r+1)*S) of the tensor, S = numel / set size; the byte size must be a multiple
+    of 16 * set size.  Only that slice of rank r's tensor receives the reduction; the rest of the tensor is left as it
+    was.  Ops: Average / Sum / Min / Max / Product.  Returns the view of this rank's reduced shard."""
+    if op == Adasum:
+        raise NotImplementedError('captured_reducescatter_ does not support op=Adasum')
+    try:
+        _native().captured_reducescatter_(tensor, int(op), float(prescale_factor), float(postscale_factor),
+                                          process_set.process_set_id, int(max_ctas))
+    except (RuntimeError, ValueError) as e:
+        raise HorovodInternalError(e)
+    return _shard_view(tensor, process_set)
+
+
+def captured_allgather_(tensor, process_set=global_process_set, max_ctas=0):
+    """In-place allgather of a contiguous registered tensor (the counterpart of `captured_reducescatter_`, same launch
+    contract): every rank's contiguous 1/N slice of its own tensor is copied into that slice of every peer's tensor.
+    The byte size must be a multiple of 16 * set size.  Returns the tensor."""
+    try:
+        _native().captured_allgather_(tensor, process_set.process_set_id, int(max_ctas))
+    except (RuntimeError, ValueError) as e:
+        raise HorovodInternalError(e)
+    return tensor
+
+
 def symm_available(process_set=global_process_set):
     """True when the zero-copy path can be used: CUDA, more than one rank, everything on one NVLink domain."""
     return torch.cuda.is_available() and is_initialized() and process_set.size() is not None and process_set.size() > 1 \

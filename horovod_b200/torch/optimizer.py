@@ -781,11 +781,18 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
 
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none, backward_passes_per_step=1,
                          op=Average, gradient_predivide_factor=1.0, num_groups=0, groups=None, sparse_as_dense=False,
-                         process_set=global_process_set, fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None):
+                         process_set=global_process_set, fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None,
+                         shard_optimizer_state=False):
     """Wraps `optimizer` so gradients are combined across ranks before the parameter update.
 
     Arguments follow the reference (horovod/torch/optimizer.py:516-608). `fused=True` (new) runs the SGD /
-    Adam(W) update as one multi-tensor CUDA kernel."""
+    Adam(W) update as one multi-tensor CUDA kernel.
+
+    `shard_optimizer_state=True` (new, ZeRO stage 1) keeps the optimizer state of 1/N of the parameters on each of the N
+    ranks: gradients are reduce-scattered, each rank updates its shard with the fused kernel and the parameters are
+    allgathered (see horovod_b200/torch/sharded_optimizer.py).  SGD / Adam / AdamW with op Average or Sum on one host;
+    raises ValueError otherwise.  The sharded update always runs the fused kernel, whatever `fused` says.  With one
+    rank it is the ordinary optimizer."""
     if gradient_predivide_factor != 1.0:
         if rocm_built_safe():
             raise ValueError('gradient_predivide_factor not supported yet with ROCm')
@@ -795,6 +802,14 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
         warnings.warn('Parameter `num_groups` has been replaced by `groups` and will be removed', DeprecationWarning)
         if groups is None:
             groups = num_groups
+    if shard_optimizer_state and (process_set.size() or 1) > 1:
+        if bucket_wire_dtype is not None or zero_copy is False:
+            raise ValueError('shard_optimizer_state keeps its buckets in registered memory in the parameter dtype: '
+                             'bucket_wire_dtype and zero_copy=False are not supported')
+        from horovod_b200.torch.sharded_optimizer import _ShardedDistributedOptimizer
+        cls = type(optimizer.__class__.__name__, (_ShardedDistributedOptimizer, optimizer.__class__), {})
+        return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,
+                   gradient_predivide_factor, groups, sparse_as_dense, process_set, bucket_cap_mb)
     if op != Adasum or size() == 1:
         cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedOptimizer.__dict__))
         return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,

@@ -1,0 +1,466 @@
+"""Sharded optimizer state (ZeRO stage 1) for `hvd.DistributedOptimizer(..., shard_optimizer_state=True)`.
+
+Parameters and gradients of every (param group, dtype) live in flat buckets of registered symmetric memory, padded so
+that each bucket splits into N equal, 128 B aligned, contiguous shards.  Rank r owns shard r of every bucket and keeps
+optimizer state for that shard only.  A step is
+
+    reduce-scatter the gradient bucket   (hvd.captured_reducescatter_, launched as soon as the bucket is ready)
+    update the own shard                 (one fused SGD / Adam(W) kernel per param group and dtype)
+    allgather the parameter bucket       (hvd.captured_allgather_)
+
+which moves the same NVLink bytes as the allreduce it replaces, while the update does 1/N of the work and the state
+takes 1/N of the memory.  The allgather runs after the update and does not overlap backward.
+"""
+import os
+import warnings
+from contextlib import contextmanager
+
+import torch
+
+from horovod_b200.common.process_sets import global_process_set
+from horovod_b200.torch import mpi_ops
+from horovod_b200.torch.compression import Compression
+from horovod_b200.torch.mpi_ops import Average, Sum
+from horovod_b200.torch.optimizer import _find_duplicates
+
+ALIGN = 128  # bytes: every parameter and every shard starts at a multiple of this
+
+
+def _itemsize(dtype):
+    return torch.empty(0, dtype=dtype).element_size()
+
+
+def shard_layout(groups, nranks, cap_bytes):
+    """Pure layout of the sharded buckets.
+
+    groups: one list per param group of (numel, dtype) of its trainable parameters, in registration order.
+    Returns a list of buckets, each a dict with
+      'group'    index of the param group,
+      'dtype'    the parameters' dtype,
+      'members'  [(index of the parameter in `groups[group]`, element offset in the bucket, numel)],
+      'numel'    padded element count (its byte size is a multiple of nranks * 128),
+      'shard'    elements per rank (numel // nranks).
+    Parameters are taken in reverse order inside a group (gradients become ready roughly in that order), split by dtype,
+    packed at 128 B alignment and cut into buckets of at most `cap_bytes` (a larger parameter gets a bucket of its own)."""
+    buckets = []
+    for gi, params in enumerate(groups):
+        by_dtype = {}
+        for i in reversed(range(len(params))):
+            numel, dtype = params[i]
+            by_dtype.setdefault(dtype, []).append((i, numel))
+        for dtype, members in by_dtype.items():
+            item = _itemsize(dtype)
+            cur, cur_bytes = [], 0
+            layouts = []
+            for i, numel in members:
+                nbytes = (numel * item + ALIGN - 1) // ALIGN * ALIGN
+                if cur and cur_bytes + nbytes > cap_bytes:
+                    layouts.append((cur, cur_bytes))
+                    cur, cur_bytes = [], 0
+                cur.append((i, cur_bytes // item, numel))
+                cur_bytes += nbytes
+            if cur:
+                layouts.append((cur, cur_bytes))
+            unit = nranks * ALIGN
+            for mem, nbytes in layouts:
+                padded = (nbytes + unit - 1) // unit * unit
+                numel = padded // item
+                buckets.append({'group': gi, 'dtype': dtype, 'members': mem, 'numel': numel, 'shard': numel // nranks})
+    return buckets
+
+
+def shard_range(bucket, rank):
+    """Elements [lo, hi) of the bucket that `rank` owns."""
+    return rank * bucket['shard'], (rank + 1) * bucket['shard']
+
+
+def shard_slices(bucket, rank):
+    """The parameter pieces inside `rank`'s shard: [(member position, first element in the parameter, last + 1,
+    first element in the shard)]."""
+    lo, hi = shard_range(bucket, rank)
+    out = []
+    for k, (_, off, numel) in enumerate(bucket['members']):
+        a, b = max(lo, off), min(hi, off + numel)
+        if a < b:
+            out.append((k, a - off, b - off, a - lo))
+    return out
+
+
+def _memory_order(t, stride):
+    """The elements of `t` in the memory order of a dense tensor of its shape with strides `stride` (None: row-major)."""
+    if stride is None:
+        return t.reshape(-1)
+    x = torch.empty_strided(t.shape, stride, dtype=t.dtype, device=t.device)
+    x.copy_(t)
+    return x.as_strided((x.numel(),), (1,))
+
+
+def shard_from_full(bucket, rank, full, strides=None, dtype=torch.float32, device=None):
+    """This rank's shard of one state tensor.  full[k]: the state of member k (its parameter's shape) or None (zeros);
+    strides[k]: the parameter's strides, i.e. the order in which its elements lie in the bucket (None: row-major).
+    Padding is zero."""
+    out = torch.zeros(bucket['shard'], dtype=dtype, device=device)
+    for k, plo, phi, slo in shard_slices(bucket, rank):
+        t = full[k]
+        if t is not None:
+            out[slo:slo + phi - plo].copy_(_memory_order(t, strides[k] if strides else None)[plo:phi])
+    return out
+
+
+def full_from_shards(bucket, shards, shapes, strides=None):
+    """Inverse of shard_from_full: the N shards of a state tensor (in rank order) -> one tensor per member, shaped
+    `shapes[k]` with strides `strides[k]` (None: row-major)."""
+    flat = torch.cat([s.reshape(-1) for s in shards])
+    out = []
+    for k, (_, off, numel) in enumerate(bucket['members']):
+        seg = flat[off:off + numel]
+        out.append(seg.reshape(shapes[k]) if not strides else seg.as_strided(shapes[k], strides[k]))
+    return out
+
+
+class _ShardedDistributedOptimizer(torch.optim.Optimizer):
+    """Wraps SGD / Adam / AdamW so that every rank keeps optimizer state for 1/N of the parameters (ZeRO stage 1).
+    Built by `hvd.DistributedOptimizer(opt, shard_optimizer_state=True)`; the dynamic class derives from this one and from
+    the wrapped optimizer's class."""
+
+    def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
+                 gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
+                 bucket_cap_mb=32):
+        super().__init__(params)
+        is_sgd = isinstance(self, torch.optim.SGD)
+        is_adam = isinstance(self, (torch.optim.Adam, torch.optim.AdamW))
+        if not (is_sgd or is_adam):
+            raise ValueError('shard_optimizer_state supports SGD, Adam and AdamW only, not %s' % type(self).__name__)
+        for g in self.param_groups:
+            if g.get('maximize', False) or (is_adam and g.get('amsgrad', False)):
+                raise ValueError('shard_optimizer_state does not support maximize=True or amsgrad=True')
+        if op not in (Average, Sum):
+            raise ValueError('shard_optimizer_state supports op=Average or op=Sum only')
+        if compression is not Compression.none or groups is not None or sparse_as_dense:
+            raise ValueError('shard_optimizer_state does not support compression, groups or sparse_as_dense')
+        if named_parameters is not None:
+            named_parameters = list(named_parameters)
+            if any(not isinstance(x, tuple) for x in named_parameters):
+                raise ValueError('named_parameters should be a sequence of tuples (name, parameter), usually produced by '
+                                 'model.named_parameters().')
+            dups = _find_duplicates([k for k, _ in named_parameters])
+            if dups:
+                raise ValueError('Parameter names in named_parameters must be unique. Found duplicates: %s' % ', '.join(dups))
+            if {id(v) for g in self.param_groups for v in g['params']} - {id(v) for _, v in named_parameters}:
+                raise ValueError('named_parameters was specified, but one or more model parameters were not named.')
+        trainable = [[p for p in g['params'] if p.requires_grad] for g in self.param_groups]
+        for ps in trainable:
+            for p in ps:
+                if not (p.is_cuda and mpi_ops._is_dense(p) and p.dtype in (torch.float32, torch.bfloat16, torch.float16)):
+                    raise ValueError('shard_optimizer_state needs dense CUDA fp32 / bf16 / fp16 parameters')
+                if is_adam and p.dtype == torch.float16:
+                    raise ValueError('shard_optimizer_state: the fused Adam kernel has no fp16 parameter variant')
+        if not (process_set.included() and mpi_ops.symm_available(process_set) and mpi_ops.cross_size() == 1):
+            raise ValueError('shard_optimizer_state needs registered symmetric memory (P2P backend, one host, not elastic)')
+
+        self._is_sgd = is_sgd
+        self.process_set = process_set
+        self.op = op
+        self.gradient_predivide_factor = gradient_predivide_factor
+        self.backward_passes_per_step = backward_passes_per_step
+        self._nranks, self._rank = process_set.size(), process_set.rank()
+        self._graph_mode = False        # set by hvd.GraphedStep
+        self._graph_capture = None      # while hvd.GraphedStep captures: {'comm': stream}
+        self._graph_comm_captured = False
+        self._should_synchronize = True
+        self._synchronized = False
+        _, hi_pri = torch.cuda.Stream.priority_range()
+        device = trainable[0][0].device if any(trainable) else torch.device('cuda', torch.cuda.current_device())
+        self._comm = torch.cuda.Stream(device=device, priority=hi_pri)
+
+        self._buckets = shard_layout([[(p.numel(), p.dtype) for p in ps] for ps in trainable], self._nranks,
+                                     int(bucket_cap_mb * 1024 * 1024))
+        self._p_to_bucket = {}
+        with torch.no_grad():
+            for bi, b in enumerate(self._buckets):
+                ps = [trainable[b['group']][i] for i, _, _ in b['members']]
+                pflat = mpi_ops.symm_empty(b['numel'], dtype=b['dtype'], device=device, process_set=process_set)
+                gflat = mpi_ops.symm_empty(b['numel'], dtype=b['dtype'], device=device, process_set=process_set)
+                pflat.zero_()
+                gflat.zero_()
+                b.update({'params': ps, 'pflat': pflat, 'gflat': gflat, 'views': {}, 'index': bi, 'step': 0,
+                          'mom_init': False, 'pending': 0, 'ready': False})
+                for p, (_, off, numel) in zip(ps, b['members']):
+                    # keep the parameter's memory format (channels_last stays channels_last)
+                    pview = pflat[off:off + numel].as_strided(p.size(), p.stride())
+                    gview = gflat[off:off + numel].as_strided(p.size(), p.stride())
+                    pview.copy_(p.data)
+                    if p.grad is not None:
+                        gview.copy_(p.grad)
+                    p.data = pview
+                    p.grad = gview
+                    b['views'][p] = (off, gview)
+                    self._p_to_bucket[p] = b
+                lo, hi = shard_range(b, self._rank)
+                b['pshard'], b['gshard'] = pflat[lo:hi], gflat[lo:hi]
+                if is_sgd:
+                    # the fused SGD kernel keeps momentum in the parameter dtype
+                    b['state'] = {'momentum_buffer': torch.zeros(b['shard'], dtype=b['dtype'], device=device)} \
+                        if self.param_groups[b['group']].get('momentum', 0.0) != 0.0 else {}
+                else:
+                    b['state'] = {'exp_avg': torch.zeros(b['shard'], dtype=torch.float32, device=device),
+                                  'exp_avg_sq': torch.zeros(b['shard'], dtype=torch.float32, device=device)}
+        self._delay = {p: backward_passes_per_step for p in self._p_to_bucket}
+        self._seen = set()  # parameters whose gradient hook fired since the last synchronize()
+        self._reset_launch_order()
+        self._hooks = [p.register_post_accumulate_grad_hook(self._make_hook(p)) for p in self._p_to_bucket]
+
+    # ---- launch order ---------------------------------------------------------------------------------------------------
+    def _reset_launch_order(self):
+        self._next = 0
+        for b in self._buckets:
+            b['pending'], b['ready'] = len(b['params']), False
+
+    def _scales(self):
+        if self.op == Average:
+            return 1.0 / self.gradient_predivide_factor, self.gradient_predivide_factor
+        return 1.0, 1.0
+
+    def _comm_stream(self):
+        return self._graph_capture['comm'] if self._graph_capture is not None else self._comm
+
+    def _mark_ready(self, bucket):
+        """A bucket's reduce-scatter is launched once the bucket and every lower-numbered bucket are ready: all ranks issue
+        the same sequence without negotiating, and buckets that complete in order still overlap backward."""
+        bucket['ready'] = True
+        while self._next < len(self._buckets) and self._buckets[self._next]['ready']:
+            b = self._buckets[self._next]
+            comm = self._comm_stream()
+            comm.wait_stream(torch.cuda.current_stream())
+            pre, post = self._scales()
+            with torch.cuda.stream(comm):
+                mpi_ops.captured_reducescatter_(b['gflat'], op=self.op, prescale_factor=pre, postscale_factor=post,
+                                                process_set=self.process_set)
+            self._next += 1
+
+    def _make_hook(self, p):
+        def hook(*ignore):
+            if self._graph_mode and self._graph_capture is None:
+                return  # GraphedStep warm-up / replay: the reductions are issued by the capture or by step()
+            bucket = self._p_to_bucket[p]
+            off, view = bucket['views'][p]
+            if p.grad.data_ptr() != view.data_ptr():
+                # model.zero_grad() (set_to_none) dropped the bucket view and autograd allocated a fresh gradient
+                view.copy_(p.grad)
+                p.grad = view
+            if self._graph_capture is not None:
+                bucket['pending'] -= 1
+                if bucket['pending'] == 0:
+                    self._mark_ready(bucket)
+                return
+            if self._delay[p] <= 0:
+                raise AssertionError('Gradients were computed more than backward_passes_per_step times before call to step(). '
+                                     'Increase backward_passes_per_step to accumulate gradients locally.')
+            self._delay[p] -= 1
+            self._seen.add(p)
+            if self._delay[p] == 0:
+                bucket['pending'] -= 1
+                if bucket['pending'] == 0:
+                    self._mark_ready(bucket)
+        return hook
+
+    def _adopt_missing_grads(self, bucket):
+        """Gradients that were not produced on this rank count as zeros; fresh gradient tensors move into the bucket."""
+        for p in bucket['params']:
+            off, view = bucket['views'][p]
+            if p.grad is None:
+                if p not in self._seen:
+                    view.zero_()
+                p.grad = view
+            elif p.grad.data_ptr() != view.data_ptr():
+                view.copy_(p.grad)
+                p.grad = view
+
+    # ---- public API -------------------------------------------------------------------------------------------------------
+    def synchronize(self):
+        """Reduce-scatters every gradient bucket whose hook has not launched it yet (missing gradients count as zeros) and
+        makes the current stream wait for all of them.  Afterwards only THIS rank's shard of each gradient bucket holds the
+        reduced gradient; the rest of p.grad keeps this rank's local values, so ranks see different p.grad.  Anything that
+        reads the whole p.grad and decides per rank is therefore unsupported with sharded optimizer state: gradient
+        clipping on the full gradient, and torch.amp.GradScaler (its inf check would skip step() on some ranks only).
+        A step() after an explicit synchronize() does not reduce again."""
+        if not (self._graph_mode and self._graph_comm_captured):
+            for b in self._buckets[self._next:]:
+                self._adopt_missing_grads(b)
+            for b in self._buckets[self._next:]:
+                self._mark_ready(b)
+            torch.cuda.current_stream().wait_stream(self._comm)
+        self._reset_launch_order()
+        self._delay = {p: self.backward_passes_per_step for p in self._delay}
+        self._seen.clear()
+        self._synchronized = True
+
+    @contextmanager
+    def skip_synchronize(self):
+        """Use after an explicit optimizer.synchronize() so that step() does not synchronize again."""
+        self._should_synchronize = False
+        try:
+            yield
+        finally:
+            self._should_synchronize = True
+
+    def _update_shards(self):
+        """One fused kernel per param group and dtype over this rank's shards; hyper-parameters are read now, so LR
+        schedulers work."""
+        native = mpi_ops._native()
+        by_group = {}
+        for b in self._buckets:
+            by_group.setdefault((b['group'], b['dtype']), []).append(b)
+        with torch.no_grad():
+            for (gi, _), bs in by_group.items():
+                group = self.param_groups[gi]
+                ps, gs = [b['pshard'] for b in bs], [b['gshard'] for b in bs]
+                if self._is_sgd:
+                    mom = group.get('momentum', 0.0)
+                    bufs = [b['state']['momentum_buffer'] for b in bs] if mom != 0.0 else []
+                    first = mom != 0.0 and not bs[0]['mom_init']
+                    native.fused_sgd_step(ps, gs, bufs, float(group['lr']), float(mom), float(group.get('dampening', 0.0)),
+                                          float(group.get('weight_decay', 0.0)), bool(group.get('nesterov', False)), 1.0, first)
+                    for b in bs:
+                        b['mom_init'] = b['mom_init'] or mom != 0.0
+                else:
+                    for b in bs:
+                        b['step'] += 1
+                    b1, b2 = group['betas']
+                    adamw = isinstance(self, torch.optim.AdamW) or bool(group.get('decoupled_weight_decay', False))
+                    native.fused_adam_step(ps, gs, [b['state']['exp_avg'] for b in bs], [b['state']['exp_avg_sq'] for b in bs],
+                                           float(group['lr']), float(b1), float(b2), float(group['eps']),
+                                           float(group.get('weight_decay', 0.0)), bs[0]['step'], 1.0, adamw)
+
+    def _allgather_params(self):
+        comm = self._comm
+        comm.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(comm):
+            for b in self._buckets:
+                mpi_ops.captured_allgather_(b['pflat'], process_set=self.process_set)
+        torch.cuda.current_stream().wait_stream(comm)
+
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        if self._should_synchronize:
+            if self._synchronized:
+                # a reduce-scatter is not idempotent: running it again would mix the reduced shard with the peers' local
+                # gradients, so the reduction done by synchronize() is used as it is
+                warnings.warn('optimizer.step() called without optimizer.skip_synchronize() context after '
+                              'optimizer.synchronize(); the gradients are not reduced a second time.')
+            else:
+                self.synchronize()
+        self._synchronized = False
+        self._update_shards()
+        self._allgather_params()
+        return loss
+
+    def zero_grad(self, set_to_none=True):
+        """Zeroes the gradient buckets in place: p.grad stays a view of registered memory (set_to_none is ignored)."""
+        if self._next > 0 or self._seen:
+            # a launched reduce-scatter may still be reading this rank's gradients for a peer
+            raise AssertionError('optimizer.zero_grad() was called after loss.backward() but before optimizer.step() or '
+                                 'optimizer.synchronize(). This is prohibited as it can cause a race condition.')
+        for b in self._buckets:
+            b['gflat'].zero_()
+            for p in b['params']:
+                if p.grad is None:
+                    p.grad = b['views'][p][1]
+
+    def set_backward_passes_per_step(self, passes):
+        self.backward_passes_per_step = passes
+        self._delay = {p: passes for p in self._delay}
+
+    # ---- hvd.GraphedStep -----------------------------------------------------------------------------------------------
+    def _begin_graph_capture(self):
+        """Called by hvd.GraphedStep right after stream capture began: the reduce-scatters become graph nodes."""
+        self._graph_comm_captured = False
+        if self.backward_passes_per_step != 1 or os.environ.get('HVD_GRAPH_COMM', '1') == '0':
+            return False
+        self._graph_capture = {'comm': torch.cuda.Stream(device=self._comm.device, priority=self._comm.priority)}
+        self._reset_launch_order()
+        return True
+
+    def _end_graph_capture(self):
+        cap = self._graph_capture
+        if cap is None:
+            return
+        for b in self._buckets[self._next:]:
+            self._mark_ready(b)
+        torch.cuda.current_stream().wait_stream(cap['comm'])
+        self._graph_capture = None
+        self._reset_launch_order()
+        self._graph_comm_captured = True
+
+    # ---- checkpoints ------------------------------------------------------------------------------------------------------
+    def state_dict(self):
+        """COLLECTIVE.  Gathers the shards bucket by bucket and returns the wrapped optimizer's own format with per-parameter
+        state tensors on the CPU, so the checkpoint loads into a sharded or an unsharded DistributedOptimizer alike."""
+        sd = torch.optim.Optimizer.state_dict(self)
+        index = {id(p): i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
+        state = {}
+        for b in self._buckets:
+            if (b['step'] == 0) if not self._is_sgd else not b['mom_init']:
+                continue  # no state yet (the same on every rank)
+            gathered = {}
+            for key, shard in b['state'].items():
+                full = mpi_ops.allgather(shard, name='sharded_opt.state.%d.%s' % (b['index'], key), process_set=self.process_set)
+                gathered[key] = full_from_shards(b, [full], [p.shape for p in b['params']], [p.stride() for p in b['params']])
+            for k, p in enumerate(b['params']):
+                st = {key: vals[k].detach().cpu().clone() for key, vals in gathered.items()}
+                if not self._is_sgd:
+                    st['step'] = torch.tensor(float(b['step']))
+                state[index[id(p)]] = st
+        sd['state'] = state
+        return sd
+
+    def load_state_dict(self, state_dict):
+        """Accepts the format of state_dict() from a sharded or an unsharded optimizer and keeps this rank's slice only.
+        Does not communicate."""
+        groups = state_dict['param_groups']
+        if len(groups) != len(self.param_groups) or any(len(a['params']) != len(b['params']) for a, b in zip(groups, self.param_groups)):
+            raise ValueError('loaded state dict does not match the optimizer\'s parameter groups')
+        for mine, saved in zip(self.param_groups, groups):
+            for k, v in saved.items():
+                if k != 'params':
+                    mine[k] = v
+        ids = {}
+        for saved, mine in zip(groups, self.param_groups):
+            for i, p in zip(saved['params'], mine['params']):
+                ids[p] = i
+        saved_state = state_dict['state']
+        with torch.no_grad():
+            for b in self._buckets:
+                per = [saved_state.get(ids[p], saved_state.get(str(ids[p]), {})) for p in b['params']]
+                for key, shard in b['state'].items():
+                    full = [st.get(key) for st in per]
+                    shard.copy_(shard_from_full(b, self._rank, [None if t is None else t.detach() for t in full],
+                                                [p.stride() for p in b['params']], dtype=shard.dtype, device='cpu'))
+                    if key == 'momentum_buffer':
+                        b['mom_init'] = any(t is not None for t in full)
+                steps = [float(st['step']) for st in per if 'step' in st]
+                b['step'] = int(max(steps)) if steps else 0
+        self._reset_launch_order()
+        self._delay = {p: self.backward_passes_per_step for p in self._delay}
+        self._seen.clear()
+
+    def _broadcast_state(self, root_rank):
+        """hvd.broadcast_optimizer_state for sharded state: every shard has a single owner, so only the hyper-parameters
+        and the per-bucket step counts travel.  The moments of a shard cannot come from the root, so every rank must
+        already hold the same step counts (a fresh start, or load_state_dict() on every rank): if they differ, e.g. after
+        loading a checkpoint on the root only, every rank raises ValueError instead of resuming with zero moments."""
+        from horovod_b200.torch.functions import allgather_object, broadcast_object
+        mine = {'steps': [b['step'] for b in self._buckets], 'mom_init': [b['mom_init'] for b in self._buckets]}
+        meta = dict(mine, param_groups=[{k: v for k, v in g.items() if k != 'params'} for g in self.param_groups])
+        meta = broadcast_object(meta, root_rank, 'sharded_opt.meta', self.process_set)
+        same = mine == {'steps': meta['steps'], 'mom_init': meta['mom_init']}
+        if not all(allgather_object(same, 'sharded_opt.same', self.process_set)):
+            raise ValueError('broadcast_optimizer_state: the sharded optimizer state differs between ranks (was the '
+                             'checkpoint loaded on the root rank only?); call load_state_dict() on every rank')
+        for g, saved in zip(self.param_groups, meta['param_groups']):
+            g.update(saved)
+        for b, s, m in zip(self._buckets, meta['steps'], meta['mom_init']):
+            b['step'], b['mom_init'] = s, m
