@@ -319,14 +319,21 @@ class HorovodBasics(object):
         return bool(self._check(self.lib.hvd_process_set_included(int(process_set_id))))
 
     def _get_process_set_ids_and_ranks(self):
+        """{id: ranks} of the registered process sets. The table can change between the calls below: when any rank
+        shuts down, every rank's background loop exits and drops its sets, possibly while this rank is still inside
+        hvd.init(). A set that is gone by the time it is queried is left out instead of failing init()."""
         n = self.lib.hvd_number_of_process_sets()
         ids = (ctypes.c_int * max(1, n))()
         self.lib.hvd_process_set_ids(ids)
         out = {}
         for i in range(n):
-            sz = self._check(self.lib.hvd_process_set_size(ids[i]))
-            ranks = (ctypes.c_int * max(1, sz))()
-            self.lib.hvd_process_set_ranks(ids[i], ranks)
+            sz = self.lib.hvd_process_set_size(ids[i])
+            if sz < 0:
+                continue
+            ranks = (ctypes.c_int * max(1, sz, self.lib.hvd_size()))()
+            sz = self.lib.hvd_process_set_ranks(ids[i], ranks)
+            if sz < 0:
+                continue
             out[ids[i]] = [ranks[j] for j in range(sz)]
         return out
 

@@ -150,6 +150,7 @@ cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, 
   if (param_dtype == 7 && grad_dtype == 7) fused_adam_kernel<float, float><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, adamw);
   else if (param_dtype == 7 && grad_dtype == 10) fused_adam_kernel<float, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, adamw);
   else if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, adamw);
+  else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, adamw);
   else return cudaErrorInvalidValue;
   CountKernelLaunch();
   return cudaGetLastError();

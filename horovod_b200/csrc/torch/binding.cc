@@ -477,19 +477,46 @@ void CapturedAllgather(at::Tensor tensor, int process_set_id, int max_ctas) {
 }
 
 // ---- fused optimizer kernels (an extra of this library; see kernels/optim_kernels.cu) --------------
+// The kernels address every tensor of entry i with the element index of params[i] and take one element type per list, so
+// each companion tensor must have the param's sizes and strides, one dtype per list, and live on the param's device.
+// Checked here, before anything is staged: a mismatch would otherwise become an out-of-bounds access or silent garbage.
+void CheckOptimizerPeer(const char* op, const char* what, size_t i, const at::Tensor& param, const at::Tensor& t,
+                        at::ScalarType dtype) {
+  TORCH_CHECK(t.device() == param.device(), op, ": ", what, "[", i, "] is on ", t.device(), ", params[", i, "] on ",
+              param.device());
+  TORCH_CHECK(t.scalar_type() == dtype, op, ": ", what, "[", i, "] is ", t.scalar_type(), ", expected ", dtype);
+  TORCH_CHECK(t.sizes() == param.sizes(), op, ": ", what, "[", i, "] has size ", t.sizes(), ", params[", i, "] has ",
+              param.sizes());
+  TORCH_CHECK(t.strides() == param.strides(), op, ": ", what, "[", i, "] has strides ", t.strides(), ", params[", i,
+              "] has ", param.strides());
+}
+
+void CheckOptimizerParam(const char* op, size_t i, const at::Tensor& param, const at::Tensor& first) {
+  TORCH_CHECK(param.is_cuda() && param.is_non_overlapping_and_dense(), op, ": params[", i, "] must be a dense CUDA tensor");
+  TORCH_CHECK(param.device() == first.device(), op, ": params[", i, "] is on ", param.device(), ", params[0] on ",
+              first.device());
+  TORCH_CHECK(param.scalar_type() == first.scalar_type(), op, ": params[", i, "] is ", param.scalar_type(),
+              ", params[0] is ", first.scalar_type(), " (one dtype per call)");
+}
+
 void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momenta, double lr,
                   double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step) {
-  TORCH_CHECK(params.size() == grads.size(), "fused_sgd: list sizes differ");
-  if (params.empty()) return;
   const bool has_mom = momentum != 0.0;
-  TORCH_CHECK(!has_mom || momenta.size() == params.size(), "fused_sgd: momentum buffers missing");
+  TORCH_CHECK(params.size() == grads.size(), "fused_sgd: list sizes differ");
+  TORCH_CHECK(momenta.size() == params.size() || (!has_mom && momenta.empty()),
+              "fused_sgd: ", momenta.size(), " momentum buffers for ", params.size(), " params");
+  if (params.empty()) return;
+  for (size_t i = 0; i < params.size(); ++i) {
+    CheckOptimizerParam("fused_sgd", i, params[i], params[0]);
+    CheckOptimizerPeer("fused_sgd", "grads", i, params[i], grads[i], grads[0].scalar_type());
+    if (has_mom) CheckOptimizerPeer("fused_sgd", "momentum_buffers", i, params[i], momenta[i], params[i].scalar_type());
+  }
   int device = (int)params[0].get_device();
   c10::cuda::CUDAGuard guard(params[0].device());
   cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
   std::vector<kern::SgdTensor> table(params.size());
   int64_t maxc = 0;
   for (size_t i = 0; i < params.size(); ++i) {
-    TORCH_CHECK(params[i].is_cuda() && params[i].is_non_overlapping_and_dense() && grads[i].strides() == params[i].strides(), "fused_sgd: params/grads must be dense CUDA tensors with identical layout");
     table[i].param = params[i].data_ptr(); table[i].grad = grads[i].data_ptr();
     table[i].momentum = has_mom ? momenta[i].data_ptr() : nullptr;
     table[i].count = params[i].numel();
@@ -507,14 +534,21 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
                    std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
                    int64_t step, double grad_scale, bool adamw) {
   TORCH_CHECK(params.size() == grads.size() && params.size() == exp_avg.size() && params.size() == exp_avg_sq.size(), "fused_adam: list sizes differ");
+  // step is 1-based: step 0 would make the bias correction 1 - beta1^0 = 0 and every parameter inf / NaN
+  TORCH_CHECK(step >= 1, "fused_adam: step must be >= 1, got ", step);
   if (params.empty()) return;
+  for (size_t i = 0; i < params.size(); ++i) {
+    CheckOptimizerParam("fused_adam", i, params[i], params[0]);
+    CheckOptimizerPeer("fused_adam", "grads", i, params[i], grads[i], grads[0].scalar_type());
+    CheckOptimizerPeer("fused_adam", "exp_avgs", i, params[i], exp_avg[i], at::kFloat);
+    CheckOptimizerPeer("fused_adam", "exp_avg_sqs", i, params[i], exp_avg_sq[i], at::kFloat);
+  }
   int device = (int)params[0].get_device();
   c10::cuda::CUDAGuard guard(params[0].device());
   cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
   std::vector<kern::AdamTensor> table(params.size());
   int64_t maxc = 0;
   for (size_t i = 0; i < params.size(); ++i) {
-    TORCH_CHECK(params[i].is_cuda() && params[i].is_non_overlapping_and_dense() && grads[i].strides() == params[i].strides(), "fused_adam: params/grads must be dense CUDA tensors with identical layout");
     table[i].param = params[i].data_ptr(); table[i].grad = grads[i].data_ptr();
     table[i].exp_avg = exp_avg[i].data_ptr(); table[i].exp_avg_sq = exp_avg_sq[i].data_ptr();
     table[i].count = params[i].numel();

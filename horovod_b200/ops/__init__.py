@@ -23,7 +23,9 @@ def fused_sgd_step(params, grads, momentum_buffers, lr, momentum=0.0, dampening=
 
 def fused_adam_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, step=1,
                     grad_scale=1.0, adamw=True):
-    """One launch of Adam / AdamW for the whole parameter list (fp32 state; `step` is the 1-based step count)."""
+    """One launch of Adam / AdamW for the whole parameter list (fp32 / bf16 / fp16 parameters, fp32 or matching
+    gradients, fp32 state with the parameters' sizes and strides; `step` is the 1-based step count). Mismatched
+    lists, dtypes, sizes, strides or devices raise RuntimeError before anything is launched."""
     return _native().fused_adam_step(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1), float(beta2),
                                      float(eps), float(weight_decay), int(step), float(grad_scale), bool(adamw))
 

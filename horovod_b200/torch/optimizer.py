@@ -114,6 +114,21 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         for p in self._allreduce_delay:
             self._allreduce_delay[p] = self.backward_passes_per_step
         super(self.__class__, self).load_state_dict(*args, **kwargs)
+        if self._fused and isinstance(self, (torch.optim.Adam, torch.optim.AdamW)):
+            self._keep_fp32_moments(args[0] if args else kwargs['state_dict'])
+
+    def _keep_fp32_moments(self, state_dict):
+        """torch casts every loaded floating state tensor to its parameter's dtype. The fused Adam kernel keeps fp32
+        moments for bf16 / fp16 parameters too, so take the checkpoint's fp32 values back: a checkpoint round-trips
+        exactly instead of losing the moments' low bits."""
+        saved = [i for g in state_dict['param_groups'] for i in g['params']]
+        params = [p for g in self.param_groups for p in g['params']]
+        for pid, p in zip(saved, params):
+            st = state_dict['state'].get(pid, {})
+            for key in ('exp_avg', 'exp_avg_sq'):
+                t = st.get(key)
+                if torch.is_tensor(t) and t.dtype == torch.float32 and p.dtype != torch.float32 and key in self.state[p]:
+                    self.state[p][key] = _state_like(p, t, torch.float32)
 
     @staticmethod
     def find_duplicates(lst):
@@ -593,10 +608,13 @@ def _fused_step(opt):
                 if mom != 0.0:
                     for p in ps:
                         st = opt.state[p]
-                        if st.get('momentum_buffer') is None:
-                            st['momentum_buffer'] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                        buf = st.get('momentum_buffer')
+                        if buf is None:
+                            buf = st['momentum_buffer'] = torch.zeros_like(p, memory_format=torch.preserve_format)
                             first = True
-                        bufs.append(st['momentum_buffer'])
+                        elif buf.dtype != p.dtype or buf.stride() != p.stride():
+                            buf = st['momentum_buffer'] = _state_like(p, buf, p.dtype)
+                        bufs.append(buf)
                 native.fused_sgd_step(ps, grads, bufs, float(group['lr']), float(mom), float(group.get('dampening', 0.0)),
                                       float(group.get('weight_decay', 0.0)), bool(group.get('nesterov', False)), 1.0, first)
             else:
@@ -607,6 +625,14 @@ def _fused_step(opt):
                         st['step'] = torch.tensor(0.0)
                         st['exp_avg'] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
                         st['exp_avg_sq'] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
+                    else:
+                        # torch's own step (closure, broadcast_optimizer_state's initialisation) and load_state_dict
+                        # leave moments in the parameter's dtype or a checkpoint's layout; the kernel reads fp32 moments
+                        # element for element with the parameter
+                        for key in ('exp_avg', 'exp_avg_sq'):
+                            t = st[key]
+                            if t.dtype != torch.float32 or t.stride() != p.stride():
+                                st[key] = _state_like(p, t, torch.float32)
                     if not torch.is_tensor(st['step']):
                         st['step'] = torch.tensor(float(st['step']))
                     steps.append(st['step'])
@@ -619,12 +645,32 @@ def _fused_step(opt):
                 for t in steps:
                     if t.is_cuda:
                         t.add_(1)
-                step = int(steps[0].item())
+                # the bias corrections follow each parameter's own step count (a parameter without a gradient does not
+                # advance, a checkpoint may mix counts): one launch per distinct count, normally exactly one
+                counts = torch.stack(cpu_steps).tolist() if len(cpu_steps) == len(steps) else [int(t.item()) for t in steps]
+                by_step = {}
+                for i, c in enumerate(counts):
+                    by_step.setdefault(int(c), []).append(i)
                 b1, b2 = group['betas']
                 adamw = isinstance(opt, torch.optim.AdamW) or bool(group.get('decoupled_weight_decay', False))
-                native.fused_adam_step(ps, grads, exp_avg, exp_avg_sq, float(group['lr']), float(b1), float(b2),
-                                       float(group['eps']), float(group.get('weight_decay', 0.0)), step, 1.0, adamw)
+                for step, idx in by_step.items():
+                    if len(by_step) > 1:
+                        sub = lambda xs: [xs[i] for i in idx]  # noqa: E731
+                        args = (sub(ps), sub(grads), sub(exp_avg), sub(exp_avg_sq))
+                    else:
+                        args = (ps, grads, exp_avg, exp_avg_sq)
+                    native.fused_adam_step(*args, float(group['lr']), float(b1), float(b2), float(group['eps']),
+                                           float(group.get('weight_decay', 0.0)), step, 1.0, adamw)
     return True
+
+
+def _state_like(p, t, dtype):
+    """A copy of optimizer state `t` in `dtype` with exactly p's strides, so the fused kernels can index it like p."""
+    if t.shape != p.shape:
+        raise RuntimeError('optimizer state of shape %s does not fit a parameter of shape %s' % (tuple(t.shape), tuple(p.shape)))
+    out = torch.empty_like(p, dtype=dtype, memory_format=torch.preserve_format)
+    out.copy_(t)
+    return out
 
 
 class _DistributedAdasumOptimizer(torch.optim.Optimizer):

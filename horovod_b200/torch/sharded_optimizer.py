@@ -153,8 +153,6 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             for p in ps:
                 if not (p.is_cuda and mpi_ops._is_dense(p) and p.dtype in (torch.float32, torch.bfloat16, torch.float16)):
                     raise ValueError('shard_optimizer_state needs dense CUDA fp32 / bf16 / fp16 parameters')
-                if is_adam and p.dtype == torch.float16:
-                    raise ValueError('shard_optimizer_state: the fused Adam kernel has no fp16 parameter variant')
         if not (process_set.included() and mpi_ops.symm_available(process_set) and mpi_ops.cross_size() == 1):
             raise ValueError('shard_optimizer_state needs registered symmetric memory (P2P backend, one host, not elastic)')
 

@@ -48,5 +48,31 @@ for n in (2, 4):
         exp = torch.arange(n, device='cuda', dtype=torch.float32).view(n, 1).expand(n, 1000)
         assert torch.equal(got, exp), ('allgather mismatch', n, r, got[:, 0].tolist(), got[:, -1].tolist(),
                                        int((got != exp).sum()))
+
+# fused SGD / Adam(W): every dtype pair, sizes around the 4-element vector and the 4096-element block, views at storage
+# offsets 0-3 (unaligned params, grads and state), one launch over all of them. Each tensor is a view of an exactly
+# sized buffer, so a store past a tail or before a head is an out-of-bounds access memcheck reports.
+from horovod_b200 import ops  # noqa: E402
+
+
+def _view(n, dtype, off):
+    return torch.zeros(off + n, device='cuda', dtype=dtype)[off:]
+
+
+sizes = [0, 1, 3, 4, 5, 4095, 4096, 4097, 3 * 4096 + 1]
+for pdt, gdt in ((torch.float32, torch.float32), (torch.float32, torch.bfloat16), (torch.bfloat16, torch.bfloat16),
+                 (torch.float16, torch.float16)):
+    offs = [(i % 4, (i + 1) % 4, (i + 2) % 4) for i in range(len(sizes))]
+    ps = [_view(n, pdt, a).fill_(1) for n, (a, _, _) in zip(sizes, offs)]
+    gs = [_view(n, gdt, b).fill_(1) for n, (_, b, _) in zip(sizes, offs)]
+    bufs = [_view(n, pdt, c) for n, (_, _, c) in zip(sizes, offs)]
+    ms = [_view(n, torch.float32, c) for n, (_, _, c) in zip(sizes, offs)]
+    vs = [_view(n, torch.float32, (c + 1) % 4) for n, (_, _, c) in zip(sizes, offs)]
+    ops.fused_sgd_step(ps, gs, bufs, lr=0.5, momentum=0.9, nesterov=True, first_step=True)
+    ops.fused_sgd_step(ps, gs, bufs, lr=0.5, momentum=0.9, weight_decay=0.1)
+    ops.fused_adam_step(ps, gs, ms, vs, lr=1e-2, weight_decay=0.1, step=1, adamw=True)
+    ops.fused_adam_step(ps, gs, ms, vs, lr=1e-2, weight_decay=0.1, step=2, adamw=False)
+    torch.cuda.synchronize()
+    assert all(float(p[-1]) < 0.5 for p in ps if p.numel()), [float(p[-1]) for p in ps if p.numel()]
 torch.cuda.synchronize()
 print('SANITIZER TARGET OK')

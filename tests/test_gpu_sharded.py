@@ -199,10 +199,11 @@ class _ConvNet(torch.nn.Module):
         return y + self.unused(x[:, 0, 0, :4]) if use_all else y
 
 
-@pytest.mark.parametrize("kind", ["adamw", "sgd"])
+@pytest.mark.parametrize("kind", ["adamw", "sgd", "adamw-fp16"])
 def test_sharded_optimizer_on_simulated_ranks(hvd, monkeypatch, kind):
     """The sharded DistributedOptimizer itself (buckets, hooks, launch order, missing gradients, fused shard update,
-    synchronize() followed by step()) on 4 simulated ranks, against plain torch on averaged gradients."""
+    synchronize() followed by step()) on 4 simulated ranks, against plain torch on averaged gradients. The fp16 model
+    is compared with an fp32 reference model, so only to fp16 accuracy; the ranks must still agree bit for bit."""
     import copy
     import warnings
     from horovod_b200.torch import mpi_ops
@@ -214,20 +215,22 @@ def test_sharded_optimizer_on_simulated_ranks(hvd, monkeypatch, kind):
     monkeypatch.setattr(mpi_ops, 'cross_size', lambda: 1)
     monkeypatch.setattr(mpi_ops, 'captured_reducescatter_', team.reducescatter)
     monkeypatch.setattr(mpi_ops, 'captured_allgather_', team.allgather)
+    dt = torch.float16 if kind == 'adamw-fp16' else torch.float32
+    tol = dict(rtol=1e-4, atol=1e-5) if dt == torch.float32 else dict(rtol=2e-2, atol=2e-3)
     torch.manual_seed(0)
-    base = _ConvNet().cuda().to(memory_format=torch.channels_last)
+    base = _ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
 
     def make(m):
-        if kind == 'adamw':
+        if kind.startswith('adamw'):
             return torch.optim.AdamW(m.parameters(), lr=1e-2, weight_decay=0.05)
         return torch.optim.SGD(m.parameters(), lr=0.05, momentum=0.9, nesterov=True, weight_decay=1e-4)
 
     models = [copy.deepcopy(base) for _ in range(n)]
     opts = [hvd.DistributedOptimizer(make(m), named_parameters=m.named_parameters(), shard_optimizer_state=True,
-                                     process_set=_FakeSet(n, r), bucket_cap_mb=0.01) for r, m in enumerate(models)]
+                                     process_set=_FakeSet(n, r), bucket_cap_mb=0.01 * dt.itemsize / 4) for r, m in enumerate(models)]
     assert all(isinstance(o, _ShardedDistributedOptimizer) for o in opts) and len(opts[0]._buckets) > 2
     assert models[0].conv.weight.is_contiguous(memory_format=torch.channels_last)
-    ref = copy.deepcopy(base)
+    ref = copy.deepcopy(base).float()
     ref_opt = make(ref)
 
     def batch(step, r):
@@ -251,7 +254,7 @@ def test_sharded_optimizer_on_simulated_ranks(hvd, monkeypatch, kind):
         for r in range(n):
             opts[r].zero_grad()
             x, y = batch(step, r)
-            torch.nn.functional.cross_entropy(models[r](x, use(r)), y).backward()
+            torch.nn.functional.cross_entropy(models[r](x.to(dt), use(r)), y).backward()
         if step == 1:
             with pytest.raises(AssertionError):
                 opts[0].zero_grad()  # reduce-scatters may be in flight
@@ -270,7 +273,7 @@ def test_sharded_optimizer_on_simulated_ranks(hvd, monkeypatch, kind):
         team.flush()
         for r in range(n):
             for (name, a), b in zip(models[r].named_parameters(), ref.parameters()):
-                torch.testing.assert_close(a, b, rtol=1e-4, atol=1e-5, msg=lambda m: '%s step %d rank %d: %s' % (name, step, r, m))
+                torch.testing.assert_close(a.float(), b, **tol, msg=lambda m: '%s step %d rank %d: %s' % (name, step, r, m))
                 assert torch.equal(a, dict(models[0].named_parameters())[name])
     assert models[0].conv.weight.is_contiguous(memory_format=torch.channels_last)
 

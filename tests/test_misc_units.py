@@ -203,3 +203,38 @@ def test_fused_step_validation_is_pure_and_falls_back_cleanly(native_built):
                 assert '_hvd_init' not in st
     finally:
         hvd.shutdown()
+
+
+@pytest.mark.parametrize("left", [{0: [0, 1]}, {}])
+def test_process_set_listing_skips_sets_that_vanish(left):
+    """When any rank shuts down, every rank's background loop drops its process sets, possibly while this rank is still
+    inside hvd.init() listing them: a set that is gone by the time its ranks are read is left out, init() does not fail."""
+    from horovod_b200.common.basics import HorovodBasics
+
+    class _Lib:
+        sets = {0: [0, 1], 1: [1], 2: [0]}
+
+        def hvd_number_of_process_sets(self):
+            return len(self.sets)
+
+        def hvd_process_set_ids(self, out):
+            for i, k in enumerate(sorted(self.sets)):
+                out[i] = k
+            self.sets = dict(left)  # the table changes right after the ids were listed
+
+        def hvd_size(self):
+            return 2
+
+        def hvd_process_set_size(self, ps_id):
+            return len(self.sets[ps_id]) if ps_id in self.sets else -1
+
+        def hvd_process_set_ranks(self, ps_id, out):
+            if ps_id not in self.sets:
+                return -1
+            for i, r in enumerate(self.sets[ps_id]):
+                out[i] = r
+            return len(self.sets[ps_id])
+
+    b = HorovodBasics()
+    b._lib = _Lib()
+    assert b._get_process_set_ids_and_ranks() == left

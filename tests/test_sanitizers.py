@@ -1,7 +1,7 @@
 """Sanitizer jobs (SURVEY.md 5.2: the reference has none).
 
 * ThreadSanitizer build of the C++ runtime running the native self-test (4 engines in one process) — CPU.
-* compute-sanitizer memcheck over the P2P kernels in the single-GPU simulation — GPU.
+* compute-sanitizer memcheck over the P2P kernels in the single-GPU simulation and the fused optimizer kernels — GPU.
 """
 import os
 import shutil
