@@ -52,14 +52,17 @@ template <typename T> __device__ __forceinline__ void store4(T* p, int64_t i, in
 }
 template <typename T> __device__ __forceinline__ bool is_aligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) % (sizeof(T) * kOptVec)) == 0; }
 
+// `grad_scale_dev` (nullptr: 1) is a factor that lives on the device, e.g. a clip coefficient computed by earlier kernels:
+// it reaches the update without a host synchronisation.  Multiplying by 1.f is exact, so nullptr changes no result.
 template <typename P, typename G>
 __global__ void __launch_bounds__(kOptThreads)
 fused_sgd_kernel(const SgdTensor* __restrict__ table, float lr, float momentum, float dampening, float wd, int nesterov,
-                 float grad_scale, int first_step) {
+                 float grad_scale, const float* __restrict__ grad_scale_dev, int first_step) {
   const SgdTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
   if (base >= n) return;
+  grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
   P* p = reinterpret_cast<P*>(t.param);
   const G* g = reinterpret_cast<const G*>(t.grad);
   P* mbuf = reinterpret_cast<P*>(t.momentum);
@@ -91,11 +94,12 @@ fused_sgd_kernel(const SgdTensor* __restrict__ table, float lr, float momentum, 
 template <typename P, typename G>
 __global__ void __launch_bounds__(kOptThreads)
 fused_adam_kernel(const AdamTensor* __restrict__ table, float lr, float b1, float b2, float eps, float wd, float c1, float c2,
-                  float grad_scale, int adamw) {
+                  float grad_scale, const float* __restrict__ grad_scale_dev, int adamw) {
   const AdamTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
   if (base >= n) return;
+  grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
   P* p = reinterpret_cast<P*>(t.param);
   const G* g = reinterpret_cast<const G*>(t.grad);
   float* m = reinterpret_cast<float*>(t.exp_avg);
@@ -126,17 +130,108 @@ fused_adam_kernel(const AdamTensor* __restrict__ table, float lr, float b1, floa
   }
 }
 
+// max that keeps a NaN once it has seen one (fmaxf drops it), so an inf-norm of NaN gradients is NaN as in torch
+__device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
+__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
+
+// Gradient statistics of a table of flat gradient shards in one read pass: optional in-place scaling by *inv_scale, the
+// sum of squares (norm_inf = 0) or the max |g| (norm_inf = 1) of the scaled values as stored, and a non-finite flag.
+// Every CTA writes one partial; the last CTA to finish (atomic ticket, which it resets for the next launch) combines them
+// in fp64, always in the same order, and folds the result into out[0] (+= or max) and out[1] (max of 0 / 1).  So the
+// same input gives the same bits on every call, and one launch per gradient dtype accumulates into one output.
+template <typename G>
+__global__ void __launch_bounds__(kOptThreads)
+grad_shard_stats_kernel(const StatTensor* __restrict__ table, const float* __restrict__ inv_scale, int norm_inf,
+                        float* __restrict__ partial, int* __restrict__ partial_flag, unsigned* ticket, float* out) {
+  __shared__ double red[kOptThreads];
+  __shared__ int red_flag[kOptThreads / 32];
+  __shared__ bool last;
+  const StatTensor t = table[blockIdx.y];
+  const int64_t n = t.count;
+  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  float acc = 0.f;
+  int bad = 0;
+  if (base < n) {
+    G* g = reinterpret_cast<G*>(t.grad);
+    const bool ga = is_aligned<G>(g);
+    const float s = inv_scale ? *inv_scale : 1.f;
+#pragma unroll
+    for (int it = 0; it < kOptIters; ++it) {
+      const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
+      if (i >= n) break;
+      float gv[kOptVec];
+      load4<G>(g, i, n, ga, gv);  // elements past the end read as 0, which changes neither statistic
+      if (inv_scale) {
+#pragma unroll
+        for (int k = 0; k < kOptVec; ++k) gv[k] = to_f<G>(from_f<G>(gv[k] * s));  // the value as stored
+        store4<G>(g, i, n, ga, gv);
+      }
+#pragma unroll
+      for (int k = 0; k < kOptVec; ++k) {
+        bad |= !isfinite(gv[k]);
+        acc = norm_inf ? nan_max(acc, fabsf(gv[k])) : fmaf(gv[k], gv[k], acc);
+      }
+    }
+  }
+  // CTA partial: a fixed shuffle tree per warp, then the warps in order
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float y = __shfl_xor_sync(0xffffffffu, acc, o);
+    acc = norm_inf ? nan_max(acc, y) : acc + y;
+  }
+  bad = __any_sync(0xffffffffu, bad);
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  if (lane == 0) { red[warp] = acc; red_flag[warp] = bad; }
+  __syncthreads();
+  const unsigned ctas = gridDim.x * gridDim.y, cta = blockIdx.y * gridDim.x + blockIdx.x;
+  if (threadIdx.x == 0) {
+    float a = 0.f;
+    int f = 0;
+    for (int w = 0; w < kOptThreads / 32; ++w) {
+      a = norm_inf ? nan_max(a, (float)red[w]) : a + (float)red[w];
+      f |= red_flag[w];
+    }
+    partial[cta] = a;
+    partial_flag[cta] = f;
+    __threadfence();
+    last = atomicAdd(ticket, 1u) == ctas - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  // the last CTA: every thread combines a fixed strided subset in index order, then a fixed tree over the threads
+  double a = 0.0;
+  int f = 0;
+  for (unsigned j = threadIdx.x; j < ctas; j += kOptThreads) {
+    const double x = (double)__ldcg(partial + j);
+    a = norm_inf ? nan_max(a, x) : a + x;
+    f |= __ldcg(partial_flag + j);
+  }
+  red[threadIdx.x] = a;
+  f = __syncthreads_or(f);
+#pragma unroll
+  for (int h = kOptThreads / 2; h > 0; h >>= 1) {
+    if (threadIdx.x < h) red[threadIdx.x] = norm_inf ? nan_max(red[threadIdx.x], red[threadIdx.x + h]) : red[threadIdx.x] + red[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    out[0] = norm_inf ? (float)nan_max((double)out[0], red[0]) : (float)((double)out[0] + red[0]);
+    out[1] = fmaxf(out[1], f ? 1.f : 0.f);
+    *ticket = 0u;  // ready for the next launch on this stream
+  }
+}
+
 }  // namespace
 
 cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
                            float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
-                           int grad_dtype, cudaStream_t stream) {
+                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
   dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)n);
-  if (param_dtype == 7 && grad_dtype == 7) fused_sgd_kernel<float, float><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, first_step);
-  else if (param_dtype == 7 && grad_dtype == 10) fused_sgd_kernel<float, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, first_step);
-  else if (param_dtype == 10 && grad_dtype == 10) fused_sgd_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, first_step);
-  else if (param_dtype == 6 && grad_dtype == 6) fused_sgd_kernel<__half, __half><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, first_step);
+  if (param_dtype == 7 && grad_dtype == 7) fused_sgd_kernel<float, float><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  else if (param_dtype == 7 && grad_dtype == 10) fused_sgd_kernel<float, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  else if (param_dtype == 10 && grad_dtype == 10) fused_sgd_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  else if (param_dtype == 6 && grad_dtype == 6) fused_sgd_kernel<__half, __half><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
   else return cudaErrorInvalidValue;
   CountKernelLaunch();
   return cudaGetLastError();
@@ -144,13 +239,30 @@ cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, flo
 
 cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
                              float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale, int adamw,
-                             int param_dtype, int grad_dtype, cudaStream_t stream) {
+                             int param_dtype, int grad_dtype, cudaStream_t stream, const float* grad_scale_dev) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
   dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)n);
-  if (param_dtype == 7 && grad_dtype == 7) fused_adam_kernel<float, float><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, adamw);
-  else if (param_dtype == 7 && grad_dtype == 10) fused_adam_kernel<float, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, adamw);
-  else if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, adamw);
-  else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, adamw);
+  if (param_dtype == 7 && grad_dtype == 7) fused_adam_kernel<float, float><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  else if (param_dtype == 7 && grad_dtype == 10) fused_adam_kernel<float, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  else if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  else return cudaErrorInvalidValue;
+  CountKernelLaunch();
+  return cudaGetLastError();
+}
+
+int64_t GradShardStatsCtas(int n, int64_t max_count) {
+  return n <= 0 || max_count <= 0 ? 0 : (max_count + kOptPerBlock - 1) / kOptPerBlock * n;
+}
+
+cudaError_t LaunchGradShardStats(const StatTensor* table, int n, int64_t max_count, const float* inv_scale, int norm_inf,
+                                 float* partial, int* partial_flag, unsigned* ticket, float* out, int grad_dtype,
+                                 cudaStream_t stream) {
+  if (n <= 0 || max_count <= 0) return cudaSuccess;
+  dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)n);
+  if (grad_dtype == 7) grad_shard_stats_kernel<float><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
+  else if (grad_dtype == 10) grad_shard_stats_kernel<__nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
+  else if (grad_dtype == 6) grad_shard_stats_kernel<__half><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
   else return cudaErrorInvalidValue;
   CountKernelLaunch();
   return cudaGetLastError();

@@ -174,15 +174,26 @@ cudaError_t LaunchAdasumStep(const CommParams& cp, const AdasumArgs& args, doubl
                              int only);
 int AdasumNumLaunches(int nranks);
 
-// Fused multi-tensor optimizer updates (see optim_kernels.cu)
+// Fused multi-tensor optimizer updates (see optim_kernels.cu).  The gradient factor is grad_scale * *grad_scale_dev
+// (nullptr: grad_scale alone, bit for bit).
 struct SgdTensor { void* param; const void* grad; void* momentum; int64_t count; };
 cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
                            float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
-                           int grad_dtype, cudaStream_t stream);
+                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev = nullptr);
 struct AdamTensor { void* param; const void* grad; void* exp_avg; void* exp_avg_sq; int64_t count; };
 cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
                              float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale,
-                             int adamw, int param_dtype, int grad_dtype, cudaStream_t stream);
+                             int adamw, int param_dtype, int grad_dtype, cudaStream_t stream,
+                             const float* grad_scale_dev = nullptr);
+// Gradient statistics of flat gradient shards in one pass (see optim_kernels.cu): optional in-place scaling by
+// *inv_scale, then out[0] += sum of squares (norm_inf: out[0] = max(out[0], max |g|)) and out[1] = max(out[1], non-finite).
+// `partial` / `partial_flag` hold GradShardStatsCtas() entries; `ticket` is a zeroed counter that the kernel leaves zeroed,
+// which launches running at the same time must not share.
+struct StatTensor { void* grad; int64_t count; };
+int64_t GradShardStatsCtas(int n, int64_t max_count);
+cudaError_t LaunchGradShardStats(const StatTensor* table, int n, int64_t max_count, const float* inv_scale, int norm_inf,
+                                 float* partial, int* partial_flag, unsigned* ticket, float* out, int grad_dtype,
+                                 cudaStream_t stream);
 
 }  // namespace kern
 }  // namespace hvd

@@ -16,6 +16,7 @@
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
+#include <map>
 #include <mutex>
 #include <unordered_map>
 #include "../common/engine.h"
@@ -499,8 +500,18 @@ void CheckOptimizerParam(const char* op, size_t i, const at::Tensor& param, cons
               ", params[0] is ", first.scalar_type(), " (one dtype per call)");
 }
 
+// A device-side scalar the kernels read: one fp32 element on the params' device (nullptr when absent).
+const float* DeviceScalar(const char* op, const char* what, const c10::optional<at::Tensor>& t, const at::Tensor& param) {
+  if (!t.has_value() || !t->defined()) return nullptr;
+  TORCH_CHECK(t->is_cuda() && t->device() == param.device(), op, ": ", what, " must be on ", param.device(), ", got ", t->device());
+  TORCH_CHECK(t->scalar_type() == at::kFloat, op, ": ", what, " must be float32, got ", t->scalar_type());
+  TORCH_CHECK(t->numel() == 1, op, ": ", what, " must have one element, got ", t->numel());
+  return t->data_ptr<float>();
+}
+
 void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momenta, double lr,
-                  double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step) {
+                  double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step,
+                  c10::optional<at::Tensor> grad_scale_dev) {
   const bool has_mom = momentum != 0.0;
   TORCH_CHECK(params.size() == grads.size(), "fused_sgd: list sizes differ");
   TORCH_CHECK(momenta.size() == params.size() || (!has_mom && momenta.empty()),
@@ -511,6 +522,7 @@ void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads,
     CheckOptimizerPeer("fused_sgd", "grads", i, params[i], grads[i], grads[0].scalar_type());
     if (has_mom) CheckOptimizerPeer("fused_sgd", "momentum_buffers", i, params[i], momenta[i], params[i].scalar_type());
   }
+  const float* gsd = DeviceScalar("fused_sgd", "grad_scale_dev", grad_scale_dev, params[0]);
   int device = (int)params[0].get_device();
   c10::cuda::CUDAGuard guard(params[0].device());
   cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
@@ -526,13 +538,13 @@ void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads,
   TORCH_CHECK(dt != nullptr, "fused_sgd: table too large");
   cudaError_t e = kern::LaunchFusedSgd(dt, (int)table.size(), maxc, (float)lr, (float)momentum, (float)dampening, (float)weight_decay,
                                        nesterov ? 1 : 0, (float)grad_scale, first_step ? 1 : 0,
-                                       (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s);
+                                       (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s, gsd);
   TORCH_CHECK(e == cudaSuccess, "fused_sgd launch failed: ", cudaGetErrorString(e));
 }
 
 void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
                    std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
-                   int64_t step, double grad_scale, bool adamw) {
+                   int64_t step, double grad_scale, bool adamw, c10::optional<at::Tensor> grad_scale_dev) {
   TORCH_CHECK(params.size() == grads.size() && params.size() == exp_avg.size() && params.size() == exp_avg_sq.size(), "fused_adam: list sizes differ");
   // step is 1-based: step 0 would make the bias correction 1 - beta1^0 = 0 and every parameter inf / NaN
   TORCH_CHECK(step >= 1, "fused_adam: step must be >= 1, got ", step);
@@ -543,6 +555,7 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
     CheckOptimizerPeer("fused_adam", "exp_avgs", i, params[i], exp_avg[i], at::kFloat);
     CheckOptimizerPeer("fused_adam", "exp_avg_sqs", i, params[i], exp_avg_sq[i], at::kFloat);
   }
+  const float* gsd = DeviceScalar("fused_adam", "grad_scale_dev", grad_scale_dev, params[0]);
   int device = (int)params[0].get_device();
   c10::cuda::CUDAGuard guard(params[0].device());
   cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
@@ -559,8 +572,65 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   const float c1 = 1.0f - (float)std::pow(beta1, (double)step), c2 = 1.0f - (float)std::pow(beta2, (double)step);
   cudaError_t e = kern::LaunchFusedAdamW(dt, (int)table.size(), maxc, (float)lr, (float)beta1, (float)beta2, (float)eps,
                                          (float)weight_decay, c1, c2, (float)grad_scale, adamw ? 1 : 0,
-                                         (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s);
+                                         (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s, gsd);
   TORCH_CHECK(e == cudaSuccess, "fused_adam launch failed: ", cudaGetErrorString(e));
+}
+
+// The stats kernel's last-CTA ticket: one zeroed counter per (device, stream), which every launch leaves zeroed again.
+// Launches on one stream run one after the other, so they can share it; launches on different streams may overlap and
+// must not.  Kept for the life of the process (4 bytes per stream that ever ran the kernel).
+unsigned* StatsTicket(int device, cudaStream_t s) {
+  static std::mutex mu;
+  static std::map<std::pair<int, cudaStream_t>, unsigned*> tickets;
+  std::lock_guard<std::mutex> l(mu);
+  unsigned*& t = tickets[{device, s}];
+  if (!t) {
+    void* p = nullptr;
+    TORCH_CHECK(cudaMalloc(&p, sizeof(unsigned)) == cudaSuccess, "grad_shard_stats: cannot allocate the ticket counter");
+    TORCH_CHECK(cudaMemset(p, 0, sizeof(unsigned)) == cudaSuccess, "grad_shard_stats: cannot zero the ticket counter");
+    t = static_cast<unsigned*>(p);
+  }
+  return t;
+}
+
+// One launch of the gradient statistics kernel over `grads` (one dtype: fp32 / bf16 / fp16), folded into out[0:2].
+void GradShardStats(std::vector<at::Tensor> grads, at::Tensor out, c10::optional<at::Tensor> inv_scale, bool norm_inf) {
+  TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kFloat && out.is_contiguous() && out.numel() >= 2,
+              "grad_shard_stats: out must be a contiguous float32 CUDA tensor with at least 2 elements");
+  for (size_t i = 0; i < grads.size(); ++i) {
+    TORCH_CHECK(grads[i].is_cuda() && grads[i].is_non_overlapping_and_dense(), "grad_shard_stats: tensors[", i,
+                "] must be a dense CUDA tensor");
+    TORCH_CHECK(grads[i].device() == out.device(), "grad_shard_stats: tensors[", i, "] is on ", grads[i].device(),
+                ", out on ", out.device());
+    TORCH_CHECK(grads[i].scalar_type() == grads[0].scalar_type(), "grad_shard_stats: tensors[", i, "] is ",
+                grads[i].scalar_type(), ", tensors[0] is ", grads[0].scalar_type(), " (one dtype per call)");
+  }
+  if (!grads.empty()) {
+    const auto st = grads[0].scalar_type();
+    TORCH_CHECK(st == at::kFloat || st == at::kBFloat16 || st == at::kHalf,
+                "grad_shard_stats: gradients must be float32, bfloat16 or float16, got ", st);
+  }
+  const float* isc = DeviceScalar("grad_shard_stats", "inv_scale", inv_scale, out);
+  std::vector<kern::StatTensor> table;
+  int64_t maxc = 0;
+  for (auto& g : grads) {
+    if (g.numel() == 0) continue;
+    table.push_back({g.data_ptr(), g.numel()});
+    maxc = std::max(maxc, (int64_t)g.numel());
+  }
+  if (table.empty()) return;
+  int device = (int)out.get_device();
+  c10::cuda::CUDAGuard guard(out.device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
+  const int64_t ctas = kern::GradShardStatsCtas((int)table.size(), maxc);
+  // stream-ordered scratch from torch's caching allocator: fp32 partials followed by int flags
+  at::Tensor work = at::empty({2 * ctas}, out.options());
+  const auto* dt = (const kern::StatTensor*)GpuContext::Get().Stage(device, table.data(), table.size() * sizeof(kern::StatTensor), s);
+  TORCH_CHECK(dt != nullptr, "grad_shard_stats: table too large");
+  cudaError_t e = kern::LaunchGradShardStats(dt, (int)table.size(), maxc, isc, norm_inf ? 1 : 0, work.data_ptr<float>(),
+                                             reinterpret_cast<int*>(work.data_ptr<float>() + ctas), StatsTicket(device, s),
+                                             out.data_ptr<float>(), (int)MapDtype(grads[0].scalar_type()), s);
+  TORCH_CHECK(e == cudaSuccess, "grad_shard_stats launch failed: ", cudaGetErrorString(e));
 }
 
 }  // namespace
@@ -585,6 +655,12 @@ PYBIND11_MODULE(_hvd_torch, m) {
   m.def("captured_allreduce_", &CapturedAllreduce);
   m.def("captured_reducescatter_", &CapturedReducescatter);
   m.def("captured_allgather_", &CapturedAllgather);
-  m.def("fused_sgd_step", &FusedSgdStep);
-  m.def("fused_adam_step", &FusedAdamStep);
+  m.def("fused_sgd_step", &FusedSgdStep, py::arg("params"), py::arg("grads"), py::arg("momenta"), py::arg("lr"),
+        py::arg("momentum"), py::arg("dampening"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("grad_scale"),
+        py::arg("first_step"), py::arg("grad_scale_dev") = py::none());
+  m.def("fused_adam_step", &FusedAdamStep, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+        py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
+        py::arg("grad_scale"), py::arg("adamw"), py::arg("grad_scale_dev") = py::none());
+  m.def("grad_shard_stats", &GradShardStats, py::arg("grads"), py::arg("out"), py::arg("inv_scale") = py::none(),
+        py::arg("norm_inf") = false);
 }

@@ -10,7 +10,12 @@ optimizer state for that shard only.  A step is
 
 which moves the same NVLink bytes as the allreduce it replaces, while the update does 1/N of the work and the state
 takes 1/N of the memory.  The allgather runs after the update and does not overlap backward.
+
+Global-norm clipping (`clip_grad_norm_`) and AMP loss scaling (`ShardedGradScaler`) read only the owned shards: one
+statistics kernel per gradient dtype and one scalar allreduce give every rank the same norm and the same inf / NaN
+verdict, and the clip coefficient reaches the update on the device.
 """
+import math
 import os
 import warnings
 from contextlib import contextmanager
@@ -166,7 +171,10 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._graph_capture = None      # while hvd.GraphedStep captures: {'comm': stream}
         self._graph_comm_captured = False
         self._should_synchronize = True
-        self._synchronized = False
+        self._synchronized = False      # set by a user's synchronize(): step() warns and does not reduce again
+        self._reduced = False           # set by clip_grad_norm_ / ShardedGradScaler: step() does not reduce again, silently
+        self._clip_coef = None          # 0-dim fp32 device tensor from clip_grad_norm_, applied by the next step()
+        self._stats_cache = None        # [sum of squares, non-finite] of the unscaled gradients from ShardedGradScaler
         _, hi_pri = torch.cuda.Stream.priority_range()
         device = trainable[0][0].device if any(trainable) else torch.device('cuda', torch.cuda.current_device())
         self._comm = torch.cuda.Stream(device=device, priority=hi_pri)
@@ -203,6 +211,11 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 else:
                     b['state'] = {'exp_avg': torch.zeros(b['shard'], dtype=torch.float32, device=device),
                                   'exp_avg_sq': torch.zeros(b['shard'], dtype=torch.float32, device=device)}
+        # cross-rank gradient statistics: [sum of squares or max |g|, non-finite] in registered memory, padded so that the
+        # in-place allreduce can split it across the ranks
+        self._stats = mpi_ops.symm_empty(ALIGN // 4 * self._nranks, dtype=torch.float32, device=device,
+                                         process_set=process_set)
+        self._stats.zero_()
         self._delay = {p: backward_passes_per_step for p in self._p_to_bucket}
         self._seen = set()  # parameters whose gradient hook fired since the last synchronize()
         self._reset_launch_order()
@@ -251,6 +264,9 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 if bucket['pending'] == 0:
                     self._mark_ready(bucket)
                 return
+            if self._reduced or self._synchronized or self._clip_coef is not None or self._stats_cache is not None:
+                # a new backward after an iteration whose step() was skipped (e.g. GradScaler found inf): start afresh
+                self._drop_iteration_state()
             if self._delay[p] <= 0:
                 raise AssertionError('Gradients were computed more than backward_passes_per_step times before call to step(). '
                                      'Increase backward_passes_per_step to accumulate gradients locally.')
@@ -280,8 +296,13 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         makes the current stream wait for all of them.  Afterwards only THIS rank's shard of each gradient bucket holds the
         reduced gradient; the rest of p.grad keeps this rank's local values, so ranks see different p.grad.  Anything that
         reads the whole p.grad and decides per rank is therefore unsupported with sharded optimizer state: gradient
-        clipping on the full gradient, and torch.amp.GradScaler (its inf check would skip step() on some ranks only).
+        clipping on the full gradient, and torch.amp.GradScaler (its inf check would skip step() on some ranks only):
+        use optimizer.clip_grad_norm_() and hvd.ShardedGradScaler instead.
         A step() after an explicit synchronize() does not reduce again."""
+        self._reduce_pending()
+        self._synchronized = True
+
+    def _reduce_pending(self):
         if not (self._graph_mode and self._graph_comm_captured):
             for b in self._buckets[self._next:]:
                 self._adopt_missing_grads(b)
@@ -291,7 +312,67 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._reset_launch_order()
         self._delay = {p: self.backward_passes_per_step for p in self._delay}
         self._seen.clear()
-        self._synchronized = True
+
+    def _reduce_once(self):
+        """Reduces what is still pending unless this iteration's gradients are reduced already; the following step()
+        neither reduces again nor warns."""
+        if self._graph_capture is not None:
+            raise RuntimeError('clip_grad_norm_ and ShardedGradScaler work in eager mode only, not inside hvd.GraphedStep')
+        if not (self._synchronized or self._reduced):
+            self._reduce_pending()
+            self._reduced = True
+
+    def _drop_iteration_state(self):
+        self._synchronized = self._reduced = False
+        self._clip_coef = self._stats_cache = None
+
+    def _shard_stats(self, norm_type, inv_scale=None):
+        """[sum of squares (norm_type 2) or max |g| (inf), non-finite flag] of the reduced gradients over all ranks'
+        owned shards, as a new 2-element fp32 tensor: one stats kernel per gradient dtype on this rank's shards (scaling
+        them in place by inv_scale first, if given), then one allreduce of the small stats buffer.  No host sync."""
+        from horovod_b200 import ops
+        self._stats.zero_()
+        ops.grad_shard_stats([b['gshard'] for b in self._buckets], self._stats, inv_scale=inv_scale, norm_type=norm_type)
+        mpi_ops.captured_allreduce_(self._stats, op=Sum if norm_type == 2.0 else mpi_ops.Max, process_set=self.process_set)
+        return self._stats[:2].clone()
+
+    def _unscale_and_check(self, inv_scale, found_inf):
+        """ShardedGradScaler._unscale_grads_: unscales the owned shards in place (fp16 included) and sets found_inf to
+        the global non-finite flag, so that every rank skips or takes the step alike."""
+        self._reduce_once()
+        stats = self._shard_stats(2.0, inv_scale=inv_scale.float())
+        found_inf.copy_(stats[1].clamp(max=1.0).reshape(found_inf.shape))
+        self._stats_cache = stats
+        return found_inf
+
+    def clip_grad_norm_(self, max_norm, norm_type=2.0, error_if_nonfinite=False):
+        """Global-norm gradient clipping for sharded optimizer state, the counterpart of
+        torch.nn.utils.clip_grad_norm_(model.parameters(), ...): call it after backward (and after
+        ShardedGradScaler.unscale_, if used) and before step().
+
+        Reduces the gradients that are still pending (the following step() does not reduce again), computes the norm of
+        the whole averaged gradient from the ranks' owned shards with one scalar allreduce, and returns it as a 0-dim
+        fp32 CUDA tensor with the same bits on every rank.  The clip coefficient min(max_norm / (norm + 1e-6), 1) stays on
+        the device and is applied by the next step() inside the fused update: unlike torch, p.grad itself is not
+        rescaled.  norm_type is 2 or inf.  error_if_nonfinite=True synchronises with the host, as torch's does."""
+        norm_type = float(norm_type)
+        if norm_type not in (2.0, math.inf):
+            raise ValueError('clip_grad_norm_ with sharded optimizer state supports norm_type 2 and inf, got %r' % norm_type)
+        self._reduce_once()
+        if norm_type == 2.0 and self._stats_cache is not None:
+            stats = self._stats_cache  # ShardedGradScaler.unscale_ computed them in its pass over the same gradients
+        else:
+            stats = self._shard_stats(norm_type)
+        total = stats[0].sqrt() if norm_type == 2.0 else stats[0].clone()
+        if self._clip_coef is not None:
+            total = total * self._clip_coef  # clipping twice: the norm of the gradient as the first clip left it
+        if error_if_nonfinite and bool(torch.logical_or(total.isnan(), total.isinf())):
+            raise RuntimeError('The total norm of order %s for gradients from `parameters` is non-finite, so it cannot be '
+                               'clipped. To disable this error and scale the gradients by the non-finite norm anyway, set '
+                               '`error_if_nonfinite=False`' % norm_type)
+        coef = torch.clamp(max_norm / (total + 1e-6), max=1.0)
+        self._clip_coef = coef if self._clip_coef is None else self._clip_coef * coef
+        return total
 
     @contextmanager
     def skip_synchronize(self):
@@ -302,9 +383,9 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         finally:
             self._should_synchronize = True
 
-    def _update_shards(self):
+    def _update_shards(self, coef=None):
         """One fused kernel per param group and dtype over this rank's shards; hyper-parameters are read now, so LR
-        schedulers work."""
+        schedulers work.  coef: the clip coefficient on the device, or None."""
         native = mpi_ops._native()
         by_group = {}
         for b in self._buckets:
@@ -318,7 +399,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                     bufs = [b['state']['momentum_buffer'] for b in bs] if mom != 0.0 else []
                     first = mom != 0.0 and not bs[0]['mom_init']
                     native.fused_sgd_step(ps, gs, bufs, float(group['lr']), float(mom), float(group.get('dampening', 0.0)),
-                                          float(group.get('weight_decay', 0.0)), bool(group.get('nesterov', False)), 1.0, first)
+                                          float(group.get('weight_decay', 0.0)), bool(group.get('nesterov', False)), 1.0, first,
+                                          coef)
                     for b in bs:
                         b['mom_init'] = b['mom_init'] or mom != 0.0
                 else:
@@ -328,7 +410,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                     adamw = isinstance(self, torch.optim.AdamW) or bool(group.get('decoupled_weight_decay', False))
                     native.fused_adam_step(ps, gs, [b['state']['exp_avg'] for b in bs], [b['state']['exp_avg_sq'] for b in bs],
                                            float(group['lr']), float(b1), float(b2), float(group['eps']),
-                                           float(group.get('weight_decay', 0.0)), bs[0]['step'], 1.0, adamw)
+                                           float(group.get('weight_decay', 0.0)), bs[0]['step'], 1.0, adamw, coef)
 
     def _allgather_params(self):
         comm = self._comm
@@ -343,7 +425,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        if self._should_synchronize:
+        if self._should_synchronize and not self._reduced:
             if self._synchronized:
                 # a reduce-scatter is not idempotent: running it again would mix the reduced shard with the peers' local
                 # gradients, so the reduction done by synchronize() is used as it is
@@ -351,8 +433,9 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                               'optimizer.synchronize(); the gradients are not reduced a second time.')
             else:
                 self.synchronize()
-        self._synchronized = False
-        self._update_shards()
+        coef = self._clip_coef
+        self._drop_iteration_state()
+        self._update_shards(coef)
         self._allgather_params()
         return loss
 
@@ -362,6 +445,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             # a launched reduce-scatter may still be reading this rank's gradients for a peer
             raise AssertionError('optimizer.zero_grad() was called after loss.backward() but before optimizer.step() or '
                                  'optimizer.synchronize(). This is prohibited as it can cause a race condition.')
+        self._drop_iteration_state()  # an iteration whose step() was skipped leaves nothing behind
         for b in self._buckets:
             b['gflat'].zero_()
             for p in b['params']:
@@ -462,3 +546,26 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             g.update(saved)
         for b, s, m in zip(self._buckets, meta['steps'], meta['mom_init']):
             b['step'], b['mom_init'] = s, m
+
+
+class ShardedGradScaler(torch.amp.GradScaler):
+    """torch.amp.GradScaler for `hvd.DistributedOptimizer(..., shard_optimizer_state=True)`; any other optimizer gets
+    torch's behaviour unchanged.
+
+    With sharded optimizer state only this rank's shard of each gradient bucket is reduced, so torch's per-rank inf / NaN
+    check would let ranks disagree and skip step() on some of them only.  Here unscale_ reduces the pending gradients,
+    unscales the owned shards in place (fp16 gradients included) in the same pass that checks them, and allreduces the
+    verdict, so every rank sees the same found_inf: step() is taken or skipped, and the scale backed off, alike on all
+    ranks.  The pass also yields the 2-norm, which a following optimizer.clip_grad_norm_(max_norm) reuses:
+
+        scaler.scale(loss).backward()
+        scaler.unscale_(opt)
+        opt.clip_grad_norm_(1.0)
+        scaler.step(opt)
+        scaler.update()
+    """
+
+    def _unscale_grads_(self, optimizer, inv_scale, found_inf, allow_fp16):
+        if not isinstance(optimizer, _ShardedDistributedOptimizer):
+            return super()._unscale_grads_(optimizer, inv_scale, found_inf, allow_fp16)
+        return {found_inf.device: optimizer._unscale_and_check(inv_scale, found_inf)}
