@@ -2,12 +2,16 @@
 
     torchrun --nproc_per_node 8 bench/sharded_optimizer.py --model bert-large
     hvdrun -np 2 python bench/sharded_optimizer.py --model gpt2-medium
+    hvdrun -np 8 python bench/sharded_optimizer.py --model bert-large --master-weights
 
 Builds the model from horovod_b200.models, wraps AdamW in hvd.DistributedOptimizer and trains with bf16 autocast,
 alternating `shard_optimizer_state=True` and the unsharded `fused=True` optimizer (fresh model and optimizer each time)
 in one run, so both see the same GPUs, clocks and neighbours; with one rank both configurations are the unsharded one.  Prints one JSON line per rank and configuration:
 optimizer-state bytes, torch.cuda.max_memory_allocated (above what was allocated before the run) and the device-timed step time (CUDA events around >= 30 steps
 after warm-up), plus the GPU name and power limit read in the same run.
+
+--master-weights trains a bf16 model (no autocast) with fp32 master weights (`master_weights=True`) instead, so the
+optimizer-state bytes include the masters: 12 B per parameter unsharded, 12 / N B per rank sharded.
 
 Parameters and gradients in registered symmetric memory are VMM allocations made by this library, not by PyTorch's
 caching allocator: max_memory_allocated does not count them (in either configuration; the unsharded optimizer keeps its
@@ -38,15 +42,15 @@ def _gpu_info(device):
     return name, out or 'unknown'
 
 
-def _model(name, bs, seq, device):
+def _model(name, bs, seq, device, dtype):
     if name == 'bert-large':
-        model = models.bert_large().to(device)
+        model = models.bert_large().to(device, dtype)
         g = torch.Generator(device=device).manual_seed(hvd.rank())
         ids = torch.randint(0, 30522, (bs, seq), device=device, generator=g)
         labels = torch.where(torch.rand(bs, seq, device=device, generator=g) < 0.15, ids, torch.full_like(ids, -100))
         nsp = torch.randint(0, 2, (bs,), device=device, generator=g)
         return model, lambda: model(ids, labels=labels, next_sentence_label=nsp)
-    model = models.gpt2_medium().to(device)
+    model = models.gpt2_medium().to(device, dtype)
     g = torch.Generator(device=device).manual_seed(hvd.rank())
     ids = torch.randint(0, 50257, (bs, seq), device=device, generator=g)
     return model, lambda: model(ids, labels=ids)
@@ -63,13 +67,15 @@ def run(args, sharded, device):
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats(device)
     base = torch.cuda.memory_allocated(device)  # whatever earlier runs left behind is not this run's
-    model, loss_fn = _model(args.model, args.batch_size, args.seq_len, device)
+    model, loss_fn = _model(args.model, args.batch_size, args.seq_len, device,
+                            torch.bfloat16 if args.master_weights else torch.float32)
     opt = torch.optim.AdamW(model.parameters(), lr=1e-4, weight_decay=0.01)
-    opt = hvd.DistributedOptimizer(opt, named_parameters=model.named_parameters(), fused=True, shard_optimizer_state=sharded)
+    opt = hvd.DistributedOptimizer(opt, named_parameters=model.named_parameters(), fused=True, shard_optimizer_state=sharded,
+                                   master_weights=args.master_weights)
 
     def step():
         opt.zero_grad()
-        with torch.autocast('cuda', dtype=torch.bfloat16):
+        with torch.autocast('cuda', dtype=torch.bfloat16, enabled=not args.master_weights):
             loss = loss_fn()
         loss.backward()
         opt.step()
@@ -85,7 +91,8 @@ def run(args, sharded, device):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / args.steps
-    res = {'config': 'sharded' if sharded else 'unsharded fused', 'optimizer_state_bytes': _state_bytes(opt),
+    res = {'config': ('sharded' if sharded else 'unsharded fused') + (' + bf16 master weights' if args.master_weights else ''),
+           'optimizer_state_bytes': _state_bytes(opt),
            'max_memory_allocated': torch.cuda.max_memory_allocated(device) - base, 'step_ms': round(ms, 3),
            'loss': float(loss)}
     del opt, model, loss_fn
@@ -102,6 +109,7 @@ def main():
     p.add_argument('--steps', type=int, default=30)
     p.add_argument('--warmup', type=int, default=5)
     p.add_argument('--rounds', type=int, default=2, help='sharded / unsharded alternations')
+    p.add_argument('--master-weights', action='store_true', help='bf16 model with fp32 master weights instead of autocast')
     args = p.parse_args()
     if args.steps < 30:
         p.error('--steps must be >= 30')

@@ -7,6 +7,7 @@
 // update instead of a separate elementwise pass.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <type_traits>
 #include "p2p_kernels.h"
 
 namespace hvd {
@@ -52,12 +53,26 @@ template <typename T> __device__ __forceinline__ void store4(T* p, int64_t i, in
 }
 template <typename T> __device__ __forceinline__ bool is_aligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) % (sizeof(T) * kOptVec)) == 0; }
 
+// fp32 master weights (kMaster): P is bf16 / fp16 and every table entry carries `master`, an fp32 copy of its parameter.
+// The update runs on the master with exactly the arithmetic of the fp32-parameter instantiation, then the master is
+// stored and the parameter receives it rounded to nearest-even.  Reconcile: where the stored bits of the parameter are
+// not those of round(master) -- a write from outside the optimizer (load_state_dict, broadcast_parameters, an in-place
+// edit) or a zero-filled master -- the master restarts from the parameter.  pv holds the parameter on entry and the
+// value the update starts from on return.
+template <typename P> __device__ __forceinline__ void reconcile4(float* pv, const float* wv) {
+#pragma unroll
+  for (int k = 0; k < kOptVec; ++k)
+    if (__float_as_uint(to_f<P>(from_f<P>(wv[k]))) == __float_as_uint(pv[k])) pv[k] = wv[k];
+}
+
 // `grad_scale_dev` (nullptr: 1) is a factor that lives on the device, e.g. a clip coefficient computed by earlier kernels:
 // it reaches the update without a host synchronisation.  Multiplying by 1.f is exact, so nullptr changes no result.
-template <typename P, typename G>
+// Momentum is stored in the parameter dtype, or in fp32 with a master.
+template <typename P, typename G, bool kMaster>
 __global__ void __launch_bounds__(kOptThreads)
 fused_sgd_kernel(const SgdTensor* __restrict__ table, float lr, float momentum, float dampening, float wd, int nesterov,
                  float grad_scale, const float* __restrict__ grad_scale_dev, int first_step) {
+  using M = std::conditional_t<kMaster, float, P>;
   const SgdTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
@@ -65,8 +80,12 @@ fused_sgd_kernel(const SgdTensor* __restrict__ table, float lr, float momentum, 
   grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
   P* p = reinterpret_cast<P*>(t.param);
   const G* g = reinterpret_cast<const G*>(t.grad);
-  P* mbuf = reinterpret_cast<P*>(t.momentum);
-  const bool pa = is_aligned<P>(p) && (!mbuf || is_aligned<P>(mbuf)), ga = is_aligned<G>(g);
+  M* mbuf = reinterpret_cast<M*>(t.momentum);
+  float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
+  // pa: the parameter (and, without a master, the momentum); wa: the fp32 master and momentum
+  const bool pa = is_aligned<P>(p) && (kMaster || !mbuf || is_aligned<M>(mbuf)), ga = is_aligned<G>(g);
+  const bool wa = kMaster && is_aligned<float>(w) && (!mbuf || is_aligned<M>(mbuf));
+  const bool ma = kMaster ? wa : pa;
 #pragma unroll
   for (int it = 0; it < kOptIters; ++it) {
     const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
@@ -74,7 +93,12 @@ fused_sgd_kernel(const SgdTensor* __restrict__ table, float lr, float momentum, 
     float pv[kOptVec], gv[kOptVec], mv[kOptVec];
     load4<P>(p, i, n, pa, pv);
     load4<G>(g, i, n, ga, gv);
-    if (mbuf && !first_step) load4<P>(mbuf, i, n, pa, mv);
+    if (mbuf && !first_step) load4<M>(mbuf, i, n, ma, mv);
+    if constexpr (kMaster) {
+      float wv[kOptVec];
+      load4<float>(w, i, n, wa, wv);
+      reconcile4<P>(pv, wv);
+    }
 #pragma unroll
     for (int k = 0; k < kOptVec; ++k) {
       float d = gv[k] * grad_scale;
@@ -86,12 +110,13 @@ fused_sgd_kernel(const SgdTensor* __restrict__ table, float lr, float momentum, 
       }
       pv[k] = fmaf(-lr, d, pv[k]);
     }
+    if constexpr (kMaster) store4<float>(w, i, n, wa, pv);
     store4<P>(p, i, n, pa, pv);
-    if (mbuf) store4<P>(mbuf, i, n, pa, mv);
+    if (mbuf) store4<M>(mbuf, i, n, ma, mv);
   }
 }
 
-template <typename P, typename G>
+template <typename P, typename G, bool kMaster>
 __global__ void __launch_bounds__(kOptThreads)
 fused_adam_kernel(const AdamTensor* __restrict__ table, float lr, float b1, float b2, float eps, float wd, float c1, float c2,
                   float grad_scale, const float* __restrict__ grad_scale_dev, int adamw) {
@@ -104,7 +129,9 @@ fused_adam_kernel(const AdamTensor* __restrict__ table, float lr, float b1, floa
   const G* g = reinterpret_cast<const G*>(t.grad);
   float* m = reinterpret_cast<float*>(t.exp_avg);
   float* v = reinterpret_cast<float*>(t.exp_avg_sq);
-  const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g), sa = is_aligned<float>(m) && is_aligned<float>(v);
+  float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
+  const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g),
+             sa = is_aligned<float>(m) && is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
   const float rsc2 = rsqrtf(c2), step = lr / c1;
 #pragma unroll
   for (int it = 0; it < kOptIters; ++it) {
@@ -115,6 +142,11 @@ fused_adam_kernel(const AdamTensor* __restrict__ table, float lr, float b1, floa
     load4<G>(g, i, n, ga, gv);
     load4<float>(m, i, n, sa, mv);
     load4<float>(v, i, n, sa, vv);
+    if constexpr (kMaster) {
+      float wv[kOptVec];
+      load4<float>(w, i, n, sa, wv);
+      reconcile4<P>(pv, wv);
+    }
 #pragma unroll
     for (int k = 0; k < kOptVec; ++k) {
       float d = gv[k] * grad_scale;
@@ -124,6 +156,7 @@ fused_adam_kernel(const AdamTensor* __restrict__ table, float lr, float b1, floa
       const float denom = sqrtf(vv[k]) * rsc2 + eps;
       pv[k] -= step * mv[k] / denom;
     }
+    if constexpr (kMaster) store4<float>(w, i, n, sa, pv);
     store4<P>(p, i, n, pa, pv);
     store4<float>(m, i, n, sa, mv);
     store4<float>(v, i, n, sa, vv);
@@ -225,13 +258,18 @@ grad_shard_stats_kernel(const StatTensor* __restrict__ table, const float* __res
 
 cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
                            float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
-                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev) {
+                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev, bool master) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
   dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)n);
-  if (param_dtype == 7 && grad_dtype == 7) fused_sgd_kernel<float, float><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
-  else if (param_dtype == 7 && grad_dtype == 10) fused_sgd_kernel<float, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
-  else if (param_dtype == 10 && grad_dtype == 10) fused_sgd_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
-  else if (param_dtype == 6 && grad_dtype == 6) fused_sgd_kernel<__half, __half><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  if (master) {
+    if (param_dtype == 10 && grad_dtype == 10) fused_sgd_kernel<__nv_bfloat16, __nv_bfloat16, true><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+    else if (param_dtype == 6 && grad_dtype == 6) fused_sgd_kernel<__half, __half, true><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+    else return cudaErrorInvalidValue;
+  }
+  else if (param_dtype == 7 && grad_dtype == 7) fused_sgd_kernel<float, float, false><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  else if (param_dtype == 7 && grad_dtype == 10) fused_sgd_kernel<float, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  else if (param_dtype == 10 && grad_dtype == 10) fused_sgd_kernel<__nv_bfloat16, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  else if (param_dtype == 6 && grad_dtype == 6) fused_sgd_kernel<__half, __half, false><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
   else return cudaErrorInvalidValue;
   CountKernelLaunch();
   return cudaGetLastError();
@@ -239,13 +277,19 @@ cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, flo
 
 cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
                              float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale, int adamw,
-                             int param_dtype, int grad_dtype, cudaStream_t stream, const float* grad_scale_dev) {
+                             int param_dtype, int grad_dtype, cudaStream_t stream, const float* grad_scale_dev,
+                             bool master) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
   dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)n);
-  if (param_dtype == 7 && grad_dtype == 7) fused_adam_kernel<float, float><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-  else if (param_dtype == 7 && grad_dtype == 10) fused_adam_kernel<float, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-  else if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-  else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  if (master) {
+    if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16, true><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+    else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half, true><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+    else return cudaErrorInvalidValue;
+  }
+  else if (param_dtype == 7 && grad_dtype == 7) fused_adam_kernel<float, float, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  else if (param_dtype == 7 && grad_dtype == 10) fused_adam_kernel<float, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  else if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
   else return cudaErrorInvalidValue;
   CountKernelLaunch();
   return cudaGetLastError();

@@ -175,16 +175,17 @@ cudaError_t LaunchAdasumStep(const CommParams& cp, const AdasumArgs& args, doubl
 int AdasumNumLaunches(int nranks);
 
 // Fused multi-tensor optimizer updates (see optim_kernels.cu).  The gradient factor is grad_scale * *grad_scale_dev
-// (nullptr: grad_scale alone, bit for bit).
-struct SgdTensor { void* param; const void* grad; void* momentum; int64_t count; };
+// (nullptr: grad_scale alone, bit for bit).  `master` (bf16 / bf16 and fp16 / fp16 only): every entry's `master` is an
+// fp32 copy of its parameter that the update runs on (SGD momentum is then fp32); without it `master` is not read.
+struct SgdTensor { void* param; const void* grad; void* momentum; int64_t count; void* master; };
 cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
                            float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
-                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev = nullptr);
-struct AdamTensor { void* param; const void* grad; void* exp_avg; void* exp_avg_sq; int64_t count; };
+                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev = nullptr, bool master = false);
+struct AdamTensor { void* param; const void* grad; void* exp_avg; void* exp_avg_sq; int64_t count; void* master; };
 cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
                              float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale,
                              int adamw, int param_dtype, int grad_dtype, cudaStream_t stream,
-                             const float* grad_scale_dev = nullptr);
+                             const float* grad_scale_dev = nullptr, bool master = false);
 // Gradient statistics of flat gradient shards in one pass (see optim_kernels.cu): optional in-place scaling by
 // *inv_scale, then out[0] += sum of squares (norm_inf: out[0] = max(out[0], max |g|)) and out[1] = max(out[1], non-finite).
 // `partial` / `partial_flag` hold GradShardStatsCtas() entries; `ticket` is a zeroed counter that the kernel leaves zeroed,

@@ -509,19 +509,36 @@ const float* DeviceScalar(const char* op, const char* what, const c10::optional<
   return t->data_ptr<float>();
 }
 
+// fp32 master weights (optional, empty: none): one fp32 tensor per param with its sizes, strides and device.  Only for
+// bf16 / fp16 params with gradients of the same dtype, the pairs the master kernels are instantiated for.  Call after
+// the params themselves are checked.  Returns whether masters are in use.
+bool CheckMasters(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
+                  const std::vector<at::Tensor>& masters) {
+  if (masters.empty()) return false;
+  const auto pt = params[0].scalar_type();
+  TORCH_CHECK(pt == at::kBFloat16 || pt == at::kHalf, op, ": master_params are for bfloat16 / float16 params, params are ", pt);
+  TORCH_CHECK(grads[0].scalar_type() == pt, op, ": with master_params the grads must be ", pt, ", got ", grads[0].scalar_type());
+  for (size_t i = 0; i < params.size(); ++i) CheckOptimizerPeer(op, "master_params", i, params[i], masters[i], at::kFloat);
+  return true;
+}
+
 void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momenta, double lr,
                   double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step,
-                  c10::optional<at::Tensor> grad_scale_dev) {
+                  c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
   const bool has_mom = momentum != 0.0;
   TORCH_CHECK(params.size() == grads.size(), "fused_sgd: list sizes differ");
   TORCH_CHECK(momenta.size() == params.size() || (!has_mom && momenta.empty()),
               "fused_sgd: ", momenta.size(), " momentum buffers for ", params.size(), " params");
+  TORCH_CHECK(masters.empty() || masters.size() == params.size(), "fused_sgd: ", masters.size(), " master params for ",
+              params.size(), " params");
   if (params.empty()) return;
   for (size_t i = 0; i < params.size(); ++i) {
     CheckOptimizerParam("fused_sgd", i, params[i], params[0]);
     CheckOptimizerPeer("fused_sgd", "grads", i, params[i], grads[i], grads[0].scalar_type());
-    if (has_mom) CheckOptimizerPeer("fused_sgd", "momentum_buffers", i, params[i], momenta[i], params[i].scalar_type());
   }
+  const bool has_master = CheckMasters("fused_sgd", params, grads, masters);
+  for (size_t i = 0; has_mom && i < params.size(); ++i)  // fp32 momentum with a master, else the param dtype
+    CheckOptimizerPeer("fused_sgd", "momentum_buffers", i, params[i], momenta[i], has_master ? at::kFloat : params[i].scalar_type());
   const float* gsd = DeviceScalar("fused_sgd", "grad_scale_dev", grad_scale_dev, params[0]);
   int device = (int)params[0].get_device();
   c10::cuda::CUDAGuard guard(params[0].device());
@@ -532,20 +549,25 @@ void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads,
     table[i].param = params[i].data_ptr(); table[i].grad = grads[i].data_ptr();
     table[i].momentum = has_mom ? momenta[i].data_ptr() : nullptr;
     table[i].count = params[i].numel();
+    table[i].master = has_master ? masters[i].data_ptr() : nullptr;
     maxc = std::max(maxc, table[i].count);
   }
   const auto* dt = (const kern::SgdTensor*)GpuContext::Get().Stage(device, table.data(), table.size() * sizeof(kern::SgdTensor), s);
   TORCH_CHECK(dt != nullptr, "fused_sgd: table too large");
   cudaError_t e = kern::LaunchFusedSgd(dt, (int)table.size(), maxc, (float)lr, (float)momentum, (float)dampening, (float)weight_decay,
                                        nesterov ? 1 : 0, (float)grad_scale, first_step ? 1 : 0,
-                                       (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s, gsd);
+                                       (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s, gsd,
+                                       has_master);
   TORCH_CHECK(e == cudaSuccess, "fused_sgd launch failed: ", cudaGetErrorString(e));
 }
 
 void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
                    std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
-                   int64_t step, double grad_scale, bool adamw, c10::optional<at::Tensor> grad_scale_dev) {
+                   int64_t step, double grad_scale, bool adamw, c10::optional<at::Tensor> grad_scale_dev,
+                   std::vector<at::Tensor> masters) {
   TORCH_CHECK(params.size() == grads.size() && params.size() == exp_avg.size() && params.size() == exp_avg_sq.size(), "fused_adam: list sizes differ");
+  TORCH_CHECK(masters.empty() || masters.size() == params.size(), "fused_adam: ", masters.size(), " master params for ",
+              params.size(), " params");
   // step is 1-based: step 0 would make the bias correction 1 - beta1^0 = 0 and every parameter inf / NaN
   TORCH_CHECK(step >= 1, "fused_adam: step must be >= 1, got ", step);
   if (params.empty()) return;
@@ -555,6 +577,7 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
     CheckOptimizerPeer("fused_adam", "exp_avgs", i, params[i], exp_avg[i], at::kFloat);
     CheckOptimizerPeer("fused_adam", "exp_avg_sqs", i, params[i], exp_avg_sq[i], at::kFloat);
   }
+  const bool has_master = CheckMasters("fused_adam", params, grads, masters);
   const float* gsd = DeviceScalar("fused_adam", "grad_scale_dev", grad_scale_dev, params[0]);
   int device = (int)params[0].get_device();
   c10::cuda::CUDAGuard guard(params[0].device());
@@ -565,6 +588,7 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
     table[i].param = params[i].data_ptr(); table[i].grad = grads[i].data_ptr();
     table[i].exp_avg = exp_avg[i].data_ptr(); table[i].exp_avg_sq = exp_avg_sq[i].data_ptr();
     table[i].count = params[i].numel();
+    table[i].master = has_master ? masters[i].data_ptr() : nullptr;
     maxc = std::max(maxc, table[i].count);
   }
   const auto* dt = (const kern::AdamTensor*)GpuContext::Get().Stage(device, table.data(), table.size() * sizeof(kern::AdamTensor), s);
@@ -572,7 +596,8 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   const float c1 = 1.0f - (float)std::pow(beta1, (double)step), c2 = 1.0f - (float)std::pow(beta2, (double)step);
   cudaError_t e = kern::LaunchFusedAdamW(dt, (int)table.size(), maxc, (float)lr, (float)beta1, (float)beta2, (float)eps,
                                          (float)weight_decay, c1, c2, (float)grad_scale, adamw ? 1 : 0,
-                                         (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s, gsd);
+                                         (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s, gsd,
+                                         has_master);
   TORCH_CHECK(e == cudaSuccess, "fused_adam launch failed: ", cudaGetErrorString(e));
 }
 
@@ -657,10 +682,11 @@ PYBIND11_MODULE(_hvd_torch, m) {
   m.def("captured_allgather_", &CapturedAllgather);
   m.def("fused_sgd_step", &FusedSgdStep, py::arg("params"), py::arg("grads"), py::arg("momenta"), py::arg("lr"),
         py::arg("momentum"), py::arg("dampening"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("grad_scale"),
-        py::arg("first_step"), py::arg("grad_scale_dev") = py::none());
+        py::arg("first_step"), py::arg("grad_scale_dev") = py::none(), py::arg("master_params") = std::vector<at::Tensor>());
   m.def("fused_adam_step", &FusedAdamStep, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
         py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
-        py::arg("grad_scale"), py::arg("adamw"), py::arg("grad_scale_dev") = py::none());
+        py::arg("grad_scale"), py::arg("adamw"), py::arg("grad_scale_dev") = py::none(),
+        py::arg("master_params") = std::vector<at::Tensor>());
   m.def("grad_shard_stats", &GradShardStats, py::arg("grads"), py::arg("out"), py::arg("inv_scale") = py::none(),
         py::arg("norm_inf") = false);
 }

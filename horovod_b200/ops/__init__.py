@@ -16,22 +16,29 @@ def _native():
 
 
 def fused_sgd_step(params, grads, momentum_buffers, lr, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False,
-                   grad_scale=1.0, first_step=False, grad_scale_dev=None):
+                   grad_scale=1.0, first_step=False, grad_scale_dev=None, master_params=None):
     """One launch for the whole parameter list (fp32 / bf16 / fp16 parameters, fp32 or matching gradients).
     `grad_scale_dev`: an optional 1-element fp32 tensor on the parameters' device; the gradients are multiplied by
-    grad_scale * grad_scale_dev[0], read by the kernel, so no host synchronisation is needed."""
+    grad_scale * grad_scale_dev[0], read by the kernel, so no host synchronisation is needed.
+
+    `master_params`: optional fp32 master copies of bf16 / fp16 parameters (gradients of the parameters' dtype), one per
+    parameter with its sizes and strides; momentum buffers are then fp32 too. The update runs on the master and the
+    parameter receives it rounded to nearest-even. Where a parameter no longer equals its rounded master (it was
+    written from outside, or the master is zero-filled), the master first restarts from the parameter."""
     return _native().fused_sgd_step(list(params), list(grads), list(momentum_buffers), float(lr), float(momentum), float(dampening),
-                                    float(weight_decay), bool(nesterov), float(grad_scale), bool(first_step), grad_scale_dev)
+                                    float(weight_decay), bool(nesterov), float(grad_scale), bool(first_step), grad_scale_dev,
+                                    list(master_params or []))
 
 
 def fused_adam_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, step=1,
-                    grad_scale=1.0, adamw=True, grad_scale_dev=None):
+                    grad_scale=1.0, adamw=True, grad_scale_dev=None, master_params=None):
     """One launch of Adam / AdamW for the whole parameter list (fp32 / bf16 / fp16 parameters, fp32 or matching
     gradients, fp32 state with the parameters' sizes and strides; `step` is the 1-based step count). Mismatched
-    lists, dtypes, sizes, strides or devices raise RuntimeError before anything is launched. `grad_scale_dev` as in
-    fused_sgd_step."""
+    lists, dtypes, sizes, strides or devices raise RuntimeError before anything is launched. `grad_scale_dev` and
+    `master_params` as in fused_sgd_step."""
     return _native().fused_adam_step(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1), float(beta2),
-                                     float(eps), float(weight_decay), int(step), float(grad_scale), bool(adamw), grad_scale_dev)
+                                     float(eps), float(weight_decay), int(step), float(grad_scale), bool(adamw), grad_scale_dev,
+                                     list(master_params or []))
 
 
 def grad_shard_stats(tensors, out, inv_scale=None, norm_type=2.0):

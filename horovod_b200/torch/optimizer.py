@@ -26,9 +26,13 @@ from horovod_b200.torch.mpi_ops import (Adasum, Average, Sum, allreduce_async_, 
 class _DistributedOptimizer(torch.optim.Optimizer):
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
-                 fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None):
+                 fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None, master_weights=False):
         super(self.__class__, self).__init__(params)
         self._compression = compression
+        # fp32 master copies of bf16 / fp16 parameters, kept as optimizer state ('master_param') and updated by the fused
+        # kernels only: master_weights implies fused, and step() never hands those parameters to torch's own update
+        self._master_weights = bool(master_weights)
+        fused = fused or self._master_weights
         # opt-in: fp32 gradient buckets travel as bf16 / fp16 (a registered shadow bucket of half the bytes is what the
         # zero-copy kernel reduces; the switch accumulates in fp32).  Not validated on hardware yet (docs/roadmap.md B3).
         if bucket_wire_dtype is None:
@@ -114,18 +118,19 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         for p in self._allreduce_delay:
             self._allreduce_delay[p] = self.backward_passes_per_step
         super(self.__class__, self).load_state_dict(*args, **kwargs)
-        if self._fused and isinstance(self, (torch.optim.Adam, torch.optim.AdamW)):
+        if self._fused and (isinstance(self, (torch.optim.Adam, torch.optim.AdamW)) or self._master_weights):
             self._keep_fp32_moments(args[0] if args else kwargs['state_dict'])
 
     def _keep_fp32_moments(self, state_dict):
         """torch casts every loaded floating state tensor to its parameter's dtype. The fused Adam kernel keeps fp32
-        moments for bf16 / fp16 parameters too, so take the checkpoint's fp32 values back: a checkpoint round-trips
-        exactly instead of losing the moments' low bits."""
+        moments for bf16 / fp16 parameters too, and with master weights the fp32 master copy and SGD momentum, so take
+        the checkpoint's fp32 values back: a checkpoint round-trips exactly instead of losing their low bits."""
         saved = [i for g in state_dict['param_groups'] for i in g['params']]
         params = [p for g in self.param_groups for p in g['params']]
+        keys = ('exp_avg', 'exp_avg_sq') + (('master_param', 'momentum_buffer') if self._master_weights else ())
         for pid, p in zip(saved, params):
             st = state_dict['state'].get(pid, {})
-            for key in ('exp_avg', 'exp_avg_sq'):
+            for key in keys:
                 t = st.get(key)
                 if torch.is_tensor(t) and t.dtype == torch.float32 and p.dtype != torch.float32 and key in self.state[p]:
                     self.state[p][key] = _state_like(p, t, torch.float32)
@@ -523,6 +528,16 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                               "code.")
             self.synchronize(_defer_shadow_copy=self._fused and closure is None)
         self._synchronized = False
+        if self._master_weights:
+            # the masters live in the fused kernels only: evaluate the closure, then the fused update (or an error)
+            loss = None
+            if closure is not None:
+                with torch.enable_grad():
+                    loss = closure()
+            _fused_step(self)
+            for bucket in self._buckets:
+                bucket['shadow_fresh'] = False
+            return loss
         if self._fused and closure is None and _fused_step(self):
             for bucket in self._buckets:
                 bucket['shadow_fresh'] = False
@@ -562,13 +577,20 @@ def _find_duplicates(lst):
     return dups
 
 
-def _fused_plan(opt):
+def _fused_plan(opt, why=None):
     """Pure eligibility pass of the fused optimizer step: returns the launch plan [(group, params, grads)] or None.
-    Nothing is mutated here, so a `None` leaves the wrapped optimizer's own step() as a clean fallback."""
+    Nothing is mutated here, so a `None` leaves the wrapped optimizer's own step() as a clean fallback; the reason is
+    appended to the list `why`, if given."""
+    def no(reason):
+        if why is not None:
+            why.append(reason)
+        return None
+
+    master = getattr(opt, '_master_weights', False)
     is_sgd = isinstance(opt, torch.optim.SGD)
     is_adam = isinstance(opt, (torch.optim.Adam, torch.optim.AdamW))
     if not (is_sgd or is_adam):
-        return None
+        return no('the optimizer is %s, not SGD, Adam or AdamW' % type(opt).__name__)
     grad_of = getattr(opt, '_grad_for_update', lambda q: q.grad)
     plan = []
     for group in opt.param_groups:
@@ -576,16 +598,18 @@ def _fused_plan(opt):
         if not params:
             continue
         if group.get('maximize', False) or (is_adam and group.get('amsgrad', False)):
-            return None
+            return no('maximize=True or amsgrad=True')
         if not all(p.is_cuda and not p.grad.is_sparse and mpi_ops._is_dense(p) and p.grad.stride() == p.stride() for p in params):
-            return None
+            return no('a parameter is not a dense CUDA tensor, its gradient is sparse, or its strides differ from the gradient\'s')
         by_dtype = {}
         for p in params:
             by_dtype.setdefault((p.dtype, grad_of(p).dtype), []).append(p)
         if any(pd == torch.float32 and gd == torch.float16 for pd, gd in by_dtype):
-            return None  # no fp32-parameter / fp16-gradient kernel
+            return no('fp16 gradients of fp32 parameters')  # no fp32-parameter / fp16-gradient kernel
+        if master and any(pd != torch.float32 and gd != pd for pd, gd in by_dtype):
+            return no('bf16 / fp16 parameters with gradients of another dtype')  # master kernels: (bf16, bf16), (fp16, fp16)
         for ps in by_dtype.values():
-            if is_sgd and group.get('momentum', 0.0) != 0.0:
+            if is_sgd and group.get('momentum', 0.0) != 0.0 and not master:
                 have = [opt.state[p].get('momentum_buffer') is not None for p in ps]
                 if any(have) and not all(have):
                     return None  # partially initialised momentum (parameters added later): let torch handle it
@@ -593,30 +617,61 @@ def _fused_plan(opt):
     return plan
 
 
+def _master_param(opt, p):
+    """p's fp32 master copy with p's strides, created from p on first use (a checkpoint's or a stray layout is
+    normalised). A master that p's value no longer matches is reconciled by the kernel itself."""
+    st = opt.state[p]
+    w = st.get('master_param')
+    if w is None:
+        w = st['master_param'] = _state_like(p, p.detach(), torch.float32)
+    elif w.dtype != torch.float32 or w.stride() != p.stride() or w.device != p.device:
+        w = st['master_param'] = _state_like(p, w, torch.float32)
+    return w
+
+
 def _fused_step(opt):
-    """One multi-tensor kernel for the whole model when the wrapped optimizer is SGD or Adam/AdamW on CUDA."""
+    """One multi-tensor kernel for the whole model when the wrapped optimizer is SGD or Adam/AdamW on CUDA. With master
+    weights a plan that cannot be fused raises RuntimeError instead of returning False."""
     native = mpi_ops._native()
-    plan = _fused_plan(opt)
+    use_master = getattr(opt, '_master_weights', False)
+    why = []
+    plan = _fused_plan(opt, why)
     if plan is None:
+        if use_master:
+            raise RuntimeError('master_weights: the fused optimizer update cannot run (%s), and torch\'s own update would '
+                               'bypass the fp32 master weights' % (why[0] if why else 'not eligible'))
         return False
     is_sgd = isinstance(opt, torch.optim.SGD)
     with torch.no_grad():
         for group, ps, grads in plan:
+            master = use_master and ps[0].dtype != torch.float32
+            masters = [_master_param(opt, p) for p in ps] if master else []
             if is_sgd:
                 mom = group.get('momentum', 0.0)
-                bufs, first = [], False
+                sdt = torch.float32 if master else None  # momentum dtype: fp32 with masters, else the parameter's
+                bufs, fresh = [], []
                 if mom != 0.0:
                     for p in ps:
                         st = opt.state[p]
                         buf = st.get('momentum_buffer')
                         if buf is None:
-                            buf = st['momentum_buffer'] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                            first = True
-                        elif buf.dtype != p.dtype or buf.stride() != p.stride():
-                            buf = st['momentum_buffer'] = _state_like(p, buf, p.dtype)
+                            buf = st['momentum_buffer'] = torch.zeros_like(p, dtype=sdt, memory_format=torch.preserve_format)
+                            fresh.append(True)
+                        else:
+                            if buf.dtype != (sdt or p.dtype) or buf.stride() != p.stride():
+                                buf = st['momentum_buffer'] = _state_like(p, buf, sdt or p.dtype)
+                            fresh.append(False)
                         bufs.append(buf)
-                native.fused_sgd_step(ps, grads, bufs, float(group['lr']), float(mom), float(group.get('dampening', 0.0)),
-                                      float(group.get('weight_decay', 0.0)), bool(group.get('nesterov', False)), 1.0, first)
+                # with masters a parameter that joins later (frozen so far) starts its momentum while the others continue:
+                # one launch for each (without masters the plan only admits all-fresh or none-fresh)
+                parts = [[i for i, f in enumerate(fresh) if f == want] for want in (True, False)] if any(fresh) and not all(fresh) \
+                    else [list(range(len(ps)))]
+                for idx in parts:
+                    pick = lambda xs: [xs[i] for i in idx] if xs else xs  # noqa: E731
+                    kw = {'master_params': pick(masters)} if master else {}
+                    native.fused_sgd_step(pick(ps), pick(grads), pick(bufs), float(group['lr']), float(mom),
+                                          float(group.get('dampening', 0.0)), float(group.get('weight_decay', 0.0)),
+                                          bool(group.get('nesterov', False)), 1.0, bool(fresh) and fresh[idx[0]], **kw)
             else:
                 exp_avg, exp_avg_sq, steps = [], [], []
                 for p in ps:
@@ -657,10 +712,12 @@ def _fused_step(opt):
                     if len(by_step) > 1:
                         sub = lambda xs: [xs[i] for i in idx]  # noqa: E731
                         args = (sub(ps), sub(grads), sub(exp_avg), sub(exp_avg_sq))
+                        kw = {'master_params': sub(masters)} if master else {}
                     else:
                         args = (ps, grads, exp_avg, exp_avg_sq)
+                        kw = {'master_params': masters} if master else {}
                     native.fused_adam_step(*args, float(group['lr']), float(b1), float(b2), float(group['eps']),
-                                           float(group.get('weight_decay', 0.0)), step, 1.0, adamw)
+                                           float(group.get('weight_decay', 0.0)), step, 1.0, adamw, **kw)
     return True
 
 
@@ -828,7 +885,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none, backward_passes_per_step=1,
                          op=Average, gradient_predivide_factor=1.0, num_groups=0, groups=None, sparse_as_dense=False,
                          process_set=global_process_set, fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None,
-                         shard_optimizer_state=False):
+                         shard_optimizer_state=False, master_weights=False):
     """Wraps `optimizer` so gradients are combined across ranks before the parameter update.
 
     Arguments follow the reference (horovod/torch/optimizer.py:516-608). `fused=True` (new) runs the SGD /
@@ -838,7 +895,24 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     ranks: gradients are reduce-scattered, each rank updates its shard with the fused kernel and the parameters are
     allgathered (see horovod_b200/torch/sharded_optimizer.py).  SGD / Adam / AdamW with op Average or Sum on one host;
     raises ValueError otherwise.  The sharded update always runs the fused kernel, whatever `fused` says.  With one
-    rank it is the ordinary optimizer."""
+    rank it is the ordinary optimizer.
+
+    `master_weights=True` (new) gives every bf16 / fp16 trainable parameter an fp32 master copy, held as optimizer state
+    ('master_param', sharded like the moments with shard_optimizer_state): the update runs in fp32 on the master and the
+    parameter receives it rounded to nearest-even, so updates smaller than half an ulp of the parameter are not lost.
+    SGD momentum is then fp32 as well.  fp32 parameters are unaffected.  Implies fused=True; SGD / Adam / AdamW only,
+    without maximize, amsgrad or op=Adasum (ValueError).  A parameter written from outside the optimizer
+    (load_state_dict, broadcast_parameters, an in-place edit) is picked up by the next step: where it no longer equals
+    its rounded master, the master restarts from it."""
+    if master_weights:
+        if op == Adasum:
+            raise ValueError('master_weights is not supported with op=Adasum')
+        if not isinstance(optimizer, (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW)):
+            raise ValueError('master_weights supports SGD, Adam and AdamW only, not %s' % type(optimizer).__name__)
+        for g in optimizer.param_groups:
+            if g.get('maximize', False) or g.get('amsgrad', False):
+                raise ValueError('master_weights does not support maximize=True or amsgrad=True')
+        fused = True
     if gradient_predivide_factor != 1.0:
         if rocm_built_safe():
             raise ValueError('gradient_predivide_factor not supported yet with ROCm')
@@ -855,11 +929,12 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
         from horovod_b200.torch.sharded_optimizer import _ShardedDistributedOptimizer
         cls = type(optimizer.__class__.__name__, (_ShardedDistributedOptimizer, optimizer.__class__), {})
         return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,
-                   gradient_predivide_factor, groups, sparse_as_dense, process_set, bucket_cap_mb)
+                   gradient_predivide_factor, groups, sparse_as_dense, process_set, bucket_cap_mb, master_weights)
     if op != Adasum or size() == 1:
         cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedOptimizer.__dict__))
         return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,
-                   gradient_predivide_factor, groups, sparse_as_dense, process_set, fused, zero_copy, bucket_cap_mb, bucket_wire_dtype)
+                   gradient_predivide_factor, groups, sparse_as_dense, process_set, fused, zero_copy, bucket_cap_mb, bucket_wire_dtype,
+                   master_weights)
     if process_set != global_process_set:
         raise NotImplementedError("Adasum does not support non-global process sets yet.")
     cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedAdasumOptimizer.__dict__))

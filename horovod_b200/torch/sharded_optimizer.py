@@ -14,6 +14,9 @@ takes 1/N of the memory.  The allgather runs after the update and does not overl
 Global-norm clipping (`clip_grad_norm_`) and AMP loss scaling (`ShardedGradScaler`) read only the owned shards: one
 statistics kernel per gradient dtype and one scalar allreduce give every rank the same norm and the same inf / NaN
 verdict, and the clip coefficient reaches the update on the device.
+
+With `master_weights=True` every bf16 / fp16 bucket also keeps an fp32 master copy of its owned shard ('master_param'),
+which the fused kernel updates and rounds into the parameter shard before the allgather.
 """
 import math
 import os
@@ -130,7 +133,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
 
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
-                 bucket_cap_mb=32):
+                 bucket_cap_mb=32, master_weights=False):
         super().__init__(params)
         is_sgd = isinstance(self, torch.optim.SGD)
         is_adam = isinstance(self, (torch.optim.Adam, torch.optim.AdamW))
@@ -204,13 +207,19 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                     self._p_to_bucket[p] = b
                 lo, hi = shard_range(b, self._rank)
                 b['pshard'], b['gshard'] = pflat[lo:hi], gflat[lo:hi]
+                master = master_weights and b['dtype'] != torch.float32
                 if is_sgd:
-                    # the fused SGD kernel keeps momentum in the parameter dtype
-                    b['state'] = {'momentum_buffer': torch.zeros(b['shard'], dtype=b['dtype'], device=device)} \
+                    # the fused SGD kernel keeps momentum in the parameter dtype, or in fp32 with master weights
+                    b['state'] = {'momentum_buffer': torch.zeros(b['shard'], dtype=torch.float32 if master else b['dtype'],
+                                                                 device=device)} \
                         if self.param_groups[b['group']].get('momentum', 0.0) != 0.0 else {}
                 else:
                     b['state'] = {'exp_avg': torch.zeros(b['shard'], dtype=torch.float32, device=device),
                                   'exp_avg_sq': torch.zeros(b['shard'], dtype=torch.float32, device=device)}
+                if master:
+                    # fp32 master copy of the owned shard of a bf16 / fp16 bucket: optimizer state, sharded like the moments
+                    b['state']['master_param'] = b['pshard'].float()
+                b['stepped'] = False
         # cross-rank gradient statistics: [sum of squares or max |g|, non-finite] in registered memory, padded so that the
         # in-place allreduce can split it across the ranks
         self._stats = mpi_ops.symm_empty(ALIGN // 4 * self._nranks, dtype=torch.float32, device=device,
@@ -394,13 +403,15 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             for (gi, _), bs in by_group.items():
                 group = self.param_groups[gi]
                 ps, gs = [b['pshard'] for b in bs], [b['gshard'] for b in bs]
+                # every bucket of a (group, dtype) has a master or none has
+                kw = {'master_params': [b['state']['master_param'] for b in bs]} if 'master_param' in bs[0]['state'] else {}
                 if self._is_sgd:
                     mom = group.get('momentum', 0.0)
                     bufs = [b['state']['momentum_buffer'] for b in bs] if mom != 0.0 else []
                     first = mom != 0.0 and not bs[0]['mom_init']
                     native.fused_sgd_step(ps, gs, bufs, float(group['lr']), float(mom), float(group.get('dampening', 0.0)),
                                           float(group.get('weight_decay', 0.0)), bool(group.get('nesterov', False)), 1.0, first,
-                                          coef)
+                                          coef, **kw)
                     for b in bs:
                         b['mom_init'] = b['mom_init'] or mom != 0.0
                 else:
@@ -410,7 +421,9 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                     adamw = isinstance(self, torch.optim.AdamW) or bool(group.get('decoupled_weight_decay', False))
                     native.fused_adam_step(ps, gs, [b['state']['exp_avg'] for b in bs], [b['state']['exp_avg_sq'] for b in bs],
                                            float(group['lr']), float(b1), float(b2), float(group['eps']),
-                                           float(group.get('weight_decay', 0.0)), bs[0]['step'], 1.0, adamw, coef)
+                                           float(group.get('weight_decay', 0.0)), bs[0]['step'], 1.0, adamw, coef, **kw)
+                for b in bs:
+                    b['stepped'] = True
 
     def _allgather_params(self):
         comm = self._comm
@@ -485,8 +498,9 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         index = {id(p): i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
         state = {}
         for b in self._buckets:
-            if (b['step'] == 0) if not self._is_sgd else not b['mom_init']:
-                continue  # no state yet (the same on every rank)
+            if not b['state'] or ((b['step'] == 0) if not self._is_sgd else
+                                  not (b['mom_init'] or ('master_param' in b['state'] and b['stepped']))):
+                continue  # no state yet (the same on every rank); a plain-SGD bucket may still hold masters
             gathered = {}
             for key, shard in b['state'].items():
                 full = mpi_ops.allgather(shard, name='sharded_opt.state.%d.%s' % (b['index'], key), process_set=self.process_set)
@@ -523,6 +537,9 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                                                 [p.stride() for p in b['params']], dtype=shard.dtype, device='cpu'))
                     if key == 'momentum_buffer':
                         b['mom_init'] = any(t is not None for t in full)
+                    if key == 'master_param':
+                        # members without a saved master get zeros, which the kernel replaces by the parameter's value
+                        b['stepped'] = any(t is not None for t in full)
                 steps = [float(st['step']) for st in per if 'step' in st]
                 b['step'] = int(max(steps)) if steps else 0
         self._reset_launch_order()
