@@ -163,6 +163,144 @@ fused_adam_kernel(const AdamTensor* __restrict__ table, float lr, float b1, floa
   }
 }
 
+// LAMB (You et al., "Large Batch Optimization for Deep Learning"): the bias-corrected Adam direction plus decoupled weight
+// decay, u = (m / c1) / (sqrt(v / c2) + eps) + wd * w, applied as w -= lr * r * u with the per-tensor trust ratio
+// r = ||w|| / ||u|| (1 if either norm is 0, or if the caller does not adapt).  The norms cover whole tensors, which may be
+// split over several table entries (and ranks) sharing one `slot`, so the step is three launches: stage 1 updates the
+// moments and writes one (sum w^2, sum u^2) partial per CTA, the finalize kernel adds each entry's partials in fp64 in a
+// fixed order into norms[2 * slot], norms[2 * slot + 1], and stage 2 recomputes u from the stored moments and applies it.
+// Deterministic, no atomics, nothing left behind between launches.  Only stage 1 reads the gradient.
+__device__ __forceinline__ float lamb_u(float m, float v, float w, float c1, float c2, float eps, float wd) {
+  return fmaf(wd, w, (m / c1) / (sqrtf(v / c2) + eps));
+}
+
+template <typename P, typename G, bool kMaster>
+__global__ void __launch_bounds__(kOptThreads)
+fused_lamb_norms_kernel(const LambTensor* __restrict__ table, float b1, float b2, float eps, float wd, float c1, float c2,
+                        float grad_scale, const float* __restrict__ grad_scale_dev, float2* __restrict__ partial) {
+  __shared__ float2 red[kOptThreads / 32];
+  const LambTensor t = table[blockIdx.y];
+  const int64_t n = t.count;
+  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  if (base >= n) return;
+  grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
+  const P* p = reinterpret_cast<const P*>(t.param);
+  const G* g = reinterpret_cast<const G*>(t.grad);
+  float* m = reinterpret_cast<float*>(t.exp_avg);
+  float* v = reinterpret_cast<float*>(t.exp_avg_sq);
+  const float* w = kMaster ? reinterpret_cast<const float*>(t.master) : nullptr;
+  const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g),
+             sa = is_aligned<float>(m) && is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
+  float sw = 0.f, su = 0.f;
+#pragma unroll
+  for (int it = 0; it < kOptIters; ++it) {
+    const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
+    if (i >= n) break;
+    float pv[kOptVec], gv[kOptVec], mv[kOptVec], vv[kOptVec];
+    load4<P>(p, i, n, pa, pv);
+    load4<G>(g, i, n, ga, gv);
+    load4<float>(m, i, n, sa, mv);
+    load4<float>(v, i, n, sa, vv);
+    if constexpr (kMaster) {
+      float wv[kOptVec];
+      load4<float>(w, i, n, sa, wv);
+      reconcile4<P>(pv, wv);
+    }
+#pragma unroll
+    for (int k = 0; k < kOptVec; ++k) {
+      const float d = gv[k] * grad_scale;
+      mv[k] = fmaf(b1, mv[k], (1.f - b1) * d);
+      vv[k] = fmaf(b2, vv[k], (1.f - b2) * d * d);
+      if (i + k < n) {  // past the end u would be 0 / eps, NaN for eps = 0
+        const float u = lamb_u(mv[k], vv[k], pv[k], c1, c2, eps, wd);
+        sw = fmaf(pv[k], pv[k], sw);
+        su = fmaf(u, u, su);
+      }
+    }
+    store4<float>(m, i, n, sa, mv);
+    store4<float>(v, i, n, sa, vv);
+  }
+  // CTA partial: a fixed shuffle tree per warp, then the warps in order
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    sw += __shfl_xor_sync(0xffffffffu, sw, o);
+    su += __shfl_xor_sync(0xffffffffu, su, o);
+  }
+  if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = make_float2(sw, su);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float2 a = red[0];
+    for (int k = 1; k < kOptThreads / 32; ++k) { a.x += red[k].x; a.y += red[k].y; }
+    partial[t.partial + blockIdx.x] = a;
+  }
+}
+
+// One CTA per entry: its partials in fp64, a fixed strided subset per thread, then a fixed tree; added into its slot.
+// Every slot appears at most once per launch (checked by the host), so the read-modify-write does not race.
+__global__ void __launch_bounds__(kOptThreads)
+lamb_finalize_kernel(const LambTensor* __restrict__ table, const float2* __restrict__ partial, float* __restrict__ norms) {
+  __shared__ double rw[kOptThreads], ru[kOptThreads];
+  const LambTensor t = table[blockIdx.x];
+  const int64_t nb = (t.count + kOptPerBlock - 1) / kOptPerBlock;
+  double a = 0.0, b = 0.0;
+  for (int64_t j = threadIdx.x; j < nb; j += kOptThreads) {
+    const float2 x = partial[t.partial + j];
+    a += (double)x.x;
+    b += (double)x.y;
+  }
+  rw[threadIdx.x] = a;
+  ru[threadIdx.x] = b;
+  __syncthreads();
+#pragma unroll
+  for (int h = kOptThreads / 2; h > 0; h >>= 1) {
+    if (threadIdx.x < h) { rw[threadIdx.x] += rw[threadIdx.x + h]; ru[threadIdx.x] += ru[threadIdx.x + h]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    norms[2 * t.slot] = (float)((double)norms[2 * t.slot] + rw[0]);
+    norms[2 * t.slot + 1] = (float)((double)norms[2 * t.slot + 1] + ru[0]);
+  }
+}
+
+template <typename P, bool kMaster>
+__global__ void __launch_bounds__(kOptThreads)
+fused_lamb_apply_kernel(const LambTensor* __restrict__ table, float lr, float eps, float wd, float c1, float c2, int adapt,
+                        const float* __restrict__ norms) {
+  const LambTensor t = table[blockIdx.y];
+  const int64_t n = t.count;
+  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  if (base >= n) return;
+  float r = 1.f;
+  if (adapt) {
+    const float wn = sqrtf(norms[2 * t.slot]), un = sqrtf(norms[2 * t.slot + 1]);
+    if (wn > 0.f && un > 0.f) r = wn / un;
+  }
+  const float step = lr * r;
+  P* p = reinterpret_cast<P*>(t.param);
+  const float* m = reinterpret_cast<const float*>(t.exp_avg);
+  const float* v = reinterpret_cast<const float*>(t.exp_avg_sq);
+  float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
+  const bool pa = is_aligned<P>(p), sa = is_aligned<float>(m) && is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
+#pragma unroll
+  for (int it = 0; it < kOptIters; ++it) {
+    const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
+    if (i >= n) break;
+    float pv[kOptVec], mv[kOptVec], vv[kOptVec];
+    load4<P>(p, i, n, pa, pv);
+    load4<float>(m, i, n, sa, mv);
+    load4<float>(v, i, n, sa, vv);
+    if constexpr (kMaster) {
+      float wv[kOptVec];
+      load4<float>(w, i, n, sa, wv);
+      reconcile4<P>(pv, wv);  // the same value stage 1 started from: nothing wrote p or the master in between
+    }
+#pragma unroll
+    for (int k = 0; k < kOptVec; ++k) pv[k] = fmaf(-step, lamb_u(mv[k], vv[k], pv[k], c1, c2, eps, wd), pv[k]);
+    if constexpr (kMaster) store4<float>(w, i, n, sa, pv);
+    store4<P>(p, i, n, pa, pv);
+  }
+}
+
 // max that keeps a NaN once it has seen one (fmaxf drops it), so an inf-norm of NaN gradients is NaN as in torch
 __device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
 __device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
@@ -291,6 +429,54 @@ cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, 
   else if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
   else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
   else return cudaErrorInvalidValue;
+  CountKernelLaunch();
+  return cudaGetLastError();
+}
+
+int64_t LambPartials(int64_t count) { return (count + kOptPerBlock - 1) / kOptPerBlock; }
+
+cudaError_t LaunchLambNorms(const LambTensor* table, int n, int64_t max_count, float beta1, float beta2, float eps,
+                            float weight_decay, float bias_c1, float bias_c2, float grad_scale, const float* grad_scale_dev,
+                            float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream) {
+  if (n <= 0 || max_count <= 0) return cudaSuccess;
+  dim3 grid((unsigned)LambPartials(max_count), (unsigned)n);
+  float2* part = reinterpret_cast<float2*>(partial);
+#define HVD_LAMB_NORMS(P, G, M) fused_lamb_norms_kernel<P, G, M><<<grid, kOptThreads, 0, stream>>>(table, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, part)
+  if (master) {
+    if (param_dtype == 10 && grad_dtype == 10) HVD_LAMB_NORMS(__nv_bfloat16, __nv_bfloat16, true);
+    else if (param_dtype == 6 && grad_dtype == 6) HVD_LAMB_NORMS(__half, __half, true);
+    else return cudaErrorInvalidValue;
+  }
+  else if (param_dtype == 7 && grad_dtype == 7) HVD_LAMB_NORMS(float, float, false);
+  else if (param_dtype == 7 && grad_dtype == 10) HVD_LAMB_NORMS(float, __nv_bfloat16, false);
+  else if (param_dtype == 10 && grad_dtype == 10) HVD_LAMB_NORMS(__nv_bfloat16, __nv_bfloat16, false);
+  else if (param_dtype == 6 && grad_dtype == 6) HVD_LAMB_NORMS(__half, __half, false);
+  else return cudaErrorInvalidValue;
+#undef HVD_LAMB_NORMS
+  CountKernelLaunch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  lamb_finalize_kernel<<<(unsigned)n, kOptThreads, 0, stream>>>(table, part, norms);
+  CountKernelLaunch();
+  return cudaGetLastError();
+}
+
+cudaError_t LaunchLambApply(const LambTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
+                            float bias_c1, float bias_c2, int adapt, const float* norms, int param_dtype, bool master,
+                            cudaStream_t stream) {
+  if (n <= 0 || max_count <= 0) return cudaSuccess;
+  dim3 grid((unsigned)LambPartials(max_count), (unsigned)n);
+#define HVD_LAMB_APPLY(P, M) fused_lamb_apply_kernel<P, M><<<grid, kOptThreads, 0, stream>>>(table, lr, eps, weight_decay, bias_c1, bias_c2, adapt, norms)
+  if (master) {
+    if (param_dtype == 10) HVD_LAMB_APPLY(__nv_bfloat16, true);
+    else if (param_dtype == 6) HVD_LAMB_APPLY(__half, true);
+    else return cudaErrorInvalidValue;
+  }
+  else if (param_dtype == 7) HVD_LAMB_APPLY(float, false);
+  else if (param_dtype == 10) HVD_LAMB_APPLY(__nv_bfloat16, false);
+  else if (param_dtype == 6) HVD_LAMB_APPLY(__half, false);
+  else return cudaErrorInvalidValue;
+#undef HVD_LAMB_APPLY
   CountKernelLaunch();
   return cudaGetLastError();
 }

@@ -186,6 +186,22 @@ cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, 
                              float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale,
                              int adamw, int param_dtype, int grad_dtype, cudaStream_t stream,
                              const float* grad_scale_dev = nullptr, bool master = false);
+// Fused LAMB in two phases (see optim_kernels.cu), so that the norms can be allreduced in between.  Entry i covers
+// `count` elements of a parameter whose whole-tensor norms live in norms[2 * slot] (sum w^2) and norms[2 * slot + 1]
+// (sum u^2); its stage-1 CTA partials start at `partial`, the running sum of LambPartials(count) over the entries before
+// it.  No two entries of one launch may share a slot.
+// LaunchLambNorms: moments updated, then the entries' squared norms ADDED into `norms` (two launches; `partial` holds
+// 2 * sum LambPartials floats).  LaunchLambApply: w -= lr * r * u (one launch; the gradient is not read).  (param, grad)
+// dtypes as LaunchFusedAdamW, `master` likewise.
+struct LambTensor { void* param; const void* grad; void* exp_avg; void* exp_avg_sq; int64_t count; void* master;
+                    int64_t partial; int64_t slot; };
+int64_t LambPartials(int64_t count);
+cudaError_t LaunchLambNorms(const LambTensor* table, int n, int64_t max_count, float beta1, float beta2, float eps,
+                            float weight_decay, float bias_c1, float bias_c2, float grad_scale, const float* grad_scale_dev,
+                            float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
+cudaError_t LaunchLambApply(const LambTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
+                            float bias_c1, float bias_c2, int adapt, const float* norms, int param_dtype, bool master,
+                            cudaStream_t stream);
 // Gradient statistics of flat gradient shards in one pass (see optim_kernels.cu): optional in-place scaling by
 // *inv_scale, then out[0] += sum of squares (norm_inf: out[0] = max(out[0], max |g|)) and out[1] = max(out[1], non-finite).
 // `partial` / `partial_flag` hold GradShardStatsCtas() entries; `ticket` is a zeroed counter that the kernel leaves zeroed,

@@ -18,6 +18,7 @@
 #include <condition_variable>
 #include <map>
 #include <mutex>
+#include <set>
 #include <unordered_map>
 #include "../common/engine.h"
 #include "../kernels/p2p_kernels.h"
@@ -601,6 +602,144 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   TORCH_CHECK(e == cudaSuccess, "fused_adam launch failed: ", cudaGetErrorString(e));
 }
 
+// ---- fused LAMB (kern::LaunchLambNorms / LaunchLambApply) ----
+// Checks every argument of one LAMB phase and builds its table: entry i is params[i] with norm slot slots[i] (empty:
+// i) of `norms`, a contiguous fp32 tensor on the params' device with 2 floats per slot.  Zero-size params get no entry.
+struct LambPlan {
+  std::vector<kern::LambTensor> table;
+  int64_t max_count = 0, partials = 0;
+  bool master = false;
+  float c1 = 1.f, c2 = 1.f;
+};
+
+LambPlan PlanLamb(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
+                  const std::vector<at::Tensor>& exp_avg, const std::vector<at::Tensor>& exp_avg_sq,
+                  const std::vector<at::Tensor>& masters, const at::Tensor& norms, const std::vector<int64_t>& slots,
+                  double beta1, double beta2, int64_t step, bool bias_correction) {
+  TORCH_CHECK(params.size() == grads.size() && params.size() == exp_avg.size() && params.size() == exp_avg_sq.size(), op,
+              ": list sizes differ");
+  TORCH_CHECK(masters.empty() || masters.size() == params.size(), op, ": ", masters.size(), " master params for ",
+              params.size(), " params");
+  TORCH_CHECK(slots.empty() || slots.size() == params.size(), op, ": ", slots.size(), " slots for ", params.size(), " params");
+  TORCH_CHECK(step >= 1, op, ": step must be >= 1, got ", step);
+  LambPlan plan;
+  if (params.empty()) return plan;
+  for (size_t i = 0; i < params.size(); ++i) {
+    CheckOptimizerParam(op, i, params[i], params[0]);
+    CheckOptimizerPeer(op, "grads", i, params[i], grads[i], grads[0].scalar_type());
+    CheckOptimizerPeer(op, "exp_avgs", i, params[i], exp_avg[i], at::kFloat);
+    CheckOptimizerPeer(op, "exp_avg_sqs", i, params[i], exp_avg_sq[i], at::kFloat);
+  }
+  plan.master = CheckMasters(op, params, grads, masters);
+  TORCH_CHECK(norms.is_cuda() && norms.device() == params[0].device() && norms.scalar_type() == at::kFloat &&
+              norms.is_contiguous(), op, ": norms must be a contiguous float32 tensor on ", params[0].device());
+  const int64_t nslots = norms.numel() / 2;
+  std::set<int64_t> seen;
+  for (size_t i = 0; i < params.size(); ++i) {
+    const int64_t s = slots.empty() ? (int64_t)i : slots[i];
+    TORCH_CHECK(s >= 0 && s < nslots, op, ": slot ", s, " of params[", i, "] is out of range for norms with room for ",
+                nslots, " slots");
+    TORCH_CHECK(seen.insert(s).second, op, ": slot ", s, " appears twice in one call");
+  }
+  for (size_t i = 0; i < params.size(); ++i) {
+    if (params[i].numel() == 0) continue;
+    kern::LambTensor t;
+    t.param = params[i].data_ptr(); t.grad = grads[i].data_ptr();
+    t.exp_avg = exp_avg[i].data_ptr(); t.exp_avg_sq = exp_avg_sq[i].data_ptr();
+    t.count = params[i].numel();
+    t.master = plan.master ? masters[i].data_ptr() : nullptr;
+    t.partial = plan.partials;
+    t.slot = slots.empty() ? (int64_t)i : slots[i];
+    plan.partials += kern::LambPartials(t.count);
+    plan.max_count = std::max(plan.max_count, t.count);
+    plan.table.push_back(t);
+  }
+  if (bias_correction) {
+    plan.c1 = 1.0f - (float)std::pow(beta1, (double)step);
+    plan.c2 = 1.0f - (float)std::pow(beta2, (double)step);
+  }
+  return plan;
+}
+
+const kern::LambTensor* StageLamb(const char* op, const LambPlan& plan, int device, cudaStream_t s) {
+  const auto* dt = (const kern::LambTensor*)GpuContext::Get().Stage(device, plan.table.data(),
+                                                                     plan.table.size() * sizeof(kern::LambTensor), s);
+  TORCH_CHECK(dt != nullptr, op, ": table too large");
+  return dt;
+}
+
+void LaunchLambNormsPhase(const char* op, const LambPlan& plan, const kern::LambTensor* dt, const at::Tensor& param0,
+                          const at::Tensor& grad0, double beta1, double beta2, double eps, double weight_decay,
+                          double grad_scale, const float* gsd, at::Tensor& norms, cudaStream_t s) {
+  // stream-ordered scratch from torch's caching allocator: one (sum w^2, sum u^2) pair per stage-1 CTA
+  at::Tensor work = at::empty({2 * plan.partials}, norms.options());
+  cudaError_t e = kern::LaunchLambNorms(dt, (int)plan.table.size(), plan.max_count, (float)beta1, (float)beta2, (float)eps,
+                                        (float)weight_decay, plan.c1, plan.c2, (float)grad_scale, gsd, work.data_ptr<float>(),
+                                        norms.data_ptr<float>(), (int)MapDtype(param0.scalar_type()),
+                                        (int)MapDtype(grad0.scalar_type()), plan.master, s);
+  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+}
+
+void LaunchLambApplyPhase(const char* op, const LambPlan& plan, const kern::LambTensor* dt, const at::Tensor& param0,
+                          double lr, double eps, double weight_decay, bool adapt, const at::Tensor& norms, cudaStream_t s) {
+  cudaError_t e = kern::LaunchLambApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)eps, (float)weight_decay,
+                                        plan.c1, plan.c2, adapt ? 1 : 0, norms.data_ptr<float>(),
+                                        (int)MapDtype(param0.scalar_type()), plan.master, s);
+  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+}
+
+// Phase 1: moments, then the squared norms of every entry ADDED into norms[2 * slot], norms[2 * slot + 1].
+void LambNorms(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
+               std::vector<at::Tensor> exp_avg_sq, double beta1, double beta2, double eps, double weight_decay, int64_t step,
+               bool bias_correction, double grad_scale, c10::optional<at::Tensor> grad_scale_dev,
+               std::vector<at::Tensor> masters, at::Tensor out, std::vector<int64_t> slots) {
+  LambPlan plan = PlanLamb("lamb_norms", params, grads, exp_avg, exp_avg_sq, masters, out, slots, beta1, beta2, step,
+                           bias_correction);
+  if (params.empty()) return;
+  const float* gsd = DeviceScalar("lamb_norms", "grad_scale_dev", grad_scale_dev, params[0]);
+  if (plan.table.empty()) return;
+  int device = (int)params[0].get_device();
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
+  const auto* dt = StageLamb("lamb_norms", plan, device, s);
+  LaunchLambNormsPhase("lamb_norms", plan, dt, params[0], grads[0], beta1, beta2, eps, weight_decay, grad_scale, gsd, out, s);
+}
+
+// Phase 2: w -= lr * r * u with r from the (allreduced) norms.  `grads` are checked like phase 1's, not read.
+void LambApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
+               std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
+               int64_t step, bool bias_correction, bool adapt, std::vector<at::Tensor> masters, at::Tensor norms,
+               std::vector<int64_t> slots) {
+  LambPlan plan = PlanLamb("lamb_apply", params, grads, exp_avg, exp_avg_sq, masters, norms, slots, beta1, beta2, step,
+                           bias_correction);
+  if (plan.table.empty()) return;
+  int device = (int)params[0].get_device();
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
+  const auto* dt = StageLamb("lamb_apply", plan, device, s);
+  LaunchLambApplyPhase("lamb_apply", plan, dt, params[0], lr, eps, weight_decay, adapt, norms, s);
+}
+
+// Both phases on one device with a fresh norms buffer (slot i = params[i]): three launches, one staged table.
+void FusedLambStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
+                   std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
+                   int64_t step, bool bias_correction, bool adapt, double grad_scale,
+                   c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
+  TORCH_CHECK(params.empty() || params[0].is_cuda(), "fused_lamb: params[0] must be a dense CUDA tensor");
+  at::Tensor norms = params.empty() ? at::Tensor() : at::zeros({2 * (int64_t)params.size()}, params[0].options().dtype(at::kFloat));
+  LambPlan plan = PlanLamb("fused_lamb", params, grads, exp_avg, exp_avg_sq, masters, norms, {}, beta1, beta2, step,
+                           bias_correction);
+  if (params.empty()) return;
+  const float* gsd = DeviceScalar("fused_lamb", "grad_scale_dev", grad_scale_dev, params[0]);
+  if (plan.table.empty()) return;
+  int device = (int)params[0].get_device();
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
+  const auto* dt = StageLamb("fused_lamb", plan, device, s);
+  LaunchLambNormsPhase("fused_lamb", plan, dt, params[0], grads[0], beta1, beta2, eps, weight_decay, grad_scale, gsd, norms, s);
+  LaunchLambApplyPhase("fused_lamb", plan, dt, params[0], lr, eps, weight_decay, adapt, norms, s);
+}
+
 // The stats kernel's last-CTA ticket: one zeroed counter per (device, stream), which every launch leaves zeroed again.
 // Launches on one stream run one after the other, so they can share it; launches on different streams may overlap and
 // must not.  Kept for the life of the process (4 bytes per stream that ever ran the kernel).
@@ -687,6 +826,17 @@ PYBIND11_MODULE(_hvd_torch, m) {
         py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
         py::arg("grad_scale"), py::arg("adamw"), py::arg("grad_scale_dev") = py::none(),
         py::arg("master_params") = std::vector<at::Tensor>());
+  m.def("fused_lamb_step", &FusedLambStep, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+        py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
+        py::arg("bias_correction"), py::arg("adapt"), py::arg("grad_scale"), py::arg("grad_scale_dev") = py::none(),
+        py::arg("master_params") = std::vector<at::Tensor>());
+  m.def("lamb_norms", &LambNorms, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+        py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
+        py::arg("bias_correction"), py::arg("grad_scale"), py::arg("grad_scale_dev"), py::arg("master_params"),
+        py::arg("out"), py::arg("slots"));
+  m.def("lamb_apply", &LambApply, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+        py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
+        py::arg("bias_correction"), py::arg("adapt"), py::arg("master_params"), py::arg("norms"), py::arg("slots"));
   m.def("grad_shard_stats", &GradShardStats, py::arg("grads"), py::arg("out"), py::arg("inv_scale") = py::none(),
         py::arg("norm_inf") = false);
 }

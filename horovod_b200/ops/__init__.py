@@ -1,6 +1,8 @@
 """Python access to the native sm_90a operations that are not collectives of the `hvd.*` API:
 
 * `fused_sgd_step`, `fused_adam_step` — multi-tensor optimizer kernels (`csrc/kernels/optim_kernels.cu`);
+* `fused_lamb_step`, and its two phases `lamb_norms` / `lamb_apply` — multi-tensor LAMB with per-tensor trust ratios
+  (same file);
 * `grad_shard_stats` — one-pass gradient norm statistics, non-finite check and optional in-place unscale (same file);
 * `symm_empty`, `symm_available` — registered symmetric memory for the zero-copy allreduce path;
 * `sim` — the single-GPU simulation harness (N ranks = N concurrently running kernels on one device) used by the
@@ -39,6 +41,46 @@ def fused_adam_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1=0.9, beta2=0
     return _native().fused_adam_step(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1), float(beta2),
                                      float(eps), float(weight_decay), int(step), float(grad_scale), bool(adamw), grad_scale_dev,
                                      list(master_params or []))
+
+
+def fused_lamb_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1, beta2, eps, weight_decay, step, bias_correction=True,
+                    adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None):
+    """One LAMB step for the whole parameter list in three launches (moments and per-CTA norm partials, the per-tensor
+    norms, the update), with the argument rules of fused_adam_step. For each parameter w (1-based `step`):
+
+        g = grad * grad_scale [* grad_scale_dev[0]];  m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g^2
+        u = (m / c1) / (sqrt(v / c2) + eps) + weight_decay * w      (c1 = 1 - b1^step, c2 = 1 - b2^step; 1 without bias_correction)
+        w -= lr * r * u,   r = ||w|| / ||u|| if adapt and both norms are > 0, else 1
+
+    Deterministic: the same input gives the same bits on every call. Nothing is synchronised with the host."""
+    return _native().fused_lamb_step(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1),
+                                     float(beta2), float(eps), float(weight_decay), int(step), bool(bias_correction),
+                                     bool(adapt), float(grad_scale), grad_scale_dev, list(master_params or []))
+
+
+def lamb_norms(params, grads, exp_avgs, exp_avg_sqs, beta1, beta2, eps, weight_decay, step, out, slots=None,
+               bias_correction=True, grad_scale=1.0, grad_scale_dev=None, master_params=None):
+    """First phase of fused_lamb_step, for parameters split into pieces (e.g. over the ranks' shards): updates the
+    moments and ADDS each piece's sum of w^2 and of u^2 into out[2 * slot] and out[2 * slot + 1]. `out` is a contiguous
+    float32 tensor on the parameters' device that the caller zeroes; `slots` (default 0, 1, ...) gives each piece the
+    slot of the tensor it belongs to, so that pieces of one tensor add up, at most once per call. Two launches."""
+    n = len(params)
+    return _native().lamb_norms(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(beta1), float(beta2),
+                                float(eps), float(weight_decay), int(step), bool(bias_correction), float(grad_scale),
+                                grad_scale_dev, list(master_params or []), out,
+                                list(range(n)) if slots is None else [int(s) for s in slots])
+
+
+def lamb_apply(params, grads, exp_avgs, exp_avg_sqs, lr, beta1, beta2, eps, weight_decay, step, norms, slots=None,
+               bias_correction=True, adapt=True, master_params=None):
+    """Second phase: w -= lr * r * u, with u recomputed from the moments of lamb_norms and r from the whole-tensor sums of
+    squares in `norms` (e.g. after adding up every rank's pieces). `grads` are checked as in lamb_norms but not read.
+    One launch."""
+    n = len(params)
+    return _native().lamb_apply(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1),
+                                float(beta2), float(eps), float(weight_decay), int(step), bool(bias_correction),
+                                bool(adapt), list(master_params or []), norms,
+                                list(range(n)) if slots is None else [int(s) for s in slots])
 
 
 def grad_shard_stats(tensors, out, inv_scale=None, norm_type=2.0):

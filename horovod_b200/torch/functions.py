@@ -95,7 +95,7 @@ def broadcast_optimizer_state(optimizer, root_rank, model=None, process_set=glob
                     created.append(p)
         # a zero-grad step must not move the weights: snapshot and restore
         saved = [[p.data.clone() for p in g['params']] for g in optimizer.param_groups]
-        if optimizer.__class__.__module__.startswith('horovod_b200') or hasattr(optimizer, '_hvd_super_step'):
+        if hasattr(optimizer, '_hvd_super_step'):  # a DistributedOptimizer: the wrapped optimizer's own step
             optimizer._hvd_super_step()
         else:
             optimizer.step()

@@ -11,6 +11,10 @@ optimizer state for that shard only.  A step is
 which moves the same NVLink bytes as the allreduce it replaces, while the update does 1/N of the work and the state
 takes 1/N of the memory.  The allgather runs after the update and does not overlap backward.
 
+LAMB (hvd.Lamb) needs the norms of whole parameters, which the shards cut at arbitrary elements: its update is split
+into lamb_norms over the owned pieces, one allreduce of a small registered buffer of per-parameter sums of squares,
+and lamb_apply, so every rank computes each trust ratio from the same bits.
+
 Global-norm clipping (`clip_grad_norm_`) and AMP loss scaling (`ShardedGradScaler`) read only the owned shards: one
 statistics kernel per gradient dtype and one scalar allreduce give every rank the same norm and the same inf / NaN
 verdict, and the clip coefficient reaches the update on the device.
@@ -28,6 +32,7 @@ import torch
 from horovod_b200.common.process_sets import global_process_set
 from horovod_b200.torch import mpi_ops
 from horovod_b200.torch.compression import Compression
+from horovod_b200.torch.lamb import Lamb
 from horovod_b200.torch.mpi_ops import Average, Sum
 from horovod_b200.torch.optimizer import _find_duplicates
 
@@ -127,7 +132,7 @@ def full_from_shards(bucket, shards, shapes, strides=None):
 
 
 class _ShardedDistributedOptimizer(torch.optim.Optimizer):
-    """Wraps SGD / Adam / AdamW so that every rank keeps optimizer state for 1/N of the parameters (ZeRO stage 1).
+    """Wraps SGD / Adam / AdamW / Lamb so that every rank keeps optimizer state for 1/N of the parameters (ZeRO stage 1).
     Built by `hvd.DistributedOptimizer(opt, shard_optimizer_state=True)`; the dynamic class derives from this one and from
     the wrapped optimizer's class."""
 
@@ -135,12 +140,17 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
                  bucket_cap_mb=32, master_weights=False):
         super().__init__(params)
-        is_sgd = isinstance(self, torch.optim.SGD)
-        is_adam = isinstance(self, (torch.optim.Adam, torch.optim.AdamW))
-        if not (is_sgd or is_adam):
-            raise ValueError('shard_optimizer_state supports SGD, Adam and AdamW only, not %s' % type(self).__name__)
+        if isinstance(self, torch.optim.SGD):
+            kind = 'sgd'
+        elif isinstance(self, (torch.optim.Adam, torch.optim.AdamW)):
+            kind = 'adam'
+        elif isinstance(self, Lamb):
+            kind = 'lamb'
+        else:
+            raise ValueError('shard_optimizer_state supports SGD, Adam and AdamW, and hvd.Lamb, only, not %s'
+                             % type(self).__name__)
         for g in self.param_groups:
-            if g.get('maximize', False) or (is_adam and g.get('amsgrad', False)):
+            if g.get('maximize', False) or (kind == 'adam' and g.get('amsgrad', False)):
                 raise ValueError('shard_optimizer_state does not support maximize=True or amsgrad=True')
         if op not in (Average, Sum):
             raise ValueError('shard_optimizer_state supports op=Average or op=Sum only')
@@ -164,7 +174,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         if not (process_set.included() and mpi_ops.symm_available(process_set) and mpi_ops.cross_size() == 1):
             raise ValueError('shard_optimizer_state needs registered symmetric memory (P2P backend, one host, not elastic)')
 
-        self._is_sgd = is_sgd
+        self._kind = kind
         self.process_set = process_set
         self.op = op
         self.gradient_predivide_factor = gradient_predivide_factor
@@ -208,7 +218,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 lo, hi = shard_range(b, self._rank)
                 b['pshard'], b['gshard'] = pflat[lo:hi], gflat[lo:hi]
                 master = master_weights and b['dtype'] != torch.float32
-                if is_sgd:
+                if kind == 'sgd':
                     # the fused SGD kernel keeps momentum in the parameter dtype, or in fp32 with master weights
                     b['state'] = {'momentum_buffer': torch.zeros(b['shard'], dtype=torch.float32 if master else b['dtype'],
                                                                  device=device)} \
@@ -225,6 +235,14 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._stats = mpi_ops.symm_empty(ALIGN // 4 * self._nranks, dtype=torch.float32, device=device,
                                          process_set=process_set)
         self._stats.zero_()
+        self._lamb_norms = None
+        if kind == 'lamb':
+            # LAMB's whole-parameter (sum w^2, sum u^2) in slot = the parameter's index in param_groups order: every rank
+            # adds the pieces of its own shards and one allreduce sums them.  Padded like _stats.
+            self._slot = {p: i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
+            unit = ALIGN // 4 * self._nranks
+            self._lamb_norms = mpi_ops.symm_empty((2 * len(self._slot) + unit - 1) // unit * unit, dtype=torch.float32,
+                                                  device=device, process_set=process_set)
         self._delay = {p: backward_passes_per_step for p in self._p_to_bucket}
         self._seen = set()  # parameters whose gradient hook fired since the last synchronize()
         self._reset_launch_order()
@@ -400,12 +418,15 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         for b in self._buckets:
             by_group.setdefault((b['group'], b['dtype']), []).append(b)
         with torch.no_grad():
+            if self._kind == 'lamb':
+                self._update_shards_lamb(by_group, coef)
+                return
             for (gi, _), bs in by_group.items():
                 group = self.param_groups[gi]
                 ps, gs = [b['pshard'] for b in bs], [b['gshard'] for b in bs]
                 # every bucket of a (group, dtype) has a master or none has
                 kw = {'master_params': [b['state']['master_param'] for b in bs]} if 'master_param' in bs[0]['state'] else {}
-                if self._is_sgd:
+                if self._kind == 'sgd':
                     mom = group.get('momentum', 0.0)
                     bufs = [b['state']['momentum_buffer'] for b in bs] if mom != 0.0 else []
                     first = mom != 0.0 and not bs[0]['mom_init']
@@ -424,6 +445,40 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                                            float(group.get('weight_decay', 0.0)), bs[0]['step'], 1.0, adamw, coef, **kw)
                 for b in bs:
                     b['stepped'] = True
+
+    def _update_shards_lamb(self, by_group, coef):
+        """LAMB's trust ratio needs the norms of whole parameters, which the shards cut at arbitrary elements.  One table
+        entry per parameter piece in this rank's shards, in the slot of its parameter: lamb_norms per (group, dtype)
+        adds the pieces' sums of squares into the registered norms buffer, one allreduce sums them over the ranks, and
+        lamb_apply per (group, dtype) updates the pieces with the same r on every rank.  Padding is not touched."""
+        native = mpi_ops._native()
+        calls = []
+        for (gi, _), bs in by_group.items():
+            group = self.param_groups[gi]
+            lists, masters, slots = ([], [], [], []), [], []
+            for b in bs:
+                st = b['state']
+                b['step'] += 1
+                b['stepped'] = True
+                for k, plo, phi, slo in shard_slices(b, self._rank):
+                    cut = slice(slo, slo + phi - plo)
+                    for out, t in zip(lists, (b['pshard'], b['gshard'], st['exp_avg'], st['exp_avg_sq'])):
+                        out.append(t[cut])
+                    if 'master_param' in st:
+                        masters.append(st['master_param'][cut])
+                    slots.append(self._slot[b['params'][k]])
+            calls.append((group, bs[0]['step'], lists, masters, slots))
+        self._lamb_norms.zero_()
+        for group, step, lists, masters, slots in calls:
+            b1, b2 = group['betas']
+            native.lamb_norms(*lists, float(b1), float(b2), float(group['eps']), float(group['weight_decay']), step,
+                              bool(group['bias_correction']), 1.0, coef, masters, self._lamb_norms, slots)
+        mpi_ops.captured_allreduce_(self._lamb_norms, op=Sum, process_set=self.process_set)
+        for group, step, lists, masters, slots in calls:
+            b1, b2 = group['betas']
+            native.lamb_apply(*lists, float(group['lr']), float(b1), float(b2), float(group['eps']),
+                              float(group['weight_decay']), step, bool(group['bias_correction']), Lamb.adapts(group),
+                              masters, self._lamb_norms, slots)
 
     def _allgather_params(self):
         comm = self._comm
@@ -498,7 +553,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         index = {id(p): i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
         state = {}
         for b in self._buckets:
-            if not b['state'] or ((b['step'] == 0) if not self._is_sgd else
+            if not b['state'] or ((b['step'] == 0) if self._kind != 'sgd' else
                                   not (b['mom_init'] or ('master_param' in b['state'] and b['stepped']))):
                 continue  # no state yet (the same on every rank); a plain-SGD bucket may still hold masters
             gathered = {}
@@ -507,7 +562,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 gathered[key] = full_from_shards(b, [full], [p.shape for p in b['params']], [p.stride() for p in b['params']])
             for k, p in enumerate(b['params']):
                 st = {key: vals[k].detach().cpu().clone() for key, vals in gathered.items()}
-                if not self._is_sgd:
+                if self._kind != 'sgd':
                     st['step'] = torch.tensor(float(b['step']))
                 state[index[id(p)]] = st
         sd['state'] = state
