@@ -40,6 +40,15 @@ Sim* GetSim(int nranks, int device, size_t buffer_bytes) {
 }
 int64_t Align128(int64_t b) { return (b + 127) / 128 * 128; }
 
+// Every simulated rank's parameters for the next collective, taken before any launch: NextSlot() flips a rank's
+// ping-pong buffer, so a launch that is rejected (bad arguments are rejected on every rank alike) must not leave the
+// ranks on different buffers, where every later collective of this rank count would read stale peer data.
+std::vector<kern::CommParams> NextParams(Sim* sim) {
+  std::vector<kern::CommParams> cps;
+  for (auto& t : sim->teams) cps.push_back(t->Params(t->NextSlot()));
+  return cps;
+}
+
 // After the device drained: a barrier that timed out (scheduling deadlock of the simulation) is an error, and the team is
 // thrown away so that the next call starts from clean flags / epochs.
 int Finish(int nranks, cudaError_t sync_result) {
@@ -87,6 +96,7 @@ int hvd_sim_allreduce(int nranks, int device, int ntensors, const int64_t* count
   cudaDeviceSynchronize();
   cudaEventRecord(e0, sim->streams[0]);
   for (int it = 0; it < repeats; ++it) {
+    const std::vector<kern::CommParams> cps = NextParams(sim);
     for (int r = 0; r < nranks; ++r) {
       kern::AllreduceArgs a {};
       a.descs = dtabs[r]; a.ndesc = ntensors; a.total_bytes = total; a.reduce_lo = 0; a.reduce_hi = total;
@@ -103,8 +113,7 @@ int hvd_sim_allreduce(int nranks, int device, int ntensors, const int64_t* count
         a.pipe_use_nvls = 0;
         a.pipe_rblock_bytes = 8192;
       }
-      kern::CommParams cp = sim->teams[r]->Params(sim->teams[r]->NextSlot());
-      cudaError_t e = kern::LaunchAllreduce(cp, a, sim->streams[r]);
+      cudaError_t e = kern::LaunchAllreduce(cps[r], a, sim->streams[r]);
       if (e != cudaSuccess) return (int)e;
     }
   }
@@ -120,6 +129,7 @@ int hvd_sim_allgather(int nranks, int device, int64_t bytes, const uint64_t* in_
   if (cudaSetDevice(device) != cudaSuccess) return -1;
   Sim* sim = GetSim(nranks, device, (size_t)std::max<int64_t>(bytes, 1 << 20));
   if (!sim) return -1;
+  const std::vector<kern::CommParams> cps = NextParams(sim);
   for (int r = 0; r < nranks; ++r) {
     std::vector<kern::CopyDesc> t;
     t.push_back({(const void*)in_ptrs[r], nullptr, 0, bytes, r, 0});
@@ -131,8 +141,7 @@ int hvd_sim_allgather(int nranks, int device, int64_t bytes, const uint64_t* in_
     if (!dt) return -2;
     kern::ExchangeArgs a {};
     a.sends = dt; a.nsend = 1; a.recvs = dt + 1; a.nrecv = nranks; a.ctas = ctas;
-    kern::CommParams cp = sim->teams[r]->Params(sim->teams[r]->NextSlot());
-    cudaError_t e = kern::LaunchExchange(cp, a, sim->streams[r]);
+    cudaError_t e = kern::LaunchExchange(cps[r], a, sim->streams[r]);
     if (e != cudaSuccess) return (int)e;
   }
   return Finish(nranks, cudaDeviceSynchronize());
@@ -150,7 +159,7 @@ int hvd_sim_adasum(int nranks, int device, int ntensors, const int64_t* counts, 
   // Step-major launch order (step k of EVERY rank before step k+1 of any rank): the streams of the simulated ranks may
   // share a hardware queue, and a rank-major order would park rank 1's kernels behind rank 0's spinning ones.
   std::vector<const kern::TensorDesc*> dtabs(nranks);
-  std::vector<kern::CommParams> cps(nranks);
+  const std::vector<kern::CommParams> cps = NextParams(sim);
   for (int r = 0; r < nranks; ++r) {
     std::vector<kern::TensorDesc> d(ntensors);
     for (int i = 0; i < ntensors; ++i) {
@@ -161,7 +170,6 @@ int hvd_sim_adasum(int nranks, int device, int ntensors, const int64_t* counts, 
     }
     dtabs[r] = (const kern::TensorDesc*)GpuContext::Get().Stage(device, d.data(), d.size() * sizeof(kern::TensorDesc), sim->streams[r]);
     if (!dtabs[r]) return -2;
-    cps[r] = sim->teams[r]->Params(sim->teams[r]->NextSlot());
   }
   // HVD_ADASUM_PERSISTENT (default 1): the single-launch kernel; every simulated rank gets its own scratch + grid-sync block
   const char* pe = getenv("HVD_ADASUM_PERSISTENT");
@@ -202,12 +210,12 @@ int hvd_sim_inplace(int nranks, int device, int64_t bytes, const uint64_t* ptrs,
   cudaDeviceSynchronize();
   cudaEventRecord(e0, sim->streams[0]);
   for (int it = 0; it < repeats; ++it) {
+    const std::vector<kern::CommParams> cps = NextParams(sim);
     for (int r = 0; r < nranks; ++r) {
       kern::InplaceArgs a {};
       for (int p = 0; p < nranks; ++p) a.ptr[p] = (void*)ptrs[p];
       a.mc = nullptr; a.bytes = bytes; a.scale = scale; a.op = op; a.dtype = dtype; a.use_multicast = 0; a.ctas = ctas;
-      kern::CommParams cp = sim->teams[r]->Params(sim->teams[r]->NextSlot());
-      cudaError_t e = kern::LaunchInplaceAllreduce(cp, a, sim->streams[r]);
+      cudaError_t e = kern::LaunchInplaceAllreduce(cps[r], a, sim->streams[r]);
       if (e != cudaSuccess) return (int)e;
     }
   }
@@ -228,13 +236,13 @@ static int hvd_sim_inplace_sharded(int nranks, int device, int64_t bytes, const 
   if (!sim) return -1;
   cudaDeviceSynchronize();
   for (int it = 0; it < repeats; ++it) {
+    const std::vector<kern::CommParams> cps = NextParams(sim);
     for (int r = 0; r < nranks; ++r) {
       kern::InplaceArgs a {};
       for (int p = 0; p < nranks; ++p) a.ptr[p] = (void*)ptrs[p];
       a.mc = nullptr; a.bytes = bytes; a.scale = scale; a.op = op; a.dtype = dtype; a.use_multicast = 0; a.ctas = ctas;
-      kern::CommParams cp = sim->teams[r]->Params(sim->teams[r]->NextSlot());
-      cudaError_t e = reducescatter ? kern::LaunchInplaceReducescatter(cp, a, sim->streams[r])
-                                    : kern::LaunchInplaceAllgather(cp, a, sim->streams[r]);
+      cudaError_t e = reducescatter ? kern::LaunchInplaceReducescatter(cps[r], a, sim->streams[r])
+                                    : kern::LaunchInplaceAllgather(cps[r], a, sim->streams[r]);
       if (e != cudaSuccess) return (int)e;
     }
   }

@@ -162,15 +162,42 @@ __device__ __forceinline__ void unpack_range(const TensorDesc* descs, int nd, in
   }
 }
 
-// Issues the loads of the vector at byte offset `o` from all peers.
-template <int NR> __device__ __forceinline__ void peer_loads(const CommParams& cp, int64_t o, uint4* v) {
+// Issues the loads of one trip, the U rows at byte offsets o0 + j * kRowBytes below `hi`, from all N peers (base[p] + o)
+// into v[j][p].  Every rank starts at its own buffer and rotates, so that at any instant the N ranks pull from N
+// different peers; v[j][] is indexed by peer, so that peer_combine adds in rank order.  One uniform dispatch on (nranks,
+// rank) per trip makes every index a compile-time constant (v[] stays in registers).  A kernel instantiated for NR peers
+// runs nranks in (NR/2, NR], and 1 .. 2 for NR = 2.
+template <int NR, int U, int N, int R>
+__device__ __forceinline__ void peer_loads_from(void* const* base, int64_t o0, int64_t hi, uint4 (*v)[NR]) {
 #pragma unroll
-  for (int k = 0; k < NR; ++k) {
-    // start at my own buffer and rotate so that at any instant the N ranks pull from N different peers
-    int p = cp.rank + k; if (p >= cp.nranks) p -= cp.nranks;
-    if (k < cp.nranks) v[k] = ld_stream(reinterpret_cast<const char*>(cp.buf[p]) + o);
+  for (int j = 0; j < U; ++j) {
+    const int64_t o = o0 + (int64_t)j * kRowBytes;
+    if (j == 0 || o < hi) {  // (callers loop while o0 < hi)
+#pragma unroll
+      for (int k = 0; k < N; ++k) {
+        const int p = (R + k) % N;
+        v[j][p] = ld_stream(reinterpret_cast<const char*>(base[p]) + o);
+      }
+    }
   }
 }
+template <int NR, int U, int N, int R = 0>
+__device__ __forceinline__ void peer_loads_rank(int rank, void* const* base, int64_t o0, int64_t hi, uint4 (*v)[NR]) {
+  if constexpr (R + 1 < N) {
+    if (rank != R) { peer_loads_rank<NR, U, N, R + 1>(rank, base, o0, hi, v); return; }
+  }
+  peer_loads_from<NR, U, N, R>(base, o0, hi, v);
+}
+template <int NR, int U, int N = NR>
+__device__ __forceinline__ void peer_loads(const CommParams& cp, void* const* base, int64_t o0, int64_t hi, uint4 (*v)[NR]) {
+  if constexpr (N > (NR == 2 ? 1 : NR / 2 + 1)) {
+    if (cp.nranks != N) { peer_loads<NR, U, N - 1>(cp, base, o0, hi, v); return; }
+  }
+  peer_loads_rank<NR, U, N>(cp.rank, base, o0, hi, v);
+}
+// Combines the N contributions in rank order 0 .. N-1 (v[p] = peer p): floating-point sums and products are not
+// associative and MIN / MAX keep the first of two NaN-unordered operands, so only one fixed order gives every rank, and
+// every variant, the same bits.
 template <typename W, int NR>
 __device__ __forceinline__ void peer_combine(const CommParams& cp, const uint4* v, int op, typename Traits<W>::Acc* acc) {
   using A = typename Traits<W>::Acc;
@@ -255,11 +282,7 @@ allreduce_kernel(const __grid_constant__ CommParams cp, const __grid_constant__ 
       }
       for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)U * kRowBytes) {
         uint4 v[U][NR];
-#pragma unroll
-        for (int j = 0; j < U; ++j) {
-          const int64_t o = o0 + (int64_t)j * kRowBytes;
-          if (o < hi) peer_loads<NR>(cp, o, v[j]);
-        }
+        peer_loads<NR, U>(cp, cp.buf, o0, hi, v);
 #pragma unroll
         for (int j = 0; j < U; ++j) {
           const int64_t o = o0 + (int64_t)j * kRowBytes;
@@ -313,11 +336,7 @@ allreduce_kernel(const __grid_constant__ CommParams cp, const __grid_constant__ 
       } else {
         for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)U * kRowBytes) {
           uint4 v[U][NR];
-#pragma unroll
-          for (int j = 0; j < U; ++j) {
-            const int64_t o = o0 + (int64_t)j * kRowBytes;
-            if (o < hi) peer_loads<NR>(cp, o, v[j]);
-          }
+          peer_loads<NR, U>(cp, cp.buf, o0, hi, v);
 #pragma unroll
           for (int j = 0; j < U; ++j) {
             const int64_t o = o0 + (int64_t)j * kRowBytes;
@@ -413,17 +432,7 @@ inplace_allreduce_kernel(const __grid_constant__ CommParams cp, const __grid_con
     } else {
       for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)U * kRowBytes) {
         uint4 v[U][NR];
-#pragma unroll
-        for (int j = 0; j < U; ++j) {
-          const int64_t o = o0 + (int64_t)j * kRowBytes;
-          if (o < hi) {
-#pragma unroll
-            for (int p = 0; p < NR; ++p) {
-              int q = cp.rank + p; if (q >= cp.nranks) q -= cp.nranks;
-              if (p < cp.nranks) v[j][p] = ld_stream(reinterpret_cast<const char*>(a.ptr[q]) + o);
-            }
-          }
-        }
+        peer_loads<NR, U>(cp, a.ptr, o0, hi, v);
 #pragma unroll
         for (int j = 0; j < U; ++j) {
           const int64_t o = o0 + (int64_t)j * kRowBytes;
@@ -513,17 +522,7 @@ inplace_reducescatter_kernel(const __grid_constant__ CommParams cp, const __grid
     } else {
       for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)U * kRowBytes) {
         uint4 v[U][NR];
-#pragma unroll
-        for (int j = 0; j < U; ++j) {
-          const int64_t o = o0 + (int64_t)j * kRowBytes;
-          if (o < hi) {
-#pragma unroll
-            for (int p = 0; p < NR; ++p) {
-              int q = cp.rank + p; if (q >= cp.nranks) q -= cp.nranks;
-              if (p < cp.nranks) v[j][p] = ld_stream(reinterpret_cast<const char*>(a.ptr[q]) + o);
-            }
-          }
-        }
+        peer_loads<NR, U>(cp, a.ptr, o0, hi, v);
 #pragma unroll
         for (int j = 0; j < U; ++j) {
           const int64_t o = o0 + (int64_t)j * kRowBytes;
@@ -666,11 +665,7 @@ __device__ __forceinline__ void pipe_p2p_reduce(const CommParams& cp, int64_t de
   constexpr int U = 8 / NR;
   for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)U * kRowBytes) {
     uint4 v[U][NR];
-#pragma unroll
-    for (int j = 0; j < U; ++j) {
-      const int64_t o = o0 + (int64_t)j * kRowBytes;
-      if (o < hi) peer_loads<NR>(cp, delta + o, v[j]);
-    }
+    peer_loads<NR, U>(cp, cp.buf, delta + o0, delta + hi, v);
 #pragma unroll
     for (int j = 0; j < U; ++j) {
       const int64_t o = o0 + (int64_t)j * kRowBytes;

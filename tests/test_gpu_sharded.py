@@ -33,34 +33,57 @@ def _inputs(n, shard, dtype, seed):
     return [torch.randint(-50, 50, (n * shard,), device='cuda', generator=g).to(dtype) for _ in range(n)]
 
 
-@pytest.mark.parametrize("n", [2, 4, 8])
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16, torch.int32])
-def test_sim_reducescatter(hvd, n, dtype):
+RS_DTYPES = [torch.float32, torch.bfloat16, torch.float16, torch.int32, torch.float64, torch.int64]
+SUM, MIN, MAX = 1, 3, 4
+RS_CASES = ([pytest.param(d, SUM, id='dtype%d' % i) for i, d in enumerate(RS_DTYPES)] +
+            [pytest.param(d, op, id='dtype%d-%s' % (i, name)) for op, name in ((MIN, 'min'), (MAX, 'max'))
+             for i, d in enumerate(RS_DTYPES)])
+
+
+@pytest.mark.parametrize("n", [2, 3, 4, 5, 6, 8])
+@pytest.mark.parametrize("dtype,op", RS_CASES)
+def test_sim_reducescatter(hvd, n, dtype, op):
     from horovod_b200.ops import sim
     repeats = 3
-    scale = 1.0 if dtype == torch.int32 else 1.0 / n  # int32: SUM; floats: AVERAGE as SUM with scale
+    # integers: SUM / MIN / MAX; floats: AVERAGE as SUM with scale (and a scaled MIN / MAX)
+    scale = 1.0 if not dtype.is_floating_point else 1.0 / n
     for shard in SHARDS:
         ts = _inputs(n, shard, dtype, seed=shard + n)
         before = [t.clone() for t in ts]
-        sim.inplace_reducescatter(ts, op=sim.SUM, ctas=8, scale=scale, repeats=repeats)
+        sim.inplace_reducescatter(ts, op=op, ctas=8, scale=scale, repeats=repeats)
         torch.cuda.synchronize()
         for r in range(n):
             lo, hi = r * shard, (r + 1) * shard
             # each repeat re-reduces: rank r's own shard already holds the previous result, the peers' shards do not
-            others = sum(before[q][lo:hi].double() for q in range(n) if q != r)
-            ref = before[r][lo:hi].double()
-            for _ in range(repeats):
-                ref = ((ref + others) * scale).to(dtype).double()
-            if dtype == torch.int32:
-                assert torch.equal(ts[r][lo:hi], ref.to(dtype))
+            if op == SUM:
+                others = sum(before[q][lo:hi].double() for q in range(n) if q != r)
+                ref = before[r][lo:hi].double()
+                for _ in range(repeats):
+                    ref = ((ref + others) * scale).to(dtype).double()
             else:
-                tol = 1e-5 if dtype == torch.float32 else 2e-2
+                # MIN / MAX select one input, then scale in the fp32 (fp64 for fp64) accumulator and round: exact
+                pick = (lambda a, b: torch.minimum(a, b)) if op == MIN else (lambda a, b: torch.maximum(a, b))
+                others = before[(r + 1) % n][lo:hi]
+                for q in range(n):
+                    if q != r:
+                        others = pick(others, before[q][lo:hi])
+                acc = torch.float64 if dtype == torch.float64 else torch.float32
+                ref = before[r][lo:hi]
+                for _ in range(repeats):
+                    ref = pick(ref, others)
+                    if dtype.is_floating_point:
+                        ref = (ref.double() * float(torch.tensor(scale, dtype=acc))).to(acc).to(dtype)
+                ref = ref.double()
+            if not dtype.is_floating_point or op != SUM:
+                assert torch.equal(ts[r][lo:hi].double(), ref)
+            else:
+                tol = {torch.float32: 1e-5, torch.float64: 1e-12}.get(dtype, 2e-2)
                 torch.testing.assert_close(ts[r][lo:hi].double(), ref, rtol=tol, atol=tol)
             # nothing outside the own shard was written (catches stray peer stores)
             assert torch.equal(ts[r][:lo], before[r][:lo]) and torch.equal(ts[r][hi:], before[r][hi:])
 
 
-@pytest.mark.parametrize("n", [2, 4, 8])
+@pytest.mark.parametrize("n", [2, 3, 4, 5, 6, 8])
 def test_sim_allgather_is_byte_exact(hvd, n):
     from horovod_b200.ops import sim
     for shard_bytes in (16, 96032, 1 << 20):
