@@ -1004,7 +1004,7 @@ void* Engine::AllocSymmetric(size_t bytes, int device, int32_t psid, std::string
 }
 
 Status Engine::CapturedAllreduce(void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale, double postscale,
-                                 int32_t psid, int max_ctas, void* stream) {
+                                 int32_t psid, int max_ctas, void* stream, int channel) {
   std::shared_ptr<ProcessSet> ps;
   Status st = CheckSet(psid, &ps);
   if (!st.ok()) return st;
@@ -1012,7 +1012,8 @@ Status Engine::CapturedAllreduce(void* ptr, int64_t bytes, DataType dtype, Reduc
   if (op == ReduceOp::AVERAGE) { op = ReduceOp::SUM; postscale /= (double)ps->set_size(); }
   if (ps->set_size() == 1) return Status::OK();
   captured_launches_.fetch_add(1, std::memory_order_relaxed);
-  return gpu_ops_->CapturedAllreduce(*ps, ptr, bytes, dtype, op, prescale, postscale, max_ctas, (cudaStream_t)stream);
+  return gpu_ops_->CapturedAllreduce(*ps, ptr, bytes, dtype, op, prescale, postscale, max_ctas, (cudaStream_t)stream,
+                                     channel);
 }
 
 Status Engine::CapturedReducescatter(void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale, double postscale,
@@ -1027,13 +1028,13 @@ Status Engine::CapturedReducescatter(void* ptr, int64_t bytes, DataType dtype, R
   return gpu_ops_->CapturedReducescatter(*ps, ptr, bytes, dtype, op, prescale, postscale, max_ctas, (cudaStream_t)stream);
 }
 
-Status Engine::CapturedAllgather(void* ptr, int64_t bytes, int32_t psid, int max_ctas, void* stream) {
+Status Engine::CapturedAllgather(void* ptr, int64_t bytes, int32_t psid, int max_ctas, void* stream, int channel) {
   std::shared_ptr<ProcessSet> ps;
   Status st = CheckSet(psid, &ps);
   if (!st.ok()) return st;
   if (ps->set_size() == 1) return Status::OK();
   captured_launches_.fetch_add(1, std::memory_order_relaxed);
-  return gpu_ops_->CapturedAllgather(*ps, ptr, bytes, max_ctas, (cudaStream_t)stream);
+  return gpu_ops_->CapturedAllgather(*ps, ptr, bytes, max_ctas, (cudaStream_t)stream, channel);
 }
 
 Status Engine::StartTimeline(const std::string& file, bool mark_cycles) {

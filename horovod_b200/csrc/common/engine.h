@@ -81,13 +81,14 @@ class Engine {
   void* AllocSymmetric(size_t bytes, int device, int32_t process_set_id, std::string* err, std::shared_ptr<void>* keep_alive = nullptr);
 
   // Zero-copy allreduce of a registered tensor launched on the caller's stream (CUDA-graph capturable, no negotiation);
-  // `stream` is a cudaStream_t.  See GpuOps::CapturedAllreduce.
+  // `stream` is a cudaStream_t.  See GpuOps::CapturedAllreduce.  `channel`: the barrier channel (kern::kGraphChannel,
+  // or kern::kSyncBnChannel for hvd.SyncBatchNorm).
   Status CapturedAllreduce(void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale, double postscale,
-                           int32_t process_set_id, int max_ctas, void* stream);
+                           int32_t process_set_id, int max_ctas, void* stream, int channel = 1);
   // The two halves of a sharded optimizer step, same contract (see GpuOps::CapturedReducescatter / CapturedAllgather).
   Status CapturedReducescatter(void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale, double postscale,
                                int32_t process_set_id, int max_ctas, void* stream);
-  Status CapturedAllgather(void* ptr, int64_t bytes, int32_t process_set_id, int max_ctas, void* stream);
+  Status CapturedAllgather(void* ptr, int64_t bytes, int32_t process_set_id, int max_ctas, void* stream, int channel = 1);
 
   // ---- timeline ----
   Status StartTimeline(const std::string& file, bool mark_cycles);

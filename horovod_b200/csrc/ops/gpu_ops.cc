@@ -416,7 +416,7 @@ bool GpuOps::BuildInplaceArgs(SymmTeam& team, const void* ptr, int64_t bytes, Da
 // does; the kernel's own flag barrier is the only synchronisation, so a replayed step needs no host work at all.
 // Nothing like it exists in the reference (its cycle loop negotiates every tensor every step, controller.cc:209-252).
 Status GpuOps::CapturedAllreduce(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
-                                 double postscale, int max_ctas, cudaStream_t stream) {
+                                 double postscale, int max_ctas, cudaStream_t stream, int channel) {
   std::shared_ptr<SymmTeam> team;
   { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
   if (!team) return Status::PreconditionError("captured allreduce: the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
@@ -426,7 +426,7 @@ Status GpuOps::CapturedAllreduce(ProcessSet& ps, void* ptr, int64_t bytes, DataT
   if (!BuildInplaceArgs(*team, ptr, bytes, dtype, op, prescale, postscale, -1, std::min(max_ctas, kern::kMaxCtas), &ia))
     return Status::InvalidArgument("captured allreduce: tensor is not (entirely) inside registered symmetric memory, is not 16 B "
                                    "aligned, or combines MIN/MAX/PRODUCT with scale factors");
-  cudaError_t ce = kern::LaunchInplaceAllreduce(team->Params(0, kern::kGraphChannel), ia, stream);
+  cudaError_t ce = kern::LaunchInplaceAllreduce(team->Params(0, channel), ia, stream);
   if (ce != cudaSuccess) return Status::UnknownError(std::string("captured allreduce launch failed: ") + cudaGetErrorString(ce));
   return Status::OK();
 }
@@ -451,7 +451,7 @@ Status GpuOps::CapturedReducescatter(ProcessSet& ps, void* ptr, int64_t bytes, D
   return Status::OK();
 }
 
-Status GpuOps::CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int max_ctas, cudaStream_t stream) {
+Status GpuOps::CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int max_ctas, cudaStream_t stream, int channel) {
   std::shared_ptr<SymmTeam> team;
   { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
   if (!team) return Status::PreconditionError("captured allgather: the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
@@ -463,7 +463,7 @@ Status GpuOps::CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int m
   // a byte copy: described as an fp32 SUM so that the multicast store follows the same policy as the reductions
   if (!BuildInplaceArgs(*team, ptr, bytes, DataType::FLOAT32, ReduceOp::SUM, 1.0, 1.0, -1, std::min(max_ctas, kern::kMaxCtas), &ia))
     return Status::InvalidArgument("captured allgather: tensor is not (entirely) inside registered symmetric memory or is not 16 B aligned");
-  cudaError_t ce = kern::LaunchInplaceAllgather(team->Params(0, kern::kGraphChannel), ia, stream);
+  cudaError_t ce = kern::LaunchInplaceAllgather(team->Params(0, channel), ia, stream);
   if (ce != cudaSuccess) return Status::UnknownError(std::string("captured allgather launch failed: ") + cudaGetErrorString(ce));
   return Status::OK();
 }

@@ -121,16 +121,17 @@ class GpuOps {
   // Description of the data path chosen for a set (for hvd.gpu_backend_info()).
   std::string Describe(ProcessSet& ps);
 
-  // Zero-copy allreduce of a registered tensor as ONE kernel on `stream` (which may be capturing into a CUDA graph), on the
-  // graph channel, with no negotiation: callable from framework threads.
+  // Zero-copy allreduce of a registered tensor as ONE kernel on `stream` (which may be capturing into a CUDA graph), on
+  // barrier channel `channel` (kern::kGraphChannel; kern::kSyncBnChannel for hvd.SyncBatchNorm), with no negotiation:
+  // callable from framework threads.
   Status CapturedAllreduce(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
-                           double postscale, int max_ctas, cudaStream_t stream);
+                           double postscale, int max_ctas, cudaStream_t stream, int channel);
   // Sharded optimizer step (ZeRO-1), same launch contract as CapturedAllreduce: rank r owns [r*S, (r+1)*S), S = bytes / n,
   // and bytes must be a multiple of 16 * n.  Reduce-scatter: rank r's shard of its own tensor receives the reduction.
   // Allgather: every owner's shard is copied into every peer's tensor.
   Status CapturedReducescatter(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                                double postscale, int max_ctas, cudaStream_t stream);
-  Status CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int max_ctas, cudaStream_t stream);
+  Status CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int max_ctas, cudaStream_t stream, int channel);
   bool BuildInplaceArgs(SymmTeam& team, const void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                         double postscale, int64_t expect_off, int max_ctas, kern::InplaceArgs* out);
 

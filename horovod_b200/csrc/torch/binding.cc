@@ -447,14 +447,23 @@ at::Tensor SymmEmpty(int64_t nbytes, int device, int process_set_id) {
 // In-place allreduce of a tensor that lives in registered symmetric memory, launched as ONE kernel on the current CUDA
 // stream of the calling thread — which may be capturing into a CUDA graph.  No handle, no negotiation, no host
 // synchronisation: ordering is the stream's.  reduce_op follows hvd.ReduceOp (0 Average, 1 Sum, 3 Min, 4 Max, 5 Product).
-void CapturedAllreduce(at::Tensor tensor, int reduce_op, double prescale, double postscale, int process_set_id, int max_ctas) {
+// `channel`: the barrier channel, kGraphChannel for the public hvd.captured_* functions, kSyncBnChannel for
+// hvd.SyncBatchNorm, whose collectives can be resident together with graph-channel ones.
+void CheckCapturedChannel(const char* op, int channel) {
+  TORCH_CHECK(channel == kern::kGraphChannel || channel == kern::kSyncBnChannel, op, ": channel must be ",
+              kern::kGraphChannel, " or ", kern::kSyncBnChannel, ", got ", channel);
+}
+
+void CapturedAllreduce(at::Tensor tensor, int reduce_op, double prescale, double postscale, int process_set_id, int max_ctas,
+                       int channel) {
+  CheckCapturedChannel("captured_allreduce_", channel);
   TORCH_CHECK(tensor.is_cuda(), "captured_allreduce_: CUDA tensor expected");
   TORCH_CHECK(tensor.is_non_overlapping_and_dense(), "captured_allreduce_: tensor must be dense");
   c10::cuda::CUDAGuard guard(tensor.device());
   cudaStream_t stream = c10::cuda::getCurrentCUDAStream(tensor.get_device());
   const int64_t bytes = (int64_t)tensor.numel() * (int64_t)tensor.element_size();
   ThrowIfError(Engine::Get().CapturedAllreduce(tensor.data_ptr(), bytes, MapDtype(tensor.scalar_type()), (ReduceOp)reduce_op, prescale,
-                                               postscale, process_set_id, max_ctas, (void*)stream));
+                                               postscale, process_set_id, max_ctas, (void*)stream, channel));
 }
 
 // The two halves of a sharded optimizer step on a registered tensor, launched like CapturedAllreduce.  Rank r owns the
@@ -469,13 +478,14 @@ void CapturedReducescatter(at::Tensor tensor, int reduce_op, double prescale, do
                                                    prescale, postscale, process_set_id, max_ctas, (void*)stream));
 }
 
-void CapturedAllgather(at::Tensor tensor, int process_set_id, int max_ctas) {
+void CapturedAllgather(at::Tensor tensor, int process_set_id, int max_ctas, int channel) {
+  CheckCapturedChannel("captured_allgather_", channel);
   TORCH_CHECK(tensor.is_cuda(), "captured_allgather_: CUDA tensor expected");
   TORCH_CHECK(tensor.is_non_overlapping_and_dense(), "captured_allgather_: tensor must be dense");
   c10::cuda::CUDAGuard guard(tensor.device());
   cudaStream_t stream = c10::cuda::getCurrentCUDAStream(tensor.get_device());
   const int64_t bytes = (int64_t)tensor.numel() * (int64_t)tensor.element_size();
-  ThrowIfError(Engine::Get().CapturedAllgather(tensor.data_ptr(), bytes, process_set_id, max_ctas, (void*)stream));
+  ThrowIfError(Engine::Get().CapturedAllgather(tensor.data_ptr(), bytes, process_set_id, max_ctas, (void*)stream, channel));
 }
 
 // ---- fused optimizer kernels (an extra of this library; see kernels/optim_kernels.cu) --------------
@@ -797,6 +807,202 @@ void GradShardStats(std::vector<at::Tensor> grads, at::Tensor out, c10::optional
   TORCH_CHECK(e == cudaSuccess, "grad_shard_stats launch failed: ", cudaGetErrorString(e));
 }
 
+// ---- hvd.SyncBatchNorm kernels (see kernels/sync_bn_kernels.cu) ------------------------------------------------------
+// Every argument is checked here, before anything is launched.
+
+// The view of an input with channels at dim 1: rows [M, C] when, walking dims 1, d-1, ..., 2, 0, the strides are those of
+// a packed array (channels_last, [N, C], spatial size 1; dims of size 1 do not matter), else planes [N, C, L] when it is
+// contiguous.  Other layouts are the caller's to make contiguous.
+kern::BnGeom BnView(const char* op, const at::Tensor& x) {
+  TORCH_CHECK(x.is_cuda() && x.dim() >= 2 && x.size(1) > 0, op, ": x must be a CUDA tensor with at least 2 dimensions "
+              "and at least one channel");
+  const auto st = x.scalar_type();
+  TORCH_CHECK(st == at::kFloat || st == at::kBFloat16 || st == at::kHalf, op, ": x must be float32, bfloat16 or float16, got ", st);
+  const int64_t d = x.dim(), C = x.size(1);
+  std::vector<int64_t> order {1};
+  for (int64_t k = d - 1; k >= 2; --k) order.push_back(k);
+  order.push_back(0);
+  bool rows = true;
+  int64_t expect = 1;
+  for (int64_t k : order) {
+    if (x.size(k) != 1 && x.stride(k) != expect) { rows = false; break; }
+    expect *= x.size(k);
+  }
+  if (rows) return kern::BnGeom {kern::kBnRows, x.numel() / C, C, 1};
+  TORCH_CHECK(x.is_contiguous(), op, ": x must be contiguous or channels-last (channels innermost), got strides ", x.strides());
+  const int64_t N = x.size(0);
+  return kern::BnGeom {kern::kBnPlanes, N, C, N > 0 ? x.numel() / (N * C) : 0};
+}
+
+// a per-channel vector: C contiguous elements on x's device, of one of `dtypes`
+void CheckBnVec(const char* op, const char* what, const at::Tensor& t, int64_t C, const at::Tensor& x,
+                std::initializer_list<at::ScalarType> dtypes) {
+  TORCH_CHECK(t.is_cuda() && t.device() == x.device(), op, ": ", what, " must be on ", x.device(), ", got ", t.device());
+  TORCH_CHECK(t.is_contiguous() && t.numel() == C, op, ": ", what, " must be contiguous with ", C, " elements, got sizes ",
+              t.sizes());
+  bool ok = false;
+  for (auto d : dtypes) ok |= t.scalar_type() == d;
+  TORCH_CHECK(ok, op, ": ", what, " has dtype ", t.scalar_type(), ", which is not allowed here");
+}
+
+// weight / bias: fp32 or x's dtype, both the same
+int BnAffineDtype(const char* op, const c10::optional<at::Tensor>& w, const c10::optional<at::Tensor>& b, int64_t C,
+                  const at::Tensor& x) {
+  const at::Tensor* first = w ? &*w : (b ? &*b : nullptr);
+  if (!first) return (int)MapDtype(at::kFloat);
+  if (w) CheckBnVec(op, "weight", *w, C, x, {at::kFloat, x.scalar_type()});
+  if (b) CheckBnVec(op, "bias", *b, C, x, {at::kFloat, x.scalar_type()});
+  TORCH_CHECK(!(w && b) || w->scalar_type() == b->scalar_type(), op, ": weight and bias must have the same dtype");
+  return (int)MapDtype(first->scalar_type());
+}
+
+// The stats kernels' last-CTA tickets: a zeroed int32 array per (device, stream), grown to the most channel tiles seen,
+// which every launch leaves zeroed.  Launches on one stream run one after another and share it.  It comes from torch's
+// allocator and is zeroed on the stream, so a stream first seen while it is being captured (hvd.GraphedStep captures on
+// a stream of its own) gets its array from the graph's pool, zeroed by the graph.  Arrays are kept for the life of the
+// process: a captured graph may still refer to them.
+unsigned* BnTickets(int device, cudaStream_t s, int64_t n) {
+  static std::mutex mu;
+  static std::map<std::pair<int, cudaStream_t>, at::Tensor> tickets;
+  static std::vector<at::Tensor> outgrown;
+  std::lock_guard<std::mutex> l(mu);
+  at::Tensor& t = tickets[{device, s}];
+  if (!t.defined() || t.numel() < n) {
+    if (t.defined()) outgrown.push_back(t);
+    t = at::zeros({std::max<int64_t>(n, 1024)}, at::TensorOptions().dtype(at::kInt).device(at::kCUDA, device));
+  }
+  return reinterpret_cast<unsigned*>(t.data_ptr<int>());
+}
+
+void CheckBnSums(const char* op, const char* what, const at::Tensor& t, int64_t need, const at::Tensor& x) {
+  TORCH_CHECK(t.is_cuda() && t.device() == x.device() && t.scalar_type() == at::kDouble && t.is_contiguous() &&
+              t.numel() >= need, op, ": ", what, " must be a contiguous float64 tensor on ", x.device(), " with at least ",
+              need, " elements");
+}
+
+// This rank's {count, mean, M2} of every channel of x, as fp64 triples, into slot[0 : 3C].
+void SyncBnStats(at::Tensor x, at::Tensor slot) {
+  const kern::BnGeom g = BnView("sync_bn_stats", x);
+  CheckBnSums("sync_bn_stats", "slot", slot, 3 * g.C, x);
+  c10::cuda::CUDAGuard guard(x.device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(x.get_device());
+  const int dt = (int)MapDtype(x.scalar_type());
+  const kern::BnPlan plan = kern::BnReducePlan(g, dt);
+  at::Tensor part = at::empty({plan.splits * g.C * 2}, x.options().dtype(at::kDouble));  // 16 B per partial
+  cudaError_t e = kern::LaunchBnStats(x.data_ptr(), g, dt, part.data_ptr(), BnTickets(x.get_device(), s, plan.tiles),
+                                      slot.data_ptr<double>(), s);
+  TORCH_CHECK(e == cudaSuccess, "sync_bn_stats launch failed: ", cudaGetErrorString(e));
+}
+
+// Merges the slots (rows of `slots`, in rank order) of C channels: returns (mean, invstd, count) as float32 and updates
+// the running statistics where given.
+std::tuple<at::Tensor, at::Tensor, at::Tensor> SyncBnCombine(at::Tensor slots, int64_t C, double eps, double momentum,
+                                                             c10::optional<at::Tensor> running_mean,
+                                                             c10::optional<at::Tensor> running_var,
+                                                             c10::optional<at::Tensor> num_batches_tracked) {
+  const char* op = "sync_bn_combine";
+  TORCH_CHECK(C > 0, op, ": C must be positive");
+  TORCH_CHECK(slots.is_cuda() && slots.scalar_type() == at::kDouble && slots.is_contiguous() && slots.dim() == 2 &&
+              slots.size(0) >= 1 && slots.size(0) <= kern::kMaxPeers && slots.size(1) >= 3 * C, op,
+              ": slots must be a contiguous float64 CUDA tensor [nranks <= ", kern::kMaxPeers, ", >= 3 * C], got ",
+              slots.scalar_type(), " ", slots.sizes());
+  TORCH_CHECK(running_mean.has_value() == running_var.has_value(), op, ": running_mean and running_var go together");
+  int sdt = (int)MapDtype(at::kFloat);
+  if (running_mean) {
+    for (const at::Tensor* t : {&*running_mean, &*running_var})
+      CheckBnVec(op, t == &*running_mean ? "running_mean" : "running_var", *t, C, slots, {at::kFloat, at::kBFloat16, at::kHalf});
+    TORCH_CHECK(running_mean->scalar_type() == running_var->scalar_type(), op, ": running stats must have one dtype");
+    sdt = (int)MapDtype(running_mean->scalar_type());
+  }
+  if (num_batches_tracked)
+    TORCH_CHECK(running_mean && num_batches_tracked->is_cuda() && num_batches_tracked->device() == slots.device() &&
+                num_batches_tracked->scalar_type() == at::kLong && num_batches_tracked->numel() == 1, op,
+                ": num_batches_tracked must be a one-element int64 tensor on ", slots.device(), ", with running stats");
+  c10::cuda::CUDAGuard guard(slots.device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(slots.get_device());
+  at::Tensor mean = at::empty({C}, slots.options().dtype(at::kFloat)), invstd = at::empty_like(mean);
+  at::Tensor count = at::empty({1}, mean.options());
+  cudaError_t e = kern::LaunchBnCombine(slots.data_ptr<double>(), (int)slots.size(0), slots.size(1), C, eps, momentum,
+                                        num_batches_tracked ? num_batches_tracked->data_ptr<int64_t>() : nullptr,
+                                        mean.data_ptr<float>(), invstd.data_ptr<float>(), count.data_ptr<float>(),
+                                        running_mean ? running_mean->data_ptr() : nullptr,
+                                        running_var ? running_var->data_ptr() : nullptr, sdt, s);
+  TORCH_CHECK(e == cudaSuccess, "sync_bn_combine launch failed: ", cudaGetErrorString(e));
+  return {mean, invstd, count};
+}
+
+at::Tensor SyncBnElemt(at::Tensor x, at::Tensor mean, at::Tensor invstd, c10::optional<at::Tensor> weight,
+                       c10::optional<at::Tensor> bias) {
+  const char* op = "sync_bn_elemt";
+  const kern::BnGeom g = BnView(op, x);
+  CheckBnVec(op, "mean", mean, g.C, x, {at::kFloat});
+  CheckBnVec(op, "invstd", invstd, g.C, x, {at::kFloat});
+  const int wdt = BnAffineDtype(op, weight, bias, g.C, x);
+  c10::cuda::CUDAGuard guard(x.device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(x.get_device());
+  at::Tensor y = at::empty_like(x);  // x is dense, so y gets its strides
+  cudaError_t e = kern::LaunchBnElemt(x.data_ptr(), y.data_ptr(), g, (int)MapDtype(x.scalar_type()), mean.data_ptr<float>(),
+                                      invstd.data_ptr<float>(), weight ? weight->data_ptr() : nullptr,
+                                      bias ? bias->data_ptr() : nullptr, wdt, s);
+  TORCH_CHECK(e == cudaSuccess, "sync_bn_elemt launch failed: ", cudaGetErrorString(e));
+  return y;
+}
+
+void CheckBnGrad(const char* op, const at::Tensor& dy, const at::Tensor& x) {
+  TORCH_CHECK(dy.device() == x.device() && dy.scalar_type() == x.scalar_type() && dy.sizes() == x.sizes() &&
+              dy.strides() == x.strides(), op, ": grad_output must have x's device, dtype, sizes and strides");
+}
+
+// sums[2c] = sum dy, sums[2c+1] = sum dy * (x - mean) over this rank's batch; returns the local (grad_weight, grad_bias)
+// in the weight's dtype where asked for (None otherwise).
+std::tuple<at::Tensor, at::Tensor> SyncBnBackwardReduce(at::Tensor dy, at::Tensor x, at::Tensor mean, at::Tensor invstd,
+                                                        c10::optional<at::Tensor> weight, at::Tensor sums,
+                                                        bool need_weight_grad, bool need_bias_grad) {
+  const char* op = "sync_bn_backward_reduce";
+  const kern::BnGeom g = BnView(op, x);
+  CheckBnGrad(op, dy, x);
+  CheckBnVec(op, "mean", mean, g.C, x, {at::kFloat});
+  CheckBnVec(op, "invstd", invstd, g.C, x, {at::kFloat});
+  CheckBnSums(op, "sums", sums, 2 * g.C, x);
+  const int wdt = BnAffineDtype(op, weight, c10::nullopt, g.C, x);
+  const auto wopt = x.options().dtype(weight ? weight->scalar_type() : at::kFloat);
+  at::Tensor gw = need_weight_grad ? at::empty({g.C}, wopt) : at::Tensor();
+  at::Tensor gb = need_bias_grad ? at::empty({g.C}, wopt) : at::Tensor();
+  c10::cuda::CUDAGuard guard(x.device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(x.get_device());
+  const int dt = (int)MapDtype(x.scalar_type());
+  const kern::BnPlan plan = kern::BnReducePlan(g, dt);
+  at::Tensor part = at::empty({plan.splits * g.C * 2}, x.options().dtype(at::kFloat));  // 8 B per partial
+  cudaError_t e = kern::LaunchBnBackwardReduce(dy.data_ptr(), x.data_ptr(), g, dt, mean.data_ptr<float>(),
+                                               invstd.data_ptr<float>(), part.data_ptr(),
+                                               BnTickets(x.get_device(), s, plan.tiles), sums.data_ptr<double>(),
+                                               gw.defined() ? gw.data_ptr() : nullptr, gb.defined() ? gb.data_ptr() : nullptr,
+                                               wdt, s);
+  TORCH_CHECK(e == cudaSuccess, "sync_bn_backward_reduce launch failed: ", cudaGetErrorString(e));
+  return {gw, gb};
+}
+
+at::Tensor SyncBnBackwardElemt(at::Tensor dy, at::Tensor x, at::Tensor mean, at::Tensor invstd,
+                               c10::optional<at::Tensor> weight, at::Tensor sums, at::Tensor count) {
+  const char* op = "sync_bn_backward_elemt";
+  const kern::BnGeom g = BnView(op, x);
+  CheckBnGrad(op, dy, x);
+  CheckBnVec(op, "mean", mean, g.C, x, {at::kFloat});
+  CheckBnVec(op, "invstd", invstd, g.C, x, {at::kFloat});
+  CheckBnSums(op, "sums", sums, 2 * g.C, x);
+  CheckBnVec(op, "count", count, 1, x, {at::kFloat});
+  const int wdt = BnAffineDtype(op, weight, c10::nullopt, g.C, x);
+  c10::cuda::CUDAGuard guard(x.device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(x.get_device());
+  at::Tensor dx = at::empty_like(x);
+  cudaError_t e = kern::LaunchBnBackwardElemt(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), g, (int)MapDtype(x.scalar_type()),
+                                              mean.data_ptr<float>(), invstd.data_ptr<float>(),
+                                              weight ? weight->data_ptr() : nullptr, wdt, sums.data_ptr<double>(),
+                                              count.data_ptr<float>(), s);
+  TORCH_CHECK(e == cudaSuccess, "sync_bn_backward_elemt launch failed: ", cudaGetErrorString(e));
+  return dx;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(_hvd_torch, m) {
@@ -816,9 +1022,11 @@ PYBIND11_MODULE(_hvd_torch, m) {
   m.def("reset", &Reset);
   m.def("reset_noname_counters", &ResetNonameCounters);
   m.def("symm_empty", &SymmEmpty);
-  m.def("captured_allreduce_", &CapturedAllreduce);
+  m.def("captured_allreduce_", &CapturedAllreduce, py::arg("tensor"), py::arg("reduce_op"), py::arg("prescale"),
+        py::arg("postscale"), py::arg("process_set_id"), py::arg("max_ctas"), py::arg("channel") = kern::kGraphChannel);
   m.def("captured_reducescatter_", &CapturedReducescatter);
-  m.def("captured_allgather_", &CapturedAllgather);
+  m.def("captured_allgather_", &CapturedAllgather, py::arg("tensor"), py::arg("process_set_id"), py::arg("max_ctas"),
+        py::arg("channel") = kern::kGraphChannel);
   m.def("fused_sgd_step", &FusedSgdStep, py::arg("params"), py::arg("grads"), py::arg("momenta"), py::arg("lr"),
         py::arg("momentum"), py::arg("dampening"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("grad_scale"),
         py::arg("first_step"), py::arg("grad_scale_dev") = py::none(), py::arg("master_params") = std::vector<at::Tensor>());
@@ -839,4 +1047,14 @@ PYBIND11_MODULE(_hvd_torch, m) {
         py::arg("bias_correction"), py::arg("adapt"), py::arg("master_params"), py::arg("norms"), py::arg("slots"));
   m.def("grad_shard_stats", &GradShardStats, py::arg("grads"), py::arg("out"), py::arg("inv_scale") = py::none(),
         py::arg("norm_inf") = false);
+  m.def("sync_bn_stats", &SyncBnStats, py::arg("x"), py::arg("slot"));
+  m.def("sync_bn_combine", &SyncBnCombine, py::arg("slots"), py::arg("num_features"), py::arg("eps"), py::arg("momentum"),
+        py::arg("running_mean") = py::none(), py::arg("running_var") = py::none(),
+        py::arg("num_batches_tracked") = py::none());
+  m.def("sync_bn_elemt", &SyncBnElemt, py::arg("x"), py::arg("mean"), py::arg("invstd"), py::arg("weight") = py::none(),
+        py::arg("bias") = py::none());
+  m.def("sync_bn_backward_reduce", &SyncBnBackwardReduce, py::arg("grad_output"), py::arg("x"), py::arg("mean"),
+        py::arg("invstd"), py::arg("weight"), py::arg("sums"), py::arg("need_weight_grad"), py::arg("need_bias_grad"));
+  m.def("sync_bn_backward_elemt", &SyncBnBackwardElemt, py::arg("grad_output"), py::arg("x"), py::arg("mean"),
+        py::arg("invstd"), py::arg("weight"), py::arg("sums"), py::arg("count"));
 }

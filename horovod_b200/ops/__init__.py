@@ -4,6 +4,8 @@
 * `fused_lamb_step`, and its two phases `lamb_norms` / `lamb_apply` — multi-tensor LAMB with per-tensor trust ratios
   (same file);
 * `grad_shard_stats` — one-pass gradient norm statistics, non-finite check and optional in-place unscale (same file);
+* `sync_bn_stats`, `sync_bn_combine`, `sync_bn_elemt`, `sync_bn_backward_reduce`, `sync_bn_backward_elemt` — the
+  kernels of hvd.SyncBatchNorm's native path (`csrc/kernels/sync_bn_kernels.cu`);
 * `symm_empty`, `symm_available` — registered symmetric memory for the zero-copy allreduce path;
 * `sim` — the single-GPU simulation harness (N ranks = N concurrently running kernels on one device) used by the
   numerics tests, `bench/kernel_micro.py` and the ncu captures;
@@ -102,6 +104,50 @@ def grad_shard_stats(tensors, out, inv_scale=None, norm_type=2.0):
     for ts in by_dtype.values():
         _native().grad_shard_stats(ts, out, inv_scale, norm_type != 2.0)
     return out
+
+
+def sync_bn_slot_doubles(num_features):
+    """float64 elements of one rank's slot in sync_bn_stats' layout: 3 per channel, padded to 16 bytes, so that N slots
+    in a row make a region of a multiple of 16 * N bytes (what the in-place allgather needs)."""
+    return (3 * int(num_features) + 1) // 2 * 2
+
+
+def sync_bn_stats(x, slot):
+    """This rank's statistics of x for SyncBatchNorm, one launch: for every channel c (dim 1), slot[3c : 3c+3] =
+    (count, mean, M2) in float64.  x is float32 / bfloat16 / float16, channels-last (channels innermost, which includes
+    [N, C] and spatial size 1) or contiguous; `slot` is a contiguous float64 CUDA tensor of at least 3C elements.
+    Welford per thread, Chan across CTAs, combined in fp64 in a fixed order: the same input gives the same bits."""
+    _native().sync_bn_stats(x, slot)
+    return slot
+
+
+def sync_bn_combine(slots, num_features, eps, momentum=0.1, running_mean=None, running_var=None, num_batches_tracked=None):
+    """Merges the rows of `slots` ([nranks, >= 3C] float64, one sync_bn_stats slot per rank) in rank order in fp64 and
+    returns (mean, invstd, count): float32 tensors of C, C and 1 elements.  Where running stats are given they are
+    updated as torch does (rv with the unbiased variance, none for a count of 1), with factor `momentum`, or
+    1 / num_batches_tracked[0] read on the device when `num_batches_tracked` is given.  One launch."""
+    return _native().sync_bn_combine(slots, int(num_features), float(eps), float(momentum), running_mean, running_var,
+                                     num_batches_tracked)
+
+
+def sync_bn_elemt(x, mean, invstd, weight=None, bias=None):
+    """y = (x - mean) * invstd * weight + bias per channel, in x's dtype and layout.  weight / bias: float32 or x's
+    dtype, or None.  One launch."""
+    return _native().sync_bn_elemt(x, mean, invstd, weight, bias)
+
+
+def sync_bn_backward_reduce(grad_output, x, mean, invstd, weight, sums, need_weight_grad=True, need_bias_grad=True):
+    """sums[2c] = sum dy and sums[2c+1] = sum dy * (x - mean) over this rank's batch (float64, `sums` has >= 2C
+    elements), to be summed over the ranks; returns this rank's (grad_weight, grad_bias) in the weight's dtype, None
+    where not asked for.  grad_output must have x's sizes and strides.  One launch, deterministic."""
+    return _native().sync_bn_backward_reduce(grad_output, x, mean, invstd, weight, sums, bool(need_weight_grad),
+                                             bool(need_bias_grad))
+
+
+def sync_bn_backward_elemt(grad_output, x, mean, invstd, weight, sums, count):
+    """dx = (dy - sum_dy / n - (x - mean) * invstd^2 * sum_dy_xmu / n) * invstd * weight, with the summed `sums` of
+    sync_bn_backward_reduce and n = count[0] of sync_bn_combine.  One launch."""
+    return _native().sync_bn_backward_elemt(grad_output, x, mean, invstd, weight, sums, count)
 
 
 def symm_empty(*args, **kwargs):
