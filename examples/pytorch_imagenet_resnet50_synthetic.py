@@ -1,6 +1,8 @@
 """ImageNet-style training program (synthetic data) with everything a long job needs: rank-0 checkpoints and resume by
 broadcast, LR warm-up scaled by the number of ranks, gradient accumulation (`backward_passes_per_step`), optional fp16 /
 bf16 gradient compression, metric averaging, pinned side-stream input prefetch, and (on GPUs) the CUDA-graph step.
+`--optimizer lars` trains with LARS (hvd.Lars, the large-batch optimizer of the MLPerf ResNet-50 reference) instead of
+momentum SGD, with BatchNorm and bias parameters excluded from weight decay and trust ratio.
 
     hvdrun -np 8 python examples/pytorch_imagenet_resnet50_synthetic.py --epochs 3 --checkpoint-format /tmp/ckpt-{epoch}.pt
     hvdrun -np 2 python examples/pytorch_imagenet_resnet50_synthetic.py --no-cuda --model tiny --steps-per-epoch 4 --batch-size 8
@@ -29,6 +31,7 @@ p.add_argument('--base-lr', type=float, default=0.0125)
 p.add_argument('--warmup-epochs', type=float, default=1.0)
 p.add_argument('--momentum', type=float, default=0.9)
 p.add_argument('--wd', type=float, default=5e-5)
+p.add_argument('--optimizer', default='sgd', choices=['sgd', 'lars'])
 p.add_argument('--compression', default='none', choices=['none', 'fp16', 'bf16'])
 p.add_argument('--checkpoint-format', default='')
 p.add_argument('--no-cuda', action='store_true')
@@ -64,7 +67,14 @@ if args.checkpoint_format and hvd.rank() == 0:
 resume_epoch = int(hvd.broadcast(torch.tensor(resume_epoch), root_rank=0, name='resume_epoch').item())
 
 lr_scaler = args.batches_per_allreduce * hvd.size()
-opt = torch.optim.SGD(model.parameters(), lr=args.base_lr * lr_scaler, momentum=args.momentum, weight_decay=args.wd)
+if args.optimizer == 'lars':
+    # BatchNorm weights and biases and every bias (the 1-D parameters) get no weight decay and so no trust ratio
+    decay = [q for q in model.parameters() if q.dim() > 1]
+    no_decay = [q for q in model.parameters() if q.dim() <= 1]
+    opt = hvd.Lars([{'params': decay, 'weight_decay': args.wd}, {'params': no_decay, 'weight_decay': 0.0}],
+                   lr=args.base_lr * lr_scaler, momentum=args.momentum)
+else:
+    opt = torch.optim.SGD(model.parameters(), lr=args.base_lr * lr_scaler, momentum=args.momentum, weight_decay=args.wd)
 compression = {'none': hvd.Compression.none, 'fp16': hvd.Compression.fp16, 'bf16': hvd.Compression.bf16}[args.compression]
 opt = hvd.DistributedOptimizer(opt, named_parameters=model.named_parameters(), compression=compression,
                                backward_passes_per_step=args.batches_per_allreduce, op=hvd.Average,

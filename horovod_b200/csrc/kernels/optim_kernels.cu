@@ -301,6 +301,106 @@ fused_lamb_apply_kernel(const LambTensor* __restrict__ table, float lr, float ep
   }
 }
 
+// LARS (You, Gitman, Ginsburg, "Large Batch Training of Convolutional Networks"; the MLPerf ResNet-50 optimizer): with
+// g the scaled gradient, d = g + wd * w, the per-tensor trust ratio r = tc * ||w|| / (||g|| + wd * ||w|| + eps) (1 if
+// either norm is 0, or if the caller does not adapt), v = momentum * v + lr * r * d, w -= v.  LAMB's three launches and
+// table, with the fp32 momentum buffer in `exp_avg` (`exp_avg_sq` is not read): stage 1 writes one (sum w^2, sum g^2)
+// partial per CTA, lamb_finalize_kernel adds them into norms[2 * slot], norms[2 * slot + 1], and stage 2 reads the
+// gradient again and applies the update.  Both stages scale the gradient alike.
+template <typename P, typename G, bool kMaster>
+__global__ void __launch_bounds__(kOptThreads)
+fused_lars_norms_kernel(const LambTensor* __restrict__ table, float grad_scale, const float* __restrict__ grad_scale_dev,
+                        float2* __restrict__ partial) {
+  __shared__ float2 red[kOptThreads / 32];
+  const LambTensor t = table[blockIdx.y];
+  const int64_t n = t.count;
+  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  if (base >= n) return;
+  grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
+  const P* p = reinterpret_cast<const P*>(t.param);
+  const G* g = reinterpret_cast<const G*>(t.grad);
+  const float* w = kMaster ? reinterpret_cast<const float*>(t.master) : nullptr;
+  const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g), wa = kMaster && is_aligned<float>(w);
+  float sw = 0.f, sg = 0.f;
+#pragma unroll
+  for (int it = 0; it < kOptIters; ++it) {
+    const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
+    if (i >= n) break;
+    float pv[kOptVec], gv[kOptVec];
+    load4<P>(p, i, n, pa, pv);
+    load4<G>(g, i, n, ga, gv);
+    if constexpr (kMaster) {
+      float wv[kOptVec];
+      load4<float>(w, i, n, wa, wv);
+      reconcile4<P>(pv, wv);
+    }
+#pragma unroll
+    for (int k = 0; k < kOptVec; ++k) {  // past the end both read as 0
+      const float d = gv[k] * grad_scale;
+      sw = fmaf(pv[k], pv[k], sw);
+      sg = fmaf(d, d, sg);
+    }
+  }
+  // CTA partial: the tree of fused_lamb_norms_kernel
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    sw += __shfl_xor_sync(0xffffffffu, sw, o);
+    sg += __shfl_xor_sync(0xffffffffu, sg, o);
+  }
+  if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = make_float2(sw, sg);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float2 a = red[0];
+    for (int k = 1; k < kOptThreads / 32; ++k) { a.x += red[k].x; a.y += red[k].y; }
+    partial[t.partial + blockIdx.x] = a;
+  }
+}
+
+template <typename P, typename G, bool kMaster>
+__global__ void __launch_bounds__(kOptThreads)
+fused_lars_apply_kernel(const LambTensor* __restrict__ table, float lr, float momentum, float wd, float tc, float eps,
+                        int adapt, float grad_scale, const float* __restrict__ grad_scale_dev, const float* __restrict__ norms) {
+  const LambTensor t = table[blockIdx.y];
+  const int64_t n = t.count;
+  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  if (base >= n) return;
+  grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
+  float r = 1.f;
+  if (adapt) {
+    const float wn = sqrtf(norms[2 * t.slot]), gn = sqrtf(norms[2 * t.slot + 1]);
+    if (wn > 0.f && gn > 0.f) r = tc * wn / (fmaf(wd, wn, gn) + eps);
+  }
+  const float step = lr * r;
+  P* p = reinterpret_cast<P*>(t.param);
+  const G* g = reinterpret_cast<const G*>(t.grad);
+  float* v = reinterpret_cast<float*>(t.exp_avg);
+  float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
+  const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g), sa = is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
+#pragma unroll
+  for (int it = 0; it < kOptIters; ++it) {
+    const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
+    if (i >= n) break;
+    float pv[kOptVec], gv[kOptVec], vv[kOptVec];
+    load4<P>(p, i, n, pa, pv);
+    load4<G>(g, i, n, ga, gv);
+    load4<float>(v, i, n, sa, vv);
+    if constexpr (kMaster) {
+      float wv[kOptVec];
+      load4<float>(w, i, n, sa, wv);
+      reconcile4<P>(pv, wv);  // the same value stage 1 started from: nothing wrote p or the master in between
+    }
+#pragma unroll
+    for (int k = 0; k < kOptVec; ++k) {
+      const float d = fmaf(wd, pv[k], gv[k] * grad_scale);
+      vv[k] = fmaf(momentum, vv[k], step * d);
+      pv[k] -= vv[k];
+    }
+    if constexpr (kMaster) store4<float>(w, i, n, sa, pv);
+    store4<P>(p, i, n, pa, pv);
+    store4<float>(v, i, n, sa, vv);
+  }
+}
+
 // max that keeps a NaN once it has seen one (fmaxf drops it), so an inf-norm of NaN gradients is NaN as in torch
 __device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
 __device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
@@ -435,6 +535,16 @@ cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, 
 
 int64_t LambPartials(int64_t count) { return (count + kOptPerBlock - 1) / kOptPerBlock; }
 
+// After a stage-1 launch: count it, then add each entry's partials into its norm slot.
+static cudaError_t FinalizeNorms(const LambTensor* table, int n, const float2* part, float* norms, cudaStream_t stream) {
+  CountKernelLaunch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  lamb_finalize_kernel<<<(unsigned)n, kOptThreads, 0, stream>>>(table, part, norms);
+  CountKernelLaunch();
+  return cudaGetLastError();
+}
+
 cudaError_t LaunchLambNorms(const LambTensor* table, int n, int64_t max_count, float beta1, float beta2, float eps,
                             float weight_decay, float bias_c1, float bias_c2, float grad_scale, const float* grad_scale_dev,
                             float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream) {
@@ -453,12 +563,7 @@ cudaError_t LaunchLambNorms(const LambTensor* table, int n, int64_t max_count, f
   else if (param_dtype == 6 && grad_dtype == 6) HVD_LAMB_NORMS(__half, __half, false);
   else return cudaErrorInvalidValue;
 #undef HVD_LAMB_NORMS
-  CountKernelLaunch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  lamb_finalize_kernel<<<(unsigned)n, kOptThreads, 0, stream>>>(table, part, norms);
-  CountKernelLaunch();
-  return cudaGetLastError();
+  return FinalizeNorms(table, n, part, norms, stream);
 }
 
 cudaError_t LaunchLambApply(const LambTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
@@ -477,6 +582,47 @@ cudaError_t LaunchLambApply(const LambTensor* table, int n, int64_t max_count, f
   else if (param_dtype == 6) HVD_LAMB_APPLY(__half, false);
   else return cudaErrorInvalidValue;
 #undef HVD_LAMB_APPLY
+  CountKernelLaunch();
+  return cudaGetLastError();
+}
+
+cudaError_t LaunchLarsNorms(const LambTensor* table, int n, int64_t max_count, float grad_scale, const float* grad_scale_dev,
+                            float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream) {
+  if (n <= 0 || max_count <= 0) return cudaSuccess;
+  dim3 grid((unsigned)LambPartials(max_count), (unsigned)n);
+  float2* part = reinterpret_cast<float2*>(partial);
+#define HVD_LARS_NORMS(P, G, M) fused_lars_norms_kernel<P, G, M><<<grid, kOptThreads, 0, stream>>>(table, grad_scale, grad_scale_dev, part)
+  if (master) {
+    if (param_dtype == 10 && grad_dtype == 10) HVD_LARS_NORMS(__nv_bfloat16, __nv_bfloat16, true);
+    else if (param_dtype == 6 && grad_dtype == 6) HVD_LARS_NORMS(__half, __half, true);
+    else return cudaErrorInvalidValue;
+  }
+  else if (param_dtype == 7 && grad_dtype == 7) HVD_LARS_NORMS(float, float, false);
+  else if (param_dtype == 7 && grad_dtype == 10) HVD_LARS_NORMS(float, __nv_bfloat16, false);
+  else if (param_dtype == 10 && grad_dtype == 10) HVD_LARS_NORMS(__nv_bfloat16, __nv_bfloat16, false);
+  else if (param_dtype == 6 && grad_dtype == 6) HVD_LARS_NORMS(__half, __half, false);
+  else return cudaErrorInvalidValue;
+#undef HVD_LARS_NORMS
+  return FinalizeNorms(table, n, part, norms, stream);
+}
+
+cudaError_t LaunchLarsApply(const LambTensor* table, int n, int64_t max_count, float lr, float momentum, float weight_decay,
+                            float trust_coefficient, float eps, int adapt, float grad_scale, const float* grad_scale_dev,
+                            const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream) {
+  if (n <= 0 || max_count <= 0) return cudaSuccess;
+  dim3 grid((unsigned)LambPartials(max_count), (unsigned)n);
+#define HVD_LARS_APPLY(P, G, M) fused_lars_apply_kernel<P, G, M><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, grad_scale_dev, norms)
+  if (master) {
+    if (param_dtype == 10 && grad_dtype == 10) HVD_LARS_APPLY(__nv_bfloat16, __nv_bfloat16, true);
+    else if (param_dtype == 6 && grad_dtype == 6) HVD_LARS_APPLY(__half, __half, true);
+    else return cudaErrorInvalidValue;
+  }
+  else if (param_dtype == 7 && grad_dtype == 7) HVD_LARS_APPLY(float, float, false);
+  else if (param_dtype == 7 && grad_dtype == 10) HVD_LARS_APPLY(float, __nv_bfloat16, false);
+  else if (param_dtype == 10 && grad_dtype == 10) HVD_LARS_APPLY(__nv_bfloat16, __nv_bfloat16, false);
+  else if (param_dtype == 6 && grad_dtype == 6) HVD_LARS_APPLY(__half, __half, false);
+  else return cudaErrorInvalidValue;
+#undef HVD_LARS_APPLY
   CountKernelLaunch();
   return cudaGetLastError();
 }

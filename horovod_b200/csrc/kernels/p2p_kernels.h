@@ -205,6 +205,15 @@ cudaError_t LaunchLambNorms(const LambTensor* table, int n, int64_t max_count, f
 cudaError_t LaunchLambApply(const LambTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
                             float bias_c1, float bias_c2, int adapt, const float* norms, int param_dtype, bool master,
                             cudaStream_t stream);
+// Fused LARS on LAMB's table and norms layout, the fp32 momentum buffer in `exp_avg` (`exp_avg_sq` unused): norms[2 * slot]
+// = sum w^2, norms[2 * slot + 1] = sum g^2 of the scaled gradient.  LaunchLarsNorms: two launches, nothing but `partial`
+// and `norms` written.  LaunchLarsApply: v = momentum * v + lr * r * (g + wd * w), w -= v (one launch; reads the gradient
+// again, scaled by grad_scale * *grad_scale_dev as in the first phase).  (param, grad) dtypes and `master` as LAMB's.
+cudaError_t LaunchLarsNorms(const LambTensor* table, int n, int64_t max_count, float grad_scale, const float* grad_scale_dev,
+                            float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
+cudaError_t LaunchLarsApply(const LambTensor* table, int n, int64_t max_count, float lr, float momentum, float weight_decay,
+                            float trust_coefficient, float eps, int adapt, float grad_scale, const float* grad_scale_dev,
+                            const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
 // Gradient statistics of flat gradient shards in one pass (see optim_kernels.cu): optional in-place scaling by
 // *inv_scale, then out[0] += sum of squares (norm_inf: out[0] = max(out[0], max |g|)) and out[1] = max(out[1], non-finite).
 // `partial` / `partial_flag` hold GradShardStatsCtas() entries; `ticket` is a zeroed counter that the kernel leaves zeroed,

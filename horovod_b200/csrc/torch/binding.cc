@@ -612,33 +612,39 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   TORCH_CHECK(e == cudaSuccess, "fused_adam launch failed: ", cudaGetErrorString(e));
 }
 
-// ---- fused LAMB (kern::LaunchLambNorms / LaunchLambApply) ----
-// Checks every argument of one LAMB phase and builds its table: entry i is params[i] with norm slot slots[i] (empty:
-// i) of `norms`, a contiguous fp32 tensor on the params' device with 2 floats per slot.  Zero-size params get no entry.
+// ---- fused LAMB and LARS (kern::LaunchLambNorms / LaunchLambApply, LaunchLarsNorms / LaunchLarsApply) ----
+// Both take one table of kern::LambTensor with a norm slot per entry.  PlanSlotted checks every argument of one phase
+// and builds the table: entry i is params[i] with norm slot slots[i] (empty: i) of `norms`, a contiguous fp32 tensor on
+// the params' device with 2 floats per slot, and each fp32 state list in its field of the entry (fields no list names
+// stay null).  Zero-size params get no entry.
 struct LambPlan {
   std::vector<kern::LambTensor> table;
   int64_t max_count = 0, partials = 0;
   bool master = false;
-  float c1 = 1.f, c2 = 1.f;
+  float c1 = 1.f, c2 = 1.f;  // LAMB's bias corrections
 };
 
-LambPlan PlanLamb(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
-                  const std::vector<at::Tensor>& exp_avg, const std::vector<at::Tensor>& exp_avg_sq,
-                  const std::vector<at::Tensor>& masters, const at::Tensor& norms, const std::vector<int64_t>& slots,
-                  double beta1, double beta2, int64_t step, bool bias_correction) {
-  TORCH_CHECK(params.size() == grads.size() && params.size() == exp_avg.size() && params.size() == exp_avg_sq.size(), op,
-              ": list sizes differ");
+struct SlottedState {
+  const char* name;
+  const std::vector<at::Tensor>& list;
+  void* kern::LambTensor::*field;
+};
+
+LambPlan PlanSlotted(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
+                     const std::vector<SlottedState>& states, const std::vector<at::Tensor>& masters,
+                     const at::Tensor& norms, const std::vector<int64_t>& slots) {
+  bool sizes = params.size() == grads.size();
+  for (const auto& st : states) sizes = sizes && st.list.size() == params.size();
+  TORCH_CHECK(sizes, op, ": list sizes differ");
   TORCH_CHECK(masters.empty() || masters.size() == params.size(), op, ": ", masters.size(), " master params for ",
               params.size(), " params");
   TORCH_CHECK(slots.empty() || slots.size() == params.size(), op, ": ", slots.size(), " slots for ", params.size(), " params");
-  TORCH_CHECK(step >= 1, op, ": step must be >= 1, got ", step);
   LambPlan plan;
   if (params.empty()) return plan;
   for (size_t i = 0; i < params.size(); ++i) {
     CheckOptimizerParam(op, i, params[i], params[0]);
     CheckOptimizerPeer(op, "grads", i, params[i], grads[i], grads[0].scalar_type());
-    CheckOptimizerPeer(op, "exp_avgs", i, params[i], exp_avg[i], at::kFloat);
-    CheckOptimizerPeer(op, "exp_avg_sqs", i, params[i], exp_avg_sq[i], at::kFloat);
+    for (const auto& st : states) CheckOptimizerPeer(op, st.name, i, params[i], st.list[i], at::kFloat);
   }
   plan.master = CheckMasters(op, params, grads, masters);
   TORCH_CHECK(norms.is_cuda() && norms.device() == params[0].device() && norms.scalar_type() == at::kFloat &&
@@ -653,9 +659,9 @@ LambPlan PlanLamb(const char* op, const std::vector<at::Tensor>& params, const s
   }
   for (size_t i = 0; i < params.size(); ++i) {
     if (params[i].numel() == 0) continue;
-    kern::LambTensor t;
+    kern::LambTensor t{};
     t.param = params[i].data_ptr(); t.grad = grads[i].data_ptr();
-    t.exp_avg = exp_avg[i].data_ptr(); t.exp_avg_sq = exp_avg_sq[i].data_ptr();
+    for (const auto& st : states) t.*st.field = st.list[i].data_ptr();
     t.count = params[i].numel();
     t.master = plan.master ? masters[i].data_ptr() : nullptr;
     t.partial = plan.partials;
@@ -664,11 +670,30 @@ LambPlan PlanLamb(const char* op, const std::vector<at::Tensor>& params, const s
     plan.max_count = std::max(plan.max_count, t.count);
     plan.table.push_back(t);
   }
+  return plan;
+}
+
+LambPlan PlanLamb(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
+                  const std::vector<at::Tensor>& exp_avg, const std::vector<at::Tensor>& exp_avg_sq,
+                  const std::vector<at::Tensor>& masters, const at::Tensor& norms, const std::vector<int64_t>& slots,
+                  double beta1, double beta2, int64_t step, bool bias_correction) {
+  TORCH_CHECK(step >= 1, op, ": step must be >= 1, got ", step);
+  LambPlan plan = PlanSlotted(op, params, grads, {{"exp_avgs", exp_avg, &kern::LambTensor::exp_avg},
+                                                  {"exp_avg_sqs", exp_avg_sq, &kern::LambTensor::exp_avg_sq}},
+                              masters, norms, slots);
   if (bias_correction) {
     plan.c1 = 1.0f - (float)std::pow(beta1, (double)step);
     plan.c2 = 1.0f - (float)std::pow(beta2, (double)step);
   }
   return plan;
+}
+
+// LARS keeps one fp32 state, the momentum buffer, in the entry's exp_avg.
+LambPlan PlanLars(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
+                  const std::vector<at::Tensor>& momentum_buffers, const std::vector<at::Tensor>& masters,
+                  const at::Tensor& norms, const std::vector<int64_t>& slots) {
+  return PlanSlotted(op, params, grads, {{"momentum_buffers", momentum_buffers, &kern::LambTensor::exp_avg}}, masters,
+                     norms, slots);
 }
 
 const kern::LambTensor* StageLamb(const char* op, const LambPlan& plan, int device, cudaStream_t s) {
@@ -748,6 +773,80 @@ void FusedLambStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   const auto* dt = StageLamb("fused_lamb", plan, device, s);
   LaunchLambNormsPhase("fused_lamb", plan, dt, params[0], grads[0], beta1, beta2, eps, weight_decay, grad_scale, gsd, norms, s);
   LaunchLambApplyPhase("fused_lamb", plan, dt, params[0], lr, eps, weight_decay, adapt, norms, s);
+}
+
+void LaunchLarsNormsPhase(const char* op, const LambPlan& plan, const kern::LambTensor* dt, const at::Tensor& param0,
+                          const at::Tensor& grad0, double grad_scale, const float* gsd, at::Tensor& norms, cudaStream_t s) {
+  // stream-ordered scratch from torch's caching allocator: one (sum w^2, sum g^2) pair per stage-1 CTA
+  at::Tensor work = at::empty({2 * plan.partials}, norms.options());
+  cudaError_t e = kern::LaunchLarsNorms(dt, (int)plan.table.size(), plan.max_count, (float)grad_scale, gsd,
+                                        work.data_ptr<float>(), norms.data_ptr<float>(), (int)MapDtype(param0.scalar_type()),
+                                        (int)MapDtype(grad0.scalar_type()), plan.master, s);
+  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+}
+
+void LaunchLarsApplyPhase(const char* op, const LambPlan& plan, const kern::LambTensor* dt, const at::Tensor& param0,
+                          const at::Tensor& grad0, double lr, double momentum, double weight_decay, double trust_coefficient,
+                          double eps, bool adapt, double grad_scale, const float* gsd, const at::Tensor& norms,
+                          cudaStream_t s) {
+  cudaError_t e = kern::LaunchLarsApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)momentum,
+                                        (float)weight_decay, (float)trust_coefficient, (float)eps, adapt ? 1 : 0,
+                                        (float)grad_scale, gsd, norms.data_ptr<float>(), (int)MapDtype(param0.scalar_type()),
+                                        (int)MapDtype(grad0.scalar_type()), plan.master, s);
+  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+}
+
+// LARS phase 1: the squared norms of every entry's parameter and scaled gradient ADDED into norms[2 * slot],
+// norms[2 * slot + 1].  The momentum buffers are checked like phase 2's, not read.
+void LarsNorms(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momentum_buffers,
+               double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters, at::Tensor out,
+               std::vector<int64_t> slots) {
+  LambPlan plan = PlanLars("lars_norms", params, grads, momentum_buffers, masters, out, slots);
+  if (params.empty()) return;
+  const float* gsd = DeviceScalar("lars_norms", "grad_scale_dev", grad_scale_dev, params[0]);
+  if (plan.table.empty()) return;
+  int device = (int)params[0].get_device();
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
+  const auto* dt = StageLamb("lars_norms", plan, device, s);
+  LaunchLarsNormsPhase("lars_norms", plan, dt, params[0], grads[0], grad_scale, gsd, out, s);
+}
+
+// LARS phase 2: momentum and parameter update with r from the (allreduced) norms; reads the gradient again, scaled the
+// same way as in phase 1.
+void LarsApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momentum_buffers,
+               double lr, double momentum, double weight_decay, double trust_coefficient, double eps, bool adapt,
+               double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters,
+               at::Tensor norms, std::vector<int64_t> slots) {
+  LambPlan plan = PlanLars("lars_apply", params, grads, momentum_buffers, masters, norms, slots);
+  if (params.empty()) return;
+  const float* gsd = DeviceScalar("lars_apply", "grad_scale_dev", grad_scale_dev, params[0]);
+  if (plan.table.empty()) return;
+  int device = (int)params[0].get_device();
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
+  const auto* dt = StageLamb("lars_apply", plan, device, s);
+  LaunchLarsApplyPhase("lars_apply", plan, dt, params[0], grads[0], lr, momentum, weight_decay, trust_coefficient, eps,
+                       adapt, grad_scale, gsd, norms, s);
+}
+
+// Both LARS phases on one device with a fresh norms buffer (slot i = params[i]): three launches, one staged table.
+void FusedLarsStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momentum_buffers,
+                   double lr, double momentum, double weight_decay, double trust_coefficient, double eps, bool adapt,
+                   double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
+  TORCH_CHECK(params.empty() || params[0].is_cuda(), "fused_lars: params[0] must be a dense CUDA tensor");
+  at::Tensor norms = params.empty() ? at::Tensor() : at::zeros({2 * (int64_t)params.size()}, params[0].options().dtype(at::kFloat));
+  LambPlan plan = PlanLars("fused_lars", params, grads, momentum_buffers, masters, norms, {});
+  if (params.empty()) return;
+  const float* gsd = DeviceScalar("fused_lars", "grad_scale_dev", grad_scale_dev, params[0]);
+  if (plan.table.empty()) return;
+  int device = (int)params[0].get_device();
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
+  const auto* dt = StageLamb("fused_lars", plan, device, s);
+  LaunchLarsNormsPhase("fused_lars", plan, dt, params[0], grads[0], grad_scale, gsd, norms, s);
+  LaunchLarsApplyPhase("fused_lars", plan, dt, params[0], grads[0], lr, momentum, weight_decay, trust_coefficient, eps,
+                       adapt, grad_scale, gsd, norms, s);
 }
 
 // The stats kernel's last-CTA ticket: one zeroed counter per (device, stream), which every launch leaves zeroed again.
@@ -1045,6 +1144,14 @@ PYBIND11_MODULE(_hvd_torch, m) {
   m.def("lamb_apply", &LambApply, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
         py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
         py::arg("bias_correction"), py::arg("adapt"), py::arg("master_params"), py::arg("norms"), py::arg("slots"));
+  m.def("fused_lars_step", &FusedLarsStep, py::arg("params"), py::arg("grads"), py::arg("momentum_buffers"), py::arg("lr"),
+        py::arg("momentum"), py::arg("weight_decay"), py::arg("trust_coefficient"), py::arg("eps"), py::arg("adapt"),
+        py::arg("grad_scale"), py::arg("grad_scale_dev") = py::none(), py::arg("master_params") = std::vector<at::Tensor>());
+  m.def("lars_norms", &LarsNorms, py::arg("params"), py::arg("grads"), py::arg("momentum_buffers"), py::arg("grad_scale"),
+        py::arg("grad_scale_dev"), py::arg("master_params"), py::arg("out"), py::arg("slots"));
+  m.def("lars_apply", &LarsApply, py::arg("params"), py::arg("grads"), py::arg("momentum_buffers"), py::arg("lr"),
+        py::arg("momentum"), py::arg("weight_decay"), py::arg("trust_coefficient"), py::arg("eps"), py::arg("adapt"),
+        py::arg("grad_scale"), py::arg("grad_scale_dev"), py::arg("master_params"), py::arg("norms"), py::arg("slots"));
   m.def("grad_shard_stats", &GradShardStats, py::arg("grads"), py::arg("out"), py::arg("inv_scale") = py::none(),
         py::arg("norm_inf") = false);
   m.def("sync_bn_stats", &SyncBnStats, py::arg("x"), py::arg("slot"));

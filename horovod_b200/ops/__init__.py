@@ -3,6 +3,8 @@
 * `fused_sgd_step`, `fused_adam_step` — multi-tensor optimizer kernels (`csrc/kernels/optim_kernels.cu`);
 * `fused_lamb_step`, and its two phases `lamb_norms` / `lamb_apply` — multi-tensor LAMB with per-tensor trust ratios
   (same file);
+* `fused_lars_step`, and its two phases `lars_norms` / `lars_apply` — multi-tensor LARS on LAMB's table and norms
+  layout (same file);
 * `grad_shard_stats` — one-pass gradient norm statistics, non-finite check and optional in-place unscale (same file);
 * `sync_bn_stats`, `sync_bn_combine`, `sync_bn_elemt`, `sync_bn_backward_reduce`, `sync_bn_backward_elemt` — the
   kernels of hvd.SyncBatchNorm's native path (`csrc/kernels/sync_bn_kernels.cu`);
@@ -82,6 +84,42 @@ def lamb_apply(params, grads, exp_avgs, exp_avg_sqs, lr, beta1, beta2, eps, weig
     return _native().lamb_apply(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1),
                                 float(beta2), float(eps), float(weight_decay), int(step), bool(bias_correction),
                                 bool(adapt), list(master_params or []), norms,
+                                list(range(n)) if slots is None else [int(s) for s in slots])
+
+
+def fused_lars_step(params, grads, momentum_buffers, lr, momentum=0.9, weight_decay=0.0, trust_coefficient=0.001, eps=0.0,
+                    adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None):
+    """One LARS step for the whole parameter list in three launches (per-CTA norm partials, the per-tensor norms, the
+    update), with the argument rules of fused_adam_step; the momentum buffers are fp32. For each parameter w:
+
+        g = grad * grad_scale [* grad_scale_dev[0]];  d = g + weight_decay * w
+        r = trust_coefficient * ||w|| / (||g|| + weight_decay * ||w|| + eps) if adapt and both norms are > 0, else 1
+        v = momentum * v + lr * r * d;  w -= v
+
+    Deterministic: the same input gives the same bits on every call. Nothing is synchronised with the host."""
+    return _native().fused_lars_step(list(params), list(grads), list(momentum_buffers), float(lr), float(momentum),
+                                     float(weight_decay), float(trust_coefficient), float(eps), bool(adapt),
+                                     float(grad_scale), grad_scale_dev, list(master_params or []))
+
+
+def lars_norms(params, grads, momentum_buffers, out, slots=None, grad_scale=1.0, grad_scale_dev=None, master_params=None):
+    """First phase of fused_lars_step, for parameters split into pieces (e.g. over the ranks' shards): ADDS each piece's
+    sum of w^2 and of g^2 (g scaled as in fused_lars_step) into out[2 * slot] and out[2 * slot + 1], with lamb_norms'
+    rules for `out` and `slots`. The momentum buffers are checked as in lars_apply but not read. Two launches."""
+    n = len(params)
+    return _native().lars_norms(list(params), list(grads), list(momentum_buffers), float(grad_scale), grad_scale_dev,
+                                list(master_params or []), out, list(range(n)) if slots is None else [int(s) for s in slots])
+
+
+def lars_apply(params, grads, momentum_buffers, lr, momentum, weight_decay, trust_coefficient, eps, norms, slots=None,
+               adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None):
+    """Second phase: the momentum and parameter update of fused_lars_step, with r from the whole-tensor sums of squares
+    in `norms` (e.g. after adding up every rank's pieces). Reads the gradient again: pass the grad_scale /
+    grad_scale_dev of lars_norms. One launch."""
+    n = len(params)
+    return _native().lars_apply(list(params), list(grads), list(momentum_buffers), float(lr), float(momentum),
+                                float(weight_decay), float(trust_coefficient), float(eps), bool(adapt), float(grad_scale),
+                                grad_scale_dev, list(master_params or []), norms,
                                 list(range(n)) if slots is None else [int(s) for s in slots])
 
 

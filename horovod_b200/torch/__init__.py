@@ -22,6 +22,7 @@ from horovod_b200.torch.mpi_ops import (  # noqa: F401
 from horovod_b200.torch.functions import (broadcast_parameters, broadcast_optimizer_state, broadcast_object,  # noqa: F401
                                           allgather_object)
 from horovod_b200.torch.lamb import Lamb  # noqa: F401
+from horovod_b200.torch.lars import Lars  # noqa: F401
 from horovod_b200.torch.optimizer import DistributedOptimizer  # noqa: F401
 from horovod_b200.torch.sharded_optimizer import ShardedGradScaler  # noqa: F401
 from horovod_b200.torch.sync_batch_norm import SyncBatchNorm  # noqa: F401

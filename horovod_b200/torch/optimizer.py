@@ -20,6 +20,7 @@ from horovod_b200.common.util import split_list
 from horovod_b200.torch import mpi_ops
 from horovod_b200.torch.compression import Compression
 from horovod_b200.torch.lamb import Lamb
+from horovod_b200.torch.lars import Lars
 from horovod_b200.torch.mpi_ops import (Adasum, Average, Sum, allreduce_async_, grouped_allreduce_async_, rank, size,
                                         synchronize)
 
@@ -119,16 +120,18 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         for p in self._allreduce_delay:
             self._allreduce_delay[p] = self.backward_passes_per_step
         super(self.__class__, self).load_state_dict(*args, **kwargs)
-        if self._fused and (isinstance(self, (torch.optim.Adam, torch.optim.AdamW, Lamb)) or self._master_weights):
+        if self._fused and (isinstance(self, (torch.optim.Adam, torch.optim.AdamW, Lamb, Lars)) or self._master_weights):
             self._keep_fp32_moments(args[0] if args else kwargs['state_dict'])
 
     def _keep_fp32_moments(self, state_dict):
         """torch casts every loaded floating state tensor to its parameter's dtype. The fused Adam and LAMB kernels keep
-        fp32 moments for bf16 / fp16 parameters too, and with master weights the fp32 master copy and SGD momentum, so take
-        the checkpoint's fp32 values back: a checkpoint round-trips exactly instead of losing their low bits."""
+        fp32 moments for bf16 / fp16 parameters too, the LARS kernels fp32 momentum, and with master weights the fp32
+        master copy and SGD momentum, so take the checkpoint's fp32 values back: a checkpoint round-trips exactly instead
+        of losing their low bits."""
         saved = [i for g in state_dict['param_groups'] for i in g['params']]
         params = [p for g in self.param_groups for p in g['params']]
-        keys = ('exp_avg', 'exp_avg_sq') + (('master_param', 'momentum_buffer') if self._master_weights else ())
+        keys = ('exp_avg', 'exp_avg_sq') + (('master_param', 'momentum_buffer') if self._master_weights else
+                                            ('momentum_buffer',) if isinstance(self, Lars) else ())
         for pid, p in zip(saved, params):
             st = state_dict['state'].get(pid, {})
             for key in keys:
@@ -590,8 +593,8 @@ def _fused_plan(opt, why=None):
     master = getattr(opt, '_master_weights', False)
     is_sgd = isinstance(opt, torch.optim.SGD)
     is_adam = isinstance(opt, (torch.optim.Adam, torch.optim.AdamW))
-    if not (is_sgd or is_adam or isinstance(opt, Lamb)):
-        return no('the optimizer is %s, not SGD, Adam or AdamW, or hvd.Lamb' % type(opt).__name__)
+    if not (is_sgd or is_adam or isinstance(opt, (Lamb, Lars))):
+        return no('the optimizer is %s, not SGD, Adam or AdamW, or hvd.Lamb or hvd.Lars' % type(opt).__name__)
     grad_of = getattr(opt, '_grad_for_update', lambda q: q.grad)
     plan = []
     for group in opt.param_groups:
@@ -632,8 +635,8 @@ def _master_param(opt, p):
 
 def _fused_step(opt):
     """One multi-tensor kernel for the whole model when the wrapped optimizer is SGD or Adam/AdamW on CUDA, three for
-    Lamb (its trust ratios need whole-tensor norms before the update). With master weights a plan that cannot be fused
-    raises RuntimeError instead of returning False."""
+    Lamb and Lars (their trust ratios need whole-tensor norms before the update). With master weights a plan that cannot
+    be fused raises RuntimeError instead of returning False."""
     native = mpi_ops._native()
     use_master = getattr(opt, '_master_weights', False)
     why = []
@@ -674,6 +677,22 @@ def _fused_step(opt):
                     native.fused_sgd_step(pick(ps), pick(grads), pick(bufs), float(group['lr']), float(mom),
                                           float(group.get('dampening', 0.0)), float(group.get('weight_decay', 0.0)),
                                           bool(group.get('nesterov', False)), 1.0, bool(fresh) and fresh[idx[0]], **kw)
+            elif isinstance(opt, Lars):
+                # fp32 momentum that starts at zero: one launch set per (group, dtype), no first-step special case
+                bufs = []
+                for p in ps:
+                    st = opt.state[p]
+                    buf = st.get('momentum_buffer')
+                    if buf is None:
+                        buf = st['momentum_buffer'] = torch.zeros_like(p, dtype=torch.float32,
+                                                                       memory_format=torch.preserve_format)
+                    elif buf.dtype != torch.float32 or buf.stride() != p.stride():
+                        buf = st['momentum_buffer'] = _state_like(p, buf, torch.float32)
+                    bufs.append(buf)
+                kw = {'master_params': masters} if master else {}
+                native.fused_lars_step(ps, grads, bufs, float(group['lr']), float(group['momentum']),
+                                       float(group['weight_decay']), float(group['trust_coefficient']), float(group['eps']),
+                                       Lars.adapts(group), 1.0, **kw)
             else:
                 exp_avg, exp_avg_sq, steps = [], [], []
                 for p in ps:
@@ -900,22 +919,23 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
 
     `shard_optimizer_state=True` (new, ZeRO stage 1) keeps the optimizer state of 1/N of the parameters on each of the N
     ranks: gradients are reduce-scattered, each rank updates its shard with the fused kernel and the parameters are
-    allgathered (see horovod_b200/torch/sharded_optimizer.py).  SGD / Adam / AdamW / Lamb with op Average or Sum on one host;
-    raises ValueError otherwise.  The sharded update always runs the fused kernel, whatever `fused` says.  With one
+    allgathered (see horovod_b200/torch/sharded_optimizer.py).  SGD / Adam / AdamW / Lamb / Lars with op Average or Sum
+    on one host; raises ValueError otherwise.  The sharded update always runs the fused kernel, whatever `fused` says.  With one
     rank it is the ordinary optimizer.
 
     `master_weights=True` (new) gives every bf16 / fp16 trainable parameter an fp32 master copy, held as optimizer state
     ('master_param', sharded like the moments with shard_optimizer_state): the update runs in fp32 on the master and the
     parameter receives it rounded to nearest-even, so updates smaller than half an ulp of the parameter are not lost.
-    SGD momentum is then fp32 as well.  fp32 parameters are unaffected.  Implies fused=True; SGD / Adam / AdamW / Lamb only,
-    without maximize, amsgrad or op=Adasum (ValueError).  A parameter written from outside the optimizer
+    SGD momentum is then fp32 as well.  fp32 parameters are unaffected.  Implies fused=True; SGD / Adam / AdamW / Lamb /
+    Lars only, without maximize, amsgrad or op=Adasum (ValueError).  A parameter written from outside the optimizer
     (load_state_dict, broadcast_parameters, an in-place edit) is picked up by the next step: where it no longer equals
     its rounded master, the master restarts from it."""
     if master_weights:
         if op == Adasum:
             raise ValueError('master_weights is not supported with op=Adasum')
-        if not isinstance(optimizer, (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW, Lamb)):
-            raise ValueError('master_weights supports SGD, Adam and AdamW, and hvd.Lamb, only, not %s' % type(optimizer).__name__)
+        if not isinstance(optimizer, (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW, Lamb, Lars)):
+            raise ValueError('master_weights supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
+                             % type(optimizer).__name__)
         for g in optimizer.param_groups:
             if g.get('maximize', False) or g.get('amsgrad', False):
                 raise ValueError('master_weights does not support maximize=True or amsgrad=True')

@@ -11,9 +11,9 @@ optimizer state for that shard only.  A step is
 which moves the same NVLink bytes as the allreduce it replaces, while the update does 1/N of the work and the state
 takes 1/N of the memory.  The allgather runs after the update and does not overlap backward.
 
-LAMB (hvd.Lamb) needs the norms of whole parameters, which the shards cut at arbitrary elements: its update is split
-into lamb_norms over the owned pieces, one allreduce of a small registered buffer of per-parameter sums of squares,
-and lamb_apply, so every rank computes each trust ratio from the same bits.
+LAMB (hvd.Lamb) and LARS (hvd.Lars) need the norms of whole parameters, which the shards cut at arbitrary elements:
+their update is split into lamb_norms / lars_norms over the owned pieces, one allreduce of a small registered buffer of
+per-parameter sums of squares, and lamb_apply / lars_apply, so every rank computes each trust ratio from the same bits.
 
 Global-norm clipping (`clip_grad_norm_`) and AMP loss scaling (`ShardedGradScaler`) read only the owned shards: one
 statistics kernel per gradient dtype and one scalar allreduce give every rank the same norm and the same inf / NaN
@@ -33,6 +33,7 @@ from horovod_b200.common.process_sets import global_process_set
 from horovod_b200.torch import mpi_ops
 from horovod_b200.torch.compression import Compression
 from horovod_b200.torch.lamb import Lamb
+from horovod_b200.torch.lars import Lars
 from horovod_b200.torch.mpi_ops import Average, Sum
 from horovod_b200.torch.optimizer import _find_duplicates
 
@@ -132,7 +133,8 @@ def full_from_shards(bucket, shards, shapes, strides=None):
 
 
 class _ShardedDistributedOptimizer(torch.optim.Optimizer):
-    """Wraps SGD / Adam / AdamW / Lamb so that every rank keeps optimizer state for 1/N of the parameters (ZeRO stage 1).
+    """Wraps SGD / Adam / AdamW / Lamb / Lars so that every rank keeps optimizer state for 1/N of the parameters (ZeRO
+    stage 1).
     Built by `hvd.DistributedOptimizer(opt, shard_optimizer_state=True)`; the dynamic class derives from this one and from
     the wrapped optimizer's class."""
 
@@ -146,8 +148,10 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             kind = 'adam'
         elif isinstance(self, Lamb):
             kind = 'lamb'
+        elif isinstance(self, Lars):
+            kind = 'lars'
         else:
-            raise ValueError('shard_optimizer_state supports SGD, Adam and AdamW, and hvd.Lamb, only, not %s'
+            raise ValueError('shard_optimizer_state supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
                              % type(self).__name__)
         for g in self.param_groups:
             if g.get('maximize', False) or (kind == 'adam' and g.get('amsgrad', False)):
@@ -223,6 +227,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                     b['state'] = {'momentum_buffer': torch.zeros(b['shard'], dtype=torch.float32 if master else b['dtype'],
                                                                  device=device)} \
                         if self.param_groups[b['group']].get('momentum', 0.0) != 0.0 else {}
+                elif kind == 'lars':
+                    b['state'] = {'momentum_buffer': torch.zeros(b['shard'], dtype=torch.float32, device=device)}
                 else:
                     b['state'] = {'exp_avg': torch.zeros(b['shard'], dtype=torch.float32, device=device),
                                   'exp_avg_sq': torch.zeros(b['shard'], dtype=torch.float32, device=device)}
@@ -236,9 +242,10 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                                          process_set=process_set)
         self._stats.zero_()
         self._lamb_norms = None
-        if kind == 'lamb':
-            # LAMB's whole-parameter (sum w^2, sum u^2) in slot = the parameter's index in param_groups order: every rank
-            # adds the pieces of its own shards and one allreduce sums them.  Padded like _stats.
+        if kind in ('lamb', 'lars'):
+            # the whole-parameter sums of squares of LAMB (w, u) or LARS (w, g) in slot = the parameter's index in
+            # param_groups order: every rank adds the pieces of its own shards and one allreduce sums them.  Padded like
+            # _stats.  (Named for LAMB, which came first.)
             self._slot = {p: i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
             unit = ALIGN // 4 * self._nranks
             self._lamb_norms = mpi_ops.symm_empty((2 * len(self._slot) + unit - 1) // unit * unit, dtype=torch.float32,
@@ -418,8 +425,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         for b in self._buckets:
             by_group.setdefault((b['group'], b['dtype']), []).append(b)
         with torch.no_grad():
-            if self._kind == 'lamb':
-                self._update_shards_lamb(by_group, coef)
+            if self._kind in ('lamb', 'lars'):
+                self._update_shards_trust(by_group, coef)
                 return
             for (gi, _), bs in by_group.items():
                 group = self.param_groups[gi]
@@ -446,39 +453,53 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 for b in bs:
                     b['stepped'] = True
 
-    def _update_shards_lamb(self, by_group, coef):
-        """LAMB's trust ratio needs the norms of whole parameters, which the shards cut at arbitrary elements.  One table
-        entry per parameter piece in this rank's shards, in the slot of its parameter: lamb_norms per (group, dtype)
-        adds the pieces' sums of squares into the registered norms buffer, one allreduce sums them over the ranks, and
-        lamb_apply per (group, dtype) updates the pieces with the same r on every rank.  Padding is not touched."""
+    def _update_shards_trust(self, by_group, coef):
+        """The trust ratios of LAMB and LARS need the norms of whole parameters, which the shards cut at arbitrary
+        elements.  One table entry per parameter piece in this rank's shards, in the slot of its parameter: the norms
+        phase per (group, dtype) adds the pieces' sums of squares into the registered norms buffer, one allreduce sums
+        them over the ranks, and the apply phase per (group, dtype) updates the pieces with the same r on every rank.
+        The clip coefficient reaches the phases that read the gradient.  Padding is not touched."""
         native = mpi_ops._native()
+        lamb = self._kind == 'lamb'
+        keys = ('exp_avg', 'exp_avg_sq') if lamb else ('momentum_buffer',)
         calls = []
         for (gi, _), bs in by_group.items():
             group = self.param_groups[gi]
-            lists, masters, slots = ([], [], [], []), [], []
+            lists, masters, slots = tuple([] for _ in range(2 + len(keys))), [], []
             for b in bs:
                 st = b['state']
                 b['step'] += 1
                 b['stepped'] = True
+                if not lamb:
+                    b['mom_init'] = True  # LARS momentum: state_dict() gathers it from now on
                 for k, plo, phi, slo in shard_slices(b, self._rank):
                     cut = slice(slo, slo + phi - plo)
-                    for out, t in zip(lists, (b['pshard'], b['gshard'], st['exp_avg'], st['exp_avg_sq'])):
+                    for out, t in zip(lists, (b['pshard'], b['gshard']) + tuple(st[key] for key in keys)):
                         out.append(t[cut])
                     if 'master_param' in st:
                         masters.append(st['master_param'][cut])
                     slots.append(self._slot[b['params'][k]])
             calls.append((group, bs[0]['step'], lists, masters, slots))
-        self._lamb_norms.zero_()
+        norms = self._lamb_norms
+        norms.zero_()
         for group, step, lists, masters, slots in calls:
-            b1, b2 = group['betas']
-            native.lamb_norms(*lists, float(b1), float(b2), float(group['eps']), float(group['weight_decay']), step,
-                              bool(group['bias_correction']), 1.0, coef, masters, self._lamb_norms, slots)
-        mpi_ops.captured_allreduce_(self._lamb_norms, op=Sum, process_set=self.process_set)
+            if lamb:
+                b1, b2 = group['betas']
+                native.lamb_norms(*lists, float(b1), float(b2), float(group['eps']), float(group['weight_decay']), step,
+                                  bool(group['bias_correction']), 1.0, coef, masters, norms, slots)
+            else:
+                native.lars_norms(*lists, 1.0, coef, masters, norms, slots)
+        mpi_ops.captured_allreduce_(norms, op=Sum, process_set=self.process_set)
         for group, step, lists, masters, slots in calls:
-            b1, b2 = group['betas']
-            native.lamb_apply(*lists, float(group['lr']), float(b1), float(b2), float(group['eps']),
-                              float(group['weight_decay']), step, bool(group['bias_correction']), Lamb.adapts(group),
-                              masters, self._lamb_norms, slots)
+            if lamb:
+                b1, b2 = group['betas']
+                native.lamb_apply(*lists, float(group['lr']), float(b1), float(b2), float(group['eps']),
+                                  float(group['weight_decay']), step, bool(group['bias_correction']), Lamb.adapts(group),
+                                  masters, norms, slots)
+            else:
+                native.lars_apply(*lists, float(group['lr']), float(group['momentum']), float(group['weight_decay']),
+                                  float(group['trust_coefficient']), float(group['eps']), Lars.adapts(group), 1.0, coef,
+                                  masters, norms, slots)
 
     def _allgather_params(self):
         comm = self._comm
@@ -553,16 +574,16 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         index = {id(p): i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
         state = {}
         for b in self._buckets:
-            if not b['state'] or ((b['step'] == 0) if self._kind != 'sgd' else
+            if not b['state'] or ((b['step'] == 0) if self._kind in ('adam', 'lamb') else
                                   not (b['mom_init'] or ('master_param' in b['state'] and b['stepped']))):
-                continue  # no state yet (the same on every rank); a plain-SGD bucket may still hold masters
+                continue  # no state yet (the same on every rank); an SGD / LARS bucket may still hold masters only
             gathered = {}
             for key, shard in b['state'].items():
                 full = mpi_ops.allgather(shard, name='sharded_opt.state.%d.%s' % (b['index'], key), process_set=self.process_set)
                 gathered[key] = full_from_shards(b, [full], [p.shape for p in b['params']], [p.stride() for p in b['params']])
             for k, p in enumerate(b['params']):
                 st = {key: vals[k].detach().cpu().clone() for key, vals in gathered.items()}
-                if self._kind != 'sgd':
+                if self._kind in ('adam', 'lamb'):
                     st['step'] = torch.tensor(float(b['step']))
                 state[index[id(p)]] = st
         sd['state'] = state
