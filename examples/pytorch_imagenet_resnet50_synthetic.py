@@ -116,13 +116,15 @@ class Synthetic:
 
 
 def loss_fn(x, y):
+    """The loss of one micro-batch, divided by the number of micro-batches per optimizer step."""
     if cuda:
         x = x.contiguous(memory_format=torch.channels_last)
     with torch.autocast('cuda', dtype=torch.bfloat16, enabled=cuda):
-        return F.cross_entropy(model(x), y)
+        return F.cross_entropy(model(x), y) / args.batches_per_allreduce
 
 
-use_graph = cuda and not args.no_graph and args.batches_per_allreduce == 1 and args.compression == 'none'
+# GraphedStep: one call per micro-batch; the optimizer steps after every batches_per_allreduce-th call
+use_graph = cuda and not args.no_graph and args.compression == 'none'
 step_fn = None
 average = MetricAverage(device=dev if cuda else None)
 for epoch in range(resume_epoch, args.epochs):
@@ -133,15 +135,20 @@ for epoch in range(resume_epoch, args.epochs):
     for step in range(args.steps_per_epoch):
         adjust_lr(epoch, step)
         if use_graph:
-            x, y = next(it)
-            if step_fn is None:
-                step_fn = hvd.GraphedStep(loss_fn, opt, (x, y))
-            loss = step_fn(x, y)
+            for _ in range(args.batches_per_allreduce):
+                x, y = next(it)
+                if step_fn is None:
+                    step_fn = hvd.GraphedStep(loss_fn, opt, (x, y))
+                    if verbose:
+                        print('GraphedStep: captured %s, comm_in_graph %s, backward_passes_per_step %d%s'
+                              % (step_fn.captured, step_fn.comm_in_graph, step_fn.k,
+                                 '' if step_fn.captured else ' (%s)' % step_fn.fallback_reason), flush=True)
+                loss = step_fn(x, y)
         else:
             opt.zero_grad()
             for _ in range(args.batches_per_allreduce):
                 x, y = next(it)
-                loss = loss_fn(x, y) / args.batches_per_allreduce
+                loss = loss_fn(x, y)
                 loss.backward()
             opt.step()
         total += float(loss.detach())

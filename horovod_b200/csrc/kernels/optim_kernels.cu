@@ -492,6 +492,44 @@ grad_shard_stats_kernel(const StatTensor* __restrict__ table, const float* __res
   }
 }
 
+// Gradient accumulation in fp32 for bf16 / fp16 gradients: every table entry pairs a 16-bit gradient g with an fp32
+// accumulator of the same element order.  kAccFirst: acc = g, g = 0.  kAccAdd: acc += g, g = 0.  kAccLast: g = acc + g
+// rounded to nearest-even once (acc is not written).  Each element is one fp32 add at most, so the result is that of the
+// same torch ops in fp32, bit for bit; inf / NaN propagate.  The table travels as a kernel parameter, so a launch
+// captured into a CUDA graph keeps its own copy.
+template <typename G>
+__global__ void __launch_bounds__(kOptThreads)
+grad_accumulate_kernel(const AccTable table, int mode) {
+  const AccTensor t = table.t[blockIdx.y];
+  const int64_t n = t.count;
+  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  if (base >= n) return;
+  G* g = reinterpret_cast<G*>(t.grad);
+  float* acc = t.acc;
+  const bool ga = is_aligned<G>(g), aa = is_aligned<float>(acc);
+#pragma unroll
+  for (int it = 0; it < kOptIters; ++it) {
+    const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
+    if (i >= n) break;
+    float gv[kOptVec], av[kOptVec];
+    load4<G>(g, i, n, ga, gv);
+    if (mode == kAccFirst) {
+      store4<float>(acc, i, n, aa, gv);
+    } else {
+      load4<float>(acc, i, n, aa, av);
+#pragma unroll
+      for (int k = 0; k < kOptVec; ++k) av[k] += gv[k];
+      if (mode == kAccLast) {
+        store4<G>(g, i, n, ga, av);
+        continue;
+      }
+      store4<float>(acc, i, n, aa, av);
+    }
+    const float zero[kOptVec] = {0.f, 0.f, 0.f, 0.f};
+    store4<G>(g, i, n, ga, zero);
+  }
+}
+
 }  // namespace
 
 cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
@@ -639,6 +677,17 @@ cudaError_t LaunchGradShardStats(const StatTensor* table, int n, int64_t max_cou
   if (grad_dtype == 7) grad_shard_stats_kernel<float><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
   else if (grad_dtype == 10) grad_shard_stats_kernel<__nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
   else if (grad_dtype == 6) grad_shard_stats_kernel<__half><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
+  else return cudaErrorInvalidValue;
+  CountKernelLaunch();
+  return cudaGetLastError();
+}
+
+cudaError_t LaunchGradAccumulate(const AccTable& table, int64_t max_count, int mode, int grad_dtype, cudaStream_t stream) {
+  if (table.n <= 0 || max_count <= 0) return cudaSuccess;
+  if (table.n > kAccMaxTensors || mode < kAccFirst || mode > kAccLast) return cudaErrorInvalidValue;
+  dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)table.n);
+  if (grad_dtype == 10) grad_accumulate_kernel<__nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, mode);
+  else if (grad_dtype == 6) grad_accumulate_kernel<__half><<<grid, kOptThreads, 0, stream>>>(table, mode);
   else return cudaErrorInvalidValue;
   CountKernelLaunch();
   return cudaGetLastError();

@@ -223,6 +223,15 @@ int64_t GradShardStatsCtas(int n, int64_t max_count);
 cudaError_t LaunchGradShardStats(const StatTensor* table, int n, int64_t max_count, const float* inv_scale, int norm_inf,
                                  float* partial, int* partial_flag, unsigned* ticket, float* out, int grad_dtype,
                                  cudaStream_t stream);
+// Gradient accumulation in fp32 (see optim_kernels.cu): `grad` is bf16 / fp16 (grad_dtype, one per launch), `acc` fp32
+// with the same element order.  kAccFirst: acc = g, g = 0; kAccAdd: acc += g, g = 0; kAccLast: g = round(acc + g).  The
+// table is passed by value (under the 4 KB kernel-parameter limit), so one launch covers at most kAccMaxTensors entries
+// and the launch can be captured into a CUDA graph.  No atomics, no state between launches.
+enum AccMode : int { kAccFirst = 0, kAccAdd = 1, kAccLast = 2 };
+constexpr int kAccMaxTensors = 160;
+struct AccTensor { void* grad; float* acc; int64_t count; };
+struct AccTable { AccTensor t[kAccMaxTensors]; int n; };
+cudaError_t LaunchGradAccumulate(const AccTable& table, int64_t max_count, int mode, int grad_dtype, cudaStream_t stream);
 
 // Batch normalization over the ranks of a process set (see sync_bn_kernels.cu).  An input with channels at dim 1 is
 // viewed as rows [M, C] with C innermost (channels_last, [N, C], spatial size 1) or planes [M, C, L] (contiguous NCHW).

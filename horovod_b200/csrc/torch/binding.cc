@@ -906,6 +906,50 @@ void GradShardStats(std::vector<at::Tensor> grads, at::Tensor out, c10::optional
   TORCH_CHECK(e == cudaSuccess, "grad_shard_stats launch failed: ", cudaGetErrorString(e));
 }
 
+// Fold bf16 / fp16 gradients into fp32 accumulators (kern::LaunchGradAccumulate): mode 0 first, 1 add, 2 last.  Every
+// argument is checked before anything is launched; one launch per kAccMaxTensors non-empty entries, on the current stream,
+// with the table as a kernel parameter, so the call can be captured into a CUDA graph.
+void GradAccumulate(std::vector<at::Tensor> grads, std::vector<at::Tensor> accs, int64_t mode) {
+  TORCH_CHECK(mode >= kern::kAccFirst && mode <= kern::kAccLast, "grad_accumulate: mode must be 0 (first), 1 (add) or 2 "
+              "(last), got ", mode);
+  TORCH_CHECK(grads.size() == accs.size(), "grad_accumulate: ", grads.size(), " gradients but ", accs.size(), " accumulators");
+  if (grads.empty()) return;
+  const auto st = grads[0].scalar_type();
+  TORCH_CHECK(st == at::kBFloat16 || st == at::kHalf, "grad_accumulate: gradients must be bfloat16 or float16, got ", st);
+  for (size_t i = 0; i < grads.size(); ++i) {
+    const at::Tensor& g = grads[i];
+    const at::Tensor& a = accs[i];
+    TORCH_CHECK(g.is_cuda() && g.is_non_overlapping_and_dense(), "grad_accumulate: grads[", i, "] must be a dense CUDA tensor");
+    TORCH_CHECK(g.scalar_type() == st, "grad_accumulate: grads[", i, "] is ", g.scalar_type(), ", grads[0] is ", st,
+                " (one dtype per call)");
+    TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kFloat, "grad_accumulate: accs[", i, "] must be a float32 CUDA tensor");
+    TORCH_CHECK(a.device() == grads[0].device() && g.device() == grads[0].device(), "grad_accumulate: entry ", i,
+                " is not on ", grads[0].device());
+    TORCH_CHECK(a.sizes() == g.sizes() && a.strides() == g.strides(), "grad_accumulate: accs[", i,
+                "] must have the shape and strides of grads[", i, "]");
+  }
+  std::vector<kern::AccTensor> entries;
+  int64_t maxc = 0;
+  for (size_t i = 0; i < grads.size(); ++i) {
+    if (grads[i].numel() == 0) continue;
+    entries.push_back({grads[i].data_ptr(), accs[i].data_ptr<float>(), grads[i].numel()});
+  }
+  if (entries.empty()) return;
+  c10::cuda::CUDAGuard guard(grads[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(grads[0].get_device());
+  for (size_t lo = 0; lo < entries.size(); lo += kern::kAccMaxTensors) {
+    kern::AccTable table;
+    table.n = (int)std::min<size_t>(kern::kAccMaxTensors, entries.size() - lo);
+    maxc = 0;
+    for (int k = 0; k < table.n; ++k) {
+      table.t[k] = entries[lo + k];
+      maxc = std::max(maxc, table.t[k].count);
+    }
+    cudaError_t e = kern::LaunchGradAccumulate(table, maxc, (int)mode, (int)MapDtype(st), s);
+    TORCH_CHECK(e == cudaSuccess, "grad_accumulate launch failed: ", cudaGetErrorString(e));
+  }
+}
+
 // ---- hvd.SyncBatchNorm kernels (see kernels/sync_bn_kernels.cu) ------------------------------------------------------
 // Every argument is checked here, before anything is launched.
 
@@ -1154,6 +1198,7 @@ PYBIND11_MODULE(_hvd_torch, m) {
         py::arg("grad_scale"), py::arg("grad_scale_dev"), py::arg("master_params"), py::arg("norms"), py::arg("slots"));
   m.def("grad_shard_stats", &GradShardStats, py::arg("grads"), py::arg("out"), py::arg("inv_scale") = py::none(),
         py::arg("norm_inf") = false);
+  m.def("grad_accumulate", &GradAccumulate, py::arg("grads"), py::arg("accs"), py::arg("mode"));
   m.def("sync_bn_stats", &SyncBnStats, py::arg("x"), py::arg("slot"));
   m.def("sync_bn_combine", &SyncBnCombine, py::arg("slots"), py::arg("num_features"), py::arg("eps"), py::arg("momentum"),
         py::arg("running_mean") = py::none(), py::arg("running_var") = py::none(),

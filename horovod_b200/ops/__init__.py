@@ -6,6 +6,7 @@
 * `fused_lars_step`, and its two phases `lars_norms` / `lars_apply` — multi-tensor LARS on LAMB's table and norms
   layout (same file);
 * `grad_shard_stats` — one-pass gradient norm statistics, non-finite check and optional in-place unscale (same file);
+* `grad_accumulate_` — folds bf16 / fp16 gradients into fp32 accumulators for gradient accumulation (same file);
 * `sync_bn_stats`, `sync_bn_combine`, `sync_bn_elemt`, `sync_bn_backward_reduce`, `sync_bn_backward_elemt` — the
   kernels of hvd.SyncBatchNorm's native path (`csrc/kernels/sync_bn_kernels.cu`);
 * `symm_empty`, `symm_available` — registered symmetric memory for the zero-copy allreduce path;
@@ -142,6 +143,37 @@ def grad_shard_stats(tensors, out, inv_scale=None, norm_type=2.0):
     for ts in by_dtype.values():
         _native().grad_shard_stats(ts, out, inv_scale, norm_type != 2.0)
     return out
+
+
+_ACC_MODES = {'first': 0, 'add': 1, 'last': 2}
+
+
+def grad_accumulate_(grads, accs, mode):
+    """Gradient accumulation in fp32 for bf16 / fp16 gradients.  grads[i] (bf16 or fp16) and accs[i] (float32, same
+    shape and strides) are folded element by element, in place:
+
+    * mode 'first': accs[i] = grads[i] in fp32, then grads[i] = 0;
+    * mode 'add':   accs[i] += grads[i] in fp32, then grads[i] = 0;
+    * mode 'last':  grads[i] = accs[i] + grads[i], computed in fp32 and rounded to nearest-even once (accs[i] is not
+      written).
+
+    So k micro-batch gradients summed as first, add, ..., add, last are rounded once instead of k times, and the results
+    are bit-identical to the same torch ops in fp32.  inf and NaN propagate (an fp16 sum above 65504 becomes inf).  One
+    launch per gradient dtype and 160 tensors, on the current stream, with no host synchronisation: the call can be
+    captured into a CUDA graph."""
+    if mode not in _ACC_MODES:
+        raise ValueError("grad_accumulate_: mode must be 'first', 'add' or 'last', got %r" % (mode,))
+    grads, accs = list(grads), list(accs)
+    if len(grads) != len(accs):
+        raise ValueError('grad_accumulate_: %d gradients but %d accumulators' % (len(grads), len(accs)))
+    by_dtype = {}
+    for g, a in zip(grads, accs):
+        gs, as_ = by_dtype.setdefault(g.dtype, ([], []))
+        gs.append(g)
+        as_.append(a)
+    for gs, as_ in by_dtype.values():
+        _native().grad_accumulate(gs, as_, _ACC_MODES[mode])
+    return grads
 
 
 def sync_bn_slot_doubles(num_features):

@@ -10,11 +10,21 @@ reduction on peer-mapped memory, flag barrier inside the kernel) on a forked hig
 reduction of bucket k overlaps the backward pass of the layers below it, and a whole data-parallel step — forward,
 backward, every collective — is ONE launch with no negotiation round and no host work.  `optimizer.step()` after the
 replay only applies the (fused) update.  If some trainable parameter is not in a registered bucket (sparse gradients,
-`zero_copy=False`, gradient accumulation) the reductions stay outside the graph and `step()` issues them as before.
+`zero_copy=False`, compression, `groups`) the reductions stay outside the graph and `step()` issues them as before.
 
     step = hvd.GraphedStep(lambda x, y: F.cross_entropy(model(x), y), optimizer, (x0, y0))
     for x, y in loader:
         loss = step(x, y)          # copies x, y into the static inputs, replays, allreduces, applies the update
+
+Gradient accumulation: with `backward_passes_per_step=k > 1` every call is one micro-batch (divide the loss by k inside
+`step_fn`, as in the eager idiom) and `optimizer.step()` runs after every k-th call only.  Up to three graphs share one
+memory pool and the static inputs: the first micro-step's (zero_grad + forward/backward), the middle ones' (k >= 3) and
+the last one's, which also holds the gradient collectives where they can be captured.  With
+`grad_accumulation_dtype=torch.float32` each graph ends with its fold of the bf16 / fp16 gradients into the fp32
+accumulators (in the last graph, each bucket's fold precedes its collective).  k is fixed when the step is built.
+As with k = 1, a call returns the static loss tensor of the graph it replayed, which that graph's next replay
+overwrites; the middle graph serves micro-steps 2 … k-1, so `.clone()` (or `.item()`) a loss that must outlive the
+next call.
 
 Constraints (those of CUDA graphs): fixed input shapes/dtypes, no host synchronisation or data-dependent control flow
 inside `step_fn`, `optimizer.zero_grad()` is part of the graph (do not call it yourself).  If capture fails the object
@@ -33,6 +43,10 @@ class GraphedStep:
         self.step_fn, self.optimizer = step_fn, optimizer
         self.captured, self.fallback_reason = False, None
         self.graph, self.static_loss = None, None
+        # backward_passes_per_step when built; k > 1: one graph and static loss per phase, replayed first, middle..., last
+        self.k = int(getattr(optimizer, 'backward_passes_per_step', 1) or 1)
+        self.graphs, self.static_losses = None, None
+        self.micro_step = 0  # micro-batches of the current optimizer step already run
         self.comm_in_graph = False  # True: the gradient allreduces are kernel nodes of the captured graph
         self.static_inputs = tuple(example_inputs)
         self.replays = 0
@@ -50,8 +64,9 @@ class GraphedStep:
             self._agree_across_ranks()
 
     # ------------------------------------------------------------------------------------------------------------------
-    def _fwd_bwd(self):
-        self.optimizer.zero_grad(set_to_none=False)
+    def _fwd_bwd(self, zero_grad=True):
+        if zero_grad:
+            self.optimizer.zero_grad(set_to_none=False)
         loss = self.step_fn(*self.static_inputs)
         loss.backward()
         return loss
@@ -70,6 +85,9 @@ class GraphedStep:
         missing = [p for g in opt.param_groups for p in g['params'] if p.requires_grad and p.grad is None]
         for p in missing:  # parameters unused by step_fn still need a static gradient for the optimizer
             p.grad = torch.zeros_like(p, memory_format=torch.preserve_format)
+        if self.k > 1:
+            self._capture_phases()
+            return
         self.graph = torch.cuda.CUDAGraph()
         try:
             with torch.cuda.graph(self.graph):
@@ -82,6 +100,35 @@ class GraphedStep:
         finally:
             if hasattr(opt, '_graph_capture'):
                 opt._graph_capture = None
+        torch.cuda.synchronize()
+        self.captured = True
+
+    def _capture_phases(self):
+        """k > 1: the first, middle (k >= 3) and last micro-steps as graphs of one memory pool.  Only the last one
+        records the gradient collectives (as the one graph of k == 1 does) and the fp32 accumulation's 'last' folds."""
+        opt = self.optimizer
+        fold = getattr(opt, '_graph_fold', None)
+        if fold is not None:
+            opt._prepare_accumulators()
+        pool = torch.cuda.graph_pool_handle()
+        phases = ('first', 'add', 'last') if self.k >= 3 else ('first', 'last')
+        self.graphs, self.static_losses = {}, {}
+        for phase in phases:
+            graph = torch.cuda.CUDAGraph()
+            try:
+                with torch.cuda.graph(graph, pool=pool):
+                    comm = phase == 'last' and bool(getattr(opt, '_begin_graph_capture', lambda: False)())
+                    loss = self._fwd_bwd(zero_grad=phase == 'first')
+                    if fold is not None:
+                        fold(phase, with_buckets=not comm)  # with comm, each bucket's fold precedes its collective
+                    if comm:
+                        opt._end_graph_capture()
+            finally:
+                if hasattr(opt, '_graph_capture'):
+                    opt._graph_capture = None
+            self.graphs[phase], self.static_losses[phase] = graph, loss
+            self.comm_in_graph = self.comm_in_graph or comm
+        self.graph, self.static_loss = self.graphs['last'], self.static_losses['last']
         torch.cuda.synchronize()
         self.captured = True
 
@@ -100,6 +147,7 @@ class GraphedStep:
 
     def _abandon(self, exc):
         self.captured, self.graph, self.comm_in_graph = False, None, False
+        self.graphs = self.static_losses = None
         self.optimizer._graph_mode = False
         if hasattr(self.optimizer, '_graph_comm_captured'):
             self.optimizer._graph_comm_captured = False
@@ -112,6 +160,12 @@ class GraphedStep:
 
     # ------------------------------------------------------------------------------------------------------------------
     def __call__(self, *inputs):
+        k = int(getattr(self.optimizer, 'backward_passes_per_step', 1) or 1)
+        if k != self.k:
+            raise RuntimeError('hvd.GraphedStep was built for backward_passes_per_step=%d, the optimizer now has %d: build '
+                               'a new GraphedStep after set_backward_passes_per_step()' % (self.k, k))
+        if self.k > 1:
+            return self._micro_step(inputs)
         if not self.captured:
             self.optimizer.zero_grad()
             loss = self.step_fn(*inputs)
@@ -125,3 +179,24 @@ class GraphedStep:
         self.replays += 1
         self.optimizer.step()
         return self.static_loss
+
+    def _micro_step(self, inputs):
+        """One micro-batch of k: the optimizer steps after the k-th.  Returns this micro-batch's loss."""
+        first, last = self.micro_step == 0, self.micro_step == self.k - 1
+        if not self.captured:
+            if first:
+                self.optimizer.zero_grad()
+            loss = self.step_fn(*inputs)
+            loss.backward()
+        else:
+            for dst, src in zip(self.static_inputs, inputs):
+                if dst is not src:
+                    dst.copy_(src, non_blocking=True)
+            phase = 'first' if first else 'last' if last else 'add'
+            self.graphs[phase].replay()
+            self.replays += 1
+            loss = self.static_losses[phase]
+        self.micro_step = 0 if last else self.micro_step + 1
+        if last:
+            self.optimizer.step()
+        return loss

@@ -28,9 +28,15 @@ from horovod_b200.torch.mpi_ops import (Adasum, Average, Sum, allreduce_async_, 
 class _DistributedOptimizer(torch.optim.Optimizer):
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
-                 fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None, master_weights=False):
+                 fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None, master_weights=False,
+                 grad_accumulation_dtype=None):
         super(self.__class__, self).__init__(params)
         self._compression = compression
+        # fp32 accumulators of bf16 / fp16 gradients over the backward passes of one step (allocated on first use, not
+        # optimizer state): bucket -> bucket['acc'], parameter outside the buckets -> self._param_accs[p]
+        self._acc_fp32 = _check_grad_accumulation_dtype(grad_accumulation_dtype)
+        self._param_accs = {}
+        self._acc_open = set()  # parameters outside the buckets folded this step whose 'last' fold is still to come
         # fp32 master copies of bf16 / fp16 parameters, kept as optimizer state ('master_param') and updated by the fused
         # kernels only: master_weights implies fused, and step() never hands those parameters to torch's own update
         self._master_weights = bool(master_weights)
@@ -119,6 +125,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._should_synchronize = True
         for p in self._allreduce_delay:
             self._allreduce_delay[p] = self.backward_passes_per_step
+        self._reset_folds()
         super(self.__class__, self).load_state_dict(*args, **kwargs)
         if self._fused and (isinstance(self, (torch.optim.Adam, torch.optim.AdamW, Lamb, Lars)) or self._master_weights):
             self._keep_fp32_moments(args[0] if args else kwargs['state_dict'])
@@ -147,6 +154,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self.backward_passes_per_step = passes
         for p in self._allreduce_delay:
             self._allreduce_delay[p] = self.backward_passes_per_step
+        self._reset_folds()
 
     def _register_hooks(self):
         if self._groups is not None:
@@ -212,7 +220,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                     flat.zero_()
                     bucket = {'flat': flat, 'params': [m[0] for m in members], 'pending': len(members),
                               'name': 'bucket.%d' % len(self._buckets), 'handle': None, 'shadow': None, 'shadow_views': None,
-                              'offsets': {m[0]: m[1] for m in members}, 'views': {}}
+                              'offsets': {m[0]: m[1] for m in members}, 'views': {}, 'acc': None, 'arrived': 0, 'folds': 0}
                     if self._bucket_wire_dtype is not None and dtype == torch.float32:
                         shadow = mpi_ops.symm_empty(total // itemsize, dtype=self._bucket_wire_dtype, device=members[0][0].device,
                                                     process_set=self.process_set)
@@ -237,6 +245,11 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._buckets, self._p_to_bucket, self._zero_copy = [], {}, False
 
     def _launch_bucket(self, bucket):
+        if bucket['folds']:
+            # gradient accumulation in fp32: the bucket's sum over the step's backward passes, rounded once, is what is
+            # reduced (the fold runs on this stream, so it precedes the allreduce)
+            _fold([bucket['flat']], [bucket['acc']], 'last')
+            bucket['folds'] = 0
         if self.op == Average:
             prescale_factor, postscale_factor = 1.0 / self.gradient_predivide_factor, self.gradient_predivide_factor
         else:
@@ -323,11 +336,23 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                     view.copy_(p.grad.to_dense() if p.grad.is_sparse else p.grad)
                     p.grad = view
                 self._handles[p] = ('bucket', None)
+                if self._accumulates(bucket['flat']):
+                    bucket['arrived'] += 1
+                    if bucket['arrived'] == len(bucket['params']):  # the bucket has this backward pass's gradients
+                        bucket['arrived'] = 0
+                        if self._allreduce_delay[p] > 0:
+                            _fold([bucket['flat']], [self._bucket_acc(bucket)], 'add' if bucket['folds'] else 'first')
+                            bucket['folds'] += 1
                 if self._allreduce_delay[p] == 0:
                     bucket['pending'] -= 1
                     if bucket['pending'] == 0:
                         self._launch_bucket(bucket)
                 return
+            if self._accumulates(p.grad):
+                if self._allreduce_delay[p] > 0:
+                    self._fold_param(p, 'add' if p in self._acc_open else 'first')
+                elif p in self._acc_open:
+                    self._fold_param(p, 'last')
             if self._allreduce_delay[p] == 0:
                 if self._groups is not None:
                     group = self._p_to_group[p]
@@ -340,12 +365,75 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._handles[p] = (handle, ctx)
         return hook
 
+    # ---- gradient accumulation in fp32 (grad_accumulation_dtype=torch.float32) -------------------------------------------
+    def _accumulates(self, grad):
+        """True when `grad` (a bucket or a parameter's gradient) is summed over the backward passes in fp32."""
+        return (self._acc_fp32 and self.backward_passes_per_step > 1 and grad is not None and grad.is_cuda
+                and not grad.is_sparse and grad.dtype in (torch.bfloat16, torch.float16))
+
+    def _bucket_acc(self, bucket):
+        if bucket['acc'] is None:  # plain device memory: the accumulator never travels
+            bucket['acc'] = torch.empty(bucket['flat'].numel(), dtype=torch.float32, device=bucket['flat'].device)
+        return bucket['acc']
+
+    def _param_acc(self, p):
+        acc = self._param_accs.get(p)
+        if acc is None or acc.shape != p.grad.shape or acc.stride() != p.grad.stride():
+            acc = self._param_accs[p] = (torch.empty_like(p.grad, dtype=torch.float32) if acc is None
+                                         else _state_like(p.grad, acc, torch.float32))
+        return acc
+
+    def _fold_param(self, p, mode):
+        _fold([p.grad], [self._param_acc(p)], mode)
+        if mode == 'last':
+            self._acc_open.discard(p)
+        else:
+            self._acc_open.add(p)
+
+    def _finish_param_folds(self):
+        """step() before every backward pass of the step arrived: parameters whose 'last' fold is missing get it now."""
+        for p in list(self._acc_open):
+            if p.grad is None:
+                p.grad = torch.zeros_like(p)
+            self._fold_param(p, 'last')
+
+    def _reset_folds(self):
+        self._acc_open.clear()
+        for bucket in self._buckets:
+            bucket['arrived'] = bucket['folds'] = 0
+
+    def _accumulator_pairs(self, with_buckets=True):
+        """(16-bit gradients, fp32 accumulators) of every accumulating bucket and parameter, allocated now if needed."""
+        grads, accs = [], []
+        if with_buckets:
+            for bucket in self._buckets:
+                if self._accumulates(bucket['flat']):
+                    grads.append(bucket['flat'])
+                    accs.append(self._bucket_acc(bucket))
+        for group in self.param_groups:
+            for p in group['params']:
+                if p.requires_grad and p not in self._p_to_bucket and self._accumulates(p.grad):
+                    grads.append(p.grad)
+                    accs.append(self._param_acc(p))
+        return grads, accs
+
+    def _prepare_accumulators(self):
+        """hvd.GraphedStep, before capture: the accumulators must exist outside the graphs' memory pool."""
+        self._accumulator_pairs()
+
+    def _graph_fold(self, mode, with_buckets=True):
+        """hvd.GraphedStep, while capturing: one fold of every accumulator after the captured backward pass."""
+        grads, accs = self._accumulator_pairs(with_buckets)
+        if grads:
+            _fold(grads, accs, mode)
+
     # ---- gradient allreduce as CUDA-graph nodes (hvd.GraphedStep) --------------------------------------------------------
     def _graph_capturable(self):
         """The whole gradient reduction can live inside the captured step: every trainable parameter sits in a registered
-        zero-copy bucket, one backward per step, a reduction the in-place kernel implements.  Depends on the model and the
-        constructor arguments only, so every rank answers the same."""
-        if not (self._zero_copy and self._buckets and self.backward_passes_per_step == 1 and self.op in (Average, Sum)):
+        zero-copy bucket and the reduction is one the in-place kernel implements.  With backward_passes_per_step > 1 the
+        reduction is part of the step's last graph only.  Depends on the model and the constructor arguments only, so
+        every rank answers the same."""
+        if not (self._zero_copy and self._buckets and self.op in (Average, Sum)):
             return False
         if not self.process_set.included() or self.process_set.size() <= 1:
             return False
@@ -364,7 +452,9 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                                # (without NVLS — teams of 2 — the P2P two-shot kernel needs more CTAs to keep up with backward)
                                'ctas': int(os.environ.get('HVD_GRAPH_COMM_CTAS', '16' if '+mc' in mpi_ops.gpu_backend_info() and self.process_set.size() >= 4 else '32')),
                                'tail_ctas': int(os.environ.get('HVD_GRAPH_COMM_TAIL_CTAS', '128')), 'tail': False,
-                               'pending': {id(b): len(b['params']) for b in self._buckets}}
+                               'pending': {id(b): len(b['params']) for b in self._buckets},
+                               # the step's last graph of an fp32 accumulation: each bucket's 'last' fold precedes its allreduce
+                               'fold': {id(b) for b in self._buckets if self._accumulates(b['flat'])}}
         return True
 
     def _graph_hook(self, p):
@@ -383,6 +473,8 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         else:
             prescale_factor = postscale_factor = 1.0
         comm = cap['comm']
+        if id(bucket) in cap['fold']:
+            _fold([bucket['flat']], [self._bucket_acc(bucket)], 'last')
         comm.wait_stream(torch.cuda.current_stream())  # fork: everything recorded so far (this bucket's gradients) precedes it
         with torch.cuda.stream(comm):
             wire = bucket['flat']
@@ -465,6 +557,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             for bucket in self._buckets:
                 synchronize(bucket['handle'])
                 bucket['handle'] = None
+                bucket['arrived'] = 0
                 if bucket.get('shadow') is not None:
                     bucket['shadow_fresh'] = True
                 for p in bucket['params']:
@@ -472,6 +565,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                     self._handles.pop(p, None)
         if self._zero_copy and not _defer_shadow_copy:
             self._restore_shadows()  # callers of synchronize() (gradient clipping, ...) read p.grad
+        self._finish_param_folds()
         pending = [p for p in self._requires_update if p not in self._handles and p not in self._p_to_bucket]
         pending += [p for p, (h, _) in self._handles.items() if h is None]
         if self._groups is not None:
@@ -579,6 +673,21 @@ def _find_duplicates(lst):
             dups.add(el)
         seen.add(el)
     return dups
+
+
+def _check_grad_accumulation_dtype(dtype):
+    """grad_accumulation_dtype: None (gradients accumulate in their own dtype) or torch.float32; True for the latter."""
+    if dtype is None:
+        return False
+    if dtype is torch.float32:
+        return True
+    raise ValueError('grad_accumulation_dtype must be None or torch.float32, got %r' % (dtype,))
+
+
+def _fold(grads, accs, mode):
+    from horovod_b200 import ops
+    with torch.no_grad():
+        ops.grad_accumulate_(grads, accs, mode)
 
 
 def _fused_plan(opt, why=None):
@@ -911,7 +1020,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none, backward_passes_per_step=1,
                          op=Average, gradient_predivide_factor=1.0, num_groups=0, groups=None, sparse_as_dense=False,
                          process_set=global_process_set, fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None,
-                         shard_optimizer_state=False, master_weights=False):
+                         shard_optimizer_state=False, master_weights=False, grad_accumulation_dtype=None):
     """Wraps `optimizer` so gradients are combined across ranks before the parameter update.
 
     Arguments follow the reference (horovod/torch/optimizer.py:516-608). `fused=True` (new) runs the SGD /
@@ -929,7 +1038,17 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     SGD momentum is then fp32 as well.  fp32 parameters are unaffected.  Implies fused=True; SGD / Adam / AdamW / Lamb /
     Lars only, without maximize, amsgrad or op=Adasum (ValueError).  A parameter written from outside the optimizer
     (load_state_dict, broadcast_parameters, an in-place edit) is picked up by the next step: where it no longer equals
-    its rounded master, the master restarts from it."""
+    its rounded master, the master restarts from it.
+
+    `grad_accumulation_dtype=torch.float32` (new; default None) sums the bf16 / fp16 gradients of the
+    `backward_passes_per_step` backward passes of one step in fp32: after each pass the gradient is folded into an fp32
+    accumulator and zeroed, and after the last pass it holds the sum rounded once, which is what is reduced and applied.
+    Between passes p.grad holds the current pass's gradient only.  fp32 gradients and backward_passes_per_step == 1 are
+    unaffected.  The accumulators (one flat buffer per zero-copy bucket, else one per parameter) are allocated on first
+    use and are not optimizer state: checkpoints are taken between steps.  Not with op=Adasum (ValueError)."""
+    _check_grad_accumulation_dtype(grad_accumulation_dtype)
+    if grad_accumulation_dtype is not None and op == Adasum:
+        raise ValueError('grad_accumulation_dtype is not supported with op=Adasum')
     if master_weights:
         if op == Adasum:
             raise ValueError('master_weights is not supported with op=Adasum')
@@ -956,12 +1075,13 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
         from horovod_b200.torch.sharded_optimizer import _ShardedDistributedOptimizer
         cls = type(optimizer.__class__.__name__, (_ShardedDistributedOptimizer, optimizer.__class__), {})
         return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,
-                   gradient_predivide_factor, groups, sparse_as_dense, process_set, bucket_cap_mb, master_weights)
+                   gradient_predivide_factor, groups, sparse_as_dense, process_set, bucket_cap_mb, master_weights,
+                   grad_accumulation_dtype)
     if op != Adasum or size() == 1:
         cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedOptimizer.__dict__))
         return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,
                    gradient_predivide_factor, groups, sparse_as_dense, process_set, fused, zero_copy, bucket_cap_mb, bucket_wire_dtype,
-                   master_weights)
+                   master_weights, grad_accumulation_dtype)
     if process_set != global_process_set:
         raise NotImplementedError("Adasum does not support non-global process sets yet.")
     cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedAdasumOptimizer.__dict__))

@@ -21,6 +21,11 @@ verdict, and the clip coefficient reaches the update on the device.
 
 With `master_weights=True` every bf16 / fp16 bucket also keeps an fp32 master copy of its owned shard ('master_param'),
 which the fused kernel updates and rounds into the parameter shard before the allgather.
+
+With `backward_passes_per_step=k > 1` and `grad_accumulation_dtype=torch.float32` every bf16 / fp16 gradient bucket has an
+fp32 accumulator of its full size: when a bucket has received a backward pass's gradients it is folded into the
+accumulator and zeroed (grad_accumulate_ 'first' / 'add'), and after the k-th pass the sum rounded once is written back
+('last') right before the bucket's reduce-scatter, on the same stream.
 """
 import math
 import os
@@ -35,7 +40,7 @@ from horovod_b200.torch.compression import Compression
 from horovod_b200.torch.lamb import Lamb
 from horovod_b200.torch.lars import Lars
 from horovod_b200.torch.mpi_ops import Average, Sum
-from horovod_b200.torch.optimizer import _find_duplicates
+from horovod_b200.torch.optimizer import _check_grad_accumulation_dtype, _find_duplicates, _fold
 
 ALIGN = 128  # bytes: every parameter and every shard starts at a multiple of this
 
@@ -140,7 +145,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
 
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
-                 bucket_cap_mb=32, master_weights=False):
+                 bucket_cap_mb=32, master_weights=False, grad_accumulation_dtype=None):
         super().__init__(params)
         if isinstance(self, torch.optim.SGD):
             kind = 'sgd'
@@ -179,6 +184,9 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             raise ValueError('shard_optimizer_state needs registered symmetric memory (P2P backend, one host, not elastic)')
 
         self._kind = kind
+        # fp32 accumulators of the bf16 / fp16 gradient buckets over the backward passes of one step (b['acc'], plain
+        # device memory allocated on first use, not optimizer state)
+        self._acc_fp32 = _check_grad_accumulation_dtype(grad_accumulation_dtype)
         self.process_set = process_set
         self.op = op
         self.gradient_predivide_factor = gradient_predivide_factor
@@ -207,7 +215,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 pflat.zero_()
                 gflat.zero_()
                 b.update({'params': ps, 'pflat': pflat, 'gflat': gflat, 'views': {}, 'index': bi, 'step': 0,
-                          'mom_init': False, 'pending': 0, 'ready': False})
+                          'mom_init': False, 'pending': 0, 'ready': False, 'acc': None, 'arrived': 0, 'folds': 0,
+                          'fold_last': False})
                 for p, (_, off, numel) in zip(ps, b['members']):
                     # keep the parameter's memory format (channels_last stays channels_last)
                     pview = pflat[off:off + numel].as_strided(p.size(), p.stride())
@@ -260,6 +269,28 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._next = 0
         for b in self._buckets:
             b['pending'], b['ready'] = len(b['params']), False
+            b['arrived'] = b['folds'] = 0
+
+    # ---- gradient accumulation in fp32 (grad_accumulation_dtype=torch.float32) -------------------------------------------
+    def _accumulates(self, bucket):
+        return self._acc_fp32 and self.backward_passes_per_step > 1 and bucket['dtype'] in (torch.bfloat16, torch.float16)
+
+    def _bucket_acc(self, bucket):
+        if bucket['acc'] is None:
+            bucket['acc'] = torch.empty(bucket['numel'], dtype=torch.float32, device=bucket['gflat'].device)
+        return bucket['acc']
+
+    def _prepare_accumulators(self):
+        """hvd.GraphedStep, before capture: the accumulators must exist outside the graphs' memory pool."""
+        for b in self._buckets:
+            if self._accumulates(b):
+                self._bucket_acc(b)
+
+    def _graph_fold(self, mode, with_buckets=True):
+        """hvd.GraphedStep, while capturing: one fold of every accumulating bucket after the captured backward pass."""
+        bs = [b for b in self._buckets if with_buckets and self._accumulates(b)]
+        if bs:
+            _fold([b['gflat'] for b in bs], [self._bucket_acc(b) for b in bs], mode)
 
     def _scales(self):
         if self.op == Average:
@@ -275,6 +306,10 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         bucket['ready'] = True
         while self._next < len(self._buckets) and self._buckets[self._next]['ready']:
             b = self._buckets[self._next]
+            if b['folds'] or (b['fold_last'] and self._graph_capture is not None):
+                # gradient accumulation in fp32: the sum over the step's backward passes, rounded once, is reduce-scattered
+                _fold([b['gflat']], [self._bucket_acc(b)], 'last')
+                b['folds'] = 0
             comm = self._comm_stream()
             comm.wait_stream(torch.cuda.current_stream())
             pre, post = self._scales()
@@ -306,6 +341,13 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                                      'Increase backward_passes_per_step to accumulate gradients locally.')
             self._delay[p] -= 1
             self._seen.add(p)
+            if self._accumulates(bucket):
+                bucket['arrived'] += 1
+                if bucket['arrived'] == len(bucket['params']):  # the bucket has this backward pass's gradients
+                    bucket['arrived'] = 0
+                    if self._delay[p] > 0:
+                        _fold([bucket['gflat']], [self._bucket_acc(bucket)], 'add' if bucket['folds'] else 'first')
+                        bucket['folds'] += 1
             if self._delay[p] == 0:
                 bucket['pending'] -= 1
                 if bucket['pending'] == 0:
@@ -544,15 +586,19 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
     def set_backward_passes_per_step(self, passes):
         self.backward_passes_per_step = passes
         self._delay = {p: passes for p in self._delay}
+        for b in self._buckets:
+            b['arrived'] = b['folds'] = 0
 
     # ---- hvd.GraphedStep -----------------------------------------------------------------------------------------------
     def _begin_graph_capture(self):
         """Called by hvd.GraphedStep right after stream capture began: the reduce-scatters become graph nodes."""
         self._graph_comm_captured = False
-        if self.backward_passes_per_step != 1 or os.environ.get('HVD_GRAPH_COMM', '1') == '0':
+        if os.environ.get('HVD_GRAPH_COMM', '1') == '0':
             return False
         self._graph_capture = {'comm': torch.cuda.Stream(device=self._comm.device, priority=self._comm.priority)}
         self._reset_launch_order()
+        for b in self._buckets:  # with backward_passes_per_step > 1 this is the step's last graph
+            b['fold_last'] = self._accumulates(b)
         return True
 
     def _end_graph_capture(self):
@@ -564,6 +610,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         torch.cuda.current_stream().wait_stream(cap['comm'])
         self._graph_capture = None
         self._reset_launch_order()
+        for b in self._buckets:
+            b['fold_last'] = False
         self._graph_comm_captured = True
 
     # ---- checkpoints ------------------------------------------------------------------------------------------------------
