@@ -6,10 +6,12 @@
 #include <cuda_runtime.h>
 #include <cstdlib>
 #include <cstring>
+#include <string>
 #include <map>
 #include <memory>
 #include <vector>
 #include "../kernels/p2p_kernels.h"
+#include "../ops/collective_plan.h"
 #include "../ops/gpu_ops.h"
 #include "../symm/symm_memory.h"
 
@@ -63,6 +65,147 @@ int Finish(int nranks, cudaError_t sync_result) {
     }
   }
   return 0;
+}
+
+// ---------------------------------------------------------------------------
+// The launch plans of reducescatter / allgather(v) / broadcast / alltoall(v) (ops/collective_plan.h) for all N ranks.
+
+enum PlanKind { kPlanReducescatter = 0, kPlanAllgather = 1, kPlanBroadcast = 2, kPlanAlltoall = 3 };
+
+// dims per tensor i: reducescatter dims[i] = dim0; allgather dims[i*n .. i*n+n) = every rank's dim0; broadcast dims[i] =
+// bytes; alltoall dims[i*n*n ..) = the split matrix (rows rank p sends to rank q at p*n+q).  rows[i]: elements per row
+// (not used by broadcast).  in_ptrs / out_ptrs: [nranks][ntensors].
+struct PlanRequest {
+  int kind, n, ntensors;
+  const int64_t* dims;
+  const int64_t* rows;
+  int dtype, op;
+  double prescale, postscale;
+  int root;
+  const uint64_t* in_ptrs;
+  const uint64_t* out_ptrs;
+  int64_t cap;
+  int ctas;
+  int grid = 0;  // > 0: every launch of every rank runs this many CTAs instead of the grid the planner sized to the data
+};
+
+// Every rank's plan and the byte ranges of its outputs (what the engine allocates for that rank).
+Status BuildPlans(const PlanRequest& q, std::vector<Plan>* plans, std::vector<std::vector<OutSpan>>* outs) {
+  const int n = q.n, t = q.ntensors;
+  if (n < 2 || n > kern::kMaxPeers || t < 0 || q.kind < 0 || q.kind > kPlanAlltoall || (q.kind == kPlanBroadcast && (q.root < 0 || q.root >= n)))
+    return Status::InvalidArgument("bad plan request");
+  const int64_t esz = q.kind == kPlanBroadcast ? 1 : (int64_t)DataTypeSize((DataType)q.dtype);
+  plans->assign(n, Plan());
+  outs->assign(n, {});
+  for (int r = 0; r < n; ++r) {
+    std::vector<PlanTensor> ts(t);
+    for (int i = 0; i < t; ++i) {
+      PlanTensor& pt = ts[i];
+      pt.in = (const void*)q.in_ptrs[(size_t)r * t + i];
+      pt.out = (void*)q.out_ptrs[(size_t)r * t + i];
+      pt.row = q.kind == kPlanBroadcast ? 1 : q.rows[i];
+      int64_t out_rows = 0;
+      if (q.kind == kPlanReducescatter) {
+        pt.dims = {q.dims[i]};
+        std::vector<int64_t> rows;
+        ReducescatterRows(q.dims[i], n, &rows);
+        out_rows = rows[r];
+      } else if (q.kind == kPlanAllgather) {
+        pt.dims.assign(q.dims + (size_t)i * n, q.dims + (size_t)(i + 1) * n);
+        for (int p = 0; p < n; ++p) out_rows += pt.dims[p];
+      } else if (q.kind == kPlanBroadcast) {
+        pt.dims = {q.dims[i]};
+        out_rows = (r == q.root && pt.out == pt.in) ? 0 : q.dims[i];
+      } else {
+        pt.dims.assign(q.dims + (size_t)i * n * n, q.dims + (size_t)(i + 1) * n * n);
+        for (int p = 0; p < n; ++p) out_rows += pt.dims[(size_t)p * n + r];
+      }
+      (*outs)[r].push_back({pt.out, out_rows * pt.row * esz});
+    }
+    Status st;
+    Plan& plan = (*plans)[r];
+    if (q.kind == kPlanReducescatter) {
+      ReduceParams rp;
+      rp.dtype = (DataType)q.dtype; rp.op = (ReduceOp)q.op; rp.prescale = q.prescale; rp.postscale = q.postscale;
+      st = PlanReducescatter(r, n, ts, rp, q.cap, q.ctas, &plan);  // the simulated team has no multicast object: rp.nvls false
+    } else if (q.kind == kPlanAllgather) {
+      st = PlanAllgather(r, n, ts, esz, q.cap, q.ctas, &plan);
+    } else if (q.kind == kPlanBroadcast) {
+      st = PlanBroadcast(r, n, q.root, ts, false, q.cap, q.ctas, &plan);
+    } else {
+      st = PlanAlltoall(r, n, ts, esz, q.cap, q.ctas, &plan);
+    }
+    if (!st.ok()) return st;
+  }
+  return Status::OK();
+}
+
+void CopyMessage(const std::string& m, char* err, int err_len) {
+  if (err && err_len > 0) { strncpy(err, m.c_str(), (size_t)err_len - 1); err[err_len - 1] = 0; }
+}
+
+// Plans all N ranks, checks them (CheckPlans) and only then launches, step-major: launch k of every rank before launch k+1
+// of any rank.  -5: no plan (the buffer is too small), -4: the ranks' plans disagree (nothing was launched).  The tables
+// of all launches go to the device in one copy before the first launch.
+int SimCollective(const PlanRequest& q, int device) {
+  if (cudaSetDevice(device) != cudaSuccess) return -1;
+  std::vector<Plan> plans;
+  std::vector<std::vector<OutSpan>> outs;
+  if (!BuildPlans(q, &plans, &outs).ok()) return -5;
+  if (q.grid > 0)
+    for (auto& plan : plans) for (auto& l : plan) l.ctas = q.grid;
+  if (!CheckPlans(plans, outs, q.cap, q.kind == kPlanBroadcast ? q.root : -1).ok()) return -4;
+  Sim* sim = GetSim(q.n, device, (size_t)std::max<int64_t>(q.cap, 1 << 20));
+  if (!sim) return -1;
+  if ((int64_t)sim->teams[0]->buffer_bytes() < q.cap) return -1;
+  const size_t nl = plans[0].size();
+  std::vector<char> host;
+  std::vector<size_t> at((size_t)q.n * nl);
+  for (size_t k = 0; k < nl; ++k) {
+    for (int r = 0; r < q.n; ++r) {
+      const PlanLaunch& l = plans[r][k];
+      at[k * q.n + r] = host.size();
+      if (l.reduce) {
+        const char* b = (const char*)l.table.data();
+        host.insert(host.end(), b, b + l.table.size() * sizeof(kern::TensorDesc));
+      } else {
+        const char* b = (const char*)l.sends.data();
+        host.insert(host.end(), b, b + l.sends.size() * sizeof(kern::CopyDesc));
+        b = (const char*)l.recvs.data();
+        host.insert(host.end(), b, b + l.recvs.size() * sizeof(kern::CopyDesc));
+      }
+      host.resize((host.size() + 255) / 256 * 256);
+    }
+  }
+  cudaDeviceSynchronize();
+  char* dev = nullptr;
+  if (!host.empty()) {
+    if (cudaMalloc(&dev, host.size()) != cudaSuccess) return -1;
+    if (cudaMemcpy(dev, host.data(), host.size(), cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(dev); return -1; }
+  }
+  cudaError_t launch_error = cudaSuccess;
+  for (size_t k = 0; k < nl && launch_error == cudaSuccess; ++k) {
+    const std::vector<kern::CommParams> cps = NextParams(sim);
+    for (int r = 0; r < q.n && launch_error == cudaSuccess; ++r) {
+      const PlanLaunch& l = plans[r][k];
+      char* t = dev + at[k * q.n + r];
+      if (l.reduce) {
+        kern::AllreduceArgs a = l.args;
+        a.descs = (const kern::TensorDesc*)t; a.out_descs = a.descs + a.ndesc; a.ctas = l.ctas;
+        launch_error = kern::LaunchAllreduce(cps[r], a, sim->streams[r]);
+      } else {
+        kern::ExchangeArgs a {};
+        a.sends = l.sends.empty() ? nullptr : (const kern::CopyDesc*)t; a.nsend = (int)l.sends.size();
+        a.recvs = l.recvs.empty() ? nullptr : (const kern::CopyDesc*)t + l.sends.size(); a.nrecv = (int)l.recvs.size();
+        a.ctas = l.ctas;
+        launch_error = kern::LaunchExchange(cps[r], a, sim->streams[r]);
+      }
+    }
+  }
+  const cudaError_t sync = cudaDeviceSynchronize();
+  if (dev) cudaFree(dev);
+  if (launch_error != cudaSuccess) return (int)launch_error;
+  return Finish(q.n, sync);
 }
 }  // namespace
 
@@ -124,27 +267,99 @@ int hvd_sim_allreduce(int nranks, int device, int ntensors, const int64_t* count
   return Finish(nranks, e);
 }
 
-// Allgather-style exchange: every rank contributes `bytes` from in_ptrs[r]; out_ptrs[r] receives nranks*bytes.
+// Allgather-style exchange: every rank contributes `bytes` from in_ptrs[r]; out_ptrs[r] receives nranks*bytes.  The
+// tables are the engine's allgather plan of one uint8 tensor, but the grid is `ctas` CTAs whatever the size (the engine
+// sizes it to the data), so that a small message also runs with CTAs that own no chunk and only take part in the barrier.
 int hvd_sim_allgather(int nranks, int device, int64_t bytes, const uint64_t* in_ptrs, const uint64_t* out_ptrs, int ctas) {
-  if (cudaSetDevice(device) != cudaSuccess) return -1;
-  Sim* sim = GetSim(nranks, device, (size_t)std::max<int64_t>(bytes, 1 << 20));
-  if (!sim) return -1;
-  const std::vector<kern::CommParams> cps = NextParams(sim);
+  std::vector<int64_t> dims(nranks, bytes);
+  const int64_t row = 1;
+  PlanRequest q {kPlanAllgather, nranks, 1, dims.data(), &row, (int)DataType::UINT8, 0, 1.0, 1.0, -1, in_ptrs, out_ptrs,
+                 std::max<int64_t>(bytes, 1 << 20), ctas};
+  q.grid = ctas;
+  return SimCollective(q, device);
+}
+
+// Reducescatter over N simulated ranks as the engine plans it: dim0s[t] / rows[t] (elements per first-dim row) of every
+// tensor, in_ptrs / out_ptrs [nranks][ntensors]; `cap` bytes of symmetric buffer per launch.  Returns 0, a cudaError_t,
+// -3 (simulated barrier timed out), -4 (the ranks' plans disagree; nothing launched) or -5 (no plan fits `cap`).
+int hvd_sim_reducescatter(int nranks, int device, int ntensors, const int64_t* dim0s, const int64_t* rows, const uint64_t* in_ptrs,
+                          const uint64_t* out_ptrs, int dtype, int op, double prescale, double postscale, int64_t cap, int ctas) {
+  PlanRequest q {kPlanReducescatter, nranks, ntensors, dim0s, rows, dtype, op, prescale, postscale, -1, in_ptrs, out_ptrs, cap, ctas};
+  return SimCollective(q, device);
+}
+
+// Allgatherv: dims[t][nranks] = every rank's first dim of tensor t; element size `esz`.  Return codes as above.
+int hvd_sim_allgatherv(int nranks, int device, int ntensors, const int64_t* dims, const int64_t* rows, int dtype,
+                       const uint64_t* in_ptrs, const uint64_t* out_ptrs, int64_t cap, int ctas) {
+  PlanRequest q {kPlanAllgather, nranks, ntensors, dims, rows, dtype, 0, 1.0, 1.0, -1, in_ptrs, out_ptrs, cap, ctas};
+  return SimCollective(q, device);
+}
+
+// Broadcast of ntensors tensors of bytes[t] bytes from `root`; out_ptrs == in_ptrs on the root is in place.
+int hvd_sim_broadcast(int nranks, int device, int ntensors, const int64_t* bytes, int root, const uint64_t* in_ptrs,
+                      const uint64_t* out_ptrs, int64_t cap, int ctas) {
+  PlanRequest q {kPlanBroadcast, nranks, ntensors, bytes, nullptr, (int)DataType::UINT8, 0, 1.0, 1.0, root, in_ptrs, out_ptrs, cap, ctas};
+  return SimCollective(q, device);
+}
+
+// Alltoallv: splits[t][nranks][nranks] = rows rank p sends to rank q (p * nranks + q) of tensor t.
+int hvd_sim_alltoallv(int nranks, int device, int ntensors, const int64_t* splits, const int64_t* rows, int dtype,
+                      const uint64_t* in_ptrs, const uint64_t* out_ptrs, int64_t cap, int ctas) {
+  PlanRequest q {kPlanAlltoall, nranks, ntensors, splits, rows, dtype, 0, 1.0, 1.0, -1, in_ptrs, out_ptrs, cap, ctas};
+  return SimCollective(q, device);
+}
+
+// The same plans on the host only (no GPU needed; the pointers are never dereferenced): `kind` 0 reducescatter,
+// 1 allgatherv, 2 broadcast, 3 alltoallv, arguments as the hvd_sim_* entries.  Runs CheckPlans and writes *nlaunch and
+// one row of 6 int64 per byte range the plans move: {0, rank, dst, src_rank, src, bytes} for every range rank `rank`
+// receives into an output (`src_rank`'s input bytes at `src`; a reduce range once per contributing rank) and
+// {1, rank, buffer offset, rank, src, bytes} for every input range rank `rank` packs.  Returns the number of rows, -5 (no
+// plan), -4 (CheckPlans failed) or -6 (more than max_rows), with the reason in `err`.
+int64_t hvd_plan_collective(int kind, int nranks, int ntensors, const int64_t* dims, const int64_t* rows, int dtype, int op,
+                            int root, const uint64_t* in_ptrs, const uint64_t* out_ptrs, int64_t cap, int ctas, int* nlaunch,
+                            int64_t* out_rows, int64_t max_rows, char* err, int err_len) {
+  PlanRequest q {kind, nranks, ntensors, dims, rows, dtype, op, 1.0, 1.0, root, in_ptrs, out_ptrs, cap, ctas};
+  std::vector<Plan> plans;
+  std::vector<std::vector<OutSpan>> outs;
+  Status st = BuildPlans(q, &plans, &outs);
+  if (!st.ok()) { CopyMessage(st.reason(), err, err_len); return -5; }
+  st = CheckPlans(plans, outs, cap, kind == kPlanBroadcast ? root : -1);
+  if (!st.ok()) { CopyMessage(st.reason(), err, err_len); return -4; }
+  *nlaunch = (int)plans[0].size();
+  int64_t m = 0;
+  auto emit = [&](int64_t a, int64_t b, int64_t c, int64_t d, int64_t e, int64_t f) {
+    if (m < max_rows) { int64_t* o = out_rows + 6 * m; o[0] = a; o[1] = b; o[2] = c; o[3] = d; o[4] = e; o[5] = f; }
+    ++m;
+  };
   for (int r = 0; r < nranks; ++r) {
-    std::vector<kern::CopyDesc> t;
-    t.push_back({(const void*)in_ptrs[r], nullptr, 0, bytes, r, 0});
-    for (int k = 0; k < nranks; ++k) {
-      int p = (r + k) % nranks;
-      t.push_back({nullptr, (char*)out_ptrs[r] + (int64_t)p * bytes, 0, bytes, p, 0});
+    for (size_t k = 0; k < plans[r].size(); ++k) {
+      const PlanLaunch& l = plans[r][k];
+      if (l.reduce) {
+        const int per = l.args.ndesc / nranks;
+        const int64_t esz = (int64_t)DataTypeSize((DataType)l.args.dtype);
+        for (int i = 0; i < l.args.ndesc; ++i)
+          if (l.table[i].count > 0) emit(1, r, l.table[i].offset, r, (int64_t)(uintptr_t)l.table[i].in, l.table[i].count * esz);
+        for (int j = 0; j < l.args.nout; ++j) {
+          const kern::TensorDesc& o = l.table[l.args.ndesc + j];
+          if (o.count > 0)
+            for (int p = 0; p < nranks; ++p)
+              emit(0, r, (int64_t)(uintptr_t)o.out, p, (int64_t)(uintptr_t)plans[p][k].table[(size_t)r * per + j].in, o.count * esz);
+        }
+        continue;
+      }
+      for (const kern::CopyDesc& s : l.sends) emit(1, r, s.offset, r, (int64_t)(uintptr_t)s.src, s.bytes);
+      for (const kern::CopyDesc& d : l.recvs) {
+        for (const kern::CopyDesc& s : plans[d.peer][k].sends) {  // CheckPlans found exactly this send
+          if (s.offset <= d.offset && d.offset + d.bytes <= s.offset + s.bytes) {
+            emit(0, r, (int64_t)(uintptr_t)d.dst, d.peer, (int64_t)(uintptr_t)s.src + (d.offset - s.offset), d.bytes);
+            break;
+          }
+        }
+      }
     }
-    const auto* dt = (const kern::CopyDesc*)GpuContext::Get().Stage(device, t.data(), t.size() * sizeof(kern::CopyDesc), sim->streams[r]);
-    if (!dt) return -2;
-    kern::ExchangeArgs a {};
-    a.sends = dt; a.nsend = 1; a.recvs = dt + 1; a.nrecv = nranks; a.ctas = ctas;
-    cudaError_t e = kern::LaunchExchange(cps[r], a, sim->streams[r]);
-    if (e != cudaSuccess) return (int)e;
   }
-  return Finish(nranks, cudaDeviceSynchronize());
+  if (m > max_rows) { CopyMessage("more than max_rows ranges", err, err_len); return -6; }
+  return m;
 }
 
 // Adasum over N simulated ranks: in_ptrs/out_ptrs [nranks][ntensors]; dtype fp32/fp16/bf16.

@@ -9,6 +9,7 @@
 #include "../common/logging.h"
 #include "../kernels/p2p_kernels.h"
 #include "../symm/symm_memory.h"
+#include "collective_plan.h"
 #include "cpu_ops.h"
 #include "ipc_registry.h"
 #include "nccl_baseline.h"
@@ -265,6 +266,7 @@ std::shared_ptr<SymmTeam> GpuOps::EnsureTeam(ProcessSet& ps, int device) {
 namespace {
 Status RunExchange(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, std::vector<kern::CopyDesc>& sends,
                    std::vector<kern::CopyDesc>& recvs, int max_ctas, int64_t grid_bytes);
+Status LaunchPlan(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, const Plan& plan, const char* what);
 }
 
 bool GpuOps::EnsureHierarchy(ProcessSet& ps, int device) {
@@ -924,70 +926,22 @@ Status GpuOps::Reducescatter(ProcessSet& ps, Entries& es, const Response& r, int
     }
     return FinishEvent(device, s, es.size(), done);
   }
-  const int64_t cap = (int64_t)team->buffer_bytes();
-  const int64_t region_cap = cap / n / 128 * 128;  // bytes available to one destination region
+  std::vector<PlanTensor> ts(items.size());
+  for (size_t ti = 0; ti < items.size(); ++ti) {
+    auto* e = items[ti].e;
+    int64_t row = 1;
+    for (int d = 1; d < e->shape.ndim(); ++d) row *= e->shape.dim(d);
+    ts[ti].in = e->input; ts[ti].out = e->output; ts[ti].row = row; ts[ti].dims = {e->shape.dim(0)};
+  }
+  ReduceParams rp;
+  rp.dtype = r.dtype; rp.op = r.reduce_op; rp.prescale = r.prescale; rp.postscale = r.postscale;
   const bool sum_like = r.reduce_op == ReduceOp::SUM || r.reduce_op == ReduceOp::AVERAGE;
   const bool float_wire = r.dtype == DataType::FLOAT32 || r.dtype == DataType::FLOAT16 || r.dtype == DataType::BFLOAT16;
-  // one launch over pieces {tensor, element window [w0, w0 + len) inside every destination block}
-  struct Piece { Item* it; int64_t w0, len; };
-  std::vector<Piece> seg;
-  std::vector<int64_t> used(n, 0);  // bytes used in region q by the current segment
-  auto flush = [&]() -> Status {
-    if (seg.empty()) return Status::OK();
-    const int64_t W = Align128(*std::max_element(used.begin(), used.end()));
-    std::vector<kern::TensorDesc> table;
-    table.reserve(seg.size() * (n + 1));
-    for (int q = 0; q < n; ++q) {
-      int64_t off = (int64_t)q * W;
-      for (auto& pc : seg) {
-        const int64_t c = std::max<int64_t>(0, std::min(pc.len, pc.it->cnt[q] - pc.w0));
-        kern::TensorDesc d;
-        d.in = (const char*)pc.it->e->input + (pc.it->boff[q] + pc.w0) * esz; d.out = nullptr; d.offset = off; d.count = c;
-        table.push_back(d);
-        off += Align128(std::max<int64_t>(0, std::min(pc.len, pc.it->cnt[q] - pc.w0)) * esz);
-      }
-    }
-    const int nin = (int)table.size();
-    int64_t off = (int64_t)me * W;
-    for (auto& pc : seg) {
-      const int64_t c = std::max<int64_t>(0, std::min(pc.len, pc.it->cnt[me] - pc.w0));
-      kern::TensorDesc d;
-      d.in = nullptr; d.out = (char*)pc.it->e->output + pc.w0 * esz; d.offset = off; d.count = c;
-      table.push_back(d);
-      off += Align128(c * esz);
-    }
-    kern::AllreduceArgs a {};
-    a.ndesc = nin;
-    a.total_bytes = (int64_t)n * W;
-    a.reduce_lo = (int64_t)me * W; a.reduce_hi = off;
-    a.prescale = r.prescale; a.postscale = r.postscale;
-    a.op = (int)r.reduce_op; a.dtype = (int)r.dtype; a.wire_dtype = (int)r.dtype;
-    a.variant = kern::kOneShot;
-    a.oneshot_nvls = (team->has_multicast() && sum_like && float_wire && n >= 4 && env_.variant != "oneshot" && env_.variant != "twoshot" &&
-                      a.total_bytes >= env_.params->nvls_min_bytes) ? 1 : 0;
-    a.ctas = (int)std::max<int64_t>(1, std::min<int64_t>(env_.params->comm_ctas, (a.total_bytes + 16383) / 16384));
-    const auto* dt = (const kern::TensorDesc*)ctx.Stage(device, table.data(), table.size() * sizeof(kern::TensorDesc), s);
-    if (!dt) return Status::UnknownError("descriptor table too large");
-    a.descs = dt; a.out_descs = dt + nin; a.nout = (int)seg.size();
-    kern::CommParams cp = team->Params(team->NextSlot());
-    cudaError_t ce = kern::LaunchAllreduce(cp, a, s);
-    if (ce != cudaSuccess) return Status::UnknownError(std::string("reducescatter kernel launch failed: ") + cudaGetErrorString(ce));
-    seg.clear(); used.assign(n, 0);
-    return Status::OK();
-  };
-  for (auto& it : items) {
-    const int64_t maxcnt = *std::max_element(it.cnt.begin(), it.cnt.end());
-    int64_t w0 = 0;
-    while (w0 < maxcnt) {
-      int64_t room = region_cap - *std::max_element(used.begin(), used.end());
-      if (room < 128) { Status st = flush(); if (!st.ok()) return st; room = region_cap; }
-      const int64_t len = std::min(maxcnt - w0, room / esz);
-      seg.push_back({&it, w0, len});
-      for (int q = 0; q < n; ++q) used[q] += Align128(std::max<int64_t>(0, std::min(len, it.cnt[q] - w0)) * esz);
-      w0 += len;
-    }
-  }
-  Status st = flush();
+  rp.nvls = team->has_multicast() && sum_like && float_wire && n >= 4 && env_.variant != "oneshot" && env_.variant != "twoshot";
+  rp.nvls_min_bytes = env_.params->nvls_min_bytes;
+  Plan plan;
+  Status st = PlanReducescatter(me, n, ts, rp, (int64_t)team->buffer_bytes(), (int)env_.params->comm_ctas, &plan);
+  if (st.ok()) st = LaunchPlan(*team, ctx, device, s, plan, "reducescatter");
   if (!st.ok()) return st;
   ctx.TempFreeAll(device, s);
   return FinishEvent(device, s, es.size(), done);
@@ -997,10 +951,8 @@ Status GpuOps::Reducescatter(ProcessSet& ps, Entries& es, const Response& r, int
 // allgather / broadcast / alltoall through the exchange kernel
 
 namespace {
-// `grid_bytes` sizes the grid and MUST be the same number on every rank (CTA b rendezvouses with CTA b of its peers): a
-// 4-byte broadcast is one CTA and one flag per peer, not comm_ctas of them.
-Status RunExchange(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, std::vector<kern::CopyDesc>& sends,
-                   std::vector<kern::CopyDesc>& recvs, int max_ctas, int64_t grid_bytes) {
+Status StageAndLaunchExchange(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, const std::vector<kern::CopyDesc>& sends,
+                              const std::vector<kern::CopyDesc>& recvs, int ctas) {
   std::vector<kern::CopyDesc> table(sends);
   table.insert(table.end(), recvs.begin(), recvs.end());
   kern::ExchangeArgs a {};
@@ -1009,13 +961,38 @@ Status RunExchange(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, 
   if (!table.empty() && !dt) return Status::UnknownError("descriptor table too large");
   a.sends = dt; a.nsend = (int)sends.size();
   a.recvs = dt ? dt + sends.size() : nullptr; a.nrecv = (int)recvs.size();
-  a.ctas = (int)std::max<int64_t>(1, std::min<int64_t>(max_ctas, (grid_bytes + 32767) / 32768));
+  a.ctas = ctas;
   kern::CommParams cp = team.Params(team.NextSlot());
   cudaError_t ce = kern::LaunchExchange(cp, a, s);
   if (ce != cudaSuccess) return Status::UnknownError(std::string("exchange kernel launch failed: ") + cudaGetErrorString(ce));
   return Status::OK();
 }
-int64_t Align16(int64_t b) { return (b + 15) / 16 * 16; }
+
+// `grid_bytes` sizes the grid and MUST be the same number on every rank (CTA b rendezvouses with CTA b of its peers).
+Status RunExchange(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, std::vector<kern::CopyDesc>& sends,
+                   std::vector<kern::CopyDesc>& recvs, int max_ctas, int64_t grid_bytes) {
+  return StageAndLaunchExchange(team, ctx, device, s, sends, recvs,
+                                (int)std::max<int64_t>(1, std::min<int64_t>(max_ctas, (grid_bytes + 32767) / 32768)));
+}
+
+// Stages and launches every entry of a plan (collective_plan.h) in order, each on the team's next buffer slot.
+Status LaunchPlan(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, const Plan& plan, const char* what) {
+  for (const PlanLaunch& l : plan) {
+    if (!l.reduce) {
+      Status st = StageAndLaunchExchange(team, ctx, device, s, l.sends, l.recvs, l.ctas);
+      if (!st.ok()) return st;
+      continue;
+    }
+    const auto* dt = (const kern::TensorDesc*)ctx.Stage(device, l.table.data(), l.table.size() * sizeof(kern::TensorDesc), s);
+    if (!dt) return Status::UnknownError("descriptor table too large");
+    kern::AllreduceArgs a = l.args;
+    a.descs = dt; a.out_descs = dt + a.ndesc; a.ctas = l.ctas;
+    kern::CommParams cp = team.Params(team.NextSlot());
+    cudaError_t ce = kern::LaunchAllreduce(cp, a, s);
+    if (ce != cudaSuccess) return Status::UnknownError(std::string(what) + " kernel launch failed: " + cudaGetErrorString(ce));
+  }
+  return Status::OK();
+}
 }  // namespace
 
 // A fused allgather response (several tensors, per-rank first dims in r.tensor_sizes) is ONE exchange launch: every rank
@@ -1066,47 +1043,17 @@ Status GpuOps::Allgather(ProcessSet& ps, Entries& es, const Response& r, int dev
     }
     return FinishEvent(device, s, es.size(), done);
   }
-  const int64_t cap = (int64_t)team->buffer_bytes() / 16 * 16;
-  // segment = tensors whose blocks fit together in every rank's symmetric buffer
-  std::vector<kern::CopyDesc> sends, recvs;
-  std::vector<int64_t> used(n, 0);
-  auto flush = [&]() -> Status {
-    if (sends.empty() && recvs.empty()) return Status::OK();
-    Status st = RunExchange(*team, ctx, device, s, sends, recvs, env_.params->comm_ctas, *std::max_element(used.begin(), used.end()));
-    sends.clear(); recvs.clear(); used.assign(n, 0);
-    return st;
-  };
-  for (auto& it : items) {
-    const int64_t maxb = *std::max_element(it.bytes.begin(), it.bytes.end());
-    if (maxb > cap) {
-      // one tensor larger than the buffer: windows of `cap` bytes, each its own launch
-      Status st = flush();
-      if (!st.ok()) return st;
-      for (int64_t w0 = 0; w0 < maxb; w0 += cap) {
-        int64_t mine = std::max<int64_t>(0, std::min(cap, it.bytes[me] - w0));
-        if (mine) sends.push_back({(const char*)it.e->input + w0, nullptr, 0, mine, me, 0});
-        for (int k = 0; k < n; ++k) {
-          int p = (me + k) % n;
-          int64_t b = std::max<int64_t>(0, std::min(cap, it.bytes[p] - w0));
-          if (b) recvs.push_back({nullptr, (char*)it.e->output + it.displ[p] + w0, 0, b, p, 0});
-          used[p] = b;
-        }
-        st = flush();
-        if (!st.ok()) return st;
-      }
-      continue;
-    }
-    bool fits = true;
-    for (int p = 0; p < n; ++p) if (used[p] + Align16(it.bytes[p]) > cap) fits = false;
-    if (!fits) { Status st = flush(); if (!st.ok()) return st; }
-    if (it.bytes[me]) sends.push_back({it.e->input, nullptr, used[me], it.bytes[me], me, 0});
-    for (int k = 0; k < n; ++k) {
-      int p = (me + k) % n;  // start at my own block and rotate: at any instant the N ranks pull from N different peers
-      if (it.bytes[p]) recvs.push_back({nullptr, (char*)it.e->output + it.displ[p], used[p], it.bytes[p], p, 0});
-    }
-    for (int p = 0; p < n; ++p) used[p] += Align16(it.bytes[p]);
+  std::vector<PlanTensor> ts(items.size());
+  for (size_t ti = 0; ti < items.size(); ++ti) {
+    auto* e = items[ti].e;
+    int64_t row = 1;
+    for (int d = 1; d < e->shape.ndim(); ++d) row *= e->shape.dim(d);
+    ts[ti].in = e->input; ts[ti].out = e->output; ts[ti].row = row;
+    ts[ti].dims.assign(r.tensor_sizes.begin() + ti * n, r.tensor_sizes.begin() + (ti + 1) * n);
   }
-  Status st = flush();
+  Plan plan;
+  Status st = PlanAllgather(me, n, ts, esz, (int64_t)team->buffer_bytes(), (int)env_.params->comm_ctas, &plan);
+  if (st.ok()) st = LaunchPlan(*team, ctx, device, s, plan, "allgather");
   if (!st.ok()) return st;
   return FinishEvent(device, s, es.size(), done);
 }
@@ -1140,31 +1087,13 @@ Status GpuOps::Broadcast(ProcessSet& ps, Entries& es, const Response& r, int dev
     return FinishEvent(device, s, es.size(), done);
   }
   const bool use_mc = env_.broadcast_multicast && team->has_multicast() && n > 2;
-  const int64_t cap = (int64_t)team->buffer_bytes() / 16 * 16;
-  std::vector<kern::CopyDesc> sends, recvs;
-  int64_t used = 0;
-  auto flush = [&]() -> Status {
-    if (used == 0) return Status::OK();
-    Status st = RunExchange(*team, ctx, device, s, sends, recvs, env_.params->comm_ctas, used);
-    sends.clear(); recvs.clear(); used = 0;
-    return st;
-  };
-  auto add = [&](const char* in, char* out, int64_t b) {
-    if (me == root) sends.push_back({in, nullptr, used, b, me, use_mc ? kern::kSendMulticast : 0});
-    if (me != root || (out && out != in)) recvs.push_back({nullptr, out, used, b, use_mc ? me : root, 0});
-    used += Align16(b);
-  };
-  for (auto& e : es) {
-    const int64_t bytes = (int64_t)e->bytes();
-    if (bytes == 0) continue;
-    for (int64_t w0 = 0; w0 < bytes; ) {
-      if (cap - used < 16) { Status st = flush(); if (!st.ok()) return st; }
-      const int64_t b = std::min(cap - used, bytes - w0);
-      add((const char*)e->input + w0, e->output ? (char*)e->output + w0 : nullptr, b);
-      w0 += b;
-    }
+  std::vector<PlanTensor> ts(es.size());
+  for (size_t ti = 0; ti < es.size(); ++ti) {
+    ts[ti].in = es[ti]->input; ts[ti].out = es[ti]->output; ts[ti].dims = {(int64_t)es[ti]->bytes()};
   }
-  Status st = flush();
+  Plan plan;
+  Status st = PlanBroadcast(me, n, root, ts, use_mc, (int64_t)team->buffer_bytes(), (int)env_.params->comm_ctas, &plan);
+  if (st.ok()) st = LaunchPlan(*team, ctx, device, s, plan, "broadcast");
   if (!st.ok()) return st;
   return FinishEvent(device, s, es.size(), done);
 }
@@ -1211,26 +1140,12 @@ Status GpuOps::Alltoall(ProcessSet& ps, Entries& es, const Response& r, int devi
       HVD_CUDA(cudaStreamSynchronize(s));
       continue;
     }
-    // window scheme: destination q's block occupies [q*win, (q+1)*win) of the sender's buffer
-    int64_t maxblock = 0;
-    for (size_t i = 0; i < all.size(); ++i) maxblock = std::max(maxblock, all[i] * row * esz);
-    const int64_t cap = (int64_t)team->buffer_bytes();
-    const int64_t win = std::min<int64_t>((maxblock + 15) / 16 * 16, cap / n / 16 * 16);
-    if (win <= 0) continue;
-    for (int64_t w0 = 0; w0 < maxblock; w0 += win) {
-      std::vector<kern::CopyDesc> sends, recvs;
-      for (int q = 0; q < n; ++q) {
-        int64_t b = std::max<int64_t>(0, std::min(win, sbytes[q] - w0));
-        if (b) sends.push_back({(const char*)e->input + sdisp[q] + w0, nullptr, q * win, b, me, 0});
-      }
-      for (int k = 0; k < n; ++k) {
-        int p = (me + k) % n;
-        int64_t b = std::max<int64_t>(0, std::min(win, rbytes[p] - w0));
-        if (b) recvs.push_back({nullptr, (char*)e->output + rdisp[p] + w0, me * win, b, p, 0});
-      }
-      Status st = RunExchange(*team, ctx, device, s, sends, recvs, env_.params->comm_ctas, std::min<int64_t>(maxblock - w0, win) * n);
-      if (!st.ok()) return st;
-    }
+    PlanTensor t;
+    t.in = e->input; t.out = e->output; t.row = row; t.dims = all;
+    Plan plan;
+    Status st = PlanAlltoall(me, n, {t}, esz, (int64_t)team->buffer_bytes(), (int)env_.params->comm_ctas, &plan);
+    if (st.ok()) st = LaunchPlan(*team, ctx, device, s, plan, "alltoall");
+    if (!st.ok()) return st;
   }
   return FinishEvent(device, s, es.size(), done);
 }

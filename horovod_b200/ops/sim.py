@@ -3,7 +3,12 @@
 Every "rank" is a set of plain device tensors plus a kernel of its own on its own stream; the cross-"GPU" flag
 protocol, chunk ownership and descriptor walking are exactly what runs across NVLink — only the address mapping differs.
 All functions take lists indexed [rank][tensor] of CUDA tensors and return the average milliseconds per repeat where that
-makes sense.  A non-zero native return code raises RuntimeError (-3 = a barrier of the simulation timed out).
+makes sense.  A non-zero native return code raises RuntimeError (-3 = a barrier of the simulation timed out, -4 = the
+ranks' launch plans disagree and nothing was launched, -5 = no plan fits the buffer size `cap`).
+
+reducescatter / allgatherv / broadcast / alltoallv run the launch plans of the engine's ops (csrc/ops/collective_plan.h)
+for every simulated rank, check that the plans agree and only then launch them.  `cap` is the symmetric buffer size one
+launch may use: small caps force the windowed multi-launch paths.
 """
 import ctypes
 
@@ -32,13 +37,21 @@ def lib():
         L.hvd_sim_inplace_reducescatter.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int64, u64p, ctypes.c_int, ctypes.c_int,
                                                     ctypes.c_int, ctypes.c_double, ctypes.c_int]
         L.hvd_sim_inplace_allgather.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int64, u64p, ctypes.c_int, ctypes.c_int]
+        plan = [ctypes.c_int, ctypes.c_int, ctypes.c_int, i64p, i64p]
+        L.hvd_sim_reducescatter.argtypes = plan + [u64p, u64p, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_double,
+                                                   ctypes.c_int64, ctypes.c_int]
+        L.hvd_sim_allgatherv.argtypes = plan + [ctypes.c_int, u64p, u64p, ctypes.c_int64, ctypes.c_int]
+        L.hvd_sim_broadcast.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, i64p, ctypes.c_int, u64p, u64p, ctypes.c_int64,
+                                        ctypes.c_int]
+        L.hvd_sim_alltoallv.argtypes = plan + [ctypes.c_int, u64p, u64p, ctypes.c_int64, ctypes.c_int]
         _lib = L
     return _lib
 
 
 def _check(rc, what):
     if rc != 0:
-        raise RuntimeError('%s failed with code %d%s' % (what, rc, ' (simulated barrier timed out)' if rc == -3 else ''))
+        why = {-3: ' (simulated barrier timed out)', -4: ' (the ranks\' launch plans disagree)', -5: ' (no plan fits the buffer)'}
+        raise RuntimeError('%s failed with code %d%s' % (what, rc, why.get(rc, '')))
 
 
 def _ptrs(rows):
@@ -101,3 +114,50 @@ def adasum(ins, outs, ctas=8, prescale=1.0, postscale=1.0, device=0):
     counts = (ctypes.c_int64 * t)(*[x.numel() for x in ins[0]])
     _check(lib().hvd_sim_adasum(n, device, t, counts, _ptrs(ins), _ptrs(outs), DTYPE_CODE[ins[0][0].dtype], ctas, prescale, postscale),
            'sim adasum')
+
+
+def _i64(vals):
+    vals = [int(v) for v in vals]
+    return (ctypes.c_int64 * max(len(vals), 1))(*vals)
+
+
+def _row(t):
+    r = 1
+    for d in t.shape[1:]:
+        r *= d
+    return r
+
+
+def reducescatter(ins, outs, op=SUM, prescale=1.0, postscale=1.0, cap=1 << 20, ctas=8, device=0):
+    """ins[r][t]: rank r's whole tensor t (the same shape on every rank); outs[r][t]: rank r's block of the result, dim 0
+    split as the engine splits it (the first dim0 % n ranks get one extra row).  One-shot reduce, rank order 0 .. n-1."""
+    n, t = len(ins), len(ins[0])
+    x = ins[0]
+    _check(lib().hvd_sim_reducescatter(n, device, t, _i64(a.shape[0] for a in x), _i64(_row(a) for a in x), _ptrs(ins), _ptrs(outs),
+                                       DTYPE_CODE[x[0].dtype], op, prescale, postscale, cap, ctas), 'sim reducescatter')
+
+
+def allgatherv(ins, outs, cap=1 << 20, ctas=8, device=0):
+    """ins[r][t]: rank r's contribution to tensor t (first dims may differ per rank, may be 0); outs[r][t]: the
+    concatenation along dim 0 in rank order."""
+    n, t = len(ins), len(ins[0])
+    dims = [ins[r][i].shape[0] for i in range(t) for r in range(n)]
+    _check(lib().hvd_sim_allgatherv(n, device, t, _i64(dims), _i64(_row(a) for a in ins[0]), DTYPE_CODE[ins[0][0].dtype], _ptrs(ins),
+                                    _ptrs(outs), cap, ctas), 'sim allgatherv')
+
+
+def broadcast(ins, outs, root, cap=1 << 20, ctas=8, device=0):
+    """ins[r][t] / outs[r][t]: every rank's tensors (the same byte sizes); outs[root][t] is ins[root][t] for an in-place
+    broadcast.  Only the root's inputs are read."""
+    n, t = len(ins), len(ins[0])
+    nbytes = [a.numel() * a.element_size() for a in ins[0]]
+    _check(lib().hvd_sim_broadcast(n, device, t, _i64(nbytes), root, _ptrs(ins), _ptrs(outs), cap, ctas), 'sim broadcast')
+
+
+def alltoallv(ins, outs, splits, cap=1 << 20, ctas=8, device=0):
+    """splits[t][p][q]: rows of tensor t that rank p sends to rank q (rank p's ins[p][t] holds them in q order); outs[q][t]
+    receives them in p order."""
+    n, t = len(ins), len(ins[0])
+    flat = [splits[i][p][q] for i in range(t) for p in range(n) for q in range(n)]
+    _check(lib().hvd_sim_alltoallv(n, device, t, _i64(flat), _i64(_row(a) for a in ins[0]), DTYPE_CODE[ins[0][0].dtype], _ptrs(ins),
+                                   _ptrs(outs), cap, ctas), 'sim alltoallv')
