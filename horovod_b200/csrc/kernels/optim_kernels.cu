@@ -70,17 +70,17 @@ template <typename P> __device__ __forceinline__ void reconcile4(float* pv, cons
 // Momentum is stored in the parameter dtype, or in fp32 with a master.
 template <typename P, typename G, bool kMaster>
 __global__ void __launch_bounds__(kOptThreads)
-fused_sgd_kernel(const SgdTensor* __restrict__ table, float lr, float momentum, float dampening, float wd, int nesterov,
+fused_sgd_kernel(const OptTensor* __restrict__ table, float lr, float momentum, float dampening, float wd, int nesterov,
                  float grad_scale, const float* __restrict__ grad_scale_dev, int first_step) {
   using M = std::conditional_t<kMaster, float, P>;
-  const SgdTensor t = table[blockIdx.y];
+  const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
   if (base >= n) return;
   grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
   P* p = reinterpret_cast<P*>(t.param);
   const G* g = reinterpret_cast<const G*>(t.grad);
-  M* mbuf = reinterpret_cast<M*>(t.momentum);
+  M* mbuf = reinterpret_cast<M*>(t.state0);
   float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
   // pa: the parameter (and, without a master, the momentum); wa: the fp32 master and momentum
   const bool pa = is_aligned<P>(p) && (kMaster || !mbuf || is_aligned<M>(mbuf)), ga = is_aligned<G>(g);
@@ -118,17 +118,17 @@ fused_sgd_kernel(const SgdTensor* __restrict__ table, float lr, float momentum, 
 
 template <typename P, typename G, bool kMaster>
 __global__ void __launch_bounds__(kOptThreads)
-fused_adam_kernel(const AdamTensor* __restrict__ table, float lr, float b1, float b2, float eps, float wd, float c1, float c2,
+fused_adam_kernel(const OptTensor* __restrict__ table, float lr, float b1, float b2, float eps, float wd, float c1, float c2,
                   float grad_scale, const float* __restrict__ grad_scale_dev, int adamw) {
-  const AdamTensor t = table[blockIdx.y];
+  const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
   if (base >= n) return;
   grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
   P* p = reinterpret_cast<P*>(t.param);
   const G* g = reinterpret_cast<const G*>(t.grad);
-  float* m = reinterpret_cast<float*>(t.exp_avg);
-  float* v = reinterpret_cast<float*>(t.exp_avg_sq);
+  float* m = reinterpret_cast<float*>(t.state0);
+  float* v = reinterpret_cast<float*>(t.state1);
   float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
   const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g),
              sa = is_aligned<float>(m) && is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
@@ -176,18 +176,18 @@ __device__ __forceinline__ float lamb_u(float m, float v, float w, float c1, flo
 
 template <typename P, typename G, bool kMaster>
 __global__ void __launch_bounds__(kOptThreads)
-fused_lamb_norms_kernel(const LambTensor* __restrict__ table, float b1, float b2, float eps, float wd, float c1, float c2,
+fused_lamb_norms_kernel(const OptTensor* __restrict__ table, float b1, float b2, float eps, float wd, float c1, float c2,
                         float grad_scale, const float* __restrict__ grad_scale_dev, float2* __restrict__ partial) {
   __shared__ float2 red[kOptThreads / 32];
-  const LambTensor t = table[blockIdx.y];
+  const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
   if (base >= n) return;
   grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
   const P* p = reinterpret_cast<const P*>(t.param);
   const G* g = reinterpret_cast<const G*>(t.grad);
-  float* m = reinterpret_cast<float*>(t.exp_avg);
-  float* v = reinterpret_cast<float*>(t.exp_avg_sq);
+  float* m = reinterpret_cast<float*>(t.state0);
+  float* v = reinterpret_cast<float*>(t.state1);
   const float* w = kMaster ? reinterpret_cast<const float*>(t.master) : nullptr;
   const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g),
              sa = is_aligned<float>(m) && is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
@@ -238,9 +238,9 @@ fused_lamb_norms_kernel(const LambTensor* __restrict__ table, float b1, float b2
 // One CTA per entry: its partials in fp64, a fixed strided subset per thread, then a fixed tree; added into its slot.
 // Every slot appears at most once per launch (checked by the host), so the read-modify-write does not race.
 __global__ void __launch_bounds__(kOptThreads)
-lamb_finalize_kernel(const LambTensor* __restrict__ table, const float2* __restrict__ partial, float* __restrict__ norms) {
+lamb_finalize_kernel(const OptTensor* __restrict__ table, const float2* __restrict__ partial, float* __restrict__ norms) {
   __shared__ double rw[kOptThreads], ru[kOptThreads];
-  const LambTensor t = table[blockIdx.x];
+  const OptTensor t = table[blockIdx.x];
   const int64_t nb = (t.count + kOptPerBlock - 1) / kOptPerBlock;
   double a = 0.0, b = 0.0;
   for (int64_t j = threadIdx.x; j < nb; j += kOptThreads) {
@@ -264,9 +264,9 @@ lamb_finalize_kernel(const LambTensor* __restrict__ table, const float2* __restr
 
 template <typename P, bool kMaster>
 __global__ void __launch_bounds__(kOptThreads)
-fused_lamb_apply_kernel(const LambTensor* __restrict__ table, float lr, float eps, float wd, float c1, float c2, int adapt,
+fused_lamb_apply_kernel(const OptTensor* __restrict__ table, float lr, float eps, float wd, float c1, float c2, int adapt,
                         const float* __restrict__ norms) {
-  const LambTensor t = table[blockIdx.y];
+  const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
   if (base >= n) return;
@@ -277,8 +277,8 @@ fused_lamb_apply_kernel(const LambTensor* __restrict__ table, float lr, float ep
   }
   const float step = lr * r;
   P* p = reinterpret_cast<P*>(t.param);
-  const float* m = reinterpret_cast<const float*>(t.exp_avg);
-  const float* v = reinterpret_cast<const float*>(t.exp_avg_sq);
+  const float* m = reinterpret_cast<const float*>(t.state0);
+  const float* v = reinterpret_cast<const float*>(t.state1);
   float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
   const bool pa = is_aligned<P>(p), sa = is_aligned<float>(m) && is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
 #pragma unroll
@@ -304,15 +304,15 @@ fused_lamb_apply_kernel(const LambTensor* __restrict__ table, float lr, float ep
 // LARS (You, Gitman, Ginsburg, "Large Batch Training of Convolutional Networks"; the MLPerf ResNet-50 optimizer): with
 // g the scaled gradient, d = g + wd * w, the per-tensor trust ratio r = tc * ||w|| / (||g|| + wd * ||w|| + eps) (1 if
 // either norm is 0, or if the caller does not adapt), v = momentum * v + lr * r * d, w -= v.  LAMB's three launches and
-// table, with the fp32 momentum buffer in `exp_avg` (`exp_avg_sq` is not read): stage 1 writes one (sum w^2, sum g^2)
+// table, with the fp32 momentum buffer in `state0` (`state1` is not read): stage 1 writes one (sum w^2, sum g^2)
 // partial per CTA, lamb_finalize_kernel adds them into norms[2 * slot], norms[2 * slot + 1], and stage 2 reads the
 // gradient again and applies the update.  Both stages scale the gradient alike.
 template <typename P, typename G, bool kMaster>
 __global__ void __launch_bounds__(kOptThreads)
-fused_lars_norms_kernel(const LambTensor* __restrict__ table, float grad_scale, const float* __restrict__ grad_scale_dev,
+fused_lars_norms_kernel(const OptTensor* __restrict__ table, float grad_scale, const float* __restrict__ grad_scale_dev,
                         float2* __restrict__ partial) {
   __shared__ float2 red[kOptThreads / 32];
-  const LambTensor t = table[blockIdx.y];
+  const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
   if (base >= n) return;
@@ -358,9 +358,9 @@ fused_lars_norms_kernel(const LambTensor* __restrict__ table, float grad_scale, 
 
 template <typename P, typename G, bool kMaster>
 __global__ void __launch_bounds__(kOptThreads)
-fused_lars_apply_kernel(const LambTensor* __restrict__ table, float lr, float momentum, float wd, float tc, float eps,
+fused_lars_apply_kernel(const OptTensor* __restrict__ table, float lr, float momentum, float wd, float tc, float eps,
                         int adapt, float grad_scale, const float* __restrict__ grad_scale_dev, const float* __restrict__ norms) {
-  const LambTensor t = table[blockIdx.y];
+  const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
   if (base >= n) return;
@@ -373,7 +373,7 @@ fused_lars_apply_kernel(const LambTensor* __restrict__ table, float lr, float mo
   const float step = lr * r;
   P* p = reinterpret_cast<P*>(t.param);
   const G* g = reinterpret_cast<const G*>(t.grad);
-  float* v = reinterpret_cast<float*>(t.exp_avg);
+  float* v = reinterpret_cast<float*>(t.state0);
   float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
   const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g), sa = is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
 #pragma unroll
@@ -530,139 +530,112 @@ grad_accumulate_kernel(const AccTable table, int mode) {
   }
 }
 
-}  // namespace
+// The (param, grad, master) instantiations of the optimizer kernels: launch(OptTypes<P, G, kMaster>()) for a pair that
+// has one, then the launch is counted and checked; cudaErrorInvalidValue without launching for any other pair.
+template <typename P_, typename G_, bool kMaster_> struct OptTypes {
+  using P = P_;
+  using G = G_;
+  static constexpr bool kMaster = kMaster_;
+};
 
-cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
-                           float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
-                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev, bool master) {
-  if (n <= 0 || max_count <= 0) return cudaSuccess;
-  dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)n);
+template <typename F> cudaError_t DispatchOpt(int param_dtype, int grad_dtype, bool master, F&& launch) {
   if (master) {
-    if (param_dtype == 10 && grad_dtype == 10) fused_sgd_kernel<__nv_bfloat16, __nv_bfloat16, true><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
-    else if (param_dtype == 6 && grad_dtype == 6) fused_sgd_kernel<__half, __half, true><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+    if (param_dtype == 10 && grad_dtype == 10) launch(OptTypes<__nv_bfloat16, __nv_bfloat16, true>());
+    else if (param_dtype == 6 && grad_dtype == 6) launch(OptTypes<__half, __half, true>());
     else return cudaErrorInvalidValue;
   }
-  else if (param_dtype == 7 && grad_dtype == 7) fused_sgd_kernel<float, float, false><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
-  else if (param_dtype == 7 && grad_dtype == 10) fused_sgd_kernel<float, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
-  else if (param_dtype == 10 && grad_dtype == 10) fused_sgd_kernel<__nv_bfloat16, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
-  else if (param_dtype == 6 && grad_dtype == 6) fused_sgd_kernel<__half, __half, false><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  else if (param_dtype == 7 && grad_dtype == 7) launch(OptTypes<float, float, false>());
+  else if (param_dtype == 7 && grad_dtype == 10) launch(OptTypes<float, __nv_bfloat16, false>());
+  else if (param_dtype == 10 && grad_dtype == 10) launch(OptTypes<__nv_bfloat16, __nv_bfloat16, false>());
+  else if (param_dtype == 6 && grad_dtype == 6) launch(OptTypes<__half, __half, false>());
   else return cudaErrorInvalidValue;
   CountKernelLaunch();
   return cudaGetLastError();
 }
 
-cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
-                             float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale, int adamw,
-                             int param_dtype, int grad_dtype, cudaStream_t stream, const float* grad_scale_dev,
-                             bool master) {
-  if (n <= 0 || max_count <= 0) return cudaSuccess;
-  dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)n);
-  if (master) {
-    if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16, true><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-    else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half, true><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-    else return cudaErrorInvalidValue;
-  }
-  else if (param_dtype == 7 && grad_dtype == 7) fused_adam_kernel<float, float, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-  else if (param_dtype == 7 && grad_dtype == 10) fused_adam_kernel<float, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-  else if (param_dtype == 10 && grad_dtype == 10) fused_adam_kernel<__nv_bfloat16, __nv_bfloat16, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-  else if (param_dtype == 6 && grad_dtype == 6) fused_adam_kernel<__half, __half, false><<<grid, kOptThreads, 0, stream>>>(table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
-  else return cudaErrorInvalidValue;
-  CountKernelLaunch();
-  return cudaGetLastError();
-}
+// blockIdx.x covers the longest entry, blockIdx.y selects the entry
+dim3 OptGrid(int n, int64_t max_count) { return dim3((unsigned)NormPartials(max_count), (unsigned)n); }
 
-int64_t LambPartials(int64_t count) { return (count + kOptPerBlock - 1) / kOptPerBlock; }
-
-// After a stage-1 launch: count it, then add each entry's partials into its norm slot.
-static cudaError_t FinalizeNorms(const LambTensor* table, int n, const float2* part, float* norms, cudaStream_t stream) {
-  CountKernelLaunch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
+// After a stage-1 launch: add each entry's partials into its norm slot.
+cudaError_t FinalizeNorms(cudaError_t stage1, const OptTensor* table, int n, const float2* part, float* norms,
+                          cudaStream_t stream) {
+  if (stage1 != cudaSuccess) return stage1;
   lamb_finalize_kernel<<<(unsigned)n, kOptThreads, 0, stream>>>(table, part, norms);
   CountKernelLaunch();
   return cudaGetLastError();
 }
 
-cudaError_t LaunchLambNorms(const LambTensor* table, int n, int64_t max_count, float beta1, float beta2, float eps,
+}  // namespace
+
+int64_t NormPartials(int64_t count) { return (count + kOptPerBlock - 1) / kOptPerBlock; }
+
+cudaError_t LaunchFusedSgd(const OptTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
+                           float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
+                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev, bool master) {
+  if (n <= 0 || max_count <= 0) return cudaSuccess;
+  return DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    fused_sgd_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+        table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+  });
+}
+
+cudaError_t LaunchFusedAdamW(const OptTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
+                             float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale, int adamw,
+                             int param_dtype, int grad_dtype, cudaStream_t stream, const float* grad_scale_dev,
+                             bool master) {
+  if (n <= 0 || max_count <= 0) return cudaSuccess;
+  return DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    fused_adam_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+        table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+  });
+}
+
+cudaError_t LaunchLambNorms(const OptTensor* table, int n, int64_t max_count, float beta1, float beta2, float eps,
                             float weight_decay, float bias_c1, float bias_c2, float grad_scale, const float* grad_scale_dev,
                             float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
-  dim3 grid((unsigned)LambPartials(max_count), (unsigned)n);
   float2* part = reinterpret_cast<float2*>(partial);
-#define HVD_LAMB_NORMS(P, G, M) fused_lamb_norms_kernel<P, G, M><<<grid, kOptThreads, 0, stream>>>(table, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, part)
-  if (master) {
-    if (param_dtype == 10 && grad_dtype == 10) HVD_LAMB_NORMS(__nv_bfloat16, __nv_bfloat16, true);
-    else if (param_dtype == 6 && grad_dtype == 6) HVD_LAMB_NORMS(__half, __half, true);
-    else return cudaErrorInvalidValue;
-  }
-  else if (param_dtype == 7 && grad_dtype == 7) HVD_LAMB_NORMS(float, float, false);
-  else if (param_dtype == 7 && grad_dtype == 10) HVD_LAMB_NORMS(float, __nv_bfloat16, false);
-  else if (param_dtype == 10 && grad_dtype == 10) HVD_LAMB_NORMS(__nv_bfloat16, __nv_bfloat16, false);
-  else if (param_dtype == 6 && grad_dtype == 6) HVD_LAMB_NORMS(__half, __half, false);
-  else return cudaErrorInvalidValue;
-#undef HVD_LAMB_NORMS
-  return FinalizeNorms(table, n, part, norms, stream);
+  return FinalizeNorms(DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    fused_lamb_norms_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+        table, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, part);
+  }), table, n, part, norms, stream);
 }
 
-cudaError_t LaunchLambApply(const LambTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
+cudaError_t LaunchLambApply(const OptTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
                             float bias_c1, float bias_c2, int adapt, const float* norms, int param_dtype, bool master,
                             cudaStream_t stream) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
-  dim3 grid((unsigned)LambPartials(max_count), (unsigned)n);
-#define HVD_LAMB_APPLY(P, M) fused_lamb_apply_kernel<P, M><<<grid, kOptThreads, 0, stream>>>(table, lr, eps, weight_decay, bias_c1, bias_c2, adapt, norms)
-  if (master) {
-    if (param_dtype == 10) HVD_LAMB_APPLY(__nv_bfloat16, true);
-    else if (param_dtype == 6) HVD_LAMB_APPLY(__half, true);
-    else return cudaErrorInvalidValue;
-  }
-  else if (param_dtype == 7) HVD_LAMB_APPLY(float, false);
-  else if (param_dtype == 10) HVD_LAMB_APPLY(__nv_bfloat16, false);
-  else if (param_dtype == 6) HVD_LAMB_APPLY(__half, false);
-  else return cudaErrorInvalidValue;
-#undef HVD_LAMB_APPLY
-  CountKernelLaunch();
-  return cudaGetLastError();
+  // the gradient is not read: dispatch on the parameter dtype alone
+  return DispatchOpt(param_dtype, param_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    fused_lamb_apply_kernel<typename T::P, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+        table, lr, eps, weight_decay, bias_c1, bias_c2, adapt, norms);
+  });
 }
 
-cudaError_t LaunchLarsNorms(const LambTensor* table, int n, int64_t max_count, float grad_scale, const float* grad_scale_dev,
+cudaError_t LaunchLarsNorms(const OptTensor* table, int n, int64_t max_count, float grad_scale, const float* grad_scale_dev,
                             float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
-  dim3 grid((unsigned)LambPartials(max_count), (unsigned)n);
   float2* part = reinterpret_cast<float2*>(partial);
-#define HVD_LARS_NORMS(P, G, M) fused_lars_norms_kernel<P, G, M><<<grid, kOptThreads, 0, stream>>>(table, grad_scale, grad_scale_dev, part)
-  if (master) {
-    if (param_dtype == 10 && grad_dtype == 10) HVD_LARS_NORMS(__nv_bfloat16, __nv_bfloat16, true);
-    else if (param_dtype == 6 && grad_dtype == 6) HVD_LARS_NORMS(__half, __half, true);
-    else return cudaErrorInvalidValue;
-  }
-  else if (param_dtype == 7 && grad_dtype == 7) HVD_LARS_NORMS(float, float, false);
-  else if (param_dtype == 7 && grad_dtype == 10) HVD_LARS_NORMS(float, __nv_bfloat16, false);
-  else if (param_dtype == 10 && grad_dtype == 10) HVD_LARS_NORMS(__nv_bfloat16, __nv_bfloat16, false);
-  else if (param_dtype == 6 && grad_dtype == 6) HVD_LARS_NORMS(__half, __half, false);
-  else return cudaErrorInvalidValue;
-#undef HVD_LARS_NORMS
-  return FinalizeNorms(table, n, part, norms, stream);
+  return FinalizeNorms(DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    fused_lars_norms_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+        table, grad_scale, grad_scale_dev, part);
+  }), table, n, part, norms, stream);
 }
 
-cudaError_t LaunchLarsApply(const LambTensor* table, int n, int64_t max_count, float lr, float momentum, float weight_decay,
+cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, float lr, float momentum, float weight_decay,
                             float trust_coefficient, float eps, int adapt, float grad_scale, const float* grad_scale_dev,
                             const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
-  dim3 grid((unsigned)LambPartials(max_count), (unsigned)n);
-#define HVD_LARS_APPLY(P, G, M) fused_lars_apply_kernel<P, G, M><<<grid, kOptThreads, 0, stream>>>(table, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, grad_scale_dev, norms)
-  if (master) {
-    if (param_dtype == 10 && grad_dtype == 10) HVD_LARS_APPLY(__nv_bfloat16, __nv_bfloat16, true);
-    else if (param_dtype == 6 && grad_dtype == 6) HVD_LARS_APPLY(__half, __half, true);
-    else return cudaErrorInvalidValue;
-  }
-  else if (param_dtype == 7 && grad_dtype == 7) HVD_LARS_APPLY(float, float, false);
-  else if (param_dtype == 7 && grad_dtype == 10) HVD_LARS_APPLY(float, __nv_bfloat16, false);
-  else if (param_dtype == 10 && grad_dtype == 10) HVD_LARS_APPLY(__nv_bfloat16, __nv_bfloat16, false);
-  else if (param_dtype == 6 && grad_dtype == 6) HVD_LARS_APPLY(__half, __half, false);
-  else return cudaErrorInvalidValue;
-#undef HVD_LARS_APPLY
-  CountKernelLaunch();
-  return cudaGetLastError();
+  return DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    fused_lars_apply_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+        table, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, grad_scale_dev, norms);
+  });
 }
 
 int64_t GradShardStatsCtas(int n, int64_t max_count) {

@@ -177,41 +177,46 @@ cudaError_t LaunchAdasumStep(const CommParams& cp, const AdasumArgs& args, doubl
                              int only);
 int AdasumNumLaunches(int nranks);
 
-// Fused multi-tensor optimizer updates (see optim_kernels.cu).  The gradient factor is grad_scale * *grad_scale_dev
-// (nullptr: grad_scale alone, bit for bit).  `master` (bf16 / bf16 and fp16 / fp16 only): every entry's `master` is an
-// fp32 copy of its parameter that the update runs on (SGD momentum is then fp32); without it `master` is not read.
-struct SgdTensor { void* param; const void* grad; void* momentum; int64_t count; void* master; };
-cudaError_t LaunchFusedSgd(const SgdTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
+// Fused multi-tensor optimizer updates (see optim_kernels.cu).  One table entry type serves SGD, Adam(W), LAMB and LARS:
+//   param, grad    the parameter and its gradient, `count` elements each
+//   master         with `master` set: the fp32 copy of the parameter that the update runs on; otherwise not read
+//   state0         SGD and LARS: the momentum buffer (SGD: nullptr without momentum); Adam and LAMB: exp_avg
+//   state1         Adam and LAMB: exp_avg_sq; SGD and LARS do not read it
+//   partial, slot  LAMB and LARS only: the entry's first stage-1 partial and its norm slot (see LaunchLambNorms)
+// Every state is fp32, except SGD momentum without `master`, which has the parameter dtype.  The (param, grad) dtypes are
+// fp32 / fp32, fp32 / bf16, bf16 / bf16 and fp16 / fp16; with `master` bf16 / bf16 and fp16 / fp16 only.  Any other
+// combination returns cudaErrorInvalidValue before anything is launched.  The gradient factor is
+// grad_scale * *grad_scale_dev (nullptr: grad_scale alone, bit for bit).
+struct OptTensor { void* param; const void* grad; void* master; void* state0; void* state1; int64_t count;
+                   int64_t partial; int64_t slot; };
+cudaError_t LaunchFusedSgd(const OptTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
                            float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
                            int grad_dtype, cudaStream_t stream, const float* grad_scale_dev = nullptr, bool master = false);
-struct AdamTensor { void* param; const void* grad; void* exp_avg; void* exp_avg_sq; int64_t count; void* master; };
-cudaError_t LaunchFusedAdamW(const AdamTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
+cudaError_t LaunchFusedAdamW(const OptTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
                              float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale,
                              int adamw, int param_dtype, int grad_dtype, cudaStream_t stream,
                              const float* grad_scale_dev = nullptr, bool master = false);
 // Fused LAMB in two phases (see optim_kernels.cu), so that the norms can be allreduced in between.  Entry i covers
 // `count` elements of a parameter whose whole-tensor norms live in norms[2 * slot] (sum w^2) and norms[2 * slot + 1]
-// (sum u^2); its stage-1 CTA partials start at `partial`, the running sum of LambPartials(count) over the entries before
+// (sum u^2); its stage-1 CTA partials start at `partial`, the running sum of NormPartials(count) over the entries before
 // it.  No two entries of one launch may share a slot.
 // LaunchLambNorms: moments updated, then the entries' squared norms ADDED into `norms` (two launches; `partial` holds
-// 2 * sum LambPartials floats).  LaunchLambApply: w -= lr * r * u (one launch; the gradient is not read).  (param, grad)
-// dtypes as LaunchFusedAdamW, `master` likewise.
-struct LambTensor { void* param; const void* grad; void* exp_avg; void* exp_avg_sq; int64_t count; void* master;
-                    int64_t partial; int64_t slot; };
-int64_t LambPartials(int64_t count);
-cudaError_t LaunchLambNorms(const LambTensor* table, int n, int64_t max_count, float beta1, float beta2, float eps,
+// 2 * sum NormPartials floats).  LaunchLambApply: w -= lr * r * u (one launch; the gradient is not read, so only the
+// parameter dtype is checked).
+int64_t NormPartials(int64_t count);
+cudaError_t LaunchLambNorms(const OptTensor* table, int n, int64_t max_count, float beta1, float beta2, float eps,
                             float weight_decay, float bias_c1, float bias_c2, float grad_scale, const float* grad_scale_dev,
                             float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
-cudaError_t LaunchLambApply(const LambTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
+cudaError_t LaunchLambApply(const OptTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
                             float bias_c1, float bias_c2, int adapt, const float* norms, int param_dtype, bool master,
                             cudaStream_t stream);
-// Fused LARS on LAMB's table and norms layout, the fp32 momentum buffer in `exp_avg` (`exp_avg_sq` unused): norms[2 * slot]
-// = sum w^2, norms[2 * slot + 1] = sum g^2 of the scaled gradient.  LaunchLarsNorms: two launches, nothing but `partial`
-// and `norms` written.  LaunchLarsApply: v = momentum * v + lr * r * (g + wd * w), w -= v (one launch; reads the gradient
-// again, scaled by grad_scale * *grad_scale_dev as in the first phase).  (param, grad) dtypes and `master` as LAMB's.
-cudaError_t LaunchLarsNorms(const LambTensor* table, int n, int64_t max_count, float grad_scale, const float* grad_scale_dev,
+// Fused LARS on LAMB's table and norms layout: norms[2 * slot] = sum w^2, norms[2 * slot + 1] = sum g^2 of the scaled
+// gradient.  LaunchLarsNorms: two launches, nothing but `partial` and `norms` written.  LaunchLarsApply:
+// v = momentum * v + lr * r * (g + wd * w), w -= v (one launch; reads the gradient again, scaled by
+// grad_scale * *grad_scale_dev as in the first phase).
+cudaError_t LaunchLarsNorms(const OptTensor* table, int n, int64_t max_count, float grad_scale, const float* grad_scale_dev,
                             float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
-cudaError_t LaunchLarsApply(const LambTensor* table, int n, int64_t max_count, float lr, float momentum, float weight_decay,
+cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, float lr, float momentum, float weight_decay,
                             float trust_coefficient, float eps, int adapt, float grad_scale, const float* grad_scale_dev,
                             const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
 // Gradient statistics of flat gradient shards in one pass (see optim_kernels.cu): optional in-place scaling by

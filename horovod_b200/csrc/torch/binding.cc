@@ -533,194 +533,164 @@ bool CheckMasters(const char* op, const std::vector<at::Tensor>& params, const s
   return true;
 }
 
-void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momenta, double lr,
-                  double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step,
-                  c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
-  const bool has_mom = momentum != 0.0;
-  TORCH_CHECK(params.size() == grads.size(), "fused_sgd: list sizes differ");
-  TORCH_CHECK(momenta.size() == params.size() || (!has_mom && momenta.empty()),
-              "fused_sgd: ", momenta.size(), " momentum buffers for ", params.size(), " params");
-  TORCH_CHECK(masters.empty() || masters.size() == params.size(), "fused_sgd: ", masters.size(), " master params for ",
-              params.size(), " params");
-  if (params.empty()) return;
-  for (size_t i = 0; i < params.size(); ++i) {
-    CheckOptimizerParam("fused_sgd", i, params[i], params[0]);
-    CheckOptimizerPeer("fused_sgd", "grads", i, params[i], grads[i], grads[0].scalar_type());
-  }
-  const bool has_master = CheckMasters("fused_sgd", params, grads, masters);
-  for (size_t i = 0; has_mom && i < params.size(); ++i)  // fp32 momentum with a master, else the param dtype
-    CheckOptimizerPeer("fused_sgd", "momentum_buffers", i, params[i], momenta[i], has_master ? at::kFloat : params[i].scalar_type());
-  const float* gsd = DeviceScalar("fused_sgd", "grad_scale_dev", grad_scale_dev, params[0]);
-  int device = (int)params[0].get_device();
-  c10::cuda::CUDAGuard guard(params[0].device());
-  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  std::vector<kern::SgdTensor> table(params.size());
-  int64_t maxc = 0;
-  for (size_t i = 0; i < params.size(); ++i) {
-    table[i].param = params[i].data_ptr(); table[i].grad = grads[i].data_ptr();
-    table[i].momentum = has_mom ? momenta[i].data_ptr() : nullptr;
-    table[i].count = params[i].numel();
-    table[i].master = has_master ? masters[i].data_ptr() : nullptr;
-    maxc = std::max(maxc, table[i].count);
-  }
-  const auto* dt = (const kern::SgdTensor*)GpuContext::Get().Stage(device, table.data(), table.size() * sizeof(kern::SgdTensor), s);
-  TORCH_CHECK(dt != nullptr, "fused_sgd: table too large");
-  cudaError_t e = kern::LaunchFusedSgd(dt, (int)table.size(), maxc, (float)lr, (float)momentum, (float)dampening, (float)weight_decay,
-                                       nesterov ? 1 : 0, (float)grad_scale, first_step ? 1 : 0,
-                                       (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s, gsd,
-                                       has_master);
-  TORCH_CHECK(e == cudaSuccess, "fused_sgd launch failed: ", cudaGetErrorString(e));
-}
-
-void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
-                   std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
-                   int64_t step, double grad_scale, bool adamw, c10::optional<at::Tensor> grad_scale_dev,
-                   std::vector<at::Tensor> masters) {
-  TORCH_CHECK(params.size() == grads.size() && params.size() == exp_avg.size() && params.size() == exp_avg_sq.size(), "fused_adam: list sizes differ");
-  TORCH_CHECK(masters.empty() || masters.size() == params.size(), "fused_adam: ", masters.size(), " master params for ",
-              params.size(), " params");
-  // step is 1-based: step 0 would make the bias correction 1 - beta1^0 = 0 and every parameter inf / NaN
-  TORCH_CHECK(step >= 1, "fused_adam: step must be >= 1, got ", step);
-  if (params.empty()) return;
-  for (size_t i = 0; i < params.size(); ++i) {
-    CheckOptimizerParam("fused_adam", i, params[i], params[0]);
-    CheckOptimizerPeer("fused_adam", "grads", i, params[i], grads[i], grads[0].scalar_type());
-    CheckOptimizerPeer("fused_adam", "exp_avgs", i, params[i], exp_avg[i], at::kFloat);
-    CheckOptimizerPeer("fused_adam", "exp_avg_sqs", i, params[i], exp_avg_sq[i], at::kFloat);
-  }
-  const bool has_master = CheckMasters("fused_adam", params, grads, masters);
-  const float* gsd = DeviceScalar("fused_adam", "grad_scale_dev", grad_scale_dev, params[0]);
-  int device = (int)params[0].get_device();
-  c10::cuda::CUDAGuard guard(params[0].device());
-  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  std::vector<kern::AdamTensor> table(params.size());
-  int64_t maxc = 0;
-  for (size_t i = 0; i < params.size(); ++i) {
-    table[i].param = params[i].data_ptr(); table[i].grad = grads[i].data_ptr();
-    table[i].exp_avg = exp_avg[i].data_ptr(); table[i].exp_avg_sq = exp_avg_sq[i].data_ptr();
-    table[i].count = params[i].numel();
-    table[i].master = has_master ? masters[i].data_ptr() : nullptr;
-    maxc = std::max(maxc, table[i].count);
-  }
-  const auto* dt = (const kern::AdamTensor*)GpuContext::Get().Stage(device, table.data(), table.size() * sizeof(kern::AdamTensor), s);
-  TORCH_CHECK(dt != nullptr, "fused_adam: table too large");
-  const float c1 = 1.0f - (float)std::pow(beta1, (double)step), c2 = 1.0f - (float)std::pow(beta2, (double)step);
-  cudaError_t e = kern::LaunchFusedAdamW(dt, (int)table.size(), maxc, (float)lr, (float)beta1, (float)beta2, (float)eps,
-                                         (float)weight_decay, c1, c2, (float)grad_scale, adamw ? 1 : 0,
-                                         (int)MapDtype(params[0].scalar_type()), (int)MapDtype(grads[0].scalar_type()), s, gsd,
-                                         has_master);
-  TORCH_CHECK(e == cudaSuccess, "fused_adam launch failed: ", cudaGetErrorString(e));
-}
-
-// ---- fused LAMB and LARS (kern::LaunchLambNorms / LaunchLambApply, LaunchLarsNorms / LaunchLarsApply) ----
-// Both take one table of kern::LambTensor with a norm slot per entry.  PlanSlotted checks every argument of one phase
-// and builds the table: entry i is params[i] with norm slot slots[i] (empty: i) of `norms`, a contiguous fp32 tensor on
-// the params' device with 2 floats per slot, and each fp32 state list in its field of the entry (fields no list names
-// stay null).  Zero-size params get no entry.
-struct LambPlan {
-  std::vector<kern::LambTensor> table;
-  int64_t max_count = 0, partials = 0;
-  bool master = false;
-  float c1 = 1.f, c2 = 1.f;  // LAMB's bias corrections
-};
-
-struct SlottedState {
+// One state list of an optimizer call and the table field it fills.  States are fp32, except a list marked
+// `param_dtype` (SGD momentum), which has the param's dtype without masters.
+struct OptState {
   const char* name;
   const std::vector<at::Tensor>& list;
-  void* kern::LambTensor::*field;
+  void* kern::OptTensor::*field;
+  bool param_dtype = false;
 };
 
-LambPlan PlanSlotted(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
-                     const std::vector<SlottedState>& states, const std::vector<at::Tensor>& masters,
-                     const at::Tensor& norms, const std::vector<int64_t>& slots) {
+// A checked call of the kern::Launch* optimizer launchers: the table, its dtypes and what the launchers take besides.
+struct OptPlan {
+  std::vector<kern::OptTensor> table;
+  int64_t max_count = 0, partials = 0;
+  int param_dtype = 0, grad_dtype = 0;
+  bool master = false;
+  const float* grad_scale_dev = nullptr;
+};
+
+// Checks every argument of one optimizer call and builds its table; nothing is staged or launched here.  Entry i is
+// params[i] with grads[i], masters[i] and each state list's element in its field.  `norms` (LAMB and LARS; nullptr:
+// none) is a contiguous fp32 tensor on the params' device with 2 floats per slot: entry i gets norm slot slots[i]
+// (empty: i) and the offset of its stage-1 partials.  Zero-size params get no entry.
+OptPlan PlanOpt(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
+                const std::vector<OptState>& states, const std::vector<at::Tensor>& masters,
+                const c10::optional<at::Tensor>& grad_scale_dev, const at::Tensor* norms = nullptr,
+                const std::vector<int64_t>& slots = {}) {
   bool sizes = params.size() == grads.size();
   for (const auto& st : states) sizes = sizes && st.list.size() == params.size();
   TORCH_CHECK(sizes, op, ": list sizes differ");
   TORCH_CHECK(masters.empty() || masters.size() == params.size(), op, ": ", masters.size(), " master params for ",
               params.size(), " params");
   TORCH_CHECK(slots.empty() || slots.size() == params.size(), op, ": ", slots.size(), " slots for ", params.size(), " params");
-  LambPlan plan;
+  OptPlan plan;
   if (params.empty()) return plan;
   for (size_t i = 0; i < params.size(); ++i) {
     CheckOptimizerParam(op, i, params[i], params[0]);
     CheckOptimizerPeer(op, "grads", i, params[i], grads[i], grads[0].scalar_type());
-    for (const auto& st : states) CheckOptimizerPeer(op, st.name, i, params[i], st.list[i], at::kFloat);
   }
   plan.master = CheckMasters(op, params, grads, masters);
-  TORCH_CHECK(norms.is_cuda() && norms.device() == params[0].device() && norms.scalar_type() == at::kFloat &&
-              norms.is_contiguous(), op, ": norms must be a contiguous float32 tensor on ", params[0].device());
-  const int64_t nslots = norms.numel() / 2;
-  std::set<int64_t> seen;
-  for (size_t i = 0; i < params.size(); ++i) {
-    const int64_t s = slots.empty() ? (int64_t)i : slots[i];
-    TORCH_CHECK(s >= 0 && s < nslots, op, ": slot ", s, " of params[", i, "] is out of range for norms with room for ",
-                nslots, " slots");
-    TORCH_CHECK(seen.insert(s).second, op, ": slot ", s, " appears twice in one call");
+  for (const auto& st : states)
+    for (size_t i = 0; i < params.size(); ++i)
+      CheckOptimizerPeer(op, st.name, i, params[i], st.list[i],
+                         st.param_dtype && !plan.master ? params[i].scalar_type() : at::kFloat);
+  if (norms != nullptr) {
+    TORCH_CHECK(norms->is_cuda() && norms->device() == params[0].device() && norms->scalar_type() == at::kFloat &&
+                norms->is_contiguous(), op, ": norms must be a contiguous float32 tensor on ", params[0].device());
+    const int64_t nslots = norms->numel() / 2;
+    std::set<int64_t> seen;
+    for (size_t i = 0; i < params.size(); ++i) {
+      const int64_t s = slots.empty() ? (int64_t)i : slots[i];
+      TORCH_CHECK(s >= 0 && s < nslots, op, ": slot ", s, " of params[", i, "] is out of range for norms with room for ",
+                  nslots, " slots");
+      TORCH_CHECK(seen.insert(s).second, op, ": slot ", s, " appears twice in one call");
+    }
   }
+  plan.grad_scale_dev = DeviceScalar(op, "grad_scale_dev", grad_scale_dev, params[0]);
+  plan.param_dtype = (int)MapDtype(params[0].scalar_type());
+  plan.grad_dtype = (int)MapDtype(grads[0].scalar_type());
   for (size_t i = 0; i < params.size(); ++i) {
     if (params[i].numel() == 0) continue;
-    kern::LambTensor t{};
+    kern::OptTensor t{};
     t.param = params[i].data_ptr(); t.grad = grads[i].data_ptr();
+    t.master = plan.master ? masters[i].data_ptr() : nullptr;
     for (const auto& st : states) t.*st.field = st.list[i].data_ptr();
     t.count = params[i].numel();
-    t.master = plan.master ? masters[i].data_ptr() : nullptr;
-    t.partial = plan.partials;
-    t.slot = slots.empty() ? (int64_t)i : slots[i];
-    plan.partials += kern::LambPartials(t.count);
+    if (norms != nullptr) {
+      t.partial = plan.partials;
+      t.slot = slots.empty() ? (int64_t)i : slots[i];
+      plan.partials += kern::NormPartials(t.count);
+    }
     plan.max_count = std::max(plan.max_count, t.count);
     plan.table.push_back(t);
   }
   return plan;
 }
 
-LambPlan PlanLamb(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
-                  const std::vector<at::Tensor>& exp_avg, const std::vector<at::Tensor>& exp_avg_sq,
-                  const std::vector<at::Tensor>& masters, const at::Tensor& norms, const std::vector<int64_t>& slots,
-                  double beta1, double beta2, int64_t step, bool bias_correction) {
-  TORCH_CHECK(step >= 1, op, ": step must be >= 1, got ", step);
-  LambPlan plan = PlanSlotted(op, params, grads, {{"exp_avgs", exp_avg, &kern::LambTensor::exp_avg},
-                                                  {"exp_avg_sqs", exp_avg_sq, &kern::LambTensor::exp_avg_sq}},
-                              masters, norms, slots);
-  if (bias_correction) {
-    plan.c1 = 1.0f - (float)std::pow(beta1, (double)step);
-    plan.c2 = 1.0f - (float)std::pow(beta2, (double)step);
-  }
-  return plan;
-}
-
-// LARS keeps one fp32 state, the momentum buffer, in the entry's exp_avg.
-LambPlan PlanLars(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
-                  const std::vector<at::Tensor>& momentum_buffers, const std::vector<at::Tensor>& masters,
-                  const at::Tensor& norms, const std::vector<int64_t>& slots) {
-  return PlanSlotted(op, params, grads, {{"momentum_buffers", momentum_buffers, &kern::LambTensor::exp_avg}}, masters,
-                     norms, slots);
-}
-
-const kern::LambTensor* StageLamb(const char* op, const LambPlan& plan, int device, cudaStream_t s) {
-  const auto* dt = (const kern::LambTensor*)GpuContext::Get().Stage(device, plan.table.data(),
-                                                                     plan.table.size() * sizeof(kern::LambTensor), s);
+// Stages the plan's table once on the params' device and runs launch(device table, current stream) there, which makes
+// one or more kern::Launch* calls and returns the first error.
+template <typename F>
+void RunPlan(const char* op, const OptPlan& plan, const std::vector<at::Tensor>& params, F&& launch) {
+  if (plan.table.empty()) return;
+  const int device = (int)params[0].get_device();
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
+  const auto* dt = (const kern::OptTensor*)GpuContext::Get().Stage(device, plan.table.data(),
+                                                                    plan.table.size() * sizeof(kern::OptTensor), s);
   TORCH_CHECK(dt != nullptr, op, ": table too large");
-  return dt;
-}
-
-void LaunchLambNormsPhase(const char* op, const LambPlan& plan, const kern::LambTensor* dt, const at::Tensor& param0,
-                          const at::Tensor& grad0, double beta1, double beta2, double eps, double weight_decay,
-                          double grad_scale, const float* gsd, at::Tensor& norms, cudaStream_t s) {
-  // stream-ordered scratch from torch's caching allocator: one (sum w^2, sum u^2) pair per stage-1 CTA
-  at::Tensor work = at::empty({2 * plan.partials}, norms.options());
-  cudaError_t e = kern::LaunchLambNorms(dt, (int)plan.table.size(), plan.max_count, (float)beta1, (float)beta2, (float)eps,
-                                        (float)weight_decay, plan.c1, plan.c2, (float)grad_scale, gsd, work.data_ptr<float>(),
-                                        norms.data_ptr<float>(), (int)MapDtype(param0.scalar_type()),
-                                        (int)MapDtype(grad0.scalar_type()), plan.master, s);
+  const cudaError_t e = launch(dt, s);
   TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
 }
 
-void LaunchLambApplyPhase(const char* op, const LambPlan& plan, const kern::LambTensor* dt, const at::Tensor& param0,
-                          double lr, double eps, double weight_decay, bool adapt, const at::Tensor& norms, cudaStream_t s) {
-  cudaError_t e = kern::LaunchLambApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)eps, (float)weight_decay,
-                                        plan.c1, plan.c2, adapt ? 1 : 0, norms.data_ptr<float>(),
-                                        (int)MapDtype(param0.scalar_type()), plan.master, s);
-  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+std::vector<OptState> MomentStates(const std::vector<at::Tensor>& exp_avg, const std::vector<at::Tensor>& exp_avg_sq) {
+  return {{"exp_avgs", exp_avg, &kern::OptTensor::state0}, {"exp_avg_sqs", exp_avg_sq, &kern::OptTensor::state1}};
+}
+
+// Adam's and LAMB's bias correction 1 - beta^step; step is 1-based: step 0 would make it 0 and every parameter inf / NaN
+float BiasCorrection(const char* op, double beta, int64_t step) {
+  TORCH_CHECK(step >= 1, op, ": step must be >= 1, got ", step);
+  return 1.0f - (float)std::pow(beta, (double)step);
+}
+
+void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momenta, double lr,
+                  double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step,
+                  c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
+  const bool has_mom = momentum != 0.0;
+  // without momentum the buffers are not read: none, or a list of the params' length
+  TORCH_CHECK(has_mom || momenta.empty() || momenta.size() == params.size(),
+              "fused_sgd: ", momenta.size(), " momentum buffers for ", params.size(), " params");
+  std::vector<OptState> states;
+  if (has_mom) states.push_back({"momentum_buffers", momenta, &kern::OptTensor::state0, true});
+  const OptPlan plan = PlanOpt("fused_sgd", params, grads, states, masters, grad_scale_dev);
+  RunPlan("fused_sgd", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
+    return kern::LaunchFusedSgd(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)momentum, (float)dampening,
+                                (float)weight_decay, nesterov ? 1 : 0, (float)grad_scale, first_step ? 1 : 0,
+                                plan.param_dtype, plan.grad_dtype, s, plan.grad_scale_dev, plan.master);
+  });
+}
+
+void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
+                   std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
+                   int64_t step, double grad_scale, bool adamw, c10::optional<at::Tensor> grad_scale_dev,
+                   std::vector<at::Tensor> masters) {
+  const float c1 = BiasCorrection("fused_adam", beta1, step), c2 = BiasCorrection("fused_adam", beta2, step);
+  const OptPlan plan = PlanOpt("fused_adam", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev);
+  RunPlan("fused_adam", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
+    return kern::LaunchFusedAdamW(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)beta1, (float)beta2,
+                                  (float)eps, (float)weight_decay, c1, c2, (float)grad_scale, adamw ? 1 : 0,
+                                  plan.param_dtype, plan.grad_dtype, s, plan.grad_scale_dev, plan.master);
+  });
+}
+
+// ---- fused LAMB and LARS: a norms phase (two launches) and an apply phase (one launch) on one table with a norm slot
+// per entry, so that the norms can be allreduced in between.
+
+// stream-ordered scratch from torch's caching allocator: one pair of sums of squares per stage-1 CTA
+at::Tensor NormsScratch(const OptPlan& plan, const at::Tensor& norms) { return at::empty({2 * plan.partials}, norms.options()); }
+
+struct LambArgs { double beta1, beta2, eps, weight_decay; float c1, c2; };
+
+LambArgs LambHyper(const char* op, double beta1, double beta2, double eps, double weight_decay, int64_t step,
+                   bool bias_correction) {
+  const float c1 = BiasCorrection(op, beta1, step), c2 = BiasCorrection(op, beta2, step);  // checks step in any case
+  return bias_correction ? LambArgs{beta1, beta2, eps, weight_decay, c1, c2} : LambArgs{beta1, beta2, eps, weight_decay, 1.f, 1.f};
+}
+
+cudaError_t LambNormsPhase(const OptPlan& plan, const kern::OptTensor* dt, const LambArgs& a, double grad_scale,
+                           at::Tensor& norms, cudaStream_t s) {
+  at::Tensor work = NormsScratch(plan, norms);
+  return kern::LaunchLambNorms(dt, (int)plan.table.size(), plan.max_count, (float)a.beta1, (float)a.beta2, (float)a.eps,
+                               (float)a.weight_decay, a.c1, a.c2, (float)grad_scale, plan.grad_scale_dev,
+                               work.data_ptr<float>(), norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype,
+                               plan.master, s);
+}
+
+cudaError_t LambApplyPhase(const OptPlan& plan, const kern::OptTensor* dt, const LambArgs& a, double lr, bool adapt,
+                           const at::Tensor& norms, cudaStream_t s) {
+  return kern::LaunchLambApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)a.eps, (float)a.weight_decay,
+                               a.c1, a.c2, adapt ? 1 : 0, norms.data_ptr<float>(), plan.param_dtype, plan.master, s);
 }
 
 // Phase 1: moments, then the squared norms of every entry ADDED into norms[2 * slot], norms[2 * slot + 1].
@@ -728,16 +698,12 @@ void LambNorms(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
                std::vector<at::Tensor> exp_avg_sq, double beta1, double beta2, double eps, double weight_decay, int64_t step,
                bool bias_correction, double grad_scale, c10::optional<at::Tensor> grad_scale_dev,
                std::vector<at::Tensor> masters, at::Tensor out, std::vector<int64_t> slots) {
-  LambPlan plan = PlanLamb("lamb_norms", params, grads, exp_avg, exp_avg_sq, masters, out, slots, beta1, beta2, step,
-                           bias_correction);
-  if (params.empty()) return;
-  const float* gsd = DeviceScalar("lamb_norms", "grad_scale_dev", grad_scale_dev, params[0]);
-  if (plan.table.empty()) return;
-  int device = (int)params[0].get_device();
-  c10::cuda::CUDAGuard guard(params[0].device());
-  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  const auto* dt = StageLamb("lamb_norms", plan, device, s);
-  LaunchLambNormsPhase("lamb_norms", plan, dt, params[0], grads[0], beta1, beta2, eps, weight_decay, grad_scale, gsd, out, s);
+  const LambArgs a = LambHyper("lamb_norms", beta1, beta2, eps, weight_decay, step, bias_correction);
+  const OptPlan plan = PlanOpt("lamb_norms", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev,
+                               &out, slots);
+  RunPlan("lamb_norms", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
+    return LambNormsPhase(plan, dt, a, grad_scale, out, s);
+  });
 }
 
 // Phase 2: w -= lr * r * u with r from the (allreduced) norms.  `grads` are checked like phase 1's, not read.
@@ -745,55 +711,54 @@ void LambApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
                std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
                int64_t step, bool bias_correction, bool adapt, std::vector<at::Tensor> masters, at::Tensor norms,
                std::vector<int64_t> slots) {
-  LambPlan plan = PlanLamb("lamb_apply", params, grads, exp_avg, exp_avg_sq, masters, norms, slots, beta1, beta2, step,
-                           bias_correction);
-  if (plan.table.empty()) return;
-  int device = (int)params[0].get_device();
-  c10::cuda::CUDAGuard guard(params[0].device());
-  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  const auto* dt = StageLamb("lamb_apply", plan, device, s);
-  LaunchLambApplyPhase("lamb_apply", plan, dt, params[0], lr, eps, weight_decay, adapt, norms, s);
+  const LambArgs a = LambHyper("lamb_apply", beta1, beta2, eps, weight_decay, step, bias_correction);
+  const OptPlan plan = PlanOpt("lamb_apply", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, c10::nullopt,
+                               &norms, slots);
+  RunPlan("lamb_apply", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
+    return LambApplyPhase(plan, dt, a, lr, adapt, norms, s);
+  });
 }
 
-// Both phases on one device with a fresh norms buffer (slot i = params[i]): three launches, one staged table.
+// A fresh norms buffer for both phases on one device (slot i = params[i]).
+at::Tensor FreshNorms(const char* op, const std::vector<at::Tensor>& params) {
+  TORCH_CHECK(params.empty() || params[0].is_cuda(), op, ": params[0] must be a dense CUDA tensor");
+  return params.empty() ? at::Tensor() : at::zeros({2 * (int64_t)params.size()}, params[0].options().dtype(at::kFloat));
+}
+
+// Both phases: three launches, one staged table.
 void FusedLambStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
                    std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
                    int64_t step, bool bias_correction, bool adapt, double grad_scale,
                    c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
-  TORCH_CHECK(params.empty() || params[0].is_cuda(), "fused_lamb: params[0] must be a dense CUDA tensor");
-  at::Tensor norms = params.empty() ? at::Tensor() : at::zeros({2 * (int64_t)params.size()}, params[0].options().dtype(at::kFloat));
-  LambPlan plan = PlanLamb("fused_lamb", params, grads, exp_avg, exp_avg_sq, masters, norms, {}, beta1, beta2, step,
-                           bias_correction);
-  if (params.empty()) return;
-  const float* gsd = DeviceScalar("fused_lamb", "grad_scale_dev", grad_scale_dev, params[0]);
-  if (plan.table.empty()) return;
-  int device = (int)params[0].get_device();
-  c10::cuda::CUDAGuard guard(params[0].device());
-  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  const auto* dt = StageLamb("fused_lamb", plan, device, s);
-  LaunchLambNormsPhase("fused_lamb", plan, dt, params[0], grads[0], beta1, beta2, eps, weight_decay, grad_scale, gsd, norms, s);
-  LaunchLambApplyPhase("fused_lamb", plan, dt, params[0], lr, eps, weight_decay, adapt, norms, s);
+  at::Tensor norms = FreshNorms("fused_lamb", params);
+  const LambArgs a = LambHyper("fused_lamb", beta1, beta2, eps, weight_decay, step, bias_correction);
+  const OptPlan plan = PlanOpt("fused_lamb", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev,
+                               &norms);
+  RunPlan("fused_lamb", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
+    const cudaError_t e = LambNormsPhase(plan, dt, a, grad_scale, norms, s);
+    return e != cudaSuccess ? e : LambApplyPhase(plan, dt, a, lr, adapt, norms, s);
+  });
 }
 
-void LaunchLarsNormsPhase(const char* op, const LambPlan& plan, const kern::LambTensor* dt, const at::Tensor& param0,
-                          const at::Tensor& grad0, double grad_scale, const float* gsd, at::Tensor& norms, cudaStream_t s) {
-  // stream-ordered scratch from torch's caching allocator: one (sum w^2, sum g^2) pair per stage-1 CTA
-  at::Tensor work = at::empty({2 * plan.partials}, norms.options());
-  cudaError_t e = kern::LaunchLarsNorms(dt, (int)plan.table.size(), plan.max_count, (float)grad_scale, gsd,
-                                        work.data_ptr<float>(), norms.data_ptr<float>(), (int)MapDtype(param0.scalar_type()),
-                                        (int)MapDtype(grad0.scalar_type()), plan.master, s);
-  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+// LARS keeps one fp32 state, the momentum buffer.
+std::vector<OptState> LarsStates(const std::vector<at::Tensor>& momentum_buffers) {
+  return {{"momentum_buffers", momentum_buffers, &kern::OptTensor::state0}};
 }
 
-void LaunchLarsApplyPhase(const char* op, const LambPlan& plan, const kern::LambTensor* dt, const at::Tensor& param0,
-                          const at::Tensor& grad0, double lr, double momentum, double weight_decay, double trust_coefficient,
-                          double eps, bool adapt, double grad_scale, const float* gsd, const at::Tensor& norms,
-                          cudaStream_t s) {
-  cudaError_t e = kern::LaunchLarsApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)momentum,
-                                        (float)weight_decay, (float)trust_coefficient, (float)eps, adapt ? 1 : 0,
-                                        (float)grad_scale, gsd, norms.data_ptr<float>(), (int)MapDtype(param0.scalar_type()),
-                                        (int)MapDtype(grad0.scalar_type()), plan.master, s);
-  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+cudaError_t LarsNormsPhase(const OptPlan& plan, const kern::OptTensor* dt, double grad_scale, at::Tensor& norms,
+                           cudaStream_t s) {
+  at::Tensor work = NormsScratch(plan, norms);
+  return kern::LaunchLarsNorms(dt, (int)plan.table.size(), plan.max_count, (float)grad_scale, plan.grad_scale_dev,
+                               work.data_ptr<float>(), norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype,
+                               plan.master, s);
+}
+
+cudaError_t LarsApplyPhase(const OptPlan& plan, const kern::OptTensor* dt, double lr, double momentum, double weight_decay,
+                           double trust_coefficient, double eps, bool adapt, double grad_scale, const at::Tensor& norms,
+                           cudaStream_t s) {
+  return kern::LaunchLarsApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)momentum, (float)weight_decay,
+                               (float)trust_coefficient, (float)eps, adapt ? 1 : 0, (float)grad_scale, plan.grad_scale_dev,
+                               norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype, plan.master, s);
 }
 
 // LARS phase 1: the squared norms of every entry's parameter and scaled gradient ADDED into norms[2 * slot],
@@ -801,15 +766,11 @@ void LaunchLarsApplyPhase(const char* op, const LambPlan& plan, const kern::Lamb
 void LarsNorms(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momentum_buffers,
                double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters, at::Tensor out,
                std::vector<int64_t> slots) {
-  LambPlan plan = PlanLars("lars_norms", params, grads, momentum_buffers, masters, out, slots);
-  if (params.empty()) return;
-  const float* gsd = DeviceScalar("lars_norms", "grad_scale_dev", grad_scale_dev, params[0]);
-  if (plan.table.empty()) return;
-  int device = (int)params[0].get_device();
-  c10::cuda::CUDAGuard guard(params[0].device());
-  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  const auto* dt = StageLamb("lars_norms", plan, device, s);
-  LaunchLarsNormsPhase("lars_norms", plan, dt, params[0], grads[0], grad_scale, gsd, out, s);
+  const OptPlan plan = PlanOpt("lars_norms", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &out,
+                               slots);
+  RunPlan("lars_norms", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
+    return LarsNormsPhase(plan, dt, grad_scale, out, s);
+  });
 }
 
 // LARS phase 2: momentum and parameter update with r from the (allreduced) norms; reads the gradient again, scaled the
@@ -818,35 +779,24 @@ void LarsApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
                double lr, double momentum, double weight_decay, double trust_coefficient, double eps, bool adapt,
                double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters,
                at::Tensor norms, std::vector<int64_t> slots) {
-  LambPlan plan = PlanLars("lars_apply", params, grads, momentum_buffers, masters, norms, slots);
-  if (params.empty()) return;
-  const float* gsd = DeviceScalar("lars_apply", "grad_scale_dev", grad_scale_dev, params[0]);
-  if (plan.table.empty()) return;
-  int device = (int)params[0].get_device();
-  c10::cuda::CUDAGuard guard(params[0].device());
-  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  const auto* dt = StageLamb("lars_apply", plan, device, s);
-  LaunchLarsApplyPhase("lars_apply", plan, dt, params[0], grads[0], lr, momentum, weight_decay, trust_coefficient, eps,
-                       adapt, grad_scale, gsd, norms, s);
+  const OptPlan plan = PlanOpt("lars_apply", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &norms,
+                               slots);
+  RunPlan("lars_apply", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
+    return LarsApplyPhase(plan, dt, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, norms, s);
+  });
 }
 
-// Both LARS phases on one device with a fresh norms buffer (slot i = params[i]): three launches, one staged table.
+// Both LARS phases: three launches, one staged table.
 void FusedLarsStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momentum_buffers,
                    double lr, double momentum, double weight_decay, double trust_coefficient, double eps, bool adapt,
                    double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
-  TORCH_CHECK(params.empty() || params[0].is_cuda(), "fused_lars: params[0] must be a dense CUDA tensor");
-  at::Tensor norms = params.empty() ? at::Tensor() : at::zeros({2 * (int64_t)params.size()}, params[0].options().dtype(at::kFloat));
-  LambPlan plan = PlanLars("fused_lars", params, grads, momentum_buffers, masters, norms, {});
-  if (params.empty()) return;
-  const float* gsd = DeviceScalar("fused_lars", "grad_scale_dev", grad_scale_dev, params[0]);
-  if (plan.table.empty()) return;
-  int device = (int)params[0].get_device();
-  c10::cuda::CUDAGuard guard(params[0].device());
-  cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  const auto* dt = StageLamb("fused_lars", plan, device, s);
-  LaunchLarsNormsPhase("fused_lars", plan, dt, params[0], grads[0], grad_scale, gsd, norms, s);
-  LaunchLarsApplyPhase("fused_lars", plan, dt, params[0], grads[0], lr, momentum, weight_decay, trust_coefficient, eps,
-                       adapt, grad_scale, gsd, norms, s);
+  at::Tensor norms = FreshNorms("fused_lars", params);
+  const OptPlan plan = PlanOpt("fused_lars", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &norms);
+  RunPlan("fused_lars", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
+    const cudaError_t e = LarsNormsPhase(plan, dt, grad_scale, norms, s);
+    return e != cudaSuccess ? e : LarsApplyPhase(plan, dt, lr, momentum, weight_decay, trust_coefficient, eps, adapt,
+                                                 grad_scale, norms, s);
+  });
 }
 
 // The stats kernel's last-CTA ticket: one zeroed counter per (device, stream), which every launch leaves zeroed again.

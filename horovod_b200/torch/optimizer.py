@@ -75,7 +75,6 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self.sparse_as_dense = sparse_as_dense
         self.process_set = process_set
         self._fused = fused
-        self._fused_steps = 0
         self._graph_mode = False  # set by hvd.GraphedStep: backward runs as a CUDA graph replay, hooks do not fire
         self._graph_capture = None      # while hvd.GraphedStep captures: {'comm': side stream, 'ctas': n, 'launched': set()}
         self._graph_comm_captured = False  # the captured graph contains the gradient allreduces (nothing left for step())
@@ -127,21 +126,20 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._allreduce_delay[p] = self.backward_passes_per_step
         self._reset_folds()
         super(self.__class__, self).load_state_dict(*args, **kwargs)
-        if self._fused and (isinstance(self, (torch.optim.Adam, torch.optim.AdamW, Lamb, Lars)) or self._master_weights):
+        if self._fused and _optimizer_kind(self):
             self._keep_fp32_moments(args[0] if args else kwargs['state_dict'])
 
     def _keep_fp32_moments(self, state_dict):
-        """torch casts every loaded floating state tensor to its parameter's dtype. The fused Adam and LAMB kernels keep
-        fp32 moments for bf16 / fp16 parameters too, the LARS kernels fp32 momentum, and with master weights the fp32
-        master copy and SGD momentum, so take the checkpoint's fp32 values back: a checkpoint round-trips exactly instead
-        of losing their low bits."""
+        """torch casts every loaded floating state tensor to its parameter's dtype. The fused kernels keep fp32 state for
+        bf16 / fp16 parameters (_state_dtype), and with master weights the fp32 master copy, so take the checkpoint's
+        fp32 values back: a checkpoint round-trips exactly instead of losing their low bits."""
+        kind = _optimizer_kind(self)
         saved = [i for g in state_dict['param_groups'] for i in g['params']]
         params = [p for g in self.param_groups for p in g['params']]
-        keys = ('exp_avg', 'exp_avg_sq') + (('master_param', 'momentum_buffer') if self._master_weights else
-                                            ('momentum_buffer',) if isinstance(self, Lars) else ())
         for pid, p in zip(saved, params):
             st = state_dict['state'].get(pid, {})
-            for key in keys:
+            keys = _STATE_KEYS[kind] if _state_dtype(kind, p.dtype, self._master_weights) == torch.float32 else ()
+            for key in keys + (('master_param',) if self._master_weights else ()):
                 t = st.get(key)
                 if torch.is_tensor(t) and t.dtype == torch.float32 and p.dtype != torch.float32 and key in self.state[p]:
                     self.state[p][key] = _state_like(p, t, torch.float32)
@@ -626,20 +624,16 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                               "code.")
             self.synchronize(_defer_shadow_copy=self._fused and closure is None)
         self._synchronized = False
-        if self._master_weights:
+        if self._master_weights or (self._fused and closure is None):
             # the masters live in the fused kernels only: evaluate the closure, then the fused update (or an error)
             loss = None
             if closure is not None:
                 with torch.enable_grad():
                     loss = closure()
-            _fused_step(self)
-            for bucket in self._buckets:
-                bucket['shadow_fresh'] = False
-            return loss
-        if self._fused and closure is None and _fused_step(self):
-            for bucket in self._buckets:
-                bucket['shadow_fresh'] = False
-            return None
+            if _fused_step(self):  # always True with masters: it raises when the update cannot be fused
+                for bucket in self._buckets:
+                    bucket['shadow_fresh'] = False
+                return loss
         self._restore_shadows()
         return super(self.__class__, self).step(closure)
 
@@ -690,6 +684,63 @@ def _fold(grads, accs, mode):
         ops.grad_accumulate_(grads, accs, mode)
 
 
+def _optimizer_kind(opt):
+    """Which fused update serves `opt`: 'sgd', 'adam' (Adam and AdamW), 'lamb' (hvd.Lamb), 'lars' (hvd.Lars), or None."""
+    kinds = ((torch.optim.SGD, 'sgd'), ((torch.optim.Adam, torch.optim.AdamW), 'adam'), (Lamb, 'lamb'), (Lars, 'lars'))
+    return next((kind for cls, kind in kinds if isinstance(opt, cls)), None)
+
+
+# The state the fused kernels keep per parameter (per owned shard with sharded state), in the order the kernels take it.
+# Every state tensor is fp32 except SGD momentum without master weights (_state_dtype).  Adam and LAMB also count steps.
+_STATE_KEYS = {'sgd': ('momentum_buffer',), 'adam': ('exp_avg', 'exp_avg_sq'), 'lamb': ('exp_avg', 'exp_avg_sq'),
+               'lars': ('momentum_buffer',)}
+_COUNTS_STEPS = ('adam', 'lamb')
+
+
+def _state_keys(kind, group):
+    return () if kind == 'sgd' and group.get('momentum', 0.0) == 0.0 else _STATE_KEYS[kind]
+
+
+def _state_dtype(kind, dtype, master):
+    return dtype if kind == 'sgd' and not master else torch.float32
+
+
+def _fused_update(opt, kind, group, ps, grads, states, masters, step=0, first_step=False, coef=None, phase=None,
+                  norms=None, slots=None):
+    """The native fused update of `kind` for params `ps` of `group` (hyper-parameters read now, so LR schedulers work),
+    with one list per state key and fp32 masters ([]: none).  coef: a device factor on the gradient (clip coefficient).
+    LAMB / LARS: both phases (phase None), or phase 'norms' / 'apply' on `norms` / `slots` to allreduce in between."""
+    native = mpi_ops._native()
+    lr, wd = float(group['lr']), float(group.get('weight_decay', 0.0))
+    if kind == 'sgd':
+        native.fused_sgd_step(ps, grads, states[0] if states else [], lr, float(group.get('momentum', 0.0)),
+                              float(group.get('dampening', 0.0)), wd, bool(group.get('nesterov', False)), 1.0,
+                              first_step, coef, masters)
+    elif kind == 'adam':
+        b1, b2 = group['betas']
+        adamw = isinstance(opt, torch.optim.AdamW) or bool(group.get('decoupled_weight_decay', False))
+        native.fused_adam_step(ps, grads, *states, lr, float(b1), float(b2), float(group['eps']), wd, step, 1.0, adamw,
+                               coef, masters)
+    elif kind == 'lamb':
+        b1, b2 = group['betas']
+        hp = (float(b1), float(b2), float(group['eps']), wd, step, bool(group['bias_correction']))
+        if phase is None:
+            native.fused_lamb_step(ps, grads, *states, lr, *hp, Lamb.adapts(group), 1.0, coef, masters)
+        elif phase == 'norms':
+            native.lamb_norms(ps, grads, *states, *hp, 1.0, coef, masters, norms, slots)
+        else:
+            native.lamb_apply(ps, grads, *states, lr, *hp, Lamb.adapts(group), masters, norms, slots)
+    else:
+        hp = (lr, float(group['momentum']), wd, float(group['trust_coefficient']), float(group['eps']), Lars.adapts(group),
+              1.0, coef, masters)
+        if phase is None:
+            native.fused_lars_step(ps, grads, *states, *hp)
+        elif phase == 'norms':
+            native.lars_norms(ps, grads, *states, 1.0, coef, masters, norms, slots)
+        else:
+            native.lars_apply(ps, grads, *states, *hp, norms, slots)
+
+
 def _fused_plan(opt, why=None):
     """Pure eligibility pass of the fused optimizer step: returns the launch plan [(group, params, grads)] or None.
     Nothing is mutated here, so a `None` leaves the wrapped optimizer's own step() as a clean fallback; the reason is
@@ -700,9 +751,8 @@ def _fused_plan(opt, why=None):
         return None
 
     master = getattr(opt, '_master_weights', False)
-    is_sgd = isinstance(opt, torch.optim.SGD)
-    is_adam = isinstance(opt, (torch.optim.Adam, torch.optim.AdamW))
-    if not (is_sgd or is_adam or isinstance(opt, (Lamb, Lars))):
+    kind = _optimizer_kind(opt)
+    if kind is None:
         return no('the optimizer is %s, not SGD, Adam or AdamW, or hvd.Lamb or hvd.Lars' % type(opt).__name__)
     grad_of = getattr(opt, '_grad_for_update', lambda q: q.grad)
     plan = []
@@ -710,7 +760,7 @@ def _fused_plan(opt, why=None):
         params = [p for p in group['params'] if p.grad is not None]
         if not params:
             continue
-        if group.get('maximize', False) or (is_adam and group.get('amsgrad', False)):
+        if group.get('maximize', False) or (kind == 'adam' and group.get('amsgrad', False)):
             return no('maximize=True or amsgrad=True')
         if not all(p.is_cuda and not p.grad.is_sparse and mpi_ops._is_dense(p) and p.grad.stride() == p.stride() for p in params):
             return no('a parameter is not a dense CUDA tensor, its gradient is sparse, or its strides differ from the gradient\'s')
@@ -722,7 +772,7 @@ def _fused_plan(opt, why=None):
         if master and any(pd != torch.float32 and gd != pd for pd, gd in by_dtype):
             return no('bf16 / fp16 parameters with gradients of another dtype')  # master kernels: (bf16, bf16), (fp16, fp16)
         for ps in by_dtype.values():
-            if is_sgd and group.get('momentum', 0.0) != 0.0 and not master:
+            if kind == 'sgd' and group.get('momentum', 0.0) != 0.0 and not master:
                 have = [opt.state[p].get('momentum_buffer') is not None for p in ps]
                 if any(have) and not all(have):
                     return None  # partially initialised momentum (parameters added later): let torch handle it
@@ -742,11 +792,30 @@ def _master_param(opt, p):
     return w
 
 
+def _param_state(opt, kind, p, keys, master):
+    """p's state `keys` for the fused kernel and whether it starts now: zeros, or in the kernel's dtype and p's strides
+    (torch's step and load_state_dict leave p's dtype or a checkpoint's layout).  The step count becomes a tensor."""
+    st = opt.state[p]
+    dtype = _state_dtype(kind, p.dtype, master)
+    fresh = bool(keys) and st.get(keys[0]) is None
+    if kind in _COUNTS_STEPS:
+        step = 0.0 if fresh else st['step']
+        st['step'] = step if torch.is_tensor(step) else torch.tensor(float(step))
+    out = []
+    for key in keys:
+        t = st.get(key)
+        if t is None:
+            t = st[key] = torch.zeros_like(p, dtype=dtype, memory_format=torch.preserve_format)
+        elif t.dtype != dtype or t.stride() != p.stride():
+            t = st[key] = _state_like(p, t, dtype)
+        out.append(t)
+    return out, fresh
+
+
 def _fused_step(opt):
     """One multi-tensor kernel for the whole model when the wrapped optimizer is SGD or Adam/AdamW on CUDA, three for
     Lamb and Lars (their trust ratios need whole-tensor norms before the update). With master weights a plan that cannot
     be fused raises RuntimeError instead of returning False."""
-    native = mpi_ops._native()
     use_master = getattr(opt, '_master_weights', False)
     why = []
     plan = _fused_plan(opt, why)
@@ -755,74 +824,20 @@ def _fused_step(opt):
             raise RuntimeError('master_weights: the fused optimizer update cannot run (%s), and torch\'s own update would '
                                'bypass the fp32 master weights' % (why[0] if why else 'not eligible'))
         return False
-    is_sgd = isinstance(opt, torch.optim.SGD)
+    kind = _optimizer_kind(opt)
     with torch.no_grad():
         for group, ps, grads in plan:
             master = use_master and ps[0].dtype != torch.float32
             masters = [_master_param(opt, p) for p in ps] if master else []
-            if is_sgd:
-                mom = group.get('momentum', 0.0)
-                sdt = torch.float32 if master else None  # momentum dtype: fp32 with masters, else the parameter's
-                bufs, fresh = [], []
-                if mom != 0.0:
-                    for p in ps:
-                        st = opt.state[p]
-                        buf = st.get('momentum_buffer')
-                        if buf is None:
-                            buf = st['momentum_buffer'] = torch.zeros_like(p, dtype=sdt, memory_format=torch.preserve_format)
-                            fresh.append(True)
-                        else:
-                            if buf.dtype != (sdt or p.dtype) or buf.stride() != p.stride():
-                                buf = st['momentum_buffer'] = _state_like(p, buf, sdt or p.dtype)
-                            fresh.append(False)
-                        bufs.append(buf)
-                # with masters a parameter that joins later (frozen so far) starts its momentum while the others continue:
-                # one launch for each (without masters the plan only admits all-fresh or none-fresh)
-                parts = [[i for i, f in enumerate(fresh) if f == want] for want in (True, False)] if any(fresh) and not all(fresh) \
-                    else [list(range(len(ps)))]
-                for idx in parts:
-                    pick = lambda xs: [xs[i] for i in idx] if xs else xs  # noqa: E731
-                    kw = {'master_params': pick(masters)} if master else {}
-                    native.fused_sgd_step(pick(ps), pick(grads), pick(bufs), float(group['lr']), float(mom),
-                                          float(group.get('dampening', 0.0)), float(group.get('weight_decay', 0.0)),
-                                          bool(group.get('nesterov', False)), 1.0, bool(fresh) and fresh[idx[0]], **kw)
-            elif isinstance(opt, Lars):
-                # fp32 momentum that starts at zero: one launch set per (group, dtype), no first-step special case
-                bufs = []
-                for p in ps:
-                    st = opt.state[p]
-                    buf = st.get('momentum_buffer')
-                    if buf is None:
-                        buf = st['momentum_buffer'] = torch.zeros_like(p, dtype=torch.float32,
-                                                                       memory_format=torch.preserve_format)
-                    elif buf.dtype != torch.float32 or buf.stride() != p.stride():
-                        buf = st['momentum_buffer'] = _state_like(p, buf, torch.float32)
-                    bufs.append(buf)
-                kw = {'master_params': masters} if master else {}
-                native.fused_lars_step(ps, grads, bufs, float(group['lr']), float(group['momentum']),
-                                       float(group['weight_decay']), float(group['trust_coefficient']), float(group['eps']),
-                                       Lars.adapts(group), 1.0, **kw)
-            else:
-                exp_avg, exp_avg_sq, steps = [], [], []
-                for p in ps:
-                    st = opt.state[p]
-                    if len(st) == 0 or 'exp_avg' not in st:
-                        st['step'] = torch.tensor(0.0)
-                        st['exp_avg'] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
-                        st['exp_avg_sq'] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
-                    else:
-                        # torch's own step (closure, broadcast_optimizer_state's initialisation) and load_state_dict
-                        # leave moments in the parameter's dtype or a checkpoint's layout; the kernel reads fp32 moments
-                        # element for element with the parameter
-                        for key in ('exp_avg', 'exp_avg_sq'):
-                            t = st[key]
-                            if t.dtype != torch.float32 or t.stride() != p.stride():
-                                st[key] = _state_like(p, t, torch.float32)
-                    if not torch.is_tensor(st['step']):
-                        st['step'] = torch.tensor(float(st['step']))
-                    steps.append(st['step'])
-                    exp_avg.append(st['exp_avg'])
-                    exp_avg_sq.append(st['exp_avg_sq'])
+            keys = _state_keys(kind, group)
+            per_param, fresh = zip(*[_param_state(opt, kind, p, keys, master) for p in ps])
+            states = [[st[k] for st in per_param] for k in range(len(keys))]
+            # one launch per (step count, momentum start), normally one: Adam's and LAMB's bias corrections follow each
+            # parameter's own count (a parameter without a gradient does not advance, a checkpoint may mix counts); with
+            # masters an SGD parameter that joins later starts its momentum while the others continue
+            counts = [0] * len(ps)
+            if kind in _COUNTS_STEPS:
+                steps = [opt.state[p]['step'] for p in ps]
                 # one host-side call for the whole group instead of a tensor op per parameter (BERT-large: ~400 of them)
                 cpu_steps = [t for t in steps if not t.is_cuda]
                 if cpu_steps:
@@ -830,29 +845,14 @@ def _fused_step(opt):
                 for t in steps:
                     if t.is_cuda:
                         t.add_(1)
-                # the bias corrections follow each parameter's own step count (a parameter without a gradient does not
-                # advance, a checkpoint may mix counts): one launch per distinct count, normally exactly one
-                counts = torch.stack(cpu_steps).tolist() if len(cpu_steps) == len(steps) else [int(t.item()) for t in steps]
-                by_step = {}
-                for i, c in enumerate(counts):
-                    by_step.setdefault(int(c), []).append(i)
-                b1, b2 = group['betas']
-                adamw = isinstance(opt, torch.optim.AdamW) or bool(group.get('decoupled_weight_decay', False))
-                for step, idx in by_step.items():
-                    if len(by_step) > 1:
-                        sub = lambda xs: [xs[i] for i in idx]  # noqa: E731
-                        args = (sub(ps), sub(grads), sub(exp_avg), sub(exp_avg_sq))
-                        kw = {'master_params': sub(masters)} if master else {}
-                    else:
-                        args = (ps, grads, exp_avg, exp_avg_sq)
-                        kw = {'master_params': masters} if master else {}
-                    if isinstance(opt, Lamb):
-                        native.fused_lamb_step(*args, float(group['lr']), float(b1), float(b2), float(group['eps']),
-                                               float(group['weight_decay']), step, bool(group['bias_correction']),
-                                               Lamb.adapts(group), 1.0, **kw)
-                    else:
-                        native.fused_adam_step(*args, float(group['lr']), float(b1), float(b2), float(group['eps']),
-                                               float(group.get('weight_decay', 0.0)), step, 1.0, adamw, **kw)
+                counts = torch.stack(cpu_steps).tolist() if len(cpu_steps) == len(steps) else [t.item() for t in steps]
+            parts = {}
+            for i, (c, f) in enumerate(zip(counts, fresh)):
+                parts.setdefault((int(c), kind == 'sgd' and f), []).append(i)
+            for (step, first), idx in parts.items():
+                pick = lambda xs: [xs[i] for i in idx] if xs else xs  # noqa: E731
+                _fused_update(opt, kind, group, pick(ps), pick(grads), [pick(s) for s in states], pick(masters),
+                              step=step, first_step=first)
     return True
 
 
@@ -1052,7 +1052,7 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     if master_weights:
         if op == Adasum:
             raise ValueError('master_weights is not supported with op=Adasum')
-        if not isinstance(optimizer, (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW, Lamb, Lars)):
+        if _optimizer_kind(optimizer) is None:
             raise ValueError('master_weights supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
                              % type(optimizer).__name__)
         for g in optimizer.param_groups:

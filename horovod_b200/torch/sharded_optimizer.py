@@ -37,10 +37,9 @@ import torch
 from horovod_b200.common.process_sets import global_process_set
 from horovod_b200.torch import mpi_ops
 from horovod_b200.torch.compression import Compression
-from horovod_b200.torch.lamb import Lamb
-from horovod_b200.torch.lars import Lars
 from horovod_b200.torch.mpi_ops import Average, Sum
-from horovod_b200.torch.optimizer import _check_grad_accumulation_dtype, _find_duplicates, _fold
+from horovod_b200.torch.optimizer import (_COUNTS_STEPS, _STATE_KEYS, _check_grad_accumulation_dtype, _find_duplicates,
+                                          _fold, _fused_update, _optimizer_kind, _state_dtype, _state_keys)
 
 ALIGN = 128  # bytes: every parameter and every shard starts at a multiple of this
 
@@ -147,15 +146,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
                  bucket_cap_mb=32, master_weights=False, grad_accumulation_dtype=None):
         super().__init__(params)
-        if isinstance(self, torch.optim.SGD):
-            kind = 'sgd'
-        elif isinstance(self, (torch.optim.Adam, torch.optim.AdamW)):
-            kind = 'adam'
-        elif isinstance(self, Lamb):
-            kind = 'lamb'
-        elif isinstance(self, Lars):
-            kind = 'lars'
-        else:
+        kind = _optimizer_kind(self)
+        if kind is None:
             raise ValueError('shard_optimizer_state supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
                              % type(self).__name__)
         for g in self.param_groups:
@@ -231,16 +223,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 lo, hi = shard_range(b, self._rank)
                 b['pshard'], b['gshard'] = pflat[lo:hi], gflat[lo:hi]
                 master = master_weights and b['dtype'] != torch.float32
-                if kind == 'sgd':
-                    # the fused SGD kernel keeps momentum in the parameter dtype, or in fp32 with master weights
-                    b['state'] = {'momentum_buffer': torch.zeros(b['shard'], dtype=torch.float32 if master else b['dtype'],
-                                                                 device=device)} \
-                        if self.param_groups[b['group']].get('momentum', 0.0) != 0.0 else {}
-                elif kind == 'lars':
-                    b['state'] = {'momentum_buffer': torch.zeros(b['shard'], dtype=torch.float32, device=device)}
-                else:
-                    b['state'] = {'exp_avg': torch.zeros(b['shard'], dtype=torch.float32, device=device),
-                                  'exp_avg_sq': torch.zeros(b['shard'], dtype=torch.float32, device=device)}
+                b['state'] = {key: torch.zeros(b['shard'], dtype=_state_dtype(kind, b['dtype'], master), device=device)
+                              for key in _state_keys(kind, self.param_groups[b['group']])}
                 if master:
                     # fp32 master copy of the owned shard of a bf16 / fp16 bucket: optimizer state, sharded like the moments
                     b['state']['master_param'] = b['pshard'].float()
@@ -250,15 +234,15 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._stats = mpi_ops.symm_empty(ALIGN // 4 * self._nranks, dtype=torch.float32, device=device,
                                          process_set=process_set)
         self._stats.zero_()
-        self._lamb_norms = None
+        self._trust_norms = None
         if kind in ('lamb', 'lars'):
-            # the whole-parameter sums of squares of LAMB (w, u) or LARS (w, g) in slot = the parameter's index in
-            # param_groups order: every rank adds the pieces of its own shards and one allreduce sums them.  Padded like
-            # _stats.  (Named for LAMB, which came first.)
+            # the whole-parameter sums of squares of LAMB (w, u) or LARS (w, g) that their trust ratios need, in slot =
+            # the parameter's index in param_groups order: every rank adds the pieces of its own shards and one allreduce
+            # sums them.  Padded like _stats.
             self._slot = {p: i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
             unit = ALIGN // 4 * self._nranks
-            self._lamb_norms = mpi_ops.symm_empty((2 * len(self._slot) + unit - 1) // unit * unit, dtype=torch.float32,
-                                                  device=device, process_set=process_set)
+            self._trust_norms = mpi_ops.symm_empty((2 * len(self._slot) + unit - 1) // unit * unit, dtype=torch.float32,
+                                                   device=device, process_set=process_set)
         self._delay = {p: backward_passes_per_step for p in self._p_to_bucket}
         self._seen = set()  # parameters whose gradient hook fired since the last synchronize()
         self._reset_launch_order()
@@ -460,9 +444,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             self._should_synchronize = True
 
     def _update_shards(self, coef=None):
-        """One fused kernel per param group and dtype over this rank's shards; hyper-parameters are read now, so LR
-        schedulers work.  coef: the clip coefficient on the device, or None."""
-        native = mpi_ops._native()
+        """One fused kernel per param group and dtype over this rank's shards.  coef: the clip coefficient on the
+        device, or None."""
         by_group = {}
         for b in self._buckets:
             by_group.setdefault((b['group'], b['dtype']), []).append(b)
@@ -472,27 +455,17 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 return
             for (gi, _), bs in by_group.items():
                 group = self.param_groups[gi]
-                ps, gs = [b['pshard'] for b in bs], [b['gshard'] for b in bs]
+                keys = _state_keys(self._kind, group)
                 # every bucket of a (group, dtype) has a master or none has
-                kw = {'master_params': [b['state']['master_param'] for b in bs]} if 'master_param' in bs[0]['state'] else {}
-                if self._kind == 'sgd':
-                    mom = group.get('momentum', 0.0)
-                    bufs = [b['state']['momentum_buffer'] for b in bs] if mom != 0.0 else []
-                    first = mom != 0.0 and not bs[0]['mom_init']
-                    native.fused_sgd_step(ps, gs, bufs, float(group['lr']), float(mom), float(group.get('dampening', 0.0)),
-                                          float(group.get('weight_decay', 0.0)), bool(group.get('nesterov', False)), 1.0, first,
-                                          coef, **kw)
-                    for b in bs:
-                        b['mom_init'] = b['mom_init'] or mom != 0.0
-                else:
+                masters = [b['state']['master_param'] for b in bs] if 'master_param' in bs[0]['state'] else []
+                if self._kind in _COUNTS_STEPS:
                     for b in bs:
                         b['step'] += 1
-                    b1, b2 = group['betas']
-                    adamw = isinstance(self, torch.optim.AdamW) or bool(group.get('decoupled_weight_decay', False))
-                    native.fused_adam_step(ps, gs, [b['state']['exp_avg'] for b in bs], [b['state']['exp_avg_sq'] for b in bs],
-                                           float(group['lr']), float(b1), float(b2), float(group['eps']),
-                                           float(group.get('weight_decay', 0.0)), bs[0]['step'], 1.0, adamw, coef, **kw)
+                _fused_update(self, self._kind, group, [b['pshard'] for b in bs], [b['gshard'] for b in bs],
+                              [[b['state'][key] for b in bs] for key in keys], masters, step=bs[0]['step'],
+                              first_step=bool(keys) and not bs[0]['mom_init'], coef=coef)
                 for b in bs:
+                    b['mom_init'] = b['mom_init'] or (self._kind == 'sgd' and bool(keys))
                     b['stepped'] = True
 
     def _update_shards_trust(self, by_group, coef):
@@ -501,18 +474,15 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         phase per (group, dtype) adds the pieces' sums of squares into the registered norms buffer, one allreduce sums
         them over the ranks, and the apply phase per (group, dtype) updates the pieces with the same r on every rank.
         The clip coefficient reaches the phases that read the gradient.  Padding is not touched."""
-        native = mpi_ops._native()
-        lamb = self._kind == 'lamb'
-        keys = ('exp_avg', 'exp_avg_sq') if lamb else ('momentum_buffer',)
+        keys = _STATE_KEYS[self._kind]
         calls = []
         for (gi, _), bs in by_group.items():
-            group = self.param_groups[gi]
             lists, masters, slots = tuple([] for _ in range(2 + len(keys))), [], []
             for b in bs:
                 st = b['state']
                 b['step'] += 1
                 b['stepped'] = True
-                if not lamb:
+                if self._kind == 'lars':
                     b['mom_init'] = True  # LARS momentum: state_dict() gathers it from now on
                 for k, plo, phi, slo in shard_slices(b, self._rank):
                     cut = slice(slo, slo + phi - plo)
@@ -521,27 +491,16 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                     if 'master_param' in st:
                         masters.append(st['master_param'][cut])
                     slots.append(self._slot[b['params'][k]])
-            calls.append((group, bs[0]['step'], lists, masters, slots))
-        norms = self._lamb_norms
+            calls.append((self.param_groups[gi], bs[0]['step'], lists, masters, slots))
+        norms = self._trust_norms
         norms.zero_()
         for group, step, lists, masters, slots in calls:
-            if lamb:
-                b1, b2 = group['betas']
-                native.lamb_norms(*lists, float(b1), float(b2), float(group['eps']), float(group['weight_decay']), step,
-                                  bool(group['bias_correction']), 1.0, coef, masters, norms, slots)
-            else:
-                native.lars_norms(*lists, 1.0, coef, masters, norms, slots)
+            _fused_update(self, self._kind, group, lists[0], lists[1], list(lists[2:]), masters, step=step, coef=coef,
+                          phase='norms', norms=norms, slots=slots)
         mpi_ops.captured_allreduce_(norms, op=Sum, process_set=self.process_set)
         for group, step, lists, masters, slots in calls:
-            if lamb:
-                b1, b2 = group['betas']
-                native.lamb_apply(*lists, float(group['lr']), float(b1), float(b2), float(group['eps']),
-                                  float(group['weight_decay']), step, bool(group['bias_correction']), Lamb.adapts(group),
-                                  masters, norms, slots)
-            else:
-                native.lars_apply(*lists, float(group['lr']), float(group['momentum']), float(group['weight_decay']),
-                                  float(group['trust_coefficient']), float(group['eps']), Lars.adapts(group), 1.0, coef,
-                                  masters, norms, slots)
+            _fused_update(self, self._kind, group, lists[0], lists[1], list(lists[2:]), masters, step=step, coef=coef,
+                          phase='apply', norms=norms, slots=slots)
 
     def _allgather_params(self):
         comm = self._comm
@@ -622,7 +581,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         index = {id(p): i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
         state = {}
         for b in self._buckets:
-            if not b['state'] or ((b['step'] == 0) if self._kind in ('adam', 'lamb') else
+            if not b['state'] or ((b['step'] == 0) if self._kind in _COUNTS_STEPS else
                                   not (b['mom_init'] or ('master_param' in b['state'] and b['stepped']))):
                 continue  # no state yet (the same on every rank); an SGD / LARS bucket may still hold masters only
             gathered = {}
@@ -631,7 +590,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 gathered[key] = full_from_shards(b, [full], [p.shape for p in b['params']], [p.stride() for p in b['params']])
             for k, p in enumerate(b['params']):
                 st = {key: vals[k].detach().cpu().clone() for key, vals in gathered.items()}
-                if self._kind in ('adam', 'lamb'):
+                if self._kind in _COUNTS_STEPS:
                     st['step'] = torch.tensor(float(b['step']))
                 state[index[id(p)]] = st
         sd['state'] = state

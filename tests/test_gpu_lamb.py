@@ -657,16 +657,16 @@ def test_sharded_lamb_with_grad_scaler(hvd, team):
                 torch.testing.assert_close(a.float(), b.float(), rtol=1e-2, atol=1e-3, msg=lambda s: '%s: %s' % (name, s))
 
 
-def test_norms_buffer_only_for_lamb(hvd, team):
+def test_trust_norms_buffer_only_for_lamb(hvd, team):
     """The sharded optimizer allocates the padded norms buffer for Lamb only."""
     torch.manual_seed(0)
     base = _ConvNet().cuda()
     models, opts = _sharded_team(hvd, team, base, torch.float32, False)
-    assert opts[0]._lamb_norms is not None and opts[0]._lamb_norms.numel() % (32 * team.n) == 0
+    assert opts[0]._trust_norms is not None and opts[0]._trust_norms.numel() % (32 * team.n) == 0
     m = copy.deepcopy(base)
     o = hvd.DistributedOptimizer(torch.optim.AdamW(m.parameters()), named_parameters=m.named_parameters(),
                                  shard_optimizer_state=True, process_set=_FakeSet(team.n, 0))
-    assert o._lamb_norms is None
+    assert o._trust_norms is None
 
 
 @pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")

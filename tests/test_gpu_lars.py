@@ -630,19 +630,19 @@ def test_sharded_lars_with_grad_scaler(hvd, team):
                 torch.testing.assert_close(a.float(), b.float(), rtol=1e-2, atol=1e-3, msg=lambda s: '%s: %s' % (name, s))
 
 
-def test_norms_buffer_only_for_lamb_and_lars(hvd, team):
+def test_trust_norms_buffer_only_for_lamb_and_lars(hvd, team):
     """The sharded optimizer allocates the padded norms buffer for Lamb and Lars only."""
     torch.manual_seed(0)
     base = _ConvNet().cuda()
     models, opts = _sharded_team(hvd, team, base, torch.float32, False)
-    assert opts[0]._lamb_norms is not None and opts[0]._lamb_norms.numel() % (32 * team.n) == 0
-    assert opts[0]._lamb_norms.numel() >= 2 * len(list(base.parameters()))
+    assert opts[0]._trust_norms is not None and opts[0]._trust_norms.numel() % (32 * team.n) == 0
+    assert opts[0]._trust_norms.numel() >= 2 * len(list(base.parameters()))
     for make in (lambda ps: hvd.Lamb(ps), lambda ps: torch.optim.SGD(ps, lr=0.1, momentum=0.9),
                  lambda ps: torch.optim.AdamW(ps)):
         m = copy.deepcopy(base)
         o = hvd.DistributedOptimizer(make(m.parameters()), named_parameters=m.named_parameters(),
                                      shard_optimizer_state=True, process_set=_FakeSet(team.n, 0))
-        assert (o._lamb_norms is not None) == isinstance(o, hvd.Lamb)
+        assert (o._trust_norms is not None) == isinstance(o, hvd.Lamb)
 
 
 @pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
