@@ -35,6 +35,7 @@ import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 
 from horovod_b200 import models, ops  # noqa: E402
+from horovod_b200.torch.grad_buckets import shard_layout  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
 BYTES = {'first': 8, 'add': 12, 'last': 8}
@@ -52,19 +53,10 @@ def _gpu_info():
 
 
 def _bucket_numels(make):
-    """Element counts of the bf16 buckets of DistributedOptimizer._setup_buckets for the model's parameters."""
+    """Element counts of the zero-copy buckets of DistributedOptimizer for the model's parameters in bf16."""
     with torch.device('meta'):
-        numels = [p.numel() for p in make().parameters() if p.requires_grad]
-    out, cur = [], 0
-    for n in reversed(numels):
-        nbytes = (n * 2 + 127) // 128 * 128
-        if cur and cur + nbytes > CAP:
-            out.append(cur // 2)
-            cur = 0
-        cur += nbytes
-    if cur:
-        out.append(cur // 2)
-    return out
+        params = [(p.numel(), torch.bfloat16) for p in make().parameters() if p.requires_grad]
+    return [b['numel'] for b in shard_layout([params], 1, CAP)]
 
 
 def _time(fn, iters):

@@ -17,8 +17,12 @@ import torch
 from horovod_b200.common.exceptions import HorovodInternalError
 from horovod_b200.common.process_sets import global_process_set
 from horovod_b200.common.util import split_list
-from horovod_b200.torch import mpi_ops
+from horovod_b200.torch import grad_buckets, mpi_ops
 from horovod_b200.torch.compression import Compression
+from horovod_b200.torch.grad_buckets import (accumulates, adopt_grad, adopt_missing_grads, bucket_accumulators,
+                                             check_grad_accumulation_dtype, check_named_parameters, find_duplicates,
+                                             fold, fold_arrived, fold_last, grad_bucket, mark_fold_last, reset_folds,
+                                             scales, shard_layout)
 from horovod_b200.torch.lamb import Lamb
 from horovod_b200.torch.lars import Lars
 from horovod_b200.torch.mpi_ops import (Adasum, Average, Sum, allreduce_async_, grouped_allreduce_async_, rank, size,
@@ -34,7 +38,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._compression = compression
         # fp32 accumulators of bf16 / fp16 gradients over the backward passes of one step (allocated on first use, not
         # optimizer state): bucket -> bucket['acc'], parameter outside the buckets -> self._param_accs[p]
-        self._acc_fp32 = _check_grad_accumulation_dtype(grad_accumulation_dtype)
+        self._acc_fp32 = check_grad_accumulation_dtype(grad_accumulation_dtype)
         self._param_accs = {}
         self._acc_open = set()  # parameters outside the buckets folded this step whose 'last' fold is still to come
         # fp32 master copies of bf16 / fp16 parameters, kept as optimizer state ('master_param') and updated by the fused
@@ -47,26 +51,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             bucket_wire_dtype = {'bf16': torch.bfloat16, 'fp16': torch.float16}.get(os.environ.get('HVD_BUCKET_WIRE_DTYPE', ''))
         self._bucket_wire_dtype = bucket_wire_dtype
 
-        if named_parameters is not None:
-            named_parameters = list(named_parameters)
-        else:
-            named_parameters = [(f'allreduce.noname.{i}.{j}', v)
-                                for i, param_group in enumerate(self.param_groups)
-                                for j, v in enumerate(param_group['params'])]
-        # make sure that named_parameters are tuples
-        if any([not isinstance(p, tuple) for p in named_parameters]):
-            raise ValueError('named_parameters should be a sequence of tuples (name, parameter), usually produced by '
-                             'model.named_parameters().')
-        dups = _find_duplicates([k for k, _ in named_parameters])
-        if len(dups) > 0:
-            raise ValueError('Parameter names in named_parameters must be unique. Found duplicates: %s' % ', '.join(dups))
-        all_param_ids = {id(v) for param_group in self.param_groups for v in param_group['params']}
-        named_param_ids = {id(v) for k, v in named_parameters}
-        unnamed_param_ids = all_param_ids - named_param_ids
-        if len(unnamed_param_ids):
-            raise ValueError('named_parameters was specified, but one or more model parameters were not named. Python '
-                             'object ids: %s' % ', '.join(str(id) for id in unnamed_param_ids))
-
+        named_parameters = check_named_parameters(self, named_parameters)
         self._parameter_names = {v: k for k, v in sorted(named_parameters)}
         self.backward_passes_per_step = backward_passes_per_step
         self._allreduce_delay = {v: self.backward_passes_per_step for _, v in sorted(named_parameters)}
@@ -146,7 +131,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     @staticmethod
     def find_duplicates(lst):
-        return _find_duplicates(lst)
+        return find_duplicates(lst)
 
     def set_backward_passes_per_step(self, passes):
         self.backward_passes_per_step = passes
@@ -192,48 +177,26 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     def _setup_buckets(self, cap_bytes):
         """Lays the gradients of all dense CUDA parameters out in a few flat buffers of registered symmetric memory
         (p.grad becomes a view, like DDP's gradient_as_bucket_view). A bucket is allreduced IN PLACE as one tensor by the
-        zero-copy NVLink kernel as soon as its last gradient is accumulated: no per-tensor negotiation, no pack/unpack."""
+        zero-copy NVLink kernel as soon as its last gradient is accumulated: no per-tensor negotiation, no pack/unpack.
+        The layout is the sharded optimizer's for one rank, with all parameters as one group."""
         params = [p for g in self.param_groups for p in g['params']
                   if p.requires_grad and p.is_cuda and mpi_ops._is_dense(p) and p.dtype in (torch.float32, torch.bfloat16, torch.float16)]
-        params.reverse()  # gradients become ready roughly in reverse registration order
-        by_dtype = {}
-        for p in params:
-            by_dtype.setdefault(p.dtype, []).append(p)
         try:
-            for dtype, ps in by_dtype.items():
-                itemsize = ps[0].element_size()
-                cur, cur_bytes = [], 0
-                layouts = []
-                for p in ps:
-                    nbytes = (p.numel() * itemsize + 127) // 128 * 128
-                    if cur and cur_bytes + nbytes > cap_bytes:
-                        layouts.append((cur, cur_bytes))
-                        cur, cur_bytes = [], 0
-                    cur.append((p, cur_bytes))
-                    cur_bytes += nbytes
-                if cur:
-                    layouts.append((cur, cur_bytes))
-                for members, total in layouts:
-                    flat = mpi_ops.symm_empty(total // itemsize, dtype=dtype, device=members[0][0].device, process_set=self.process_set)
-                    flat.zero_()
-                    bucket = {'flat': flat, 'params': [m[0] for m in members], 'pending': len(members),
-                              'name': 'bucket.%d' % len(self._buckets), 'handle': None, 'shadow': None, 'shadow_views': None,
-                              'offsets': {m[0]: m[1] for m in members}, 'views': {}, 'acc': None, 'arrived': 0, 'folds': 0}
-                    if self._bucket_wire_dtype is not None and dtype == torch.float32:
-                        shadow = mpi_ops.symm_empty(total // itemsize, dtype=self._bucket_wire_dtype, device=members[0][0].device,
-                                                    process_set=self.process_set)
-                        shadow.zero_()
-                        bucket['shadow'] = shadow
-                        bucket['shadow_views'] = {p: shadow[off // itemsize: off // itemsize + p.numel()].as_strided(p.size(), p.stride())
-                                                  for p, off in members}
-                    for p, off in members:
-                        view = flat[off // itemsize: off // itemsize + p.numel()].as_strided(p.size(), p.stride())
-                        if p.grad is not None:
-                            view.copy_(p.grad)
-                        p.grad = view
-                        bucket['views'][p] = view
-                        self._p_to_bucket[p] = bucket
-                    self._buckets.append(bucket)
+            for layout in shard_layout([[(p.numel(), p.dtype) for p in params]], 1, cap_bytes):
+                members = [params[i] for i, _, _ in layout['members']]
+                bucket = grad_bucket(layout, members, members[0].device, self.process_set)
+                bucket.update({'pending': len(members), 'name': 'bucket.%d' % len(self._buckets), 'handle': None,
+                               'shadow': None, 'shadow_views': None})
+                self._buckets.append(bucket)
+                if self._bucket_wire_dtype is not None and layout['dtype'] == torch.float32:
+                    shadow = mpi_ops.symm_empty(layout['numel'], dtype=self._bucket_wire_dtype, device=members[0].device,
+                                                process_set=self.process_set)
+                    shadow.zero_()
+                    bucket['shadow'] = shadow
+                    bucket['shadow_views'] = {p: shadow[off:off + numel].as_strided(p.size(), p.stride())
+                                              for p, (_, off, numel) in zip(members, layout['members'])}
+                for p in members:
+                    self._p_to_bucket[p] = bucket
             self._zero_copy = True
         except HorovodInternalError as e:
             warnings.warn('zero-copy gradient buckets unavailable (%s); using the fused pack/unpack path' % e)
@@ -243,22 +206,28 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._buckets, self._p_to_bucket, self._zero_copy = [], {}, False
 
     def _launch_bucket(self, bucket):
-        if bucket['folds']:
-            # gradient accumulation in fp32: the bucket's sum over the step's backward passes, rounded once, is what is
-            # reduced (the fold runs on this stream, so it precedes the allreduce)
-            _fold([bucket['flat']], [bucket['acc']], 'last')
-            bucket['folds'] = 0
-        if self.op == Average:
-            prescale_factor, postscale_factor = 1.0 / self.gradient_predivide_factor, self.gradient_predivide_factor
-        else:
-            prescale_factor = postscale_factor = 1.0
-        wire = bucket['flat']
-        if bucket.get('shadow') is not None:
-            wire = bucket['shadow']
-            wire.copy_(bucket['flat'])  # one cast kernel fp32 -> wire dtype on the caller's stream
-        bucket['handle'] = allreduce_async_(wire, name=bucket['name'], op=self.op, prescale_factor=prescale_factor,
-                                            postscale_factor=postscale_factor, process_set=self.process_set)
-        bucket['pending'] = len(bucket['params'])
+        """Allreduces the bucket in place: with allreduce_async_ on the caller's stream, or, while hvd.GraphedStep
+        captures, as a captured_allreduce_ node forked onto the side stream (so it overlaps the rest of backward)."""
+        cap = self._graph_capture
+        fold_last(bucket, cap is not None)  # on the caller's stream, so it precedes the allreduce
+        prescale_factor, postscale_factor = scales(self)
+        if cap is not None:
+            cap['comm'].wait_stream(torch.cuda.current_stream())  # fork: everything recorded so far (this bucket's gradients) precedes it
+        with torch.cuda.stream(cap['comm'] if cap is not None else None):
+            wire = bucket['gflat']
+            if bucket['shadow'] is not None:
+                wire = bucket['shadow']
+                wire.copy_(bucket['gflat'])  # one cast kernel fp32 -> wire dtype
+            if cap is None:
+                bucket['handle'] = allreduce_async_(wire, name=bucket['name'], op=self.op, prescale_factor=prescale_factor,
+                                                    postscale_factor=postscale_factor, process_set=self.process_set)
+                bucket['pending'] = len(bucket['params'])
+                return
+            # the last bucket in registration order holds the first layers' gradients: backward is over when it is ready
+            tail = cap['tail'] or bucket is self._buckets[-1]
+            mpi_ops.captured_allreduce_(wire, op=self.op, prescale_factor=prescale_factor, postscale_factor=postscale_factor,
+                                        process_set=self.process_set, max_ctas=cap['tail_ctas'] if tail else cap['ctas'])
+        cap['launched'].add(id(bucket))
 
     def _allreduce_grad_async(self, p):
         if p.grad is None:
@@ -273,13 +242,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             else:
                 return mpi_ops.sparse_allreduce_async(tensor, name=name, op=self.op, process_set=self.process_set), None
         tensor_compressed, ctx = self._compression.compress(tensor)
-        if self.op == Average:
-            # split the averaging into pre- and post-division around the sum (reference optimizer.py:197-204)
-            prescale_factor = 1.0 / self.gradient_predivide_factor
-            postscale_factor = self.gradient_predivide_factor
-        else:
-            prescale_factor = 1.0
-            postscale_factor = 1.0
+        prescale_factor, postscale_factor = scales(self)
         handle = allreduce_async_(tensor_compressed, name=name, op=self.op, prescale_factor=prescale_factor,
                                   postscale_factor=postscale_factor, process_set=self.process_set)
         return handle, ctx
@@ -290,12 +253,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             if p.grad is None:
                 p.grad = torch.zeros_like(p.data)
         tensors_compressed, ctxs = zip(*[self._compression.compress(p.grad) for p in ps])
-        if self.op == Average:
-            prescale_factor = 1.0 / self.gradient_predivide_factor
-            postscale_factor = self.gradient_predivide_factor
-        else:
-            prescale_factor = 1.0
-            postscale_factor = 1.0
+        prescale_factor, postscale_factor = scales(self)
         handle = grouped_allreduce_async_(list(tensors_compressed), name=name, op=self.op, prescale_factor=prescale_factor,
                                           postscale_factor=postscale_factor, process_set=self.process_set)
         return handle, ctxs
@@ -326,27 +284,15 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._allreduce_delay[p] -= 1
             bucket = self._p_to_bucket.get(p)
             if bucket is not None:
-                if p.grad.is_sparse or p.grad.data_ptr() != bucket['flat'].data_ptr() + bucket['offsets'][p]:
-                    # model.zero_grad() (set_to_none=True is torch's default) or `p.grad = None` dropped the bucket view and
-                    # autograd allocated a fresh gradient: move it into the registered bucket and re-point p.grad, so the
-                    # reference idiom keeps working (one extra copy for that parameter; optimizer.zero_grad() avoids it)
-                    view = bucket['views'][p]
-                    view.copy_(p.grad.to_dense() if p.grad.is_sparse else p.grad)
-                    p.grad = view
+                adopt_grad(p, bucket['views'][p], densify=True)
                 self._handles[p] = ('bucket', None)
-                if self._accumulates(bucket['flat']):
-                    bucket['arrived'] += 1
-                    if bucket['arrived'] == len(bucket['params']):  # the bucket has this backward pass's gradients
-                        bucket['arrived'] = 0
-                        if self._allreduce_delay[p] > 0:
-                            _fold([bucket['flat']], [self._bucket_acc(bucket)], 'add' if bucket['folds'] else 'first')
-                            bucket['folds'] += 1
+                fold_arrived(self, bucket, self._allreduce_delay[p] > 0)
                 if self._allreduce_delay[p] == 0:
                     bucket['pending'] -= 1
                     if bucket['pending'] == 0:
                         self._launch_bucket(bucket)
                 return
-            if self._accumulates(p.grad):
+            if accumulates(self, p.grad):
                 if self._allreduce_delay[p] > 0:
                     self._fold_param(p, 'add' if p in self._acc_open else 'first')
                 elif p in self._acc_open:
@@ -363,17 +309,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._handles[p] = (handle, ctx)
         return hook
 
-    # ---- gradient accumulation in fp32 (grad_accumulation_dtype=torch.float32) -------------------------------------------
-    def _accumulates(self, grad):
-        """True when `grad` (a bucket or a parameter's gradient) is summed over the backward passes in fp32."""
-        return (self._acc_fp32 and self.backward_passes_per_step > 1 and grad is not None and grad.is_cuda
-                and not grad.is_sparse and grad.dtype in (torch.bfloat16, torch.float16))
-
-    def _bucket_acc(self, bucket):
-        if bucket['acc'] is None:  # plain device memory: the accumulator never travels
-            bucket['acc'] = torch.empty(bucket['flat'].numel(), dtype=torch.float32, device=bucket['flat'].device)
-        return bucket['acc']
-
+    # ---- gradient accumulation in fp32 of the parameters outside the buckets (grad_buckets.py has the buckets') ----------
     def _param_acc(self, p):
         acc = self._param_accs.get(p)
         if acc is None or acc.shape != p.grad.shape or acc.stride() != p.grad.stride():
@@ -382,7 +318,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         return acc
 
     def _fold_param(self, p, mode):
-        _fold([p.grad], [self._param_acc(p)], mode)
+        fold([p.grad], [self._param_acc(p)], mode)
         if mode == 'last':
             self._acc_open.discard(p)
         else:
@@ -397,20 +333,14 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     def _reset_folds(self):
         self._acc_open.clear()
-        for bucket in self._buckets:
-            bucket['arrived'] = bucket['folds'] = 0
+        reset_folds(self._buckets)
 
     def _accumulator_pairs(self, with_buckets=True):
         """(16-bit gradients, fp32 accumulators) of every accumulating bucket and parameter, allocated now if needed."""
-        grads, accs = [], []
-        if with_buckets:
-            for bucket in self._buckets:
-                if self._accumulates(bucket['flat']):
-                    grads.append(bucket['flat'])
-                    accs.append(self._bucket_acc(bucket))
+        grads, accs = bucket_accumulators(self, with_buckets)
         for group in self.param_groups:
             for p in group['params']:
-                if p.requires_grad and p not in self._p_to_bucket and self._accumulates(p.grad):
+                if p.requires_grad and p not in self._p_to_bucket and accumulates(self, p.grad):
                     grads.append(p.grad)
                     accs.append(self._param_acc(p))
         return grads, accs
@@ -421,9 +351,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     def _graph_fold(self, mode, with_buckets=True):
         """hvd.GraphedStep, while capturing: one fold of every accumulator after the captured backward pass."""
-        grads, accs = self._accumulator_pairs(with_buckets)
-        if grads:
-            _fold(grads, accs, mode)
+        fold(*self._accumulator_pairs(with_buckets), mode)
 
     # ---- gradient allreduce as CUDA-graph nodes (hvd.GraphedStep) --------------------------------------------------------
     def _graph_capturable(self):
@@ -450,9 +378,8 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                                # (without NVLS — teams of 2 — the P2P two-shot kernel needs more CTAs to keep up with backward)
                                'ctas': int(os.environ.get('HVD_GRAPH_COMM_CTAS', '16' if '+mc' in mpi_ops.gpu_backend_info() and self.process_set.size() >= 4 else '32')),
                                'tail_ctas': int(os.environ.get('HVD_GRAPH_COMM_TAIL_CTAS', '128')), 'tail': False,
-                               'pending': {id(b): len(b['params']) for b in self._buckets},
-                               # the step's last graph of an fp32 accumulation: each bucket's 'last' fold precedes its allreduce
-                               'fold': {id(b) for b in self._buckets if self._accumulates(b['flat'])}}
+                               'pending': {id(b): len(b['params']) for b in self._buckets}}
+        mark_fold_last(self, True)  # the step's last graph of an fp32 accumulation
         return True
 
     def _graph_hook(self, p):
@@ -462,28 +389,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         cap = self._graph_capture
         cap['pending'][id(bucket)] -= 1
         if cap['pending'][id(bucket)] == 0:
-            self._graph_launch_bucket(bucket)
-
-    def _graph_launch_bucket(self, bucket):
-        cap = self._graph_capture
-        if self.op == Average:
-            prescale_factor, postscale_factor = 1.0 / self.gradient_predivide_factor, self.gradient_predivide_factor
-        else:
-            prescale_factor = postscale_factor = 1.0
-        comm = cap['comm']
-        if id(bucket) in cap['fold']:
-            _fold([bucket['flat']], [self._bucket_acc(bucket)], 'last')
-        comm.wait_stream(torch.cuda.current_stream())  # fork: everything recorded so far (this bucket's gradients) precedes it
-        with torch.cuda.stream(comm):
-            wire = bucket['flat']
-            if bucket.get('shadow') is not None:
-                wire = bucket['shadow']
-                wire.copy_(bucket['flat'])
-            # the last bucket in registration order holds the first layers' gradients: backward is over when it is ready
-            tail = cap['tail'] or bucket is self._buckets[-1]
-            mpi_ops.captured_allreduce_(wire, op=self.op, prescale_factor=prescale_factor, postscale_factor=postscale_factor,
-                                        process_set=self.process_set, max_ctas=cap['tail_ctas'] if tail else cap['ctas'])
-        cap['launched'].add(id(bucket))
+            self._launch_bucket(bucket)
 
     def _end_graph_capture(self):
         """Before stream capture ends: buckets whose last hook never fired (parameters unused by the step) are reduced
@@ -494,30 +400,17 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         cap['tail'] = True
         for bucket in self._buckets:
             if id(bucket) not in cap['launched']:
-                self._graph_launch_bucket(bucket)
+                self._launch_bucket(bucket)
         torch.cuda.current_stream().wait_stream(cap['comm'])
         self._graph_capture = None
+        mark_fold_last(self, False)
         self._graph_comm_captured = True
-
-    def _adopt_missing_grads(self, bucket):
-        """A bucket is launched from synchronize() because some hook never fired: parameters whose gradient is None (dropped
-        by model.zero_grad() and not produced this step) contribute zeros and get their bucket view back."""
-        base = bucket['flat'].data_ptr()
-        for p in bucket['params']:
-            view = bucket['views'][p]
-            if p.grad is None:
-                if p not in self._handles:
-                    view.zero_()
-                p.grad = view
-            elif p.grad.is_sparse or p.grad.data_ptr() != base + bucket['offsets'][p]:
-                view.copy_(p.grad.to_dense() if p.grad.is_sparse else p.grad)
-                p.grad = view
 
     def _restore_shadows(self):
         """Reduced values of wire-dtype shadow buckets -> the fp32 gradients that p.grad points at."""
         for bucket in self._buckets:
             if bucket.get('shadow') is not None and bucket.get('shadow_fresh'):
-                bucket['flat'].copy_(bucket['shadow'])
+                bucket['gflat'].copy_(bucket['shadow'])
                 bucket['shadow_fresh'] = False
 
     def _grad_for_update(self, p):
@@ -550,12 +443,12 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 if bucket['handle'] is None:
                     # some gradient of this bucket was not produced on this rank (or accumulation is incomplete): reduce what
                     # is there so that all ranks stay in lock-step (missing gradients are zeros)
-                    self._adopt_missing_grads(bucket)
+                    adopt_missing_grads(bucket, self._handles, densify=True)
                     self._launch_bucket(bucket)
+            reset_folds(self._buckets)
             for bucket in self._buckets:
                 synchronize(bucket['handle'])
                 bucket['handle'] = None
-                bucket['arrived'] = 0
                 if bucket.get('shadow') is not None:
                     bucket['shadow_fresh'] = True
                 for p in bucket['params']:
@@ -603,14 +496,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._group_handles.clear()
         self._synchronized = True
 
-    @contextmanager
-    def skip_synchronize(self):
-        """Use after an explicit optimizer.synchronize() (e.g. gradient clipping) so step() does not sync again."""
-        self._should_synchronize = False
-        try:
-            yield
-        finally:
-            self._should_synchronize = True
+    skip_synchronize = grad_buckets.skip_synchronize
 
     def _hvd_super_step(self, closure=None):
         return super(self.__class__, self).step(closure)
@@ -644,7 +530,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         if self._zero_copy:
             # bucketed gradients must stay views of the registered buffers: zero them in place (one memset per bucket)
             for bucket in self._buckets:
-                bucket['flat'].zero_()
+                bucket['gflat'].zero_()
             for group in self.param_groups:
                 for p in group['params']:
                     if p not in self._p_to_bucket and p.grad is not None:
@@ -657,31 +543,6 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             kwargs['set_to_none'] = False
             args = ()
         return super(self.__class__, self).zero_grad(*args, **kwargs)
-
-
-def _find_duplicates(lst):
-    seen = set()
-    dups = set()
-    for el in lst:
-        if el in seen:
-            dups.add(el)
-        seen.add(el)
-    return dups
-
-
-def _check_grad_accumulation_dtype(dtype):
-    """grad_accumulation_dtype: None (gradients accumulate in their own dtype) or torch.float32; True for the latter."""
-    if dtype is None:
-        return False
-    if dtype is torch.float32:
-        return True
-    raise ValueError('grad_accumulation_dtype must be None or torch.float32, got %r' % (dtype,))
-
-
-def _fold(grads, accs, mode):
-    from horovod_b200 import ops
-    with torch.no_grad():
-        ops.grad_accumulate_(grads, accs, mode)
 
 
 def _optimizer_kind(opt):
@@ -1046,7 +907,7 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     Between passes p.grad holds the current pass's gradient only.  fp32 gradients and backward_passes_per_step == 1 are
     unaffected.  The accumulators (one flat buffer per zero-copy bucket, else one per parameter) are allocated on first
     use and are not optimizer state: checkpoints are taken between steps.  Not with op=Adasum (ValueError)."""
-    _check_grad_accumulation_dtype(grad_accumulation_dtype)
+    check_grad_accumulation_dtype(grad_accumulation_dtype)
     if grad_accumulation_dtype is not None and op == Adasum:
         raise ValueError('grad_accumulation_dtype is not supported with op=Adasum')
     if master_weights:

@@ -30,110 +30,18 @@ accumulator and zeroed (grad_accumulate_ 'first' / 'add'), and after the k-th pa
 import math
 import os
 import warnings
-from contextlib import contextmanager
 
 import torch
 
 from horovod_b200.common.process_sets import global_process_set
-from horovod_b200.torch import mpi_ops
+from horovod_b200.torch import grad_buckets, mpi_ops
 from horovod_b200.torch.compression import Compression
+from horovod_b200.torch.grad_buckets import (ALIGN, adopt_grad, adopt_missing_grads, bucket_accumulators,
+                                             check_grad_accumulation_dtype, check_named_parameters, fold, fold_arrived,
+                                             fold_last, full_from_shards, grad_bucket, mark_fold_last, reset_folds,
+                                             scales, shard_from_full, shard_layout, shard_range, shard_slices)
 from horovod_b200.torch.mpi_ops import Average, Sum
-from horovod_b200.torch.optimizer import (_COUNTS_STEPS, _STATE_KEYS, _check_grad_accumulation_dtype, _find_duplicates,
-                                          _fold, _fused_update, _optimizer_kind, _state_dtype, _state_keys)
-
-ALIGN = 128  # bytes: every parameter and every shard starts at a multiple of this
-
-
-def _itemsize(dtype):
-    return torch.empty(0, dtype=dtype).element_size()
-
-
-def shard_layout(groups, nranks, cap_bytes):
-    """Pure layout of the sharded buckets.
-
-    groups: one list per param group of (numel, dtype) of its trainable parameters, in registration order.
-    Returns a list of buckets, each a dict with
-      'group'    index of the param group,
-      'dtype'    the parameters' dtype,
-      'members'  [(index of the parameter in `groups[group]`, element offset in the bucket, numel)],
-      'numel'    padded element count (its byte size is a multiple of nranks * 128),
-      'shard'    elements per rank (numel // nranks).
-    Parameters are taken in reverse order inside a group (gradients become ready roughly in that order), split by dtype,
-    packed at 128 B alignment and cut into buckets of at most `cap_bytes` (a larger parameter gets a bucket of its own)."""
-    buckets = []
-    for gi, params in enumerate(groups):
-        by_dtype = {}
-        for i in reversed(range(len(params))):
-            numel, dtype = params[i]
-            by_dtype.setdefault(dtype, []).append((i, numel))
-        for dtype, members in by_dtype.items():
-            item = _itemsize(dtype)
-            cur, cur_bytes = [], 0
-            layouts = []
-            for i, numel in members:
-                nbytes = (numel * item + ALIGN - 1) // ALIGN * ALIGN
-                if cur and cur_bytes + nbytes > cap_bytes:
-                    layouts.append((cur, cur_bytes))
-                    cur, cur_bytes = [], 0
-                cur.append((i, cur_bytes // item, numel))
-                cur_bytes += nbytes
-            if cur:
-                layouts.append((cur, cur_bytes))
-            unit = nranks * ALIGN
-            for mem, nbytes in layouts:
-                padded = (nbytes + unit - 1) // unit * unit
-                numel = padded // item
-                buckets.append({'group': gi, 'dtype': dtype, 'members': mem, 'numel': numel, 'shard': numel // nranks})
-    return buckets
-
-
-def shard_range(bucket, rank):
-    """Elements [lo, hi) of the bucket that `rank` owns."""
-    return rank * bucket['shard'], (rank + 1) * bucket['shard']
-
-
-def shard_slices(bucket, rank):
-    """The parameter pieces inside `rank`'s shard: [(member position, first element in the parameter, last + 1,
-    first element in the shard)]."""
-    lo, hi = shard_range(bucket, rank)
-    out = []
-    for k, (_, off, numel) in enumerate(bucket['members']):
-        a, b = max(lo, off), min(hi, off + numel)
-        if a < b:
-            out.append((k, a - off, b - off, a - lo))
-    return out
-
-
-def _memory_order(t, stride):
-    """The elements of `t` in the memory order of a dense tensor of its shape with strides `stride` (None: row-major)."""
-    if stride is None:
-        return t.reshape(-1)
-    x = torch.empty_strided(t.shape, stride, dtype=t.dtype, device=t.device)
-    x.copy_(t)
-    return x.as_strided((x.numel(),), (1,))
-
-
-def shard_from_full(bucket, rank, full, strides=None, dtype=torch.float32, device=None):
-    """This rank's shard of one state tensor.  full[k]: the state of member k (its parameter's shape) or None (zeros);
-    strides[k]: the parameter's strides, i.e. the order in which its elements lie in the bucket (None: row-major).
-    Padding is zero."""
-    out = torch.zeros(bucket['shard'], dtype=dtype, device=device)
-    for k, plo, phi, slo in shard_slices(bucket, rank):
-        t = full[k]
-        if t is not None:
-            out[slo:slo + phi - plo].copy_(_memory_order(t, strides[k] if strides else None)[plo:phi])
-    return out
-
-
-def full_from_shards(bucket, shards, shapes, strides=None):
-    """Inverse of shard_from_full: the N shards of a state tensor (in rank order) -> one tensor per member, shaped
-    `shapes[k]` with strides `strides[k]` (None: row-major)."""
-    flat = torch.cat([s.reshape(-1) for s in shards])
-    out = []
-    for k, (_, off, numel) in enumerate(bucket['members']):
-        seg = flat[off:off + numel]
-        out.append(seg.reshape(shapes[k]) if not strides else seg.as_strided(shapes[k], strides[k]))
-    return out
+from horovod_b200.torch.optimizer import _COUNTS_STEPS, _STATE_KEYS, _fused_update, _optimizer_kind, _state_dtype, _state_keys
 
 
 class _ShardedDistributedOptimizer(torch.optim.Optimizer):
@@ -157,16 +65,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             raise ValueError('shard_optimizer_state supports op=Average or op=Sum only')
         if compression is not Compression.none or groups is not None or sparse_as_dense:
             raise ValueError('shard_optimizer_state does not support compression, groups or sparse_as_dense')
-        if named_parameters is not None:
-            named_parameters = list(named_parameters)
-            if any(not isinstance(x, tuple) for x in named_parameters):
-                raise ValueError('named_parameters should be a sequence of tuples (name, parameter), usually produced by '
-                                 'model.named_parameters().')
-            dups = _find_duplicates([k for k, _ in named_parameters])
-            if dups:
-                raise ValueError('Parameter names in named_parameters must be unique. Found duplicates: %s' % ', '.join(dups))
-            if {id(v) for g in self.param_groups for v in g['params']} - {id(v) for _, v in named_parameters}:
-                raise ValueError('named_parameters was specified, but one or more model parameters were not named.')
+        check_named_parameters(self, named_parameters)
         trainable = [[p for p in g['params'] if p.requires_grad] for g in self.param_groups]
         for ps in trainable:
             for p in ps:
@@ -178,7 +77,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._kind = kind
         # fp32 accumulators of the bf16 / fp16 gradient buckets over the backward passes of one step (b['acc'], plain
         # device memory allocated on first use, not optimizer state)
-        self._acc_fp32 = _check_grad_accumulation_dtype(grad_accumulation_dtype)
+        self._acc_fp32 = check_grad_accumulation_dtype(grad_accumulation_dtype)
         self.process_set = process_set
         self.op = op
         self.gradient_predivide_factor = gradient_predivide_factor
@@ -203,25 +102,17 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             for bi, b in enumerate(self._buckets):
                 ps = [trainable[b['group']][i] for i, _, _ in b['members']]
                 pflat = mpi_ops.symm_empty(b['numel'], dtype=b['dtype'], device=device, process_set=process_set)
-                gflat = mpi_ops.symm_empty(b['numel'], dtype=b['dtype'], device=device, process_set=process_set)
                 pflat.zero_()
-                gflat.zero_()
-                b.update({'params': ps, 'pflat': pflat, 'gflat': gflat, 'views': {}, 'index': bi, 'step': 0,
-                          'mom_init': False, 'pending': 0, 'ready': False, 'acc': None, 'arrived': 0, 'folds': 0,
-                          'fold_last': False})
+                grad_bucket(b, ps, device, process_set)
+                b.update({'pflat': pflat, 'index': bi, 'step': 0, 'mom_init': False, 'pending': 0, 'ready': False})
                 for p, (_, off, numel) in zip(ps, b['members']):
                     # keep the parameter's memory format (channels_last stays channels_last)
                     pview = pflat[off:off + numel].as_strided(p.size(), p.stride())
-                    gview = gflat[off:off + numel].as_strided(p.size(), p.stride())
                     pview.copy_(p.data)
-                    if p.grad is not None:
-                        gview.copy_(p.grad)
                     p.data = pview
-                    p.grad = gview
-                    b['views'][p] = (off, gview)
                     self._p_to_bucket[p] = b
                 lo, hi = shard_range(b, self._rank)
-                b['pshard'], b['gshard'] = pflat[lo:hi], gflat[lo:hi]
+                b['pshard'], b['gshard'] = pflat[lo:hi], b['gflat'][lo:hi]
                 master = master_weights and b['dtype'] != torch.float32
                 b['state'] = {key: torch.zeros(b['shard'], dtype=_state_dtype(kind, b['dtype'], master), device=device)
                               for key in _state_keys(kind, self.param_groups[b['group']])}
@@ -253,33 +144,16 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._next = 0
         for b in self._buckets:
             b['pending'], b['ready'] = len(b['params']), False
-            b['arrived'] = b['folds'] = 0
+        reset_folds(self._buckets)
 
     # ---- gradient accumulation in fp32 (grad_accumulation_dtype=torch.float32) -------------------------------------------
-    def _accumulates(self, bucket):
-        return self._acc_fp32 and self.backward_passes_per_step > 1 and bucket['dtype'] in (torch.bfloat16, torch.float16)
-
-    def _bucket_acc(self, bucket):
-        if bucket['acc'] is None:
-            bucket['acc'] = torch.empty(bucket['numel'], dtype=torch.float32, device=bucket['gflat'].device)
-        return bucket['acc']
-
     def _prepare_accumulators(self):
         """hvd.GraphedStep, before capture: the accumulators must exist outside the graphs' memory pool."""
-        for b in self._buckets:
-            if self._accumulates(b):
-                self._bucket_acc(b)
+        bucket_accumulators(self)
 
     def _graph_fold(self, mode, with_buckets=True):
         """hvd.GraphedStep, while capturing: one fold of every accumulating bucket after the captured backward pass."""
-        bs = [b for b in self._buckets if with_buckets and self._accumulates(b)]
-        if bs:
-            _fold([b['gflat'] for b in bs], [self._bucket_acc(b) for b in bs], mode)
-
-    def _scales(self):
-        if self.op == Average:
-            return 1.0 / self.gradient_predivide_factor, self.gradient_predivide_factor
-        return 1.0, 1.0
+        fold(*bucket_accumulators(self, with_buckets), mode)
 
     def _comm_stream(self):
         return self._graph_capture['comm'] if self._graph_capture is not None else self._comm
@@ -290,13 +164,10 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         bucket['ready'] = True
         while self._next < len(self._buckets) and self._buckets[self._next]['ready']:
             b = self._buckets[self._next]
-            if b['folds'] or (b['fold_last'] and self._graph_capture is not None):
-                # gradient accumulation in fp32: the sum over the step's backward passes, rounded once, is reduce-scattered
-                _fold([b['gflat']], [self._bucket_acc(b)], 'last')
-                b['folds'] = 0
+            fold_last(b, self._graph_capture is not None)
             comm = self._comm_stream()
             comm.wait_stream(torch.cuda.current_stream())
-            pre, post = self._scales()
+            pre, post = scales(self)
             with torch.cuda.stream(comm):
                 mpi_ops.captured_reducescatter_(b['gflat'], op=self.op, prescale_factor=pre, postscale_factor=post,
                                                 process_set=self.process_set)
@@ -307,11 +178,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             if self._graph_mode and self._graph_capture is None:
                 return  # GraphedStep warm-up / replay: the reductions are issued by the capture or by step()
             bucket = self._p_to_bucket[p]
-            off, view = bucket['views'][p]
-            if p.grad.data_ptr() != view.data_ptr():
-                # model.zero_grad() (set_to_none) dropped the bucket view and autograd allocated a fresh gradient
-                view.copy_(p.grad)
-                p.grad = view
+            adopt_grad(p, bucket['views'][p], densify=False)
             if self._graph_capture is not None:
                 bucket['pending'] -= 1
                 if bucket['pending'] == 0:
@@ -325,30 +192,12 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                                      'Increase backward_passes_per_step to accumulate gradients locally.')
             self._delay[p] -= 1
             self._seen.add(p)
-            if self._accumulates(bucket):
-                bucket['arrived'] += 1
-                if bucket['arrived'] == len(bucket['params']):  # the bucket has this backward pass's gradients
-                    bucket['arrived'] = 0
-                    if self._delay[p] > 0:
-                        _fold([bucket['gflat']], [self._bucket_acc(bucket)], 'add' if bucket['folds'] else 'first')
-                        bucket['folds'] += 1
+            fold_arrived(self, bucket, self._delay[p] > 0)
             if self._delay[p] == 0:
                 bucket['pending'] -= 1
                 if bucket['pending'] == 0:
                     self._mark_ready(bucket)
         return hook
-
-    def _adopt_missing_grads(self, bucket):
-        """Gradients that were not produced on this rank count as zeros; fresh gradient tensors move into the bucket."""
-        for p in bucket['params']:
-            off, view = bucket['views'][p]
-            if p.grad is None:
-                if p not in self._seen:
-                    view.zero_()
-                p.grad = view
-            elif p.grad.data_ptr() != view.data_ptr():
-                view.copy_(p.grad)
-                p.grad = view
 
     # ---- public API -------------------------------------------------------------------------------------------------------
     def synchronize(self):
@@ -365,7 +214,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
     def _reduce_pending(self):
         if not (self._graph_mode and self._graph_comm_captured):
             for b in self._buckets[self._next:]:
-                self._adopt_missing_grads(b)
+                adopt_missing_grads(b, self._seen, densify=False)
             for b in self._buckets[self._next:]:
                 self._mark_ready(b)
             torch.cuda.current_stream().wait_stream(self._comm)
@@ -434,14 +283,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._clip_coef = coef if self._clip_coef is None else self._clip_coef * coef
         return total
 
-    @contextmanager
-    def skip_synchronize(self):
-        """Use after an explicit optimizer.synchronize() so that step() does not synchronize again."""
-        self._should_synchronize = False
-        try:
-            yield
-        finally:
-            self._should_synchronize = True
+    skip_synchronize = grad_buckets.skip_synchronize
 
     def _update_shards(self, coef=None):
         """One fused kernel per param group and dtype over this rank's shards.  coef: the clip coefficient on the
@@ -540,13 +382,12 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             b['gflat'].zero_()
             for p in b['params']:
                 if p.grad is None:
-                    p.grad = b['views'][p][1]
+                    p.grad = b['views'][p]
 
     def set_backward_passes_per_step(self, passes):
         self.backward_passes_per_step = passes
         self._delay = {p: passes for p in self._delay}
-        for b in self._buckets:
-            b['arrived'] = b['folds'] = 0
+        reset_folds(self._buckets)
 
     # ---- hvd.GraphedStep -----------------------------------------------------------------------------------------------
     def _begin_graph_capture(self):
@@ -556,8 +397,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             return False
         self._graph_capture = {'comm': torch.cuda.Stream(device=self._comm.device, priority=self._comm.priority)}
         self._reset_launch_order()
-        for b in self._buckets:  # with backward_passes_per_step > 1 this is the step's last graph
-            b['fold_last'] = self._accumulates(b)
+        mark_fold_last(self, True)  # with backward_passes_per_step > 1 this is the step's last graph
         return True
 
     def _end_graph_capture(self):
@@ -569,8 +409,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         torch.cuda.current_stream().wait_stream(cap['comm'])
         self._graph_capture = None
         self._reset_launch_order()
-        for b in self._buckets:
-            b['fold_last'] = False
+        mark_fold_last(self, False)
         self._graph_comm_captured = True
 
     # ---- checkpoints ------------------------------------------------------------------------------------------------------

@@ -508,7 +508,7 @@ def _sharded_team(hvd, team, base, dt, master):
 
 
 def _reduced_grads(opts, params):
-    from horovod_b200.torch.sharded_optimizer import full_from_shards
+    from horovod_b200.torch.grad_buckets import full_from_shards
     out = {}
     for bi, b in enumerate(opts[0]._buckets):
         full = torch.cat([o._buckets[bi]['gshard'] for o in opts])

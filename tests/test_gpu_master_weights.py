@@ -632,7 +632,7 @@ def _reference(hvd, kind, model):
 
 def _reduced_grads(opts, params):
     """Every parameter's reduced gradient, assembled from the owners' gradient shards (what the sharded update reads)."""
-    from horovod_b200.torch.sharded_optimizer import full_from_shards
+    from horovod_b200.torch.grad_buckets import full_from_shards
     out = {}
     for bi, b in enumerate(opts[0]._buckets):
         full = torch.cat([o._buckets[bi]['gshard'] for o in opts])

@@ -315,7 +315,7 @@ def _sharded(hvd, team, base, make, dt):
 
 def _reduced_grads(opts, model_params):
     """The averaged gradient of every parameter, assembled from the ranks' owned shards (what the sharded update sees)."""
-    from horovod_b200.torch.sharded_optimizer import full_from_shards, shard_range
+    from horovod_b200.torch.grad_buckets import full_from_shards, shard_range
     out = {}
     for bi, b in enumerate(opts[0]._buckets):
         shards = []
@@ -419,7 +419,7 @@ def test_sharded_grad_scaler_on_simulated_ranks(hvd, team):
     at a position rank 2 owns: every rank must skip and back off alike.  The other steps follow torch.amp.GradScaler on
     averaged gradients; unscale_ + clip_grad_norm_ + step cost one stats pass and one stats allreduce per rank."""
     from horovod_b200.ops import kernel_launches
-    from horovod_b200.torch.sharded_optimizer import shard_range, shard_slices
+    from horovod_b200.torch.grad_buckets import shard_range, shard_slices
     n = team.n
     torch.manual_seed(0)
     base = _ConvNet().cuda()

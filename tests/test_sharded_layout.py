@@ -3,7 +3,7 @@ and the round trip between a full per-parameter state and N shards."""
 import pytest
 import torch
 
-from horovod_b200.torch.sharded_optimizer import full_from_shards, shard_from_full, shard_layout, shard_range, shard_slices
+from horovod_b200.torch.grad_buckets import full_from_shards, shard_from_full, shard_layout, shard_range, shard_slices
 
 GROUPS = [[(1000, torch.float32), (7, torch.float32), (33, torch.bfloat16), (40000, torch.float32), (1, torch.bfloat16)],
           [(5, torch.float32), (129, torch.float16)]]
