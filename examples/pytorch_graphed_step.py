@@ -1,6 +1,9 @@
 """ResNet-50 synthetic training with the whole forward+backward replayed as one CUDA graph (hvd.GraphedStep).
 
-    bin/hvdrun -np 8 python examples/pytorch_graphed_step.py --batch-size 64
+    bin/hvdrun -np 8 python examples/pytorch_graphed_step.py --batch-size 64 [--max-grad-norm 1.0] [--fp16]
+
+--max-grad-norm clips the global gradient norm before every update; --fp16 trains under fp16 autocast with a
+torch.amp.GradScaler (bf16 autocast without one otherwise).
 """
 import argparse
 import time
@@ -15,6 +18,8 @@ p = argparse.ArgumentParser()
 p.add_argument('--batch-size', type=int, default=64)
 p.add_argument('--steps', type=int, default=50)
 p.add_argument('--eager', action='store_true')
+p.add_argument('--max-grad-norm', type=float, default=None)
+p.add_argument('--fp16', action='store_true')
 args = p.parse_args()
 
 hvd.init()
@@ -30,11 +35,12 @@ y = torch.randint(0, 1000, (args.batch_size,), device='cuda')
 
 
 def loss_fn(x, y):
-    with torch.autocast('cuda', dtype=torch.bfloat16):
+    with torch.autocast('cuda', dtype=torch.float16 if args.fp16 else torch.bfloat16):
         return F.cross_entropy(model(x), y)
 
 
-step = hvd.GraphedStep(loss_fn, opt, (x, y), enabled=not args.eager)
+scaler = torch.amp.GradScaler('cuda') if args.fp16 else None
+step = hvd.GraphedStep(loss_fn, opt, (x, y), enabled=not args.eager, max_grad_norm=args.max_grad_norm, scaler=scaler)
 if hvd.rank() == 0:
     print('CUDA graph captured:', step.captured, step.fallback_reason or '')
 for _ in range(5):

@@ -407,19 +407,28 @@ __device__ __forceinline__ double nan_max(double a, double b) { return (a > b ||
 
 // Gradient statistics of a table of flat gradient shards in one read pass: optional in-place scaling by *inv_scale, the
 // sum of squares (norm_inf = 0) or the max |g| (norm_inf = 1) of the scaled values as stored, and a non-finite flag.
-// Every CTA writes one partial; the last CTA to finish (atomic ticket, which it resets for the next launch) combines them
-// in fp64, always in the same order, and folds the result into out[0] (+= or max) and out[1] (max of 0 / 1).  So the
-// same input gives the same bits on every call, and one launch per gradient dtype accumulates into one output.
+// The grid has one CTA per kOptPerBlock-element tile of each tensor (entry e owns tiles [tile_begin, next tile_begin)), so
+// a list of per-parameter gradients with one large embedding costs CTAs in proportion to its total size.  Every CTA
+// writes one partial; the last CTA to finish (atomic ticket, which it resets for the next launch) combines them in fp64,
+// always in the same order, and folds the result into out[0] (+= or max) and out[1] (max of 0 / 1).  So the same input
+// gives the same bits on every call, and one launch per gradient dtype accumulates into one output.
 template <typename G>
 __global__ void __launch_bounds__(kOptThreads)
-grad_shard_stats_kernel(const StatTensor* __restrict__ table, const float* __restrict__ inv_scale, int norm_inf,
-                        float* __restrict__ partial, int* __restrict__ partial_flag, unsigned* ticket, float* out) {
+grad_shard_stats_kernel(const StatTensor* __restrict__ table, int n_entries, int64_t row_tiles,
+                        const float* __restrict__ inv_scale, int norm_inf, float* __restrict__ partial,
+                        int* __restrict__ partial_flag, unsigned* ticket, float* out) {
   __shared__ double red[kOptThreads];
   __shared__ int red_flag[kOptThreads / 32];
   __shared__ bool last;
-  const StatTensor t = table[blockIdx.y];
+  const unsigned ctas = gridDim.x, cta = blockIdx.x;
+  int lo = 0, hi = n_entries - 1;  // the entry whose tiles include this CTA: the last one with tile_begin <= cta
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) / 2;
+    if (table[mid].tile_begin <= (int64_t)cta) lo = mid; else hi = mid - 1;
+  }
+  const StatTensor t = table[lo];
   const int64_t n = t.count;
-  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  const int64_t base = ((int64_t)cta - t.tile_begin) * kOptPerBlock;
   float acc = 0.f;
   int bad = 0;
   if (base < n) {
@@ -454,7 +463,6 @@ grad_shard_stats_kernel(const StatTensor* __restrict__ table, const float* __res
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   if (lane == 0) { red[warp] = acc; red_flag[warp] = bad; }
   __syncthreads();
-  const unsigned ctas = gridDim.x * gridDim.y, cta = blockIdx.y * gridDim.x + blockIdx.x;
   if (threadIdx.x == 0) {
     float a = 0.f;
     int f = 0;
@@ -470,13 +478,21 @@ grad_shard_stats_kernel(const StatTensor* __restrict__ table, const float* __res
   __syncthreads();
   if (!last) return;
   __threadfence();
-  // the last CTA: every thread combines a fixed strided subset in index order, then a fixed tree over the threads
+  // the last CTA: every thread combines a fixed subset of the partials in a fixed order, then a fixed tree over the
+  // threads.  Thread i takes tile x of entry e when e * row_tiles + x == i (mod kOptThreads), in increasing order of that
+  // index: the order of a grid of row_tiles CTAs per entry (as wide as the largest tensor), whose CTAs past the end of
+  // their tensor would add partials of +0, which leave an fp64 sum and a max of non-negative values unchanged.  So the
+  // statistics are bit for bit those of that rectangular grid, which earlier versions launched.
   double a = 0.0;
   int f = 0;
-  for (unsigned j = threadIdx.x; j < ctas; j += kOptThreads) {
-    const double x = (double)__ldcg(partial + j);
-    a = norm_inf ? nan_max(a, x) : a + x;
-    f |= __ldcg(partial_flag + j);
+  for (int e = 0; e < n_entries; ++e) {
+    const int64_t tb = table[e].tile_begin, te = e + 1 < n_entries ? table[e + 1].tile_begin : (int64_t)ctas;
+    for (int64_t j = tb + ((int64_t)threadIdx.x + kOptThreads - (int64_t)e * row_tiles % kOptThreads) % kOptThreads;
+         j < te; j += kOptThreads) {
+      const double x = (double)__ldcg(partial + j);
+      a = norm_inf ? nan_max(a, x) : a + x;
+      f |= __ldcg(partial_flag + j);
+    }
   }
   red[threadIdx.x] = a;
   f = __syncthreads_or(f);
@@ -638,18 +654,17 @@ cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, fl
   });
 }
 
-int64_t GradShardStatsCtas(int n, int64_t max_count) {
-  return n <= 0 || max_count <= 0 ? 0 : (max_count + kOptPerBlock - 1) / kOptPerBlock * n;
-}
+int64_t GradShardStatsTiles(int64_t count) { return (count + kOptPerBlock - 1) / kOptPerBlock; }
 
-cudaError_t LaunchGradShardStats(const StatTensor* table, int n, int64_t max_count, const float* inv_scale, int norm_inf,
-                                 float* partial, int* partial_flag, unsigned* ticket, float* out, int grad_dtype,
-                                 cudaStream_t stream) {
-  if (n <= 0 || max_count <= 0) return cudaSuccess;
-  dim3 grid((unsigned)((max_count + kOptPerBlock - 1) / kOptPerBlock), (unsigned)n);
-  if (grad_dtype == 7) grad_shard_stats_kernel<float><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
-  else if (grad_dtype == 10) grad_shard_stats_kernel<__nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
-  else if (grad_dtype == 6) grad_shard_stats_kernel<__half><<<grid, kOptThreads, 0, stream>>>(table, inv_scale, norm_inf, partial, partial_flag, ticket, out);
+cudaError_t LaunchGradShardStats(const StatTensor* table, int n, int64_t tiles, int64_t row_tiles, const float* inv_scale,
+                                 int norm_inf, float* partial, int* partial_flag, unsigned* ticket, float* out,
+                                 int grad_dtype, cudaStream_t stream) {
+  if (n <= 0 || tiles <= 0) return cudaSuccess;
+  if (tiles > 0x7fffffff) return cudaErrorInvalidValue;
+  const unsigned grid = (unsigned)tiles;
+  if (grad_dtype == 7) grad_shard_stats_kernel<float><<<grid, kOptThreads, 0, stream>>>(table, n, row_tiles, inv_scale, norm_inf, partial, partial_flag, ticket, out);
+  else if (grad_dtype == 10) grad_shard_stats_kernel<__nv_bfloat16><<<grid, kOptThreads, 0, stream>>>(table, n, row_tiles, inv_scale, norm_inf, partial, partial_flag, ticket, out);
+  else if (grad_dtype == 6) grad_shard_stats_kernel<__half><<<grid, kOptThreads, 0, stream>>>(table, n, row_tiles, inv_scale, norm_inf, partial, partial_flag, ticket, out);
   else return cudaErrorInvalidValue;
   CountKernelLaunch();
   return cudaGetLastError();

@@ -221,13 +221,14 @@ cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, fl
                             const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
 // Gradient statistics of flat gradient shards in one pass (see optim_kernels.cu): optional in-place scaling by
 // *inv_scale, then out[0] += sum of squares (norm_inf: out[0] = max(out[0], max |g|)) and out[1] = max(out[1], non-finite).
-// `partial` / `partial_flag` hold GradShardStatsCtas() entries; `ticket` is a zeroed counter that the kernel leaves zeroed,
-// which launches running at the same time must not share.
-struct StatTensor { void* grad; int64_t count; };
-int64_t GradShardStatsCtas(int n, int64_t max_count);
-cudaError_t LaunchGradShardStats(const StatTensor* table, int n, int64_t max_count, const float* inv_scale, int norm_inf,
-                                 float* partial, int* partial_flag, unsigned* ticket, float* out, int grad_dtype,
-                                 cudaStream_t stream);
+// Entries are non-empty and in order; tile_begin is the sum of GradShardStatsTiles(count) of the entries before, `tiles`
+// that sum over all of them and `row_tiles` its largest term.  `partial` / `partial_flag` hold `tiles` entries; `ticket`
+// is a zeroed counter that the kernel leaves zeroed, which launches running at the same time must not share.
+struct StatTensor { void* grad; int64_t count; int64_t tile_begin; };
+int64_t GradShardStatsTiles(int64_t count);
+cudaError_t LaunchGradShardStats(const StatTensor* table, int n, int64_t tiles, int64_t row_tiles, const float* inv_scale,
+                                 int norm_inf, float* partial, int* partial_flag, unsigned* ticket, float* out,
+                                 int grad_dtype, cudaStream_t stream);
 // Gradient accumulation in fp32 (see optim_kernels.cu): `grad` is bf16 / fp16 (grad_dtype, one per launch), `acc` fp32
 // with the same element order.  kAccFirst: acc = g, g = 0; kAccAdd: acc += g, g = 0; kAccLast: g = round(acc + g).  The
 // table is passed by value (under the 4 KB kernel-parameter limit), so one launch covers at most kAccMaxTensors entries

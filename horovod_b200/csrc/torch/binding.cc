@@ -835,24 +835,27 @@ void GradShardStats(std::vector<at::Tensor> grads, at::Tensor out, c10::optional
   }
   const float* isc = DeviceScalar("grad_shard_stats", "inv_scale", inv_scale, out);
   std::vector<kern::StatTensor> table;
-  int64_t maxc = 0;
+  int64_t tiles = 0, row_tiles = 0;  // one CTA per tile of every tensor
   for (auto& g : grads) {
     if (g.numel() == 0) continue;
-    table.push_back({g.data_ptr(), g.numel()});
-    maxc = std::max(maxc, (int64_t)g.numel());
+    table.push_back({g.data_ptr(), g.numel(), tiles});
+    const int64_t t = kern::GradShardStatsTiles(g.numel());
+    tiles += t;
+    row_tiles = std::max(row_tiles, t);
   }
   if (table.empty()) return;
+  TORCH_CHECK(tiles <= 0x7fffffff, "grad_shard_stats: ", tiles, " tiles exceed one launch's grid");
   int device = (int)out.get_device();
   c10::cuda::CUDAGuard guard(out.device());
   cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  const int64_t ctas = kern::GradShardStatsCtas((int)table.size(), maxc);
   // stream-ordered scratch from torch's caching allocator: fp32 partials followed by int flags
-  at::Tensor work = at::empty({2 * ctas}, out.options());
+  at::Tensor work = at::empty({2 * tiles}, out.options());
   const auto* dt = (const kern::StatTensor*)GpuContext::Get().Stage(device, table.data(), table.size() * sizeof(kern::StatTensor), s);
   TORCH_CHECK(dt != nullptr, "grad_shard_stats: table too large");
-  cudaError_t e = kern::LaunchGradShardStats(dt, (int)table.size(), maxc, isc, norm_inf ? 1 : 0, work.data_ptr<float>(),
-                                             reinterpret_cast<int*>(work.data_ptr<float>() + ctas), StatsTicket(device, s),
-                                             out.data_ptr<float>(), (int)MapDtype(grads[0].scalar_type()), s);
+  cudaError_t e = kern::LaunchGradShardStats(dt, (int)table.size(), tiles, row_tiles, isc, norm_inf ? 1 : 0,
+                                             work.data_ptr<float>(), reinterpret_cast<int*>(work.data_ptr<float>() + tiles),
+                                             StatsTicket(device, s), out.data_ptr<float>(),
+                                             (int)MapDtype(grads[0].scalar_type()), s);
   TORCH_CHECK(e == cudaSuccess, "grad_shard_stats launch failed: ", cudaGetErrorString(e));
 }
 

@@ -26,10 +26,29 @@ As with k = 1, a call returns the static loss tensor of the graph it replayed, w
 overwrites; the middle graph serves micro-steps 2 … k-1, so `.clone()` (or `.item()`) a loss that must outlive the
 next call.
 
+Gradient clipping and AMP loss scaling: `max_grad_norm=` clips the global norm (`norm_type` 2 or inf) of the reduced
+gradients before each optimizer step, and `scaler=` (a torch.amp.GradScaler, or hvd.ShardedGradScaler with sharded
+optimizer state) scales the loss that every captured backward pass differentiates.  The update itself stays outside
+the graph; after the last backward pass of a step the call runs the documented sequence
+
+    optimizer.synchronize()                       # with a scaler: unscale_ reads the reduced gradients
+    scaler.unscale_(optimizer)                    # with a scaler
+    optimizer.clip_grad_norm_(max_grad_norm)      # with max_grad_norm: one statistics pass, no host sync
+    with optimizer.skip_synchronize():
+        scaler.step(optimizer)                    # or optimizer.step()
+    scaler.update()                               # with a scaler
+
+The graph reads the scale from the scaler's device tensor, which update() rewrites in place, so every replay uses the
+current scale; the returned loss is the unscaled one.  scaler.step() reads the inf / NaN verdict on the host, as torch
+does: one host synchronisation per step with a scaler, none with clipping alone.  A step the scaler skips leaves no
+clip coefficient or gradient statistics behind.  Not with op=Adasum, whose optimizer reduces parameter deltas rather
+than gradients (ValueError).
+
 Constraints (those of CUDA graphs): fixed input shapes/dtypes, no host synchronisation or data-dependent control flow
 inside `step_fn`, `optimizer.zero_grad()` is part of the graph (do not call it yourself).  If capture fails the object
 falls back to the eager step and says so in `.captured` / `.fallback_reason`.
 """
+import math
 import warnings
 
 import torch
@@ -37,10 +56,14 @@ import torch
 
 class GraphedStep:
     """Training step whose forward + backward are one CUDA graph replay; `step(*inputs)` returns the (static) loss tensor.
-    `.captured` tells whether the graph is in use, `.fallback_reason` why not."""
+    `.captured` tells whether the graph is in use, `.fallback_reason` why not.  `max_grad_norm` / `norm_type`: clip the
+    global gradient norm before every optimizer step; `scaler`: AMP loss scaling (see the module docstring)."""
 
-    def __init__(self, step_fn, optimizer, example_inputs, warmup_iters=3, enabled=True):
+    def __init__(self, step_fn, optimizer, example_inputs, warmup_iters=3, enabled=True, max_grad_norm=None,
+                 norm_type=2.0, scaler=None):
+        self._check_clip_and_scaler(optimizer, max_grad_norm, norm_type, scaler)
         self.step_fn, self.optimizer = step_fn, optimizer
+        self.max_grad_norm, self.norm_type, self.scaler = max_grad_norm, float(norm_type), scaler
         self.captured, self.fallback_reason = False, None
         self.graph, self.static_loss = None, None
         # backward_passes_per_step when built; k > 1: one graph and static loss per phase, replayed first, middle..., last
@@ -63,12 +86,30 @@ class GraphedStep:
                 self._abandon(e)
             self._agree_across_ranks()
 
+    @staticmethod
+    def _check_clip_and_scaler(optimizer, max_grad_norm, norm_type, scaler):
+        if float(norm_type) not in (2.0, math.inf):
+            raise ValueError('hvd.GraphedStep: norm_type must be 2 or inf, got %r' % (norm_type,))
+        if max_grad_norm is None and scaler is None:
+            return
+        from horovod_b200.torch.mpi_ops import Adasum
+        if getattr(optimizer, 'op', None) == Adasum or hasattr(optimizer, '_whole_model_step'):
+            raise ValueError('hvd.GraphedStep: max_grad_norm and scaler are not supported with op=Adasum, whose optimizer '
+                             'reduces parameter deltas, not gradients')
+        if not (hasattr(optimizer, 'clip_grad_norm_') and hasattr(optimizer, '_drop_iteration_state')):
+            raise ValueError('hvd.GraphedStep: max_grad_norm and scaler need an hvd.DistributedOptimizer')
+        if scaler is not None and not all(p.is_cuda for g in optimizer.param_groups for p in g['params']):
+            raise ValueError('hvd.GraphedStep: scaler needs an optimizer of CUDA parameters')
+
     # ------------------------------------------------------------------------------------------------------------------
+    def _backward(self, loss):
+        (loss if self.scaler is None else self.scaler.scale(loss)).backward()
+
     def _fwd_bwd(self, zero_grad=True):
         if zero_grad:
             self.optimizer.zero_grad(set_to_none=False)
         loss = self.step_fn(*self.static_inputs)
-        loss.backward()
+        self._backward(loss)
         return loss
 
     def _capture(self, warmup_iters):
@@ -169,16 +210,38 @@ class GraphedStep:
         if not self.captured:
             self.optimizer.zero_grad()
             loss = self.step_fn(*inputs)
-            loss.backward()
-            self.optimizer.step()
+            self._backward(loss)
+            self._update()
             return loss
         for dst, src in zip(self.static_inputs, inputs):
             if dst is not src:
                 dst.copy_(src, non_blocking=True)
         self.graph.replay()
         self.replays += 1
-        self.optimizer.step()
+        self._update()
         return self.static_loss
+
+    def _update(self):
+        """The optimizer step after the last backward pass of a step, with unscaling and clipping where asked for."""
+        opt = self.optimizer
+        if self.scaler is None and self.max_grad_norm is None:
+            opt.step()
+            return
+        if self.scaler is not None:
+            opt.synchronize()
+            self.scaler.unscale_(opt)
+        if self.max_grad_norm is not None:
+            opt.clip_grad_norm_(self.max_grad_norm, self.norm_type)
+        with opt.skip_synchronize():
+            if self.scaler is not None:
+                self.scaler.step(opt)
+            else:
+                opt.step()
+        if self.scaler is not None:
+            self.scaler.update()
+        # a step the scaler skipped must not leave its clip coefficient or statistics to the next one: on replay neither
+        # a gradient hook nor zero_grad() (a node of the graph) runs Python that would drop them
+        opt._drop_iteration_state()
 
     def _micro_step(self, inputs):
         """One micro-batch of k: the optimizer steps after the k-th.  Returns this micro-batch's loss."""
@@ -187,7 +250,7 @@ class GraphedStep:
             if first:
                 self.optimizer.zero_grad()
             loss = self.step_fn(*inputs)
-            loss.backward()
+            self._backward(loss)
         else:
             for dst, src in zip(self.static_inputs, inputs):
                 if dst is not src:
@@ -198,5 +261,5 @@ class GraphedStep:
             loss = self.static_losses[phase]
         self.micro_step = 0 if last else self.micro_step + 1
         if last:
-            self.optimizer.step()
+            self._update()
         return loss

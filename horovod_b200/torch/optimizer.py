@@ -8,6 +8,7 @@ with no autograd-graph surgery), completion is event-chained (no host sync per
 tensor), and `fused=True` replaces the wrapped SGD/Adam(W) math by one
 multi-tensor sm_90a kernel (csrc/kernels/optim_kernels.cu).
 """
+import math
 import os
 import warnings
 from contextlib import contextmanager
@@ -69,6 +70,8 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._requires_update = set()
         self._synchronized = False
         self._should_synchronize = True
+        self._reduced = False    # set by clip_grad_norm_: step() does not reduce again, silently
+        self._clip_coef = None   # 0-dim fp32 device tensor from clip_grad_norm_, applied by the next fused step()
 
         self._num_groups = None
         self._groups = None
@@ -273,6 +276,9 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 if self._graph_capture is not None:
                     self._graph_hook(p)
                 return
+            if self._reduced or self._clip_coef is not None:
+                # a new backward after an iteration whose step() was skipped (e.g. GradScaler found inf): start afresh
+                self._drop_iteration_state()
             if p in self._handles and self._handles[p][0] is not None:
                 if self._allreduce_delay[p] <= 0:
                     raise AssertionError(
@@ -498,35 +504,96 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     skip_synchronize = grad_buckets.skip_synchronize
 
+    def _drop_iteration_state(self):
+        self._synchronized = self._reduced = False
+        self._clip_coef = None
+
+    def _grads_to_clip(self):
+        """The gradients the next update reads, with a fresh wire-dtype shadow in place of its fp32 bucket: each zero-copy
+        bucket as one flat tensor (its padding stays zero), every other parameter's gradient on its own."""
+        grads = [b['shadow'] if b.get('shadow') is not None and b.get('shadow_fresh') else b['gflat'] for b in self._buckets]
+        grads += [p.grad for g in self.param_groups for p in g['params'] if p.grad is not None and p not in self._p_to_bucket]
+        if any(g.is_sparse for g in grads):
+            raise ValueError('clip_grad_norm_ does not support sparse gradients')
+        return grads
+
+    def clip_grad_norm_(self, max_norm, norm_type=2.0, error_if_nonfinite=False):
+        """Global-norm gradient clipping, the counterpart of torch.nn.utils.clip_grad_norm_(model.parameters(), ...):
+        call it after backward (and after GradScaler.unscale_, if used) and before step().
+
+        Reduces the gradients that are still pending, as synchronize() does (the following step() neither reduces again
+        nor warns), and returns the norm of the reduced gradients as a 0-dim fp32 tensor on their device.  All ranks hold
+        the same reduced gradients, so no further collective is needed.  On CUDA the norm is one statistics kernel per
+        gradient dtype, without a host synchronisation.  When step() runs the fused update, the clip coefficient
+        min(max_norm / (norm + 1e-6), 1) stays on the device and scales the gradient inside that update, and p.grad is
+        not rescaled; otherwise p.grad is scaled in place, as torch does.  norm_type is 2 or inf; sparse gradients raise
+        ValueError.  error_if_nonfinite=True synchronises with the host, as torch's does."""
+        norm_type = float(norm_type)
+        if norm_type not in (2.0, math.inf):
+            raise ValueError('clip_grad_norm_ supports norm_type 2 and inf, got %r' % norm_type)
+        if not (self._synchronized or self._reduced):
+            self.synchronize(_defer_shadow_copy=self._fused)
+            self._reduced = True
+        fused = self._master_weights or (self._fused and _fused_plan(self) is not None)
+        if not fused:
+            self._restore_shadows()
+        grads = self._grads_to_clip()
+        if not grads:
+            return torch.zeros((), dtype=torch.float32)
+        if grads[0].is_cuda:
+            from horovod_b200 import ops
+            stats = torch.zeros(2, dtype=torch.float32, device=grads[0].device)
+            ops.grad_shard_stats(grads, stats, norm_type=norm_type)
+            total = stats[0].sqrt() if norm_type == 2.0 else stats[0].clone()
+        else:  # CPU tensors: torch's norm
+            total = torch.nn.utils.get_total_norm(grads, norm_type)
+        if self._clip_coef is not None:
+            total = total * self._clip_coef  # clipping twice: the norm of the gradient as the first clip left it
+        if error_if_nonfinite and bool(torch.logical_or(total.isnan(), total.isinf())):
+            raise RuntimeError('The total norm of order %s for gradients from `parameters` is non-finite, so it cannot be '
+                               'clipped. To disable this error and scale the gradients by the non-finite norm anyway, set '
+                               '`error_if_nonfinite=False`' % norm_type)
+        coef = torch.clamp(max_norm / (total + 1e-6), max=1.0)
+        if fused:
+            self._clip_coef = coef if self._clip_coef is None else self._clip_coef * coef
+        else:
+            torch._foreach_mul_(grads, coef)
+        return total
+
     def _hvd_super_step(self, closure=None):
         return super(self.__class__, self).step(closure)
 
     def step(self, closure=None):
-        if self._should_synchronize:
+        if self._should_synchronize and not self._reduced:
             if self._synchronized:
                 warnings.warn("optimizer.step() called without optimizer.skip_synchronize() context after "
                               "optimizer.synchronize(). This can cause training slowdown. You may want to consider "
                               "using optimizer.skip_synchronize() context if you use optimizer.synchronize() in your "
                               "code.")
             self.synchronize(_defer_shadow_copy=self._fused and closure is None)
-        self._synchronized = False
+        coef = self._clip_coef
+        self._drop_iteration_state()
         if self._master_weights or (self._fused and closure is None):
             # the masters live in the fused kernels only: evaluate the closure, then the fused update (or an error)
             loss = None
             if closure is not None:
                 with torch.enable_grad():
                     loss = closure()
-            if _fused_step(self):  # always True with masters: it raises when the update cannot be fused
+            if _fused_step(self, coef):  # always True with masters: it raises when the update cannot be fused
                 for bucket in self._buckets:
                     bucket['shadow_fresh'] = False
                 return loss
         self._restore_shadows()
+        if coef is not None:  # clip_grad_norm_ expected the fused update, which could not run
+            torch._foreach_mul_(self._grads_to_clip(), coef)
         return super(self.__class__, self).step(closure)
 
     def zero_grad(self, *args, **kwargs):
         if self._handles:
             raise AssertionError("optimizer.zero_grad() was called after loss.backward() but before optimizer.step() or "
                                  "optimizer.synchronize(). This is prohibited as it can cause a race condition.")
+        if self._reduced or self._clip_coef is not None:
+            self._drop_iteration_state()  # an iteration whose step() was skipped leaves no clip coefficient behind
         if self._zero_copy:
             # bucketed gradients must stay views of the registered buffers: zero them in place (one memset per bucket)
             for bucket in self._buckets:
@@ -673,10 +740,10 @@ def _param_state(opt, kind, p, keys, master):
     return out, fresh
 
 
-def _fused_step(opt):
+def _fused_step(opt, coef=None):
     """One multi-tensor kernel for the whole model when the wrapped optimizer is SGD or Adam/AdamW on CUDA, three for
     Lamb and Lars (their trust ratios need whole-tensor norms before the update). With master weights a plan that cannot
-    be fused raises RuntimeError instead of returning False."""
+    be fused raises RuntimeError instead of returning False.  coef: the clip coefficient on the device, or None."""
     use_master = getattr(opt, '_master_weights', False)
     why = []
     plan = _fused_plan(opt, why)
@@ -713,7 +780,7 @@ def _fused_step(opt):
             for (step, first), idx in parts.items():
                 pick = lambda xs: [xs[i] for i in idx] if xs else xs  # noqa: E731
                 _fused_update(opt, kind, group, pick(ps), pick(grads), [pick(s) for s in states], pick(masters),
-                              step=step, first_step=first)
+                              step=step, first_step=first, coef=coef)
     return True
 
 
