@@ -2,7 +2,6 @@
 """Bandwidth sweep of the non-allreduce collectives: allgather, broadcast, alltoall, reducescatter.
 
     torchrun --nproc-per-node 8 bench/collective_sweep.py --out collectives8.json
-    HVD_EXCHANGE_TMA=1 torchrun ... bench/collective_sweep.py --ops allgather,broadcast --tag tma
 
 Every op is timed on the device (CUDA events around `iters` back-to-back calls after warm-up, max over ranks) through
 `horovod_b200.torch`, and — with `--nccl` — next to the same op issued through torch.distributed's NCCL backend on the same
@@ -127,7 +126,7 @@ for op in args.ops.split(','):
             print('  %12d B  %10.2f us  bus %8.2f GB/s%s' % (r['bytes'], r['us'], r['busbw_gbs'], extra), flush=True)
 if rank == 0 and args.out:
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    json.dump({'n_gpus': size, 'tag': args.tag, 'exchange_tma': os.environ.get('HVD_EXCHANGE_TMA', '0'), 'results': results},
+    json.dump({'n_gpus': size, 'tag': args.tag, 'results': results},
               open(args.out, 'w'), indent=1)
 if pg:
     pg.destroy_process_group()

@@ -52,8 +52,8 @@ constexpr const char* PS_ADD_PREFIX = "__process_set_add__:";
 constexpr const char* PS_REMOVE_PREFIX = "__process_set_remove__:";
 constexpr const char* SYMM_ALLOC_PREFIX = "__symm_alloc__:";
 
-// Every fused tensor starts on a 128 B boundary so that 16 B vector accesses,
-// TMA bulk copies and multimem.* never straddle two tensors (the reference pads
+// Every fused tensor starts on a 128 B boundary so that 16 B vector accesses
+// and multimem.* never straddle two tensors (the reference pads
 // to 16 B: controller.cc:922-930).
 constexpr int64_t FUSION_ALIGN_BYTES = 128;
 

@@ -256,10 +256,6 @@ void Engine::BackgroundThread() {
     genv.wire_dtype = wire == "bf16" ? DataType::BFLOAT16 : wire == "fp16" ? DataType::FLOAT16 : DataType::FLOAT32;
     genv.symm_buffer_bytes = (size_t)EnvInt(HVD_SYMM_BUFFER_BYTES, 128ll << 20);
     genv.want_multicast = EnvBool("HVD_ENABLE_NVLS", true);
-    genv.pipelined = EnvBool("HVD_PIPELINED_ALLREDUCE", false);
-    genv.pipe_chunk_bytes = std::max<int64_t>(1 << 20, EnvInt("HVD_PIPE_CHUNK_BYTES", 4 << 20) / 4096 * 4096);
-    genv.pipe_min_bytes = EnvInt("HVD_PIPE_MIN_BYTES", 32 << 20);
-    genv.pipe_rblock_bytes = std::max<int64_t>(4096, EnvInt("HVD_PIPE_RBLOCK_BYTES", 16384) / 4096 * 4096);
     genv.large_msg_ctas = std::min<int64_t>(kern::kMaxCtas, std::max<int64_t>(4, EnvInt("HVD_LARGE_MSG_CTAS", 256)));
     genv.broadcast_multicast = EnvBool("HVD_BROADCAST_MULTICAST", true);
     // on-the-fly IPC registration of plain in-place tensors (ops/ipc_registry.h); 0 disables
@@ -270,8 +266,6 @@ void Engine::BackgroundThread() {
     // the reference's knob for concurrent responses (operations.cc:465): 1 = a single stream, i.e. no latency lane
     if (EnvIsSet(HOROVOD_NUM_STREAMS) && EnvInt(HOROVOD_NUM_STREAMS, 1) <= 1 && !EnvIsSet("HVD_LATENCY_LANE_BYTES")) genv.latency_lane_bytes = 0;
     genv.adasum_persistent = EnvBool("HVD_ADASUM_PERSISTENT", true);
-    genv.dual_lane = EnvBool("HVD_DUAL_LANE_ALLREDUCE", false);
-    genv.dual_lane_min_bytes = EnvInt("HVD_DUAL_LANE_MIN_BYTES", 64 << 20);
     genv.zero_copy_nvls_min_bytes = EnvInt("HVD_ZERO_COPY_NVLS_MIN_BYTES", 1 << 20);
     genv.calibrate = EnvBool("HVD_CALIBRATE", true) && !EnvBool(HOROVOD_AUTOTUNE, false);
     genv.on_calibrated = [this](int64_t oneshot_max, int64_t nvls_min) {

@@ -245,17 +245,6 @@ int hvd_sim_allreduce(int nranks, int device, int ntensors, const int64_t* count
       a.descs = dtabs[r]; a.ndesc = ntensors; a.total_bytes = total; a.reduce_lo = 0; a.reduce_hi = total;
       a.prescale = prescale; a.postscale = postscale; a.op = op; a.dtype = dtype; a.wire_dtype = wire_dtype;
       a.variant = variant; a.ctas = ctas;
-      if (variant == kern::kPipelined) {  // small chunks so that a modest test message exercises ring reuse
-        const char* cb = getenv("HVD_PIPE_CHUNK_BYTES");
-        a.pipe_chunk_bytes = cb ? atoll(cb) / 4096 * 4096 : 65536;
-        if (a.pipe_chunk_bytes < 4096) a.pipe_chunk_bytes = 4096;
-        a.pipe_slots = (int)std::min<int64_t>(kern::kPipeMaxSlots, std::max<int64_t>(2, (int64_t)sim->bytes / a.pipe_chunk_bytes));
-        const char* sl = getenv("HVD_PIPE_SLOTS");
-        if (sl && atoi(sl) >= 2) a.pipe_slots = std::min(a.pipe_slots, atoi(sl));
-        a.pipe_base = sim->teams[r]->NextPipeBase((uint32_t)((total + a.pipe_chunk_bytes - 1) / a.pipe_chunk_bytes));
-        a.pipe_use_nvls = 0;
-        a.pipe_rblock_bytes = 8192;
-      }
       cudaError_t e = kern::LaunchAllreduce(cps[r], a, sim->streams[r]);
       if (e != cudaSuccess) return (int)e;
     }

@@ -584,186 +584,6 @@ inplace_allgather_kernel(const __grid_constant__ CommParams cp, const __grid_con
   if (threadIdx.x == 0) cp.epochs[cta] = epoch;
 }
 
-
-// ---------------------------------------------------------------------------
-// Software-pipelined allreduce for LARGE fused responses of ordinary (unregistered) tensors (opt-in,
-// HVD_PIPELINED_ALLREDUCE=1; variant kPipelined).
-//
-// The three-phase kernel above runs pack, reduce and unpack back to back: NVLink idles while HBM is busy and vice versa
-// (it trails the zero-copy kernel at 1 GiB).  Here the message is cut into chunks that
-// travel through a ring of slots in the symmetric buffer, and the CTAs are specialised by blockIdx & 3:
-//     0     pack    chunk c   : tensors -> my slot (prescale, cast)
-//     1, 2  reduce  chunk c-1 : my 1/N slice of the slot on ALL ranks: multimem.ld_reduce + multimem.st (or P2P loads /
-//                               stores), postscale folded in
-//     3     unpack  chunk c-2 : my slot -> output tensors (cast)
-// so HBM traffic of chunks c and c-2 overlaps the NVLink traffic of chunk c-1.  Hand-offs (all monotonic counters,
-// `pipe_base` + chunk index + 1, never reset):
-//     packed[r]   written by rank r's LAST pack CTA of a chunk into every rank's flag region (st.release.sys)
-//                 reduce waits for packed[q] of every rank q before touching chunk c
-//     reduced[r]  written by rank r's LAST reduce CTA of a chunk into every rank's flag region
-//                 unpack waits for reduced[q] of every rank q (all slices of my slot are final)
-//     unpack_done local: the slot of chunk c may be re-packed with chunk c + slots once chunk c is unpacked here (which
-//                 implies that every peer finished reading it)
-// "last CTA of a chunk" is found with a per-slot arrival counter (threadfence + atomicAdd, reset by the last arriver
-// BEFORE it publishes).  Roles are interleaved over blockIdx so that any resident prefix of the grid contains all of
-// them; the grid must nevertheless fit on the device (every role waits for the others).
-
-__device__ __forceinline__ uint32_t* pipe_area(const CommParams& cp, int r) {
-  return reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(cp.flags[r]) + kPipeAreaOffset);
-}
-
-// Threads [0, n) each spin on words[i] until it reaches `target` (wrap-safe), with the abort / timeout protocol of
-// peer_barrier.  Returns false when the wait was abandoned.  Ends with __syncthreads().
-__device__ __forceinline__ bool pipe_wait(const CommParams& cp, const uint32_t* words, int n, uint32_t target) {
-  __shared__ int s_abort;
-  if (threadIdx.x == 0) s_abort = 0;
-  __syncthreads();
-  if ((int)threadIdx.x < n) {
-    const uint32_t* w = words + threadIdx.x;
-    uint32_t spins = 0;
-    unsigned long long t0 = 0;
-    while ((int32_t)(ld_relaxed_sys(w) - target) < 0) {
-      if ((++spins & 0x3fff) == 0 && cp.abort_flag) {
-        if (*reinterpret_cast<volatile int*>(cp.abort_flag)) { s_abort = 1; break; }
-        if (cp.timeout_ns) {
-          unsigned long long now;
-          asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-          if (t0 == 0) t0 = now;
-          else if (now - t0 > cp.timeout_ns) { *reinterpret_cast<volatile int*>(cp.abort_flag) = 2; s_abort = 1; break; }
-        }
-      }
-    }
-    (void)ld_acquire_sys(w);
-  }
-  __syncthreads();
-  const int aborted = s_abort;
-  __syncthreads();  // everyone has read the verdict before the next call may reset it
-  return aborted == 0;
-}
-
-// All threads of the CTA call it after their last store of a chunk.  Returns true in exactly one CTA per chunk (the
-// one that arrives last); that CTA has already reset the counter for the slot's next use.
-__device__ __forceinline__ bool pipe_last_cta(uint32_t* counter, uint32_t nctas) {
-  __shared__ int s_last;
-  __threadfence_system();  // my stores (to local HBM, peers, or the multicast alias) before my arrival
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const uint32_t old = atomicAdd(counter, 1u);
-    s_last = old == nctas - 1;
-    if (s_last) { atomicExch(counter, 0u); __threadfence_system(); }
-  }
-  __syncthreads();
-  return s_last != 0;
-}
-
-template <typename W, int NR>
-__device__ __forceinline__ void pipe_p2p_reduce(const CommParams& cp, int64_t delta, int64_t lo, int64_t hi, int op,
-                                                typename ScaleOf<typename Traits<W>::Acc>::type postscale) {
-  // [lo, hi) are fused-buffer offsets; the data lives at buf[q] + delta + offset on every rank q
-  using A = typename Traits<W>::Acc;
-  constexpr int NW = 16 / (int)sizeof(W);
-  constexpr int U = 8 / NR;
-  for (int64_t o0 = lo + (int64_t)threadIdx.x * 16; o0 < hi; o0 += (int64_t)U * kRowBytes) {
-    uint4 v[U][NR];
-    peer_loads<NR, U>(cp, cp.buf, delta + o0, delta + hi, v);
-#pragma unroll
-    for (int j = 0; j < U; ++j) {
-      const int64_t o = o0 + (int64_t)j * kRowBytes;
-      if (o < hi) {
-        A acc[NW];
-        peer_combine<W, NR>(cp, v[j], op, acc);
-#pragma unroll
-        for (int i = 0; i < NW; ++i) acc[i] = apply_scale<A>(acc[i], postscale);
-        const uint4 r = pack_vec<W, NW>(acc);
-#pragma unroll
-        for (int p = 0; p < NR; ++p) {
-          int q = cp.rank + p; if (q >= cp.nranks) q -= cp.nranks;
-          if (p < cp.nranks) st_stream(reinterpret_cast<char*>(cp.buf[q]) + delta + o, r);
-        }
-      }
-    }
-  }
-}
-
-template <typename T, typename W, int NR>
-__global__ void __launch_bounds__(kThreads, 2)
-pipelined_allreduce_kernel(const __grid_constant__ CommParams cp, const __grid_constant__ AllreduceArgs a) {
-  using A = typename Traits<W>::Acc;
-  using S = typename ScaleOf<A>::type;
-  constexpr int NW = 16 / (int)sizeof(W);
-  constexpr int UP = NW >= 16 ? 4 : 8;
-  const int role = blockIdx.x & 3, quad = blockIdx.x >> 2, nquad = gridDim.x >> 2;
-  const TensorDesc* descs = a.descs ? a.descs : a.inline_descs;
-  const int64_t total = a.total_bytes, C = a.pipe_chunk_bytes;
-  const int K = a.pipe_slots;
-  const int64_t nchunks = (total + C - 1) / C;
-  const uint32_t base = a.pipe_base;
-  uint32_t* mine = pipe_area(cp, cp.rank);
-  char* mybuf = reinterpret_cast<char*>(cp.buf[cp.rank]);
-  constexpr int64_t kBlock = 8 * (int64_t)kRowBytes;  // 32 KiB work items inside a chunk
-
-  if (role == 0) {
-    // ---------------- pack ----------------
-    const S prescale = (S)a.prescale;
-    for (int64_t c = 0; c < nchunks; ++c) {
-      if (c >= K && !pipe_wait(cp, mine + kPipeUnpackDone, 1, base + (uint32_t)(c - K) + 1u)) return;
-      const int64_t clo = c * C, chi = clo + C < total ? clo + C : total;
-      const int64_t delta = (c % K) * C - clo;  // fused offset -> slot offset
-      for (int64_t o = clo + quad * kBlock; o < chi; o += (int64_t)nquad * kBlock)
-        pack_range<T, W, UP>(descs, a.ndesc, total, mybuf + delta, o, o + kBlock < chi ? o + kBlock : chi, prescale);
-      if (pipe_last_cta(mine + kPipePackCnt + (c % K), (uint32_t)nquad)) {
-        if ((int)threadIdx.x < cp.nranks) st_release_sys(pipe_area(cp, threadIdx.x) + kPipePacked + cp.rank, base + (uint32_t)c + 1u);
-      }
-    }
-  } else if (role == 3) {
-    // ---------------- unpack ----------------
-    for (int64_t c = 0; c < nchunks; ++c) {
-      if (!pipe_wait(cp, mine + kPipeReduced, cp.nranks, base + (uint32_t)c + 1u)) return;
-      const int64_t clo = c * C, chi = clo + C < total ? clo + C : total;
-      const int64_t delta = (c % K) * C - clo;
-      for (int64_t o = clo + quad * kBlock; o < chi; o += (int64_t)nquad * kBlock)
-        unpack_range<T, W, UP>(descs, a.ndesc, total, mybuf + delta, o, o + kBlock < chi ? o + kBlock : chi);
-      if (pipe_last_cta(mine + kPipeUnpackCnt + (c % K), (uint32_t)nquad)) {
-        if (threadIdx.x == 0) st_release_sys(mine + kPipeUnpackDone, base + (uint32_t)c + 1u);
-      }
-    }
-  } else {
-    // ---------------- reduce + broadcast of my slice ----------------
-    const S postscale = (S)a.postscale;
-    const int ri = quad * 2 + (role - 1), nred = nquad * 2;
-    const int64_t kRBlock = a.pipe_rblock_bytes;  // work item of one reduce CTA (multiple of the 4 KiB row)
-    for (int64_t c = 0; c < nchunks; ++c) {
-      if (!pipe_wait(cp, mine + kPipePacked, cp.nranks, base + (uint32_t)c + 1u)) return;
-      const int64_t clo = c * C, chi = clo + C < total ? clo + C : total;
-      const int64_t delta = (c % K) * C - clo;
-      const int64_t units = (chi - clo) / 16;  // chunk length is a multiple of 128
-      const int64_t slo = clo + 16 * (units * cp.rank / cp.nranks), shi = clo + 16 * (units * (cp.rank + 1) / cp.nranks);
-      for (int64_t o = slo + ri * kRBlock; o < shi; o += (int64_t)nred * kRBlock) {
-        const int64_t e = o + kRBlock < shi ? o + kRBlock : shi;
-        if (a.pipe_use_nvls) {
-          if constexpr (Nvls<W>::ok) nvls_inplace_rows<W, 4>(reinterpret_cast<char*>(cp.mc_buf) + delta, o, e, postscale);
-        } else {
-          pipe_p2p_reduce<W, NR>(cp, delta, o, e, a.op, postscale);
-        }
-      }
-      if (pipe_last_cta(mine + kPipeRedCnt + (c % K), (uint32_t)nred)) {
-        if ((int)threadIdx.x < cp.nranks) st_release_sys(pipe_area(cp, threadIdx.x) + kPipeReduced + cp.rank, base + (uint32_t)c + 1u);
-      }
-    }
-  }
-}
-
-template <typename T, typename W>
-cudaError_t launch_pipelined(const CommParams& cp, const AllreduceArgs& a, cudaStream_t s) {
-  const int grid = (a.ctas / 4) * 4;
-  if (grid < 4) return cudaErrorInvalidValue;
-  if (cp.nranks <= 2) pipelined_allreduce_kernel<T, W, 2><<<grid, kThreads, 0, s>>>(cp, a);
-  else if (cp.nranks <= 4) pipelined_allreduce_kernel<T, W, 4><<<grid, kThreads, 0, s>>>(cp, a);
-  else pipelined_allreduce_kernel<T, W, 8><<<grid, kThreads, 0, s>>>(cp, a);
-  CountKernelLaunch();
-  return cudaGetLastError();
-}
-
 template <typename W>
 cudaError_t launch_inplace(const CommParams& cp, const InplaceArgs& a, cudaStream_t s) {
   if (cp.nranks <= 2) inplace_allreduce_kernel<W, 2><<<a.ctas, kThreads, 0, s>>>(cp, a);
@@ -881,6 +701,7 @@ cudaError_t launch_pu(char* buffer, const TensorDesc* descs, int nd, int64_t tot
 
 cudaError_t LaunchAllreduce(const CommParams& cp, const AllreduceArgs& args, cudaStream_t stream) {
   if (args.ctas < 1 || args.ctas > kMaxCtas || cp.nranks < 1 || cp.nranks > kMaxPeers) return cudaErrorInvalidValue;
+  if (args.variant != kOneShot && args.variant != kTwoShot && args.variant != kNvls) return cudaErrorInvalidValue;
   if (args.total_bytes <= 0) return cudaSuccess;
   if (args.variant == kNvls) {
     const int w = args.dtype == 7 ? (args.wire_dtype == 10 || args.wire_dtype == 6 ? args.wire_dtype : 7) : args.dtype;
@@ -889,15 +710,6 @@ cudaError_t LaunchAllreduce(const CommParams& cp, const AllreduceArgs& args, cud
   if (args.oneshot_nvls) {
     const int w = args.dtype == 7 ? (args.wire_dtype == 10 || args.wire_dtype == 6 ? args.wire_dtype : 7) : args.dtype;
     if (args.variant != kOneShot || !(w == 7 || w == 6 || w == 10) || args.op != 1 || cp.mc_buf == nullptr) return cudaErrorInvalidValue;
-  }
-  if (args.variant == kPipelined) {
-    const int w = args.dtype == 7 ? (args.wire_dtype == 10 || args.wire_dtype == 6 ? args.wire_dtype : 7) : args.dtype;
-    if (args.pipe_chunk_bytes <= 0 || (args.pipe_chunk_bytes % 4096) || args.pipe_slots < 2 || args.pipe_slots > kPipeMaxSlots ||
-        args.pipe_rblock_bytes < kRowBytes || (args.pipe_rblock_bytes % kRowBytes) ||
-        args.out_descs != nullptr || args.reduce_lo != 0 || args.reduce_hi != args.total_bytes)
-      return cudaErrorInvalidValue;
-    if (args.pipe_use_nvls && (!(w == 7 || w == 6 || w == 10) || args.op != 1 || cp.mc_buf == nullptr)) return cudaErrorInvalidValue;
-    HVD_DISPATCH(args.dtype, args.wire_dtype, launch_pipelined, cp, args, stream)
   }
   // chunk size: enough chunks that every (rank, CTA) pair owns work, bounded by [8 KiB, 32 KiB]
   int64_t want = args.total_bytes / ((int64_t)args.ctas * cp.nranks);

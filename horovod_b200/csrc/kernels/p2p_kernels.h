@@ -31,8 +31,7 @@ constexpr int kFlagWords = kMaxCtas * kMaxPeers;
 // Independent barrier channels (flag words + epochs) of one team: see SymmTeam::Params
 constexpr int kNumChannels = 8;
 constexpr int kGraphChannel = 1;              // collectives captured into CUDA graphs (framework streams)
-constexpr int kLatencyChannel = 3;            // the latency lane of small allreduce responses
-constexpr int kAuxChannel = 2;                // lane 1 of the dual-lane large-message allreduce (auxiliary hvd stream)
+constexpr int kLatencyChannel = 3;            // the latency lane of small allreduce responses (channel 2 is unused)
 // hvd.SyncBatchNorm's captured collectives on the compute stream: inside hvd.GraphedStep they run while the gradient
 // buckets' allreduces (kGraphChannel, forked stream) may be resident, so they need flag words and epochs of their own
 constexpr int kSyncBnChannel = 4;
@@ -60,19 +59,8 @@ struct TensorDesc {
   int64_t count;
 };
 
-enum Variant : int { kOneShot = 0, kTwoShot = 1, kNvls = 2, kPipelined = 3 };
+enum Variant : int { kOneShot = 0, kTwoShot = 1, kNvls = 2 };
 
-// Software-pipelined variant (kPipelined): per-rank words inside the flag region, past the per-CTA barrier flags and the
-// Adasum scratch.  `packed` / `reduced` are written by the peers, the rest is local bookkeeping.
-constexpr int kPipeAreaOffset = 96 * 1024;   // bytes from the start of the flag region
-constexpr int kPipeMaxSlots = 32;
-constexpr int kPipePacked = 0;                       // [kMaxPeers] chunk counter published by every rank after its pack
-constexpr int kPipeReduced = 16;                     // [kMaxPeers] ... after its reduce + broadcast
-constexpr int kPipePackCnt = 64;                     // [kPipeMaxSlots] CTAs that finished packing the chunk in this slot
-constexpr int kPipeRedCnt = 64 + kPipeMaxSlots;      // [kPipeMaxSlots]
-constexpr int kPipeUnpackCnt = 64 + 2 * kPipeMaxSlots;
-constexpr int kPipeUnpackDone = 64 + 3 * kPipeMaxSlots;  // 1 word: chunks completely unpacked on this rank
-constexpr int kPipeAreaWords = 64 + 3 * kPipeMaxSlots + 16;
 // reduce op codes follow hvd::ReduceOp: 1 SUM (AVERAGE arrives as SUM + postscale), 3 MIN, 4 MAX, 5 PRODUCT
 // dtype codes follow hvd::DataType.
 
@@ -91,18 +79,10 @@ struct AllreduceArgs {
   const TensorDesc* out_descs;  // nullptr => same as descs
   int nout;
   int oneshot_nvls;             // kOneShot only: reduce with multimem.ld_reduce on the multicast mapping instead of N peer loads
-  // kPipelined only: the symmetric buffer is a ring of `pipe_slots` chunks of `pipe_chunk_bytes`; `pipe_base` is the
-  // team-wide running chunk counter at the start of this launch (identical on all ranks), `pipe_use_nvls` selects the
-  // in-switch reduction
-  int64_t pipe_chunk_bytes;
-  int64_t pipe_rblock_bytes;    // bytes one reduce CTA handles per trip (multiple of 4096)
-  int pipe_slots;
-  uint32_t pipe_base;
-  int pipe_use_nvls;
 };
 
 // Fused allreduce / reducescatter.  Returns cudaErrorInvalidValue for
-// unsupported dtype combinations.
+// unsupported dtype combinations and for a variant other than kOneShot, kTwoShot or kNvls.
 cudaError_t LaunchAllreduce(const CommParams& cp, const AllreduceArgs& args, cudaStream_t stream);
 
 // Zero-copy allreduce on a registered (peer-mapped) tensor: ptr[r] = the tensor's address in rank r's region as

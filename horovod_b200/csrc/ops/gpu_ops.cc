@@ -58,18 +58,6 @@ GpuContext::PerDevice& GpuContext::Dev(int device) {
 }
 
 cudaStream_t GpuContext::Stream(int device) { std::lock_guard<std::mutex> l(mu_); return Dev(device).stream; }
-cudaStream_t GpuContext::AuxStream(int device) {
-  std::lock_guard<std::mutex> l(mu_);
-  PerDevice& d = Dev(device);
-  if (!d.aux_stream) {
-    int lo = 0, hi = 0;
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    cudaStreamCreateWithPriority(&d.aux_stream, cudaStreamNonBlocking, hi);
-    cudaEventCreateWithFlags(&d.fork_ev, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&d.join_ev, cudaEventDisableTiming);
-  }
-  return d.aux_stream;
-}
 cudaStream_t GpuContext::LatencyStream(int device) {
   std::lock_guard<std::mutex> l(mu_);
   PerDevice& d = Dev(device);
@@ -89,8 +77,6 @@ void* GpuContext::GridSyncBlock(int device) {
   }
   return d.grid_sync;
 }
-cudaEvent_t GpuContext::ForkEvent(int device) { AuxStream(device); std::lock_guard<std::mutex> l(mu_); return Dev(device).fork_ev; }
-cudaEvent_t GpuContext::JoinEvent(int device) { AuxStream(device); std::lock_guard<std::mutex> l(mu_); return Dev(device).join_ev; }
 
 SharedEvent* GpuContext::NewEvent(int device, int refs) {
   std::lock_guard<std::mutex> l(mu_);
@@ -123,7 +109,6 @@ const void* GpuContext::Stage(int device, const void* host, size_t bytes, cudaSt
   if (d.ring_off + bytes > kRingBytes) {  // wrap: everything older must have been consumed, on every stream that stages here
     cudaStreamSynchronize(s);
     if (d.stream && d.stream != s) cudaStreamSynchronize(d.stream);
-    if (d.aux_stream && d.aux_stream != s) cudaStreamSynchronize(d.aux_stream);
     if (d.lat_stream && d.lat_stream != s) cudaStreamSynchronize(d.lat_stream);
     d.ring_off = 0;
   }
@@ -169,11 +154,8 @@ void GpuContext::Reset() {
     cudaSetDevice(kv.first);
     if (kv.second.pinned) cudaFreeHost(kv.second.pinned);
     if (kv.second.stream) { cudaStreamSynchronize(kv.second.stream); cudaStreamDestroy(kv.second.stream); }
-    if (kv.second.aux_stream) { cudaStreamSynchronize(kv.second.aux_stream); cudaStreamDestroy(kv.second.aux_stream); }
     if (kv.second.lat_stream) { cudaStreamSynchronize(kv.second.lat_stream); cudaStreamDestroy(kv.second.lat_stream); }
     if (kv.second.grid_sync) cudaFree(kv.second.grid_sync);
-    if (kv.second.fork_ev) cudaEventDestroy(kv.second.fork_ev);
-    if (kv.second.join_ev) cudaEventDestroy(kv.second.join_ev);
     for (auto e : kv.second.pool) cudaEventDestroy(e);
     if (kv.second.host_ring) cudaFreeHost(kv.second.host_ring);
     if (kv.second.dev_ring) cudaFree(kv.second.dev_ring);
@@ -692,32 +674,6 @@ Status GpuOps::Allreduce(ProcessSet& ps, Entries& es, const Response& r, int dev
       if (lat_lane && lat_area < env_.latency_lane_bytes) lat_lane = false;  // tiny buffers: no reserved tail (same on every rank)
       if (lat_lane) cap = lat_area / 128 * 128;
       const TunableParams& tp = *env_.params;
-      // ---- large fused messages of plain tensors: TWO LANES.  The three-phase kernel is pack (HBM) -> NVLink phase -> unpack
-      // (HBM) back to back, so the links idle while it packs and HBM idles while it reduces.  The message is cut into segments that alternate
-      // between two streams — lane 0 = the hvd stream on channel 0 / buffer slot 0, lane 1 = an auxiliary stream on its
-      // own barrier channel / slot 1 — so one lane's pack and unpack run under the other lane's NVLink phase.  No
-      // fine-grained hand-offs: the overlap comes from two ordinary kernels being resident together (2 x 128 CTAs <= 264
-      // slots).  Only the two-barrier variants (two-shot / NVLS) may reuse a slot back to back: after barrier 2 nobody reads
-      // a peer's buffer any more.
-      int64_t fused_total = 0;
-      for (auto& p : pieces) fused_total += Align128(p.count * wsz);
-      const bool dual = env_.dual_lane && env_.variant != "oneshot" && fused_total >= env_.dual_lane_min_bytes && !env_.pipelined && !lat_lane;
-      cudaStream_t lane_stream[2] = {s, s};
-      if (dual) {
-        lane_stream[1] = ctx.AuxStream(device);
-        const int64_t seg = std::max<int64_t>(16ll << 20, std::min<int64_t>(64ll << 20, (fused_total / 8 + 127) / 128 * 128));
-        cap = std::min(cap, seg);
-        // fork: the auxiliary lane starts after everything already queued on the hvd stream (earlier ops may still own slot 1)
-        HVD_CUDA(cudaEventRecord(ctx.ForkEvent(device), s));
-        HVD_CUDA(cudaStreamWaitEvent(lane_stream[1], ctx.ForkEvent(device), 0));
-        WaitReady(es, lane_stream[1]);
-      }
-      int lane = 0;
-      // lane 0 takes the slot this op would have used anyway, lane 1 the other one — which the PREVIOUS op used, possibly
-      // with a one-barrier kernel a slow peer is still reading from: lane 1 therefore starts only after lane 0's first
-      // kernel (whose barrier proves every rank has left the previous op)
-      const int first_slot = dual ? team->NextSlot() : 0;
-      bool lane1_gated = false;
       // split into segments that fit the symmetric buffer
       std::vector<kern::TensorDesc> descs;
       int64_t seg_bytes = 0;
@@ -737,50 +693,27 @@ Status GpuOps::Allreduce(ProcessSet& ps, Entries& es, const Response& r, int dev
         else if (env_.variant == "twoshot") variant = kern::kTwoShot;
         else if (env_.variant == "nvls" && nvls_ok) variant = kern::kNvls;
         else {
-          if (seg_bytes <= tp.oneshot_max_bytes && !dual) variant = kern::kOneShot;
+          if (seg_bytes <= tp.oneshot_max_bytes) variant = kern::kOneShot;
           else if (nvls_ok && n >= 4 && seg_bytes >= tp.nvls_min_bytes) variant = kern::kNvls;  // in-switch reduction pays off from 4 GPUs (measured: slower than two-shot at N=2)
-        }
-        // opt-in: software-pipelined pack / NVLS / unpack for large segments of plain tensors (docs/roadmap.md B1)
-        const bool pipelined_on = env_.pipelined;
-        const int64_t pipe_chunk = env_.pipe_chunk_bytes, pipe_min = env_.pipe_min_bytes;
-        // (at N = 2, where the reduce stage is plain P2P, the pipeline lost to the three-phase kernel at 1 GiB — it only pays
-        // when the reduce stage is the in-switch multimem one)
-        if (pipelined_on && env_.variant == "auto" && nvls_ok && n >= 4 && seg_bytes >= pipe_min && cap / pipe_chunk >= 2) {
-          variant = kern::kPipelined;
-          a.pipe_chunk_bytes = pipe_chunk;
-          a.pipe_rblock_bytes = env_.pipe_rblock_bytes;
-          a.pipe_slots = (int)std::min<int64_t>(kern::kPipeMaxSlots, cap / pipe_chunk);
-          a.pipe_base = team->NextPipeBase((uint32_t)((seg_bytes + pipe_chunk - 1) / pipe_chunk));
-          a.pipe_use_nvls = 1;
         }
         a.variant = variant;
         a.ctas = CtasFor(variant, seg_bytes, n);
-        const int64_t big_ctas = env_.large_msg_ctas;
-        if (dual) a.ctas = (int)std::max<int64_t>(8, std::min<int64_t>(big_ctas / 2, kern::kMaxCtas / 2));
-        if (variant == kern::kPipelined) a.ctas = (int)std::min<int64_t>(kern::kMaxCtas, std::max<int64_t>(tp.comm_ctas, big_ctas)) / 4 * 4;
         if (a.ndesc <= kern::kInlineDescs) {
           memcpy(a.inline_descs, descs.data(), descs.size() * sizeof(kern::TensorDesc));
           a.descs = nullptr;
         } else {
-          a.descs = (const kern::TensorDesc*)ctx.Stage(device, descs.data(), descs.size() * sizeof(kern::TensorDesc), lane_stream[lane]);
+          a.descs = (const kern::TensorDesc*)ctx.Stage(device, descs.data(), descs.size() * sizeof(kern::TensorDesc), s);
           if (!a.descs) return Status::UnknownError("descriptor table too large");
         }
-        kern::CommParams cp = dual ? team->Params(first_slot ^ lane, lane == 0 ? 0 : kern::kAuxChannel)
-                            : lat_lane ? team->Params(team->NextLatencySlot(), kern::kLatencyChannel, (int64_t)team->buffer_bytes())
+        kern::CommParams cp = lat_lane ? team->Params(team->NextLatencySlot(), kern::kLatencyChannel, (int64_t)team->buffer_bytes())
                                        : team->Params(team->NextSlot());
-        if (dual && lane == 1 && !lane1_gated) {
-          cudaStreamWaitEvent(lane_stream[1], ctx.ForkEvent(device), 0);  // re-recorded below, after lane 0's first kernel
-          lane1_gated = true;
-        }
         if (env_.timeline && env_.timeline->Initialized())
           env_.timeline->ActivityStartAll(es, variant == kern::kOneShot ? HVD_ACT_P2P_ALLREDUCE_ONESHOT
                                               : variant == kern::kNvls ? HVD_ACT_P2P_ALLREDUCE_NVLS : HVD_ACT_P2P_ALLREDUCE_TWOSHOT);
-        cudaError_t ce = kern::LaunchAllreduce(cp, a, lane_stream[lane]);
+        cudaError_t ce = kern::LaunchAllreduce(cp, a, s);
         if (ce != cudaSuccess) return Status::UnknownError(std::string("allreduce kernel launch failed: ") + cudaGetErrorString(ce));
         descs.clear();
         seg_bytes = 0;
-        if (dual && lane == 0 && !lane1_gated) cudaEventRecord(ctx.ForkEvent(device), s);  // "lane 0's first kernel is done"
-        if (dual) lane ^= 1;
         return Status::OK();
       };
       for (auto& p : pieces) {
@@ -799,10 +732,6 @@ Status GpuOps::Allreduce(ProcessSet& ps, Entries& es, const Response& r, int dev
       }
       st = flush();
       if (!st.ok()) return st;
-      if (dual) {  // join: the completion event (recorded on the hvd stream) covers the auxiliary lane
-        HVD_CUDA(cudaEventRecord(ctx.JoinEvent(device), lane_stream[1]));
-        HVD_CUDA(cudaStreamWaitEvent(s, ctx.JoinEvent(device), 0));
-      }
     }
   }
   ctx.TempFreeAll(device, s);

@@ -37,12 +37,8 @@ class GpuContext {
   bool Available();
   int DeviceCount();
   cudaStream_t Stream(int device);
-  // second private stream of the device (lane 1 of the dual-lane large-message allreduce) and its fork / join events
-  cudaStream_t AuxStream(int device);
-  cudaStream_t LatencyStream(int device);
-  void* GridSyncBlock(int device);         // 256 zeroed bytes: grid-barrier state of the persistent Adasum kernel  // small responses (GpuOpEnv::latency_lane_bytes)
-  cudaEvent_t ForkEvent(int device);
-  cudaEvent_t JoinEvent(int device);
+  cudaStream_t LatencyStream(int device);  // small responses (GpuOpEnv::latency_lane_bytes)
+  void* GridSyncBlock(int device);         // 256 zeroed bytes: grid-barrier state of the persistent Adasum kernel
   SharedEvent* NewEvent(int device, int refs);
   void Release(SharedEvent* e);
   // Copies a small host table to device memory on `s` (pinned ring -> device ring).
@@ -57,10 +53,8 @@ class GpuContext {
  private:
   struct PerDevice {
     cudaStream_t stream = nullptr;
-    cudaStream_t aux_stream = nullptr;
     cudaStream_t lat_stream = nullptr;
     void* grid_sync = nullptr;
-    cudaEvent_t fork_ev = nullptr, join_ev = nullptr;
     std::vector<cudaEvent_t> pool;
     char* host_ring = nullptr; char* dev_ring = nullptr; size_t ring_off = 0;
     std::vector<void*> temps;
@@ -82,20 +76,12 @@ struct GpuOpEnv {
   DataType wire_dtype = DataType::FLOAT32;  // FLOAT32 = no compression
   size_t symm_buffer_bytes = 128ull << 20;
   bool want_multicast = true;
-  // software-pipelined allreduce of large plain (unregistered) tensors: pack / reduce / unpack CTAs on a chunk ring
-  bool pipelined = false;  // opt-in: slower than the three-phase kernel where it was measured (8 GPUs)
-  int64_t pipe_chunk_bytes = 4 << 20, pipe_min_bytes = 32 << 20, pipe_rblock_bytes = 16384;
   int64_t large_msg_ctas = 256;   // CTAs for >= 64 MiB fused messages (two per SM)
   bool broadcast_multicast = true;
-  // large fused messages of plain tensors alternate between two streams / barrier channels / buffer slots so that one
-  // lane's pack + unpack (HBM) overlap the other lane's NVLink phase
   // allreduce responses of at most this many fused bytes run on the latency lane (own stream / barrier channel / reserved
   // buffer tail) instead of queueing behind large ones on the main stream; 0 = off
   int64_t latency_lane_bytes = 256 << 10;
   bool adasum_persistent = true;   // single-launch Adasum (grid barriers inside the kernel) instead of 2 + 2 log2(N) launches
-  bool dual_lane = false;  // opt-in: where it was measured (8 GPUs) it did not pay: each lane's
-                           // pack / unpack runs at half the CTAs and the two NVLink phases contend
-  int64_t dual_lane_min_bytes = 64 << 20;
   // teams of up to this many ranks reduce IPC-registered plain tensors in place with the P2P two-shot kernel; larger
   // teams keep the fused pack + NVLS + unpack kernel for sums and use IPC only for MIN / MAX / PRODUCT
   int ipc_max_ranks = 4;  // at 4 GPUs zero-copy P2P beat the three-phase NVLS kernel where it was measured; at 8 GPUs the two tied

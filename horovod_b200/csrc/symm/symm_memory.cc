@@ -280,8 +280,7 @@ kern::CommParams SymmTeam::Params(int which, int channel, int64_t byte_offset) c
 namespace {
 // flag words (kFlagWords * 4 = 8 KiB) followed by the two Adasum partial-dot tables (2 x kAdasumScratchStride)
 constexpr size_t kFlagRegionBytes = 256 * 1024;
-static_assert(kern::kFlagWords * 4 + 2 * kern::kAdasumScratchStride <= (long long)kern::kPipeAreaOffset, "Adasum scratch overlaps the pipeline words");
-static_assert(kern::kPipeAreaOffset + kern::kPipeAreaWords * 4 <= (long long)kern::kChannelFlagsOffset, "pipeline words overlap the channel flags");
+static_assert(kern::kFlagWords * 4 + 2 * kern::kAdasumScratchStride <= (long long)kern::kChannelFlagsOffset, "Adasum scratch overlaps the channel flags");
 static_assert(kern::kChannelFlagsOffset + (kern::kNumChannels - 1) * kern::kFlagWords * 4 <= (long long)kFlagRegionBytes, "flag region too small");
 }
 

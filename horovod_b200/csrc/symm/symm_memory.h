@@ -70,9 +70,6 @@ class SymmTeam {
   // slow peer is still reading).
   int NextSlot() { int s = slot_; slot_ ^= 1; return s; }
   int NextLatencySlot() { int s = lat_slot_; lat_slot_ ^= 1; return s; }  // the latency lane alternates on its own
-  // Running chunk counter of the software-pipelined allreduce: every rank launches the same sequence of pipelined
-  // kernels with the same chunk counts, so the value is identical on all ranks without communication.
-  uint32_t NextPipeBase(uint32_t nchunks) { uint32_t b = pipe_seq_; pipe_seq_ += nchunks; return b; }
   int* host_abort_flag() { return abort_host_; }
   void Abort() { if (abort_host_) *abort_host_ = 1; }
   // 0 = healthy, 1 = aborted by the host, 2 = a kernel timed out waiting for a peer
@@ -100,7 +97,6 @@ class SymmTeam {
   int* abort_host_ = nullptr;   // pinned, mapped
   int* abort_dev_ = nullptr;    // device alias of abort_host_
   int slot_ = 0, lat_slot_ = 0;
-  uint32_t pipe_seq_ = 0;
   unsigned long long timeout_ns_ = 0;
   std::string backend_;
   std::vector<RegionView> regions_;

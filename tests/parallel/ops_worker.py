@@ -359,8 +359,8 @@ def _():
 
 @check('large_allreduce')
 def _():
-    """Large fused responses of ordinary tensors (GPU: the three-phase / software-pipelined kernels, several segments of
-    the symmetric buffer): exact integer-valued sums so every element can be checked."""
+    """Large fused responses of ordinary tensors (GPU: the three-phase kernel, several segments of the symmetric buffer):
+    exact integer-valued sums so every element can be checked."""
     big = (5 << 20) if args.device == 'cuda' else (1 << 18)
     for dtype in (torch.float32, torch.bfloat16):
         sizes = [big + 3, 1001, big // 2 + 17, 7, big]
@@ -371,7 +371,7 @@ def _():
         for n, t in zip(sizes, ts):
             exp = ((torch.arange(n, device=DEV) % 13) * size + sum(range(size))).to(dtype)
             assert torch.equal(t, exp), (dtype, n, t[:5], exp[:5], int((t != exp).sum()))
-    # one tensor larger than a pipeline chunk ring, averaged, not in place
+    # one large tensor, averaged, not in place
     x = torch.full([3 * big + 5], float(rank + 1), device=DEV)
     y = hvd.allreduce(x, op=hvd.Average, name='large.avg')
     assert torch.allclose(y, torch.full_like(y, (size + 1) / 2.0)) and float(x[0]) == rank + 1

@@ -6,7 +6,7 @@ fp64 for fp64, int32 for 8 / 16 / 32-bit integers, int64 for int64):
 
     pack (every fused variant)   w_r = W(A(x_r * prescale))     integers: trunc(double(x_r) * prescale), wrapped
     one-shot                     T(A(sum_r w_r * postscale))
-    two-shot, pipelined          T(W(A(sum_r w_r * postscale)))  (the owner rounds to the wire before broadcasting)
+    two-shot                     T(W(A(sum_r w_r * postscale)))  (the owner rounds to the wire before broadcasting)
     zero-copy in-place           W(A(sum_r x_r * scale))
 
 Floats are compared with the accumulation bound |out - ref| <= (n-1) u_A sum_r |w_r| |postscale| (plus one rounding of
@@ -20,7 +20,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-ONESHOT, TWOSHOT, PIPELINED, INPLACE = 0, 1, 3, 'inplace'
+ONESHOT, TWOSHOT, INPLACE = 0, 1, 'inplace'
 SUM, MIN, MAX, PROD = 1, 3, 4, 5
 FLOATS = [torch.float32, torch.float64, torch.bfloat16, torch.float16]
 INTS = [torch.uint8, torch.int8, torch.int16, torch.int32, torch.int64]
@@ -81,7 +81,7 @@ def pack_int(x, pre, wire):
 def narrowing(variant, dtype, wire):
     """Casts after the accumulation that can round (each costs one ulp in the bound)."""
     acc = acc_dtype(wire)
-    chain = [wire, dtype] if variant in (TWOSHOT, PIPELINED) else [wire] if variant == INPLACE else [dtype]
+    chain = [wire, dtype] if variant == TWOSHOT else [wire] if variant == INPLACE else [dtype]
     out, prev = [], acc
     for d in chain:
         if FMT[d][0] < FMT[prev][0]:
@@ -128,7 +128,7 @@ def minmax_exact(ws, op, post, variant, dtype, wire):
     m = st.min(0).values if op == MIN else st.max(0).values
     acc = acc_dtype(wire)
     m = (m * kernel_scale(post, acc)).to(acc)
-    for d in ([wire, dtype] if variant in (TWOSHOT, PIPELINED) else [wire] if variant == INPLACE else [dtype]):
+    for d in ([wire, dtype] if variant == TWOSHOT else [wire] if variant == INPLACE else [dtype]):
         m = m.to(d)
     return m.double()
 
@@ -253,7 +253,7 @@ def inject_nonfinite(ins, i):
 
 @pytest.mark.parametrize('op', [SUM, MIN, MAX, PROD])
 @pytest.mark.parametrize('dtype', FLOATS)
-@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT, INPLACE, PIPELINED])
+@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT, INPLACE])
 @pytest.mark.parametrize('n', [2, 3, 4, 6, 8])
 def test_ranks_agree_bitwise(sim, n, variant, dtype, op):
     sizes = [81928] if variant == INPLACE else [1, 4099, 70001]
@@ -262,7 +262,7 @@ def test_ranks_agree_bitwise(sim, n, variant, dtype, op):
     keep = [[x.clone() for x in row] for row in ins]
     outs = [[torch.empty_like(x) for x in row] for row in ins]
     post = 1.0 / n if op == SUM else 1.0
-    res = run(sim, variant, ins, outs, op, ctas=16 if variant == PIPELINED else 8, post=post)
+    res = run(sim, variant, ins, outs, op, ctas=8, post=post)
     assert_ranks_agree(res, 'variant %s n=%d %s op %d' % (variant, n, dtype, op))
     if op == SUM:  # the non-finite pattern (AMP's overflow check reads it) is the reference's
         i = len(sizes) - 1
@@ -282,11 +282,11 @@ def test_variants_agree_bitwise(sim, n, dtype):
     count = 3 * 8192 + 40  # several chunks per CTA, a multiple of 16 B in every dtype
     base = make(n, [count], dtype, SUM, seed=7 + n)
     results = {}
-    for variant in (ONESHOT, TWOSHOT, INPLACE, PIPELINED):
+    for variant in (ONESHOT, TWOSHOT, INPLACE):
         ins = [[x.clone() for x in row] for row in base]
         outs = [[torch.empty_like(x) for x in row] for row in ins]
         results[variant] = run(sim, variant, ins, outs, SUM, ctas=8, post=1.0 / n)
-    for variant in (TWOSHOT, INPLACE, PIPELINED):
+    for variant in (TWOSHOT, INPLACE):
         for r in range(n):
             a, b = as_bits(results[ONESHOT][r][0]), as_bits(results[variant][r][0])
             assert torch.equal(a, b), 'variant %s rank %d differs from one-shot in %d elements' % (variant, r, int((a != b).sum()))
@@ -313,30 +313,21 @@ def test_allreduce_matches_model(sim, n, variant, dtype, op, scales):
 
 @pytest.mark.parametrize('op', [SUM, MAX])
 @pytest.mark.parametrize('wire', [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT, PIPELINED])
+@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT])
 @pytest.mark.parametrize('n', [2, 3, 5, 8])
 def test_wire_compression_matches_model(sim, n, variant, wire, op):
-    """fp32 tensors, 16-bit wire: one-shot keeps the fp32 sum, two-shot / pipelined round it to the wire."""
+    """fp32 tensors, 16-bit wire: one-shot keeps the fp32 sum, two-shot rounds it to the wire."""
     ins = make(n, C_SIZES, torch.float32, op, seed=n)
     outs = [[torch.empty_like(x) for x in row] for row in ins]
-    run(sim, variant, ins, outs, op, ctas=16 if variant == PIPELINED else 8, wire=wire, pre=0.5, post=1.0 / n)
+    run(sim, variant, ins, outs, op, ctas=8, wire=wire, pre=0.5, post=1.0 / n)
     check_against_reference(outs, ins, variant, op, torch.float32, wire, 0.5, 1.0 / n, 'variant %d' % variant)
     assert_ranks_agree(outs, 'wire %s' % wire)
-
-
-def test_pipelined_matches_model(sim):
-    for n, dtype, op in ((3, torch.float32, SUM), (5, torch.bfloat16, SUM), (8, torch.float64, PROD), (6, torch.int16, SUM),
-                         (4, torch.int64, MAX)):
-        ins = make(n, C_SIZES + [300001], dtype, op, seed=n)
-        outs = [[torch.empty_like(x) for x in row] for row in ins]
-        run(sim, PIPELINED, ins, outs, op, ctas=16, pre=0.5, post=1.0 / n)
-        check_against_reference(outs, ins, PIPELINED, op, dtype, dtype, 0.5, 1.0 / n, 'pipelined n=%d %s' % (n, dtype))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # D. integer edges: wrap-around, and int64 values no double can hold
 
-@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT, PIPELINED, INPLACE])
+@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT, INPLACE])
 @pytest.mark.parametrize('n', [2, 3, 5, 8])
 def test_integer_wrap_and_int64_exact(sim, n, variant):
     cases = [(torch.int8, 100), (torch.uint8, 200), (torch.int16, 30000), (torch.int32, (1 << 31) - 5),
@@ -352,7 +343,7 @@ def test_integer_wrap_and_int64_exact(sim, n, variant):
             rows.append([x.to(dtype).cuda()])
         keep = [[x.clone() for x in row] for row in rows]
         outs = [[torch.empty_like(x) for x in row] for row in rows]
-        res = run(sim, variant, rows, outs, SUM, ctas=16 if variant == PIPELINED else 4)
+        res = run(sim, variant, rows, outs, SUM, ctas=4)
         ref = int_ref([x[0].cpu().numpy().astype(np.int64) for x in keep], SUM, 1.0, dtype, dtype)
         for r in range(n):
             assert np.array_equal(res[r][0].cpu().numpy(), ref), (dtype, v, r)
@@ -404,11 +395,9 @@ def guarded(shape_count, dtype, offset, fill):
 
 
 @pytest.mark.parametrize('ctas', [1, 3, 8, 32])
-@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT, PIPELINED])
+@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT])
 @pytest.mark.parametrize('dtype', [torch.uint8, torch.float16, torch.float32, torch.float64])
 def test_shapes_in_one_response(sim, dtype, variant, ctas):
-    if variant == PIPELINED and ctas < 4:
-        pytest.skip('the pipelined kernel needs at least one CTA of each of its four roles')
     n = 4
     counts = boundary_counts(dtype.itemsize)
     counts = counts[:3] + [0] + counts[3:] + [0, 5]  # empty tensors between non-empty ones and before the last one
@@ -452,7 +441,7 @@ def test_shapes_in_one_response(sim, dtype, variant, ctas):
                 assert (buf[:k] == 0).all() and (buf[k + counts[i]:] == 0).all()
 
 
-@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT, PIPELINED])
+@pytest.mark.parametrize('variant', [ONESHOT, TWOSHOT])
 def test_many_tensors_one_response(sim, variant):
     n = 4
     sizes = [1, 3, 7, 64, 333, 4097, 0, 12, 1025, 2] * 32 + [100003]  # 321 tensors
@@ -468,7 +457,7 @@ def test_tiny_response_leaves_ctas_idle(sim):
     for n, ctas in ((2, 32), (4, 32), (8, 16)):
         ins = make(n, [5], torch.float32, SUM, seed=n)
         outs = [[torch.empty_like(x) for x in row] for row in ins]
-        for variant in (ONESHOT, TWOSHOT, PIPELINED):
+        for variant in (ONESHOT, TWOSHOT):
             run(sim, variant, ins, outs, SUM, ctas=ctas)
             check_against_reference(outs, ins, variant, SUM, torch.float32, torch.float32, 1.0, 1.0, 'tiny')
 
@@ -526,9 +515,11 @@ def test_inplace_rejects_sizes_not_multiple_of_16_bytes(sim):
     ts = [torch.zeros(5, device='cuda') for _ in range(n)]  # 20 B
     with pytest.raises(RuntimeError):
         sim.inplace_allreduce(ts)
-    # the rejected call leaves the simulated ranks in step: the next collectives through their buffers still add up
     ins = make(n, [4099], torch.float32, SUM, seed=1)
     outs = [[torch.empty_like(x) for x in row] for row in ins]
+    with pytest.raises(RuntimeError):  # the fused kernel has variants 0 (one-shot), 1 (two-shot) and 2 (NVLS) only
+        sim.allreduce(ins, outs, op=SUM, variant=3, ctas=8)
+    # the rejected calls leave the simulated ranks in step: the next collectives through their buffers still add up
     for variant in (ONESHOT, TWOSHOT):
         run(sim, variant, ins, outs, SUM, ctas=8)
         check_against_reference(outs, ins, variant, SUM, torch.float32, torch.float32, 1.0, 1.0, 'after a rejected call')

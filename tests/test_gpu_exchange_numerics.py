@@ -10,17 +10,11 @@ bytes, so their outputs must equal torch.cat / indexing of the inputs byte for b
 
 Every case writes into views of larger buffers filled with a sentinel, at byte offsets 0 and 1..15 (16 B vector and
 byte paths), checks that the sentinel around each output and every input are untouched, and runs three times (ping-pong
-buffer slots, barrier epochs).  Small buffer sizes (`cap`) force the windowed multi-launch paths.  The exchange cases run
-again in a subprocess with the TMA variant of the exchange kernel (HVD_EXCHANGE_TMA=1).
+buffer slots, barrier epochs).  Small buffer sizes (`cap`) force the windowed multi-launch paths.
 
 Not covered here: the broadcast root's multicast store and reducescatter's multimem reduce; the simulated team has no
 multicast object.  tests/test_gpu_multi.py covers them on real multi-GPU teams.
 """
-import os
-import subprocess
-import sys
-import textwrap
-
 import numpy as np
 import pytest
 import torch
@@ -311,23 +305,6 @@ def a2a_case(sim, n, dtype, ctas, cap):
 NS = [2, 3, 5, 8]
 
 
-def exchange_cases():
-    """(name, callable(sim)) of every exchange case, shared by the tests below and the TMA subprocess."""
-    cases = []
-    for cap in CAPS:
-        for n in NS:
-            for k, dtype in enumerate(EX_DTYPES):
-                ctas = CTAS[(n + k) % 4]
-                cases.append(('allgatherv-%d-%s-%d' % (n, dtype, cap), lambda s, n=n, d=dtype, c=ctas, b=cap: ag_case(s, n, d, c, b)))
-                cases.append(('alltoallv-%d-%s-%d' % (n, dtype, cap), lambda s, n=n, d=dtype, c=ctas, b=cap: a2a_case(s, n, d, c, b)))
-            for root in range(n):
-                for inplace in (False, True):
-                    ctas = CTAS[(root + 2 * inplace) % 4]
-                    cases.append(('broadcast-%d-%d-%d-%d' % (n, root, inplace, cap),
-                                  lambda s, n=n, r=root, i=inplace, c=ctas, b=cap: bc_case(s, n, r, i, c, b)))
-    return cases
-
-
 @pytest.mark.parametrize('cap', CAPS)
 @pytest.mark.parametrize('ctas', CTAS)
 @pytest.mark.parametrize('dtype', EX_DTYPES)
@@ -363,23 +340,3 @@ def test_buffer_without_a_plan_launches_nothing(sim):
     sim.reducescatter(ins, outs, cap=4096)
     torch.cuda.synchronize()
     assert all(torch.equal(o[0], torch.full((1, 4), float(n), device='cuda')) for o in outs)
-
-
-def test_exchange_tma_variant():
-    """Every exchange case above once more with the cp.async.bulk variant of the exchange kernel, in a subprocess: the
-    variant is selected once per process (HVD_EXCHANGE_TMA)."""
-    code = textwrap.dedent('''
-        import sys
-        sys.path.insert(0, %r)
-        from horovod_b200.ops import sim
-        import test_gpu_exchange_numerics as t
-        cases = t.exchange_cases()
-        for name, run in cases:
-            run(sim)
-        print('TMA EXCHANGE CASES OK', len(cases))
-    ''' % os.path.dirname(os.path.abspath(__file__)))
-    from conftest import REPO
-    p = subprocess.run([sys.executable, '-c', code], env=dict(os.environ, HVD_EXCHANGE_TMA='1', PYTHONPATH=REPO),
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=900)
-    out = p.stdout.decode()
-    assert p.returncode == 0 and 'TMA EXCHANGE CASES OK' in out, out[-3000:]

@@ -151,69 +151,6 @@ def test_sim_allgather_exchange():
         assert torch.equal(outs[r], ref)
 
 
-def test_sim_allgather_exchange_tma_variant():
-    """The cp.async.bulk (UBLKCP) variant of the exchange kernel: ragged sizes (16 B-aligned bulk part + byte tail) and an
-    unaligned destination (falls back to the vector path inside the same kernel).  Runs in a subprocess because the
-    variant is selected once per process (HVD_EXCHANGE_TMA)."""
-    import os, subprocess, sys, textwrap
-    code = textwrap.dedent('''
-        import ctypes, torch
-        from horovod_b200.common.basics import load_library
-        lib = load_library()
-        lib.hvd_sim_allgather.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int64, ctypes.POINTER(ctypes.c_uint64),
-                                          ctypes.POINTER(ctypes.c_uint64), ctypes.c_int]
-        for n, nbytes, shift in ((8, 1 << 20, 0), (4, (1 << 18) + 13, 0), (2, 100000, 3), (2, 7, 0)):
-            ins = [torch.randint(0, 255, (nbytes,), device='cuda', dtype=torch.uint8) for _ in range(n)]
-            bufs = [torch.zeros(n * nbytes + 64, device='cuda', dtype=torch.uint8) for _ in range(n)]
-            outs = [b[shift:shift + n * nbytes] for b in bufs]
-            ip = (ctypes.c_uint64 * n)(*[x.data_ptr() for x in ins])
-            op_ = (ctypes.c_uint64 * n)(*[x.data_ptr() for x in outs])
-            for rep in range(3):
-                assert lib.hvd_sim_allgather(n, 0, nbytes, ip, op_, 8) == 0
-            ref = torch.cat(ins)
-            for r in range(n):
-                assert torch.equal(outs[r], ref), (n, nbytes, shift, r)
-        print('TMA EXCHANGE OK')
-    ''')
-    from conftest import REPO
-    p = subprocess.run([sys.executable, '-c', code], env=dict(os.environ, HVD_EXCHANGE_TMA='1', PYTHONPATH=REPO),
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=300)
-    assert p.returncode == 0 and 'TMA EXCHANGE OK' in p.stdout.decode(), p.stdout.decode()[-3000:]
-
-
-@pytest.mark.parametrize("slots", ["2", "16"])
-def test_pipelined_allreduce_variant_in_simulation(slots):
-    """kPipelined (role-specialised CTAs, chunk ring in the symmetric buffer, packed / reduced / unpack_done counters) with
-    the P2P reduce stage on 2 / 4 / 8 simulated ranks; 64 KiB chunks and a 2-slot ring force many ring wrap-arounds."""
-    import os, subprocess, sys, textwrap
-    code = textwrap.dedent('''
-        import torch
-        from horovod_b200.ops import sim
-        PIPELINED = 3
-        for n in (2, 4, 8):
-            for dtype, tol in ((torch.float32, 1e-5), (torch.bfloat16, 2e-2)):
-                sizes = [1, 100003, 17, 262144 + 5, 4096]
-                g = torch.Generator(device='cuda').manual_seed(n)
-                ins = [[torch.randn(s, device='cuda', generator=g).to(dtype) for s in sizes] for _ in range(n)]
-                outs = [[torch.empty_like(t) for t in row] for row in ins]
-                for rep in range(3):  # the chunk counters keep running across launches
-                    sim.allreduce(ins, outs, op=sim.SUM, variant=PIPELINED, ctas=16, prescale=0.5, postscale=2.0 / n)
-                    for i in range(len(sizes)):
-                        ref = torch.stack([ins[r][i].float() * 0.5 for r in range(n)]).sum(0) * (2.0 / n)
-                        for r in range(n):
-                            torch.testing.assert_close(outs[r][i].float(), ref, rtol=tol, atol=tol)
-            big = [[torch.ones(3 << 20, device='cuda')] for _ in range(n)]   # 12 MiB: ~190 chunks
-            sim.allreduce(big, big, op=sim.SUM, variant=PIPELINED, ctas=32)
-            assert all(float(b[0][0]) == n and float(b[0][-1]) == n and float(b[0].min()) == n for b in big)
-        print('PIPELINED OK')
-    ''')
-    from conftest import REPO
-    p = subprocess.run([sys.executable, '-c', code], env=dict(os.environ, HVD_PIPE_SLOTS=slots, HVD_PIPE_CHUNK_BYTES='65536',
-                                                              HVD_KERNEL_TIMEOUT_SECONDS='20', PYTHONPATH=REPO),
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=600)
-    assert p.returncode == 0 and 'PIPELINED OK' in p.stdout.decode(), p.stdout.decode()[-3000:]
-
-
 def test_pack_reduce_bandwidth_smoke():
     """Not a benchmark: just checks a 64 MiB fused buffer moves at a sane rate on one GPU (all 'peers' are local HBM)."""
     n = 2

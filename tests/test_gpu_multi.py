@@ -89,11 +89,11 @@ def test_collectives_as_cuda_graph_nodes(native_built):
 
 
 @pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
-def test_fused_collectives_and_pipelined_allreduce(native_built):
-    """Fused allgather / reducescatter / broadcast responses (one launch each) and the software-pipelined allreduce of
-    large plain tensors."""
+def test_fused_collectives_and_large_allreduce(native_built):
+    """Fused allgather / reducescatter / broadcast responses (one launch each) and the three-phase allreduce of large
+    plain tensors."""
     n = 2 if _ngpu() < 4 else (4 if _ngpu() < 8 else 8)
-    rc, out = run_parallel("ops_worker.py", np=n, timeout=420, env={"HVD_PIPE_MIN_BYTES": str(1 << 20), "HVD_PIPE_CHUNK_BYTES": str(1 << 20)},
+    rc, out = run_parallel("ops_worker.py", np=n, timeout=420,
                            args=["--device", "cuda", "--only", "fused_other_collectives,allgather,broadcast,reducescatter,"
                                  "allreduce_sum_avg,allreduce_async_fused,large_allreduce"])
     assert "ALL OK" in out, out[-4000:]
