@@ -17,6 +17,8 @@ import numpy as np
 import pytest
 import torch
 
+from optim_cases import COUNTS, PAIRS, Slot, adam_ref, adam_ref_kernel, f32, hvd, ulp  # noqa: F401  (hvd: fixture)
+
 # ---------------------------------------------------------------------------------------------------------------------
 # float64 reference
 
@@ -43,43 +45,11 @@ def sgd_ref(p, g, buf, lr, momentum=0.0, dampening=0.0, weight_decay=0.0, nester
     return p - lr * d, buf, p.abs() + abs(lr) * ds, bs
 
 
-def adam_ref(p, g, m, v, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, step=1, adamw=True, grad_scale=1.0,
-             bias=None):
-    """One Adam (L2 weight decay) or AdamW (decoupled) step on float64 tensors, with `step` the parameter's 1-based step
-    count; eps is added after sqrt(v) / sqrt(1 - beta2^step). `bias` overrides the two bias corrections. Returns
-    (p, m, v, p_scale, m_scale, v_scale)."""
-    c1, c2 = bias if bias is not None else (1 - beta1 ** step, 1 - beta2 ** step)
-    d = g * grad_scale
-    ds = d.abs()
-    if adamw:
-        p = p * (1 - lr * weight_decay)
-    elif weight_decay != 0:
-        d = d + weight_decay * p
-        ds = ds + abs(weight_decay) * p.abs()
-    m_new = beta1 * m + (1 - beta1) * d
-    ms = beta1 * m.abs() + (1 - beta1) * ds
-    v_new = beta2 * v + (1 - beta2) * d * d
-    vs = beta2 * v + (1 - beta2) * ds * ds
-    denom = v_new.sqrt() / c2 ** 0.5 + eps
-    return p - (lr / c1) * m_new / denom, m_new, v_new, p.abs() + (lr / c1) * ms / denom, ms, vs
-
-
-def _f32(x):
-    return float(np.float32(x))
-
-
 def sgd_ref_kernel(p, g, buf, lr, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, grad_scale=1.0,
                    first_step=False):
     """sgd_ref with the hyper-parameters the kernel receives (fp32)."""
-    return sgd_ref(p, g, buf, _f32(lr), _f32(momentum), _f32(dampening), _f32(weight_decay), nesterov, _f32(grad_scale),
+    return sgd_ref(p, g, buf, f32(lr), f32(momentum), f32(dampening), f32(weight_decay), nesterov, f32(grad_scale),
                    first_step)
-
-
-def adam_ref_kernel(p, g, m, v, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, step=1, adamw=True, grad_scale=1.0):
-    """adam_ref with the hyper-parameters the kernel receives: fp32 values, bias corrections 1 - (float)beta^step."""
-    bias = (_f32(1.0 - _f32(beta1 ** step)), _f32(1.0 - _f32(beta2 ** step)))
-    return adam_ref(p, g, m, v, _f32(lr), _f32(beta1), _f32(beta2), _f32(eps), _f32(weight_decay), step, adamw,
-                    _f32(grad_scale), bias)
 
 
 def test_reference_matches_torch_optim_in_float64():
@@ -132,17 +102,6 @@ def test_reference_matches_torch_optim_in_float64():
 # ---------------------------------------------------------------------------------------------------------------------
 # helpers for the kernel tests
 
-_MANT = {torch.bfloat16: 7, torch.float16: 10}
-_EMIN = {torch.bfloat16: -126, torch.float16: -14}
-
-
-def _ulp(x, dtype):
-    """Spacing of `dtype` at |x| (x float64, already representable in dtype)."""
-    _, e = torch.frexp(x.abs())  # |x| = f * 2^e, f in [0.5, 1); frexp(0) has e = 0, zero has the subnormal spacing
-    e = torch.where(x == 0, torch.full_like(e, _EMIN[dtype] + 1), e)
-    return torch.ldexp(torch.ones_like(x), torch.clamp(e - 1, min=_EMIN[dtype]) - _MANT[dtype])
-
-
 def check(name, got, ref, scale, dtype, rtol=1e-6):
     """got (kernel, any dtype) against ref (float64). fp32: |got - ref| <= rtol * scale. bf16 / fp16: within one ulp of
     the reference rounded to the dtype, plus the fp32 arithmetic error of the kernel before its final rounding."""
@@ -152,36 +111,13 @@ def check(name, got, ref, scale, dtype, rtol=1e-6):
         want = ref
     else:
         want = ref.to(dtype).double()
-        allowed = _ulp(want, dtype) + rtol * scale
+        allowed = ulp(want, dtype) + rtol * scale
     err = (got - want).abs()
     bad = ~(err <= allowed)  # NaN counts as bad
     if bad.any():
         i = int(bad.nonzero()[0])
         raise AssertionError(f'{name}: {int(bad.sum())}/{got.numel()} elements off, first at {i}: got {got[i].item()!r} '
                              f'want {want[i].item()!r} (err {err[i].item():.3e} > {allowed[i].item():.3e})')
-
-
-class Slot:
-    """A tensor of `shape` / `dtype` placed at element `offset` of a larger buffer; the slack is random bits that must
-    survive the kernel (catches vector stores running past a tail or before a head)."""
-
-    def __init__(self, shape, dtype, offset=0, memory_format=torch.contiguous_format, fill=None, slack=67):
-        numel = int(np.prod(shape)) if len(shape) else 1
-        self.buf = torch.randn(offset + numel + slack, device='cuda').to(dtype)
-        strides = torch.empty(shape, memory_format=memory_format).stride() if len(shape) == 4 else \
-            torch.empty(shape).stride()
-        self.t = self.buf.as_strided(shape, strides, offset)
-        if fill is not None:
-            self.t.copy_(fill)
-        self.lo, self.hi = offset, offset + numel
-        self.slack = self._slack_bits().clone()
-
-    def _slack_bits(self):
-        bits = self.buf.view(torch.int16 if self.buf.element_size() == 2 else torch.int32)
-        return torch.cat([bits[:self.lo], bits[self.hi:]])
-
-    def intact(self):
-        return torch.equal(self._slack_bits(), self.slack)
 
 
 def _gen(seed):
@@ -194,12 +130,12 @@ def _make(shape, pdt, gdt, seed, offsets=(0, 0, 0), memory_format=torch.contiguo
     po, go, so = offsets
     n = int(np.prod(shape)) if len(shape) else 1
     rnd = lambda scale: (torch.randn(n, device='cuda', generator=g, dtype=torch.float64) * scale).reshape(shape)  # noqa: E731
-    slots = {'p': Slot(shape, pdt, po, memory_format, rnd(0.1)), 'g': Slot(shape, gdt, go, memory_format, rnd(1.0))}
+    slots = {'p': Slot(shape, pdt, po, rnd(0.1), memory_format), 'g': Slot(shape, gdt, go, rnd(1.0), memory_format)}
     if sgd:
-        slots['buf'] = Slot(shape, pdt, so, memory_format, rnd(0.5))
+        slots['buf'] = Slot(shape, pdt, so, rnd(0.5), memory_format)
     else:
-        slots['m'] = Slot(shape, torch.float32, so, memory_format, rnd(0.1))
-        slots['v'] = Slot(shape, torch.float32, so + 1, memory_format, rnd(0.1).square())
+        slots['m'] = Slot(shape, torch.float32, so, rnd(0.1), memory_format)
+        slots['v'] = Slot(shape, torch.float32, so + 1, rnd(0.1).square(), memory_format)
     return slots
 
 
@@ -208,26 +144,13 @@ def _intact(name, slots):
         assert s.intact(), f'{name}: the kernel wrote outside {k}'
 
 
-def _ops():
-    from horovod_b200 import ops
-    return ops
-
-
-@pytest.fixture(scope="module")
-def hvd():
-    import horovod_b200.torch as hvd
-    hvd.init()
-    torch.cuda.set_device(0)
-    yield hvd
-    hvd.shutdown()
-
-
 def run_sgd(tensors, pdt, **hp):
     """One fused SGD call over `tensors` (lists of slot dicts) and the reference check of every tensor."""
+    from horovod_b200 import ops
     has_mom = hp.get('momentum', 0.0) != 0.0
     before = [{k: s.t.double().clone() for k, s in sl.items()} for sl in tensors]
-    _ops().fused_sgd_step([sl['p'].t for sl in tensors], [sl['g'].t for sl in tensors],
-                          [sl['buf'].t for sl in tensors] if has_mom else [], **hp)
+    ops.fused_sgd_step([sl['p'].t for sl in tensors], [sl['g'].t for sl in tensors],
+                       [sl['buf'].t for sl in tensors] if has_mom else [], **hp)
     torch.cuda.synchronize()
     for i, (sl, b) in enumerate(zip(tensors, before)):
         p, buf, ps, bs = sgd_ref_kernel(b['p'], b['g'], b['buf'] if has_mom else None, **hp)
@@ -240,9 +163,10 @@ def run_sgd(tensors, pdt, **hp):
 
 
 def run_adam(tensors, pdt, **hp):
+    from horovod_b200 import ops
     before = [{k: s.t.double().clone() for k, s in sl.items()} for sl in tensors]
-    _ops().fused_adam_step([sl['p'].t for sl in tensors], [sl['g'].t for sl in tensors], [sl['m'].t for sl in tensors],
-                           [sl['v'].t for sl in tensors], **hp)
+    ops.fused_adam_step([sl['p'].t for sl in tensors], [sl['g'].t for sl in tensors], [sl['m'].t for sl in tensors],
+                        [sl['v'].t for sl in tensors], **hp)
     torch.cuda.synchronize()
     for i, (sl, b) in enumerate(zip(tensors, before)):
         p, m, v, ps, ms, vs = adam_ref_kernel(b['p'], b['g'], b['m'], b['v'], **hp)
@@ -252,11 +176,7 @@ def run_adam(tensors, pdt, **hp):
         _intact(f'adam[{i}] {hp}', sl)
 
 
-DTYPES = [(torch.float32, torch.float32), (torch.float32, torch.bfloat16), (torch.bfloat16, torch.bfloat16),
-          (torch.float16, torch.float16)]
 DTYPE_IDS = ['fp32-fp32', 'fp32-bf16', 'bf16-bf16', 'fp16-fp16']
-# around the 4-element vector, the 4096-element block (256 threads x 4 elements x 4 iterations) and a large tail
-COUNTS = [1, 3, 4, 5, 4095, 4096, 4097, 3 * 4096 + 1, (1 << 20) + 3]
 
 SGD_HP = dict(lr=0.05, momentum=0.9, dampening=0.5, weight_decay=1e-2, grad_scale=0.25)
 ADAM_HP = dict(lr=1e-2, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=1e-2)
@@ -267,7 +187,7 @@ ADAM_HP = dict(lr=1e-2, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=1e-2)
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("count", COUNTS)
-@pytest.mark.parametrize("dtypes", DTYPES, ids=DTYPE_IDS)
+@pytest.mark.parametrize("dtypes", PAIRS, ids=DTYPE_IDS)
 def test_sgd_dtypes_and_counts(hvd, dtypes, count):
     pdt, gdt = dtypes
     t = [_make((count,), pdt, gdt, seed=count, sgd=True)]
@@ -279,7 +199,7 @@ def test_sgd_dtypes_and_counts(hvd, dtypes, count):
 @pytest.mark.gpu
 @pytest.mark.parametrize("adamw", [True, False], ids=['adamw', 'adam'])
 @pytest.mark.parametrize("count", COUNTS)
-@pytest.mark.parametrize("dtypes", DTYPES, ids=DTYPE_IDS)
+@pytest.mark.parametrize("dtypes", PAIRS, ids=DTYPE_IDS)
 def test_adam_dtypes_and_counts(hvd, dtypes, count, adamw):
     pdt, gdt = dtypes
     t = [_make((count,), pdt, gdt, seed=count + 7)]
@@ -293,7 +213,7 @@ OFFSETS = [(1, 0, 0), (0, 1, 0), (0, 0, 1), (2, 0, 0), (0, 2, 2), (3, 3, 3), (0,
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("offsets", OFFSETS, ids=[f'p{a}g{b}s{c}' for a, b, c in OFFSETS])
-@pytest.mark.parametrize("dtypes", DTYPES, ids=DTYPE_IDS)
+@pytest.mark.parametrize("dtypes", PAIRS, ids=DTYPE_IDS)
 def test_unaligned_views(hvd, dtypes, offsets):
     pdt, gdt = dtypes
     for count in (5, 4097):
@@ -311,7 +231,7 @@ def _many_sizes():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("dtypes", DTYPES, ids=DTYPE_IDS)
+@pytest.mark.parametrize("dtypes", PAIRS, ids=DTYPE_IDS)
 def test_many_tensors_in_one_launch(hvd, dtypes):
     pdt, gdt = dtypes
     sizes = _many_sizes()
@@ -325,7 +245,7 @@ def test_many_tensors_in_one_launch(hvd, dtypes):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("dtypes", DTYPES, ids=DTYPE_IDS)
+@pytest.mark.parametrize("dtypes", PAIRS, ids=DTYPE_IDS)
 def test_channels_last(hvd, dtypes):
     pdt, gdt = dtypes
     cl = torch.channels_last
@@ -359,6 +279,7 @@ def test_adam_hyperparameters(hvd, pdt):
 @pytest.mark.parametrize("kind", ["sgd", "adam", "adamw"])
 def test_fp32_trajectory(hvd, kind):
     """10 steps of the kernel against 10 steps of the reference (parameters and moments stored as fp32 in between)."""
+    from horovod_b200 import ops
     n = (1 << 16) + 5
     sl = _make((n,), torch.float32, torch.float32, seed=11, offsets=(1, 2, 3), sgd=kind == 'sgd')
     ref = {k: s.t.double().clone() for k, s in sl.items()}
@@ -370,12 +291,12 @@ def test_fp32_trajectory(hvd, kind):
         sl['g'].t.copy_(g)
         if kind == 'sgd':
             hp = dict(lr=0.05, momentum=0.9, nesterov=True, weight_decay=1e-2)
-            _ops().fused_sgd_step([sl['p'].t], [sl['g'].t], [sl['buf'].t], first_step=step == 1, **hp)
+            ops.fused_sgd_step([sl['p'].t], [sl['g'].t], [sl['buf'].t], first_step=step == 1, **hp)
             p, buf, ps, _ = sgd_ref_kernel(ref['p'], g.double(), ref['buf'], first_step=step == 1, **hp)
             ref.update(p=p.float().double(), buf=buf.float().double())
         else:
             hp = dict(ADAM_HP, adamw=kind == 'adamw', step=step)
-            _ops().fused_adam_step([sl['p'].t], [sl['g'].t], [sl['m'].t], [sl['v'].t], **hp)
+            ops.fused_adam_step([sl['p'].t], [sl['g'].t], [sl['m'].t], [sl['v'].t], **hp)
             p, m, v, ps, _, _ = adam_ref_kernel(ref['p'], g.double(), ref['m'], ref['v'], **hp)
             ref.update(p=p.float().double(), m=m.float().double(), v=v.float().double())
         worst = torch.maximum(worst, ps)
@@ -398,7 +319,8 @@ def _rejects(hvd, fn, *args, **kw):
 
 @pytest.mark.gpu
 def test_adam_rejects_bad_arguments(hvd):
-    adam = _ops().fused_adam_step
+    from horovod_b200 import ops
+    adam = ops.fused_adam_step
     z = lambda n=64, dt=torch.float32, **kw: torch.zeros(n, device='cuda', dtype=dt, **kw)  # noqa: E731
     p, g = z(), z()
     p0 = p.clone()
@@ -429,7 +351,8 @@ def test_adam_rejects_bad_arguments(hvd):
 
 @pytest.mark.gpu
 def test_sgd_rejects_bad_arguments(hvd):
-    sgd = _ops().fused_sgd_step
+    from horovod_b200 import ops
+    sgd = ops.fused_sgd_step
     z = lambda n=64, dt=torch.float32: torch.zeros(n, device='cuda', dtype=dt)  # noqa: E731
     pb, gb = z(dt=torch.bfloat16), z(dt=torch.bfloat16)
     _rejects(hvd, sgd, [pb], [gb], [z()], lr=0.1, momentum=0.9)                  # momentum dtype != param dtype

@@ -5,40 +5,24 @@ unsharded fused update, and GraphedStep with k = 4 and the collectives captured 
 (capturable stand-ins), unsharded and sharded, against the eager loop; with >= 2 GPUs, across real ranks."""
 import copy
 import math
-import threading
 
 import pytest
 import torch
 
 from conftest import run_parallel
-from test_gpu_lamb import Slot, _ngpu, _same
-from test_gpu_sharded_clip import _FakeSet, _SimTeam
+from optim_cases import LOW, LOW_IDS, Slot, hvd, make_optimizer, mlp, ngpu, same  # noqa: F401  (hvd: fixture)
+from sim_ranks import (ConvNet, gteam, micro_batch, reduced_grads, ref_step, sharded_team, team,  # noqa: F401
+                       zero_copy_buckets)
 
 pytestmark = pytest.mark.gpu
 
-LOW = [torch.bfloat16, torch.float16]
-LOW_IDS = ['bf16', 'fp16']
 SIZES = [0, 1, 3, 4, 4093, (1 << 24) + 3]
-
-
-@pytest.fixture(scope="module")
-def hvd():
-    import horovod_b200.torch as hvd
-    hvd.init()
-    torch.cuda.set_device(0)
-    yield hvd
-    hvd.shutdown()
-
-
-def _ops():
-    from horovod_b200 import ops
-    return ops
 
 
 def _match(a, b):
     """Bit-identical where neither is NaN, NaN at the same places (NaN payloads are not compared)."""
     na, nb = torch.isnan(a), torch.isnan(b)
-    return torch.equal(na, nb) and _same(torch.where(na, 0, a), torch.where(nb, 0, b))
+    return torch.equal(na, nb) and same(torch.where(na, 0, a), torch.where(nb, 0, b))
 
 
 # ---- the kernel ---------------------------------------------------------------------------------------------------------
@@ -57,12 +41,12 @@ def _table(dtype, seed, offsets):
 @pytest.mark.parametrize("dtype", LOW, ids=LOW_IDS)
 @pytest.mark.parametrize("offsets", [(0, 0), (1, 0), (0, 3), (2, 1), (-1, -2)], ids=['aligned', 'g+1', 'acc+3', 'g+2-acc+1', 'mixed'])
 def test_kernel_modes_match_torch_fp32(hvd, dtype, offsets):
-    ops = _ops()
+    from horovod_b200 import ops
     grads, accs = _table(dtype, 3, offsets)
     g0, a0 = [s.t.clone() for s in grads], [s.t.clone() for s in accs]
     ops.grad_accumulate_([s.t for s in grads], [s.t for s in accs], 'first')
     for i, (g, a) in enumerate(zip(grads, accs)):
-        assert _same(a.t, g0[i].float()) and not bool(g.t.ne(0).any()) and not bool(g.t.signbit().any()), ('first', i)
+        assert same(a.t, g0[i].float()) and not bool(g.t.ne(0).any()) and not bool(g.t.signbit().any()), ('first', i)
     # add: a fresh gradient into the accumulator the 'first' fold left
     gen = torch.Generator(device='cuda').manual_seed(5)
     for g in grads:
@@ -70,21 +54,21 @@ def test_kernel_modes_match_torch_fp32(hvd, dtype, offsets):
     g1, a1 = [s.t.clone() for s in grads], [s.t.clone() for s in accs]
     ops.grad_accumulate_([s.t for s in grads], [s.t for s in accs], 'add')
     for i, (g, a) in enumerate(zip(grads, accs)):
-        assert _same(a.t, a1[i] + g1[i].float()) and not bool(g.t.ne(0).any()), ('add', i)
+        assert same(a.t, a1[i] + g1[i].float()) and not bool(g.t.ne(0).any()), ('add', i)
     for g in grads:
         g.t.copy_(torch.randn(g.t.shape, device='cuda', generator=gen))
     g2, a2 = [s.t.clone() for s in grads], [s.t.clone() for s in accs]
     ops.grad_accumulate_([s.t for s in grads], [s.t for s in accs], 'last')
     for i, (g, a) in enumerate(zip(grads, accs)):
-        assert _same(g.t, (a2[i] + g2[i].float()).to(dtype)), ('last', i)
-        assert _same(a.t, a2[i]), ('last wrote the accumulator', i)
+        assert same(g.t, (a2[i] + g2[i].float()).to(dtype)), ('last', i)
+        assert same(a.t, a2[i]), ('last wrote the accumulator', i)
     for s in grads + accs:
         assert s.intact(), 'wrote outside a tensor'
 
 
 @pytest.mark.parametrize("dtype", LOW, ids=LOW_IDS)
 def test_kernel_propagates_inf_nan_and_overflows_fp16_only_at_last(hvd, dtype):
-    ops = _ops()
+    from horovod_b200 import ops
     big = 6.0e4 if dtype == torch.float16 else 3.0e38
     g = torch.tensor([math.inf, -math.inf, math.nan, 1.0, big, -big, 2.0, 0.0] * 3, device='cuda').to(dtype)
     acc = torch.zeros(g.numel(), device='cuda')
@@ -105,7 +89,7 @@ def test_fp32_accumulation_rounds_once(hvd):
     """16 bf16 micro-gradients whose magnitudes fall from 1 to 2^-12 (every element keeps its sign, so nothing cancels):
     the fp32 path is within 1 bf16 ulp of the fp64 sum everywhere; summing in bf16, as autograd does into a bf16 p.grad,
     loses the small contributions and is off by more."""
-    ops = _ops()
+    from horovod_b200 import ops
     n = 1 << 16
     gen = torch.Generator(device='cuda').manual_seed(11)
     sign = torch.where(torch.rand(n, device='cuda', generator=gen) < 0.5, -1.0, 1.0)
@@ -126,7 +110,7 @@ def test_fp32_accumulation_rounds_once(hvd):
 
 
 def test_kernel_one_launch_no_sync_and_capturable(hvd):
-    ops = _ops()
+    from horovod_b200 import ops
     grads, accs = _table(torch.bfloat16, 9, (1, 2))
     gs, as_ = [s.t for s in grads], [s.t for s in accs]
     snap = [t.clone() for t in gs + as_]
@@ -152,11 +136,11 @@ def test_kernel_one_launch_no_sync_and_capturable(hvd):
         t.copy_(s)
     graph.replay()
     torch.cuda.synchronize()
-    assert all(_same(a, b) for a, b in zip(gs + as_, eager))
+    assert all(same(a, b) for a, b in zip(gs + as_, eager))
 
 
 def test_kernel_rejects_bad_arguments(hvd):
-    ops = _ops()
+    from horovod_b200 import ops
     g, a = torch.zeros(64, device='cuda', dtype=torch.bfloat16), torch.zeros(64, device='cuda')
     with pytest.raises(ValueError):
         ops.grad_accumulate_([g], [a], 'middle')
@@ -169,22 +153,6 @@ def test_kernel_rejects_bad_arguments(hvd):
 
 
 # ---- GraphedStep at world size 1 ----------------------------------------------------------------------------------------
-def _mlp(dtype, seed=0):
-    torch.manual_seed(seed)
-    return torch.nn.Sequential(torch.nn.Linear(24, 48), torch.nn.GELU(), torch.nn.LayerNorm(48),
-                               torch.nn.Linear(48, 8)).cuda().to(dtype)
-
-
-def _make(hvd, kind, params):
-    if kind == 'sgd':
-        return torch.optim.SGD(params, lr=0.05, momentum=0.9, weight_decay=1e-4)
-    if kind == 'adamw':
-        return torch.optim.AdamW(params, lr=1e-2, weight_decay=0.01)
-    if kind == 'lamb':
-        return hvd.Lamb(params, lr=1e-2, weight_decay=0.01)
-    return hvd.Lars(params, lr=0.5, momentum=0.9, weight_decay=1e-3, trust_coefficient=0.02)
-
-
 CASES = [('sgd', torch.float32, False), ('adamw', torch.float32, False), ('lamb', torch.float32, False),
          ('lars', torch.float32, False), ('adamw', torch.bfloat16, False), ('adamw', torch.bfloat16, True),
          ('lars', torch.bfloat16, False), ('lars', torch.bfloat16, True)]
@@ -192,12 +160,10 @@ CASE_IDS = ['sgd', 'adamw', 'lamb', 'lars', 'adamw-bf16', 'adamw-bf16-acc32', 'l
 
 
 def _run(hvd, kind, dt, acc, k, graphed, buckets=False, steps=3, monkeypatch=None):
-    if buckets:  # zero-copy buckets at world size 1: flat gradient buffers in plain device memory
-        from horovod_b200.torch import mpi_ops
-        monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-        monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-    m = _mlp(dt)
-    opt = hvd.DistributedOptimizer(_make(hvd, kind, m.parameters()), named_parameters=m.named_parameters(), fused=True,
+    if buckets:  # zero-copy buckets at world size 1
+        zero_copy_buckets(monkeypatch)
+    m = mlp(dt)
+    opt = hvd.DistributedOptimizer(make_optimizer(hvd, kind, m.parameters()), named_parameters=m.named_parameters(), fused=True,
                                    master_weights=dt != torch.float32, backward_passes_per_step=k,
                                    grad_accumulation_dtype=torch.float32 if acc else None)
     assert bool(opt._buckets) == buckets
@@ -231,14 +197,14 @@ def test_graphed_step_equals_eager_loop(hvd, monkeypatch, k, case):
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
     kind, dt, acc = case
     (a, oa, la), (b, ob, lb) = [_run(hvd, kind, dt, acc, k, graphed) for graphed in (False, True)]
-    assert all(_same(x, y) for x, y in zip(la, lb)), 'every call returns its own micro-batch loss'
+    assert all(same(x, y) for x, y in zip(la, lb)), 'every call returns its own micro-batch loss'
     for (name, p), q in zip(a.named_parameters(), b.parameters()):
-        assert _same(p.detach(), q.detach()), name
+        assert same(p.detach(), q.detach()), name
         sa, sb = oa.state[p], ob.state[q]
         assert sa.keys() == sb.keys()
         for key in sa:
             if torch.is_tensor(sa[key]) and sa[key].is_cuda:
-                assert _same(sa[key], sb[key]), (name, key)
+                assert same(sa[key], sb[key]), (name, key)
         if 'step' in sa:
             assert float(sa['step']) == float(sb['step']) == 3, 'one optimizer step per k calls'
     assert bool(ob._param_accs) == acc
@@ -251,10 +217,10 @@ def test_graphed_step_equals_eager_loop_with_buckets(hvd, monkeypatch, k, acc):
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
     (a, oa, la), (b, ob, lb) = [_run(hvd, 'lars', torch.bfloat16, acc, k, graphed, buckets=True, monkeypatch=monkeypatch)
                                 for graphed in (False, True)]
-    assert all(_same(x, y) for x, y in zip(la, lb))
+    assert all(same(x, y) for x, y in zip(la, lb))
     for (name, p), q in zip(a.named_parameters(), b.parameters()):
-        assert _same(p.detach(), q.detach()), name
-        assert _same(oa.state[p]['momentum_buffer'], ob.state[q]['momentum_buffer']), name
+        assert same(p.detach(), q.detach()), name
+        assert same(oa.state[p]['momentum_buffer'], ob.state[q]['momentum_buffer']), name
     assert all((bk['acc'] is not None) == acc for bk in ob._buckets)
 
 
@@ -264,20 +230,20 @@ def test_fp32_accumulation_differs_from_bf16_sum(hvd, monkeypatch):
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
     m16, _, _ = _run(hvd, 'lars', torch.bfloat16, False, 4, True, steps=2)
     m32, _, _ = _run(hvd, 'lars', torch.bfloat16, True, 4, True, steps=2)
-    assert not all(_same(p.detach(), q.detach()) for p, q in zip(m16.parameters(), m32.parameters()))
+    assert not all(same(p.detach(), q.detach()) for p, q in zip(m16.parameters(), m32.parameters()))
 
 
 def test_k1_with_fp32_accumulation_is_the_default(hvd, monkeypatch):
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
     (a, oa, la), (b, ob, lb) = [_run(hvd, 'adamw', torch.bfloat16, acc, 1, True) for acc in (False, True)]
     assert not ob._param_accs
-    assert all(_same(x, y) for x, y in zip(la, lb))
+    assert all(same(x, y) for x, y in zip(la, lb))
     for p, q in zip(a.parameters(), b.parameters()):
-        assert _same(p.detach(), q.detach())
+        assert same(p.detach(), q.detach())
 
 
 def test_changed_k_raises(hvd):
-    m = _mlp(torch.float32)
+    m = mlp(torch.float32)
     opt = hvd.DistributedOptimizer(torch.optim.SGD(m.parameters(), lr=0.1), named_parameters=m.named_parameters(),
                                    backward_passes_per_step=2)
     x = torch.randn(16, 24, device='cuda')
@@ -290,57 +256,7 @@ def test_changed_k_raises(hvd):
 
 
 # ---- sharded (ZeRO-1) on 4 simulated ranks ------------------------------------------------------------------------------
-@pytest.fixture
-def team(hvd, monkeypatch):
-    from horovod_b200.torch import mpi_ops
-    t = _SimTeam(4)
-    monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-    monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-    monkeypatch.setattr(mpi_ops, 'cross_size', lambda: 1)
-    monkeypatch.setattr(mpi_ops, 'captured_reducescatter_', t.reducescatter)
-    monkeypatch.setattr(mpi_ops, 'captured_allgather_', t.allgather)
-    monkeypatch.setattr(mpi_ops, 'captured_allreduce_', t.allreduce)
-    return t
-
-
-class _ConvNet(torch.nn.Module):
-    def __init__(self):
-        super().__init__()
-        self.conv = torch.nn.Conv2d(3, 8, 3)
-        self.fc = torch.nn.Linear(8 * 6 * 6, 10)
-
-    def forward(self, x):
-        return self.fc(torch.relu(self.conv(x)).flatten(1))
-
-
-def _batch(step, micro, r, dt):
-    g = torch.Generator(device='cuda').manual_seed(1000 * step + 10 * micro + r)
-    return torch.randn(5, 3, 8, 8, device='cuda', generator=g).to(dt), torch.randint(0, 10, (5,), device='cuda', generator=g)
-
-
-def _reduced_grads(opts, params):
-    from horovod_b200.torch.grad_buckets import full_from_shards
-    out = {}
-    for bi, b in enumerate(opts[0]._buckets):
-        full = torch.cat([o._buckets[bi]['gshard'] for o in opts])
-        for p, g in zip(b['params'], full_from_shards(b, [full], [p.shape for p in b['params']], [p.stride() for p in b['params']])):
-            out[p] = g
-    return [out[p] for p in params]
-
-
 K = 4
-
-
-def _sharded_team(hvd, team, kind, base, dt, master, acc):
-    models = [copy.deepcopy(base) for _ in range(team.n)]
-    opts = [hvd.DistributedOptimizer(_make(hvd, kind, m.parameters()), named_parameters=m.named_parameters(),
-                                     shard_optimizer_state=True, master_weights=master, process_set=_FakeSet(team.n, r),
-                                     bucket_cap_mb=0.01 * dt.itemsize / 4, backward_passes_per_step=K,
-                                     grad_accumulation_dtype=torch.float32 if acc else None)
-            for r, m in enumerate(models)]
-    team.opts = opts
-    assert len(opts[0]._buckets) > 1
-    return models, opts
 
 
 def _backward_all(team, models, opts, step, dt, scalers=None):
@@ -350,7 +266,7 @@ def _backward_all(team, models, opts, step, dt, scalers=None):
         opts[r].zero_grad()
         mine = len(team.log)
         for j in range(K):
-            x, y = _batch(step, j, r, dt)
+            x, y = micro_batch(step, j, r, dt)
             loss = torch.nn.functional.cross_entropy(models[r](x), y) / K
             (scalers[r].scale(loss) if scalers else loss).backward()
             if j < K - 1:
@@ -367,10 +283,12 @@ def test_sharded_accumulation_on_simulated_ranks(hvd, team, monkeypatch, kind, d
     unsharded fused on the reduced gradients, and every rank ends with the same parameters."""
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
     torch.manual_seed(0)
-    base = _ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
-    models, opts = _sharded_team(hvd, team, kind, base, dt, master, acc)
+    base = ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
+    models, opts = sharded_team(hvd, team, base, lambda m: make_optimizer(hvd, kind, m.parameters()), dt, min_buckets=2,
+                                master_weights=master, backward_passes_per_step=K,
+                                grad_accumulation_dtype=torch.float32 if acc else None)
     ref = copy.deepcopy(base)
-    ref_opt = hvd.DistributedOptimizer(_make(hvd, kind, ref.parameters()), named_parameters=ref.named_parameters(),
+    ref_opt = hvd.DistributedOptimizer(make_optimizer(hvd, kind, ref.parameters()), named_parameters=ref.named_parameters(),
                                        fused=True, master_weights=master, zero_copy=False)
     tol = dict(rtol=1e-5, atol=1e-6) if dt == torch.float32 else dict(rtol=1e-2, atol=1e-3)
     for step in range(3):
@@ -381,7 +299,7 @@ def test_sharded_accumulation_on_simulated_ranks(hvd, team, monkeypatch, kind, d
             sums = [torch.zeros_like(p, dtype=torch.float32 if acc else dt) for p in twin.parameters()]
             for j in range(K):
                 twin.zero_grad(set_to_none=True)
-                x, y = _batch(step, j, r, dt)
+                x, y = micro_batch(step, j, r, dt)
                 (torch.nn.functional.cross_entropy(twin(x), y) / K).backward()
                 for s, p in zip(sums, twin.parameters()):
                     s += p.grad.to(s.dtype)
@@ -389,23 +307,20 @@ def test_sharded_accumulation_on_simulated_ranks(hvd, team, monkeypatch, kind, d
         _backward_all(team, models, opts, step, dt)
         for r in range(team.n):  # before the reduction ran: the rank's own rounded sum sits in its gradient buckets
             for p, w in zip(models[r].parameters(), want[r]):
-                assert _same(p.grad, w), (step, r)
+                assert same(p.grad, w), (step, r)
         for o in opts:
             o.synchronize()
         team.flush()
-        grads = _reduced_grads(opts, list(models[0].parameters()))
+        grads = reduced_grads(opts, list(models[0].parameters()))
 
         def step_rank(r):
             with opts[r].skip_synchronize():
                 opts[r].step()
         team.run(step_rank)
-        ref_opt.zero_grad()
-        for p, g in zip(ref.parameters(), grads):
-            p.grad = g.clone()
-        ref_opt.step()
+        ref_step(ref, ref_opt, grads)
         for r in range(1, team.n):
             for a, b in zip(models[r].parameters(), models[0].parameters()):
-                assert _same(a.detach(), b.detach()), 'ranks differ after the allgather'
+                assert same(a.detach(), b.detach()), 'ranks differ after the allgather'
         for (name, a), b in zip(models[0].named_parameters(), ref.parameters()):
             torch.testing.assert_close(a.float(), b.float(), **tol, msg=lambda s: 'step %d %s: %s' % (step, name, s))
 
@@ -416,8 +331,9 @@ def test_sharded_accumulation_with_clip_and_scaler(hvd, team):
     the 'last' fold on rank 0 makes every rank skip and halves every scale."""
     n, dt = team.n, torch.float16
     torch.manual_seed(0)
-    base = _ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
-    models, opts = _sharded_team(hvd, team, 'lars', base, dt, True, True)
+    base = ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
+    models, opts = sharded_team(hvd, team, base, lambda m: make_optimizer(hvd, 'lars', m.parameters()), dt, min_buckets=2,
+                                master_weights=True, backward_passes_per_step=K, grad_accumulation_dtype=torch.float32)
     scalers = [hvd.ShardedGradScaler('cuda', init_scale=256.0) for _ in range(n)]
     for step in range(3):
         before = [s.get_scale() for s in scalers]
@@ -432,7 +348,7 @@ def test_sharded_accumulation_with_clip_and_scaler(hvd, team):
                         b0 = opts[0]._buckets[0]
                         b0['acc'][0] = 1.0e5
                         assert bool(torch.isfinite(b0['acc']).all())
-                    x, y = _batch(step, j, r, dt)
+                    x, y = micro_batch(step, j, r, dt)
                     scalers[r].scale(torch.nn.functional.cross_entropy(models[r](x), y) / K).backward()
         else:
             _backward_all(team, models, opts, step, dt, scalers)
@@ -440,136 +356,27 @@ def test_sharded_accumulation_with_clip_and_scaler(hvd, team):
         team.run(lambda r: scalers[r].unscale_(opts[r]))
         norms = team.run(lambda r: opts[r].clip_grad_norm_(0.05))
         assert team.count('rs', mark) == 0, 'the gradients were reduced once, after the last micro-step'
-        assert all(_same(x, norms[0]) for x in norms)
+        assert all(same(x, norms[0]) for x in norms)
         team.run(lambda r: (scalers[r].step(opts[r]), scalers[r].update()))
         if step == 1:
             assert all(s.get_scale() == before[0] / 2 for s in scalers)
-            assert all(_same(a.detach(), b) for a, b in zip(models[0].parameters(), params_before))
+            assert all(same(a.detach(), b) for a, b in zip(models[0].parameters(), params_before))
         else:
             assert all(s.get_scale() == before[0] for s in scalers)
-            assert float(norms[0]) > 0.05 and not all(_same(a.detach(), b) for a, b in zip(models[0].parameters(), params_before))
+            assert float(norms[0]) > 0.05 and not all(same(a.detach(), b) for a, b in zip(models[0].parameters(), params_before))
         for r in range(1, n):
             for a, b in zip(models[r].parameters(), models[0].parameters()):
-                assert _same(a.detach(), b.detach())
+                assert same(a.detach(), b.detach())
 
 
 # ---- GraphedStep on 4 simulated ranks, unsharded and sharded -----------------------------------------------------------
-class _GraphTeam(_SimTeam):
-    """_SimTeam with capturable stand-ins.  A collective issued while a CUDA graph is being captured records, inside the
-    graph, a copy of its tensor into a staging tensor of its own; after every rank replayed its graph, reduce_captured()
-    runs the recorded collectives on the ranks' staging copies with the same simulation kernels as flush() and copies
-    the results back into the tensors, which is what the in-place kernel would have left there.  Eager collectives are
-    queued as in _SimTeam; the gradient allreduce (op Average / Sum with scale factors) is supported as well."""
-
-    def __init__(self, n):
-        super().__init__(n)
-        self.captured = [[] for _ in range(n)]  # per rank: [kind, tensor, staging, arg, issued from the comm capture]
-        self.graph_runs = 0
-        self._graph_barrier = threading.Barrier(n, action=self.reduce_captured)
-
-    def _stand_in(self, r, kind, tensor, arg):
-        if torch.cuda.is_current_stream_capturing():
-            staging = torch.empty_like(tensor)
-            staging.copy_(tensor)
-            self.captured[r].append((kind, tensor, staging, arg, self.opts[r]._graph_capture is not None))
-            self.log.append(('captured-' + kind, r))
-        else:
-            self._issue(r, (kind, tensor, arg))
-
-    def reducescatter(self, tensor, op, prescale_factor, postscale_factor, process_set, max_ctas=0):
-        scale = prescale_factor * postscale_factor / (self.n if op == self.mpi_ops.Average else 1)
-        self._stand_in(process_set.r, 'rs', tensor, scale)
-
-    def allreduce(self, tensor, op=1, prescale_factor=1.0, postscale_factor=1.0, process_set=None, max_ctas=0):
-        if op in (self.mpi_ops.Average, self.mpi_ops.Sum) and (op == self.mpi_ops.Average or prescale_factor != 1.0
-                                                                or postscale_factor != 1.0):
-            scale = prescale_factor * postscale_factor / (self.n if op == self.mpi_ops.Average else 1)
-            self._stand_in(process_set.r, 'ars', tensor, scale)
-        else:
-            assert prescale_factor == postscale_factor == 1.0 and op in (self.mpi_ops.Sum, self.mpi_ops.Max)
-            self._stand_in(process_set.r, 'ar', tensor, op)
-        return tensor
-
-    def allreduce_async_(self, tensor, name=None, op=0, prescale_factor=1.0, postscale_factor=1.0, process_set=None):
-        """The unsharded optimizer's eager bucket allreduce; synchronize() of its handle is a no-op."""
-        self.allreduce(tensor, op, prescale_factor, postscale_factor, process_set)
-        return ('sim', name)
-
-    def _run(self, kind, ts, arg):
-        from horovod_b200.ops import sim
-        if kind == 'rs':
-            sim.inplace_reducescatter(ts, op=sim.SUM, scale=arg)
-        elif kind == 'ag':
-            sim.inplace_allgather(ts)
-        elif kind == 'ars':
-            sim.inplace_allreduce(ts, op=sim.SUM, scale=arg)
-        else:
-            sim.inplace_allreduce(ts, op=sim.SUM if arg == self.mpi_ops.Sum else sim.MAX)
-
-    def flush(self):
-        from horovod_b200.ops import kernel_launches
-        torch.cuda.synchronize()
-        before = kernel_launches()
-        assert len({len(q) for q in self.queues}) == 1, 'ranks issued different numbers of collectives'
-        for calls in zip(*self.queues):
-            assert len({(c[0], c[1].numel(), c[1].dtype, c[2]) for c in calls}) == 1, 'ranks issued different collectives'
-            self._run(calls[0][0], [c[1] for c in calls], calls[0][2])
-        torch.cuda.synchronize()
-        self.sim_launches += kernel_launches() - before
-        self.queues = [[] for _ in range(self.n)]
-
-    def reduce_captured(self):
-        torch.cuda.synchronize()
-        assert len({len(c) for c in self.captured}) == 1, 'ranks captured different numbers of collectives'
-        for calls in zip(*self.captured):
-            assert len({(c[0], c[1].numel(), c[1].dtype, c[3]) for c in calls}) == 1, 'ranks captured different collectives'
-            self._run(calls[0][0], [c[2] for c in calls], calls[0][3])
-            for c in calls:
-                c[1].copy_(c[2])
-            self.log.extend(('ran-' + calls[0][0], r) for r in range(self.n))
-        torch.cuda.synchronize()
-        self.graph_runs += 1
-
-    def before_step(self):
-        """Called by every rank's optimizer.step() after its last replay: the captured collectives run once all ranks
-        are there."""
-        self._graph_barrier.wait(timeout=120)
-
-
-@pytest.fixture
-def gteam(hvd, monkeypatch):
-    from horovod_b200.torch import mpi_ops, optimizer
-    t = _GraphTeam(4)
-    monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-    monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-    monkeypatch.setattr(mpi_ops, 'cross_size', lambda: 1)
-    monkeypatch.setattr(mpi_ops, 'captured_reducescatter_', t.reducescatter)
-    monkeypatch.setattr(mpi_ops, 'captured_allgather_', t.allgather)
-    monkeypatch.setattr(mpi_ops, 'captured_allreduce_', t.allreduce)
-    monkeypatch.setattr(optimizer, 'allreduce_async_', t.allreduce_async_)
-    monkeypatch.setattr(optimizer, 'synchronize', lambda handle: None)
-    # the ranks' agreement on the capture is a real allreduce over the process set: every simulated rank captures here
-    monkeypatch.setattr(hvd.GraphedStep, '_agree_across_ranks', lambda self: None)
-    monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
-    return t
-
-
-def _team_opts(hvd, team, kind, models, dt, shard):
-    master = dt != torch.float32
-    opts = [hvd.DistributedOptimizer(_make(hvd, kind, m.parameters()), named_parameters=m.named_parameters(), fused=True,
-                                     shard_optimizer_state=shard, master_weights=master, process_set=_FakeSet(team.n, r),
-                                     bucket_cap_mb=0.01 * dt.itemsize / 4, backward_passes_per_step=K,
-                                     grad_accumulation_dtype=torch.float32 if master else None)
-            for r, m in enumerate(models)]
-    team.opts = opts
-    assert len(opts[0]._buckets) > 1 and all(bool(o._buckets) for o in opts)
-    return opts
-
-
 def _team_run(hvd, team, kind, base, dt, shard, graphed, steps=3):
     n = team.n
-    models = [copy.deepcopy(base) for _ in range(n)]
-    opts = _team_opts(hvd, team, kind, models, dt, shard)
+    master = dt != torch.float32
+    models, opts = sharded_team(hvd, team, base, lambda m: make_optimizer(hvd, kind, m.parameters()), dt, min_buckets=2,
+                                shard_optimizer_state=shard, fused=True, master_weights=master, backward_passes_per_step=K,
+                                grad_accumulation_dtype=torch.float32 if master else None)
+    assert all(bool(o._buckets) for o in opts)
     nb = len(opts[0]._buckets)
     grad_kind = 'rs' if shard else 'ars'
     losses = [[] for _ in range(n)]
@@ -577,8 +384,7 @@ def _team_run(hvd, team, kind, base, dt, shard, graphed, steps=3):
     if graphed:
         gsteps = []
         for r in range(n):
-            team.opts = opts
-            gsteps.append(hvd.GraphedStep(fns[r], opts[r], _batch(0, 0, r, dt)))
+            gsteps.append(hvd.GraphedStep(fns[r], opts[r], micro_batch(0, 0, r, dt)))
             assert gsteps[r].captured and gsteps[r].comm_in_graph and len(gsteps[r].graphs) == 3, gsteps[r].fallback_reason
         # one collective per bucket, all of them recorded by the comm capture of the last graph
         assert all(len(c) == nb and all(x[0] == grad_kind and x[4] for x in c) for c in team.captured)
@@ -590,10 +396,10 @@ def _team_run(hvd, team, kind, base, dt, shard, graphed, steps=3):
         if graphed:
             for j in range(K - 1):
                 for r in range(n):
-                    losses[r].append(gsteps[r](*_batch(step, j, r, dt)).detach().clone())
+                    losses[r].append(gsteps[r](*micro_batch(step, j, r, dt)).detach().clone())
             assert team.count(grad_kind, mark) == team.count('ran-' + grad_kind, mark) == 0
             runs = team.graph_runs
-            out = team.run(lambda r: gsteps[r](*_batch(step, K - 1, r, dt)).detach().clone())
+            out = team.run(lambda r: gsteps[r](*micro_batch(step, K - 1, r, dt)).detach().clone())
             for r in range(n):
                 losses[r].append(out[r])
             assert team.graph_runs == runs + 1
@@ -602,7 +408,7 @@ def _team_run(hvd, team, kind, base, dt, shard, graphed, steps=3):
             for r in range(n):
                 opts[r].zero_grad(set_to_none=False)
                 for j in range(K):
-                    loss = fns[r](*_batch(step, j, r, dt))
+                    loss = fns[r](*micro_batch(step, j, r, dt))
                     loss.backward()
                     losses[r].append(loss.detach().clone())
             assert team.count(grad_kind, mark) == n * nb, 'one collective per bucket, rank and step'
@@ -616,7 +422,7 @@ def _team_run(hvd, team, kind, base, dt, shard, graphed, steps=3):
             team.run(step_rank)
         for r in range(1, n):
             for a, b in zip(models[r].parameters(), models[0].parameters()):
-                assert _same(a.detach(), b.detach()), 'ranks differ'
+                assert same(a.detach(), b.detach()), 'ranks differ'
     return models, opts, losses
 
 
@@ -628,7 +434,7 @@ def test_graphed_step_on_simulated_ranks(hvd, gteam, kind, dt):
     bucket's collective is recorded once per rank, by the last graph, and runs once per optimizer step; every rank ends
     with the same parameters, and the sharded run follows the unsharded one."""
     torch.manual_seed(0)
-    base = _ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
+    base = ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
     finals = {}
     for shard in (False, True):
         runs = []
@@ -637,20 +443,20 @@ def test_graphed_step_on_simulated_ranks(hvd, gteam, kind, dt):
             runs.append(_team_run(hvd, gteam, kind, base, dt, shard, graphed))
         (me, oe, le), (mg, og, lg) = runs
         for r in range(gteam.n):
-            assert all(_same(a, b) for a, b in zip(le[r], lg[r])), (shard, r, 'losses')
+            assert all(same(a, b) for a, b in zip(le[r], lg[r])), (shard, r, 'losses')
             for (name, a), b in zip(me[r].named_parameters(), mg[r].parameters()):
-                assert _same(a.detach(), b.detach()), (shard, r, name)
+                assert same(a.detach(), b.detach()), (shard, r, name)
         if shard:
             for be, bg in zip(oe[0]._buckets, og[0]._buckets):
                 for key in be['state']:
-                    assert _same(be['state'][key], bg['state'][key]), key
+                    assert same(be['state'][key], bg['state'][key]), key
                 if dt != torch.float32:
                     assert bg['acc'] is not None
         else:
             for pe, pg in zip(me[0].parameters(), mg[0].parameters()):
                 for key, t in oe[0].state[pe].items():
                     if torch.is_tensor(t) and t.is_cuda:
-                        assert _same(t, og[0].state[pg][key]), key
+                        assert same(t, og[0].state[pg][key]), key
             assert all((b['acc'] is not None) == (dt != torch.float32) for b in og[0]._buckets)
         finals[shard] = mg[0]
     tol = dict(rtol=1e-5, atol=1e-6) if dt == torch.float32 else dict(rtol=1e-2, atol=1e-3)
@@ -659,8 +465,8 @@ def test_graphed_step_on_simulated_ranks(hvd, gteam, kind, dt):
 
 
 # ---- real ranks ----------------------------------------------------------------------------------------------------------
-@pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
+@pytest.mark.skipif(ngpu() < 2, reason="needs >= 2 GPUs")
 def test_grad_accumulation_across_ranks(hvd):
-    n = 2 if _ngpu() < 4 else 4
+    n = 2 if ngpu() < 4 else 4
     rc, out = run_parallel("grad_accumulation_worker.py", np=n, timeout=420)
     assert "GRAD ACCUMULATION OK" in out, out[-4000:]

@@ -8,25 +8,11 @@ import math
 import pytest
 import torch
 
-from test_gpu_grad_accumulation import _GraphTeam, _batch, _make, _mlp
-from test_gpu_lamb import Slot, _same
-from test_gpu_sharded_clip import _FakeSet
+from conftest import run_parallel
+from optim_cases import Slot, hvd, make_optimizer, mlp, ngpu, same  # noqa: F401  (hvd: fixture)
+from sim_ranks import ConvNet, gteam, micro_batch, sharded_team, zero_copy_buckets  # noqa: F401  (gteam: fixture)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def hvd():
-    import horovod_b200.torch as hvd
-    hvd.init()
-    torch.cuda.set_device(0)
-    yield hvd
-    hvd.shutdown()
-
-
-def _ops():
-    from horovod_b200 import ops
-    return ops
 
 
 # ---- the statistics kernel on per-parameter gradients ---------------------------------------------------------------------
@@ -43,7 +29,7 @@ def _ragged(dtype, seed):
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16], ids=['fp32', 'bf16', 'fp16'])
 def test_stats_kernel_on_ragged_gradients(hvd, dtype):
-    ops = _ops()
+    from horovod_b200 import ops
     slots = _ragged(dtype, 3)
     views = [s.t for s in slots]
     want_sq = sum(float(v.double().square().sum()) for v in views)
@@ -60,7 +46,7 @@ def test_stats_kernel_on_ragged_gradients(hvd, dtype):
                 torch.cuda.set_sync_debug_mode(0)
             assert ops.kernel_launches() - before == 1, 'one launch per gradient dtype'
             outs.append(out)
-        assert _same(outs[0], outs[1]), 'the same input gives the same bits'
+        assert same(outs[0], outs[1]), 'the same input gives the same bits'
         assert abs(float(outs[0][0]) - want) <= 1e-5 * want, (norm_type, float(outs[0][0]), want)
         assert float(outs[0][1]) == 0.0
     # in-place unscale of a mixed-dtype list: one launch per dtype, the statistics of the stored values
@@ -71,15 +57,15 @@ def test_stats_kernel_on_ragged_gradients(hvd, dtype):
     before = ops.kernel_launches()
     ops.grad_shard_stats(mixed, out, inv_scale=inv)
     assert ops.kernel_launches() - before == 2
-    assert all(_same(v, w) for v, w in zip(mixed, want))
+    assert all(same(v, w) for v, w in zip(mixed, want))
     ref = sum(float(w.double().square().sum()) for w in want)
     assert abs(float(out[0]) - ref) <= 1e-5 * ref
     for s in slots:
-        assert _same(s._slack(), s.slack), 'the kernel wrote outside a tensor'
+        assert same(s._slack(), s.slack), 'the kernel wrote outside a tensor'
 
 
 def test_stats_kernel_flags_non_finite_in_a_large_tensor(hvd):
-    ops = _ops()
+    from horovod_b200 import ops
     g = [torch.ones(n, device='cuda') for n in (5, 31 * 1024 * 1024, 4097)]
     g[1][-1] = float('nan')
     out = torch.zeros(2, device='cuda')
@@ -88,13 +74,6 @@ def test_stats_kernel_flags_non_finite_in_a_large_tensor(hvd):
 
 
 # ---- the unsharded optimizer's clip_grad_norm_ ------------------------------------------------------------------------------
-def _with_buckets(monkeypatch):
-    """Zero-copy buckets at world size 1: flat gradient buffers in plain device memory."""
-    from horovod_b200.torch import mpi_ops
-    monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-    monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-
-
 def _xs(n, dt, seed=2):
     gen = torch.Generator(device='cuda').manual_seed(seed)
     return [torch.randn(16, 24, device='cuda', generator=gen).to(dt) for _ in range(n)]
@@ -111,13 +90,13 @@ def test_unsharded_clip_matches_torch(hvd, monkeypatch, kind, dt, buckets):
     on an fp32 copy fed the same gradients."""
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
     if buckets:
-        _with_buckets(monkeypatch)
-    m = _mlp(dt)
+        zero_copy_buckets(monkeypatch)
+    m = mlp(dt)
     ref = copy.deepcopy(m).float()
-    opt = hvd.DistributedOptimizer(_make(hvd, kind, m.parameters()), named_parameters=m.named_parameters(), fused=True,
+    opt = hvd.DistributedOptimizer(make_optimizer(hvd, kind, m.parameters()), named_parameters=m.named_parameters(), fused=True,
                                    master_weights=dt != torch.float32)
     assert bool(opt._buckets) == buckets
-    ropt = _make(hvd, kind, ref.parameters())
+    ropt = make_optimizer(hvd, kind, ref.parameters())
     tol = dict(rtol=1e-5, atol=1e-6) if dt == torch.float32 else dict(rtol=1e-2, atol=2e-3)
     for i, x in enumerate(_xs(5, dt)):
         opt.zero_grad()
@@ -143,8 +122,8 @@ def test_clip_below_max_norm_is_bit_identical_to_no_clip(hvd, monkeypatch, kind,
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
     runs = []
     for clip in (False, True):
-        m = _mlp(dt)
-        opt = hvd.DistributedOptimizer(_make(hvd, kind, m.parameters()), named_parameters=m.named_parameters(),
+        m = mlp(dt)
+        opt = hvd.DistributedOptimizer(make_optimizer(hvd, kind, m.parameters()), named_parameters=m.named_parameters(),
                                        fused=True, master_weights=dt != torch.float32)
         for x in _xs(3, dt):
             opt.zero_grad()
@@ -154,11 +133,11 @@ def test_clip_below_max_norm_is_bit_identical_to_no_clip(hvd, monkeypatch, kind,
             opt.step()
         runs.append(m)
     for a, b in zip(*[r.parameters() for r in runs]):
-        assert _same(a.detach(), b.detach())
+        assert same(a.detach(), b.detach())
 
 
 def test_unfused_clip_scales_grad_in_place(hvd):
-    m = _mlp(torch.float32)
+    m = mlp(torch.float32)
     ref = copy.deepcopy(m)
     opt = hvd.DistributedOptimizer(torch.optim.SGD(m.parameters(), lr=0.1, momentum=0.9),
                                    named_parameters=m.named_parameters(), fused=False)
@@ -194,14 +173,14 @@ MAX_NORM = 0.02  # below the model's gradient norm: every step clips
 
 
 def _opt(hvd, kind, m, dt, k, acc):
-    return hvd.DistributedOptimizer(_make(hvd, kind, m.parameters()), named_parameters=m.named_parameters(), fused=True,
+    return hvd.DistributedOptimizer(make_optimizer(hvd, kind, m.parameters()), named_parameters=m.named_parameters(), fused=True,
                                     master_weights=dt != torch.float32, backward_passes_per_step=k,
                                     grad_accumulation_dtype=torch.float32 if acc and k > 1 else None)
 
 
 def _clip_run(hvd, kind, dt, acc, k, mode, steps=3):
     """mode 'eager': the documented loop; 'graphed': GraphedStep(max_grad_norm); 'disabled': its eager fallback."""
-    m = _mlp(dt)
+    m = mlp(dt)
     opt = _opt(hvd, kind, m, dt, k, acc)
     xs = _xs(steps * k, dt)
     fn = lambda x: m(x).float().square().mean() / k  # noqa: E731
@@ -236,17 +215,17 @@ def test_graphed_clip_equals_eager_loop(hvd, monkeypatch, k, case):
     runs = [_clip_run(hvd, kind, dt, acc, k, mode) for mode in ('eager', 'graphed', 'disabled')]
     (a, oa, na) = runs[0]
     for b, ob, nb in runs[1:]:
-        assert all(_same(x, y) for x, y in zip(na, nb))
+        assert all(same(x, y) for x, y in zip(na, nb))
         for (name, p), q in zip(a.named_parameters(), b.parameters()):
-            assert _same(p.detach(), q.detach()), name
+            assert same(p.detach(), q.detach()), name
             for key in oa.state[p]:
                 if torch.is_tensor(oa.state[p][key]) and oa.state[p][key].is_cuda:
-                    assert _same(oa.state[p][key], ob.state[q][key]), (name, key)
+                    assert same(oa.state[p][key], ob.state[q][key]), (name, key)
 
 
 def test_graphed_clip_does_not_sync_with_the_host(hvd, monkeypatch):
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
-    m = _mlp(torch.float32)
+    m = mlp(torch.float32)
     opt = _opt(hvd, 'adamw', m, torch.float32, 1, False)
     xs = _xs(3, torch.float32)
     step = hvd.GraphedStep(lambda x: m(x).square().mean(), opt, (xs[0],), max_grad_norm=MAX_NORM)
@@ -263,7 +242,7 @@ def test_graphed_clip_does_not_sync_with_the_host(hvd, monkeypatch):
 
 # ---- fp16 autocast + GradScaler ----------------------------------------------------------------------------------------------
 def _amp_run(hvd, kind, graphed, overflow_step=1, steps=4):
-    m = _mlp(torch.float32)
+    m = mlp(torch.float32)
     opt = _opt(hvd, kind, m, torch.float32, 1, False)
     scaler = torch.amp.GradScaler('cuda', init_scale=2.0 ** 12)
     xs = _xs(steps, torch.float32)
@@ -303,45 +282,23 @@ def test_graphed_grad_scaler_equals_eager(hvd, monkeypatch, kind):
     monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
     eager, graphed = _amp_run(hvd, kind, False), _amp_run(hvd, kind, True)
     for i, (e, g) in enumerate(zip(eager, graphed)):
-        assert _same(e[0], g[0]) and e[1] == g[1], i
-        assert all(_same(a, b) for a, b in zip(e[2], g[2])), i
-        assert e[4].keys() == g[4].keys() and all(_same(e[4][k], g[4][k]) for k in e[4]), i
+        assert same(e[0], g[0]) and e[1] == g[1], i
+        assert all(same(a, b) for a, b in zip(e[2], g[2])), i
+        assert e[4].keys() == g[4].keys() and all(same(e[4][k], g[4][k]) for k in e[4]), i
     skipped = graphed[1]
     assert skipped[1] == graphed[0][1] / 2, 'the scale backs off on the overflowing step'
-    assert all(_same(a, b) for a, b in zip(skipped[2], skipped[3])), 'the skipped step leaves the parameters alone'
-    assert graphed[1][4].keys() == graphed[0][4].keys() and all(_same(graphed[0][4][k], graphed[1][4][k]) for k in graphed[0][4])
-    assert not all(_same(a, b) for a, b in zip(graphed[2][2], graphed[2][3])), 'the step after it updates'
+    assert all(same(a, b) for a, b in zip(skipped[2], skipped[3])), 'the skipped step leaves the parameters alone'
+    assert graphed[1][4].keys() == graphed[0][4].keys() and all(same(graphed[0][4][k], graphed[1][4][k]) for k in graphed[0][4])
+    assert not all(same(a, b) for a, b in zip(graphed[2][2], graphed[2][3])), 'the step after it updates'
 
 
 # ---- sharded (ZeRO-1) on 4 simulated ranks -----------------------------------------------------------------------------------
-@pytest.fixture
-def gteam(hvd, monkeypatch):
-    from horovod_b200.torch import mpi_ops, optimizer
-    t = _GraphTeam(4)
-    monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-    monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-    monkeypatch.setattr(mpi_ops, 'cross_size', lambda: 1)
-    monkeypatch.setattr(mpi_ops, 'captured_reducescatter_', t.reducescatter)
-    monkeypatch.setattr(mpi_ops, 'captured_allgather_', t.allgather)
-    monkeypatch.setattr(mpi_ops, 'captured_allreduce_', t.allreduce)
-    monkeypatch.setattr(optimizer, 'allreduce_async_', t.allreduce_async_)
-    monkeypatch.setattr(optimizer, 'synchronize', lambda handle: None)
-    monkeypatch.setattr(hvd.GraphedStep, '_agree_across_ranks', lambda self: None)
-    monkeypatch.setattr(torch.backends.cudnn, 'deterministic', True)
-    return t
-
-
 def _sharded_run(hvd, team, kind, k, graphed, steps=3):
     n = team.n
     torch.manual_seed(0)
-    from test_gpu_grad_accumulation import _ConvNet
-    base = _ConvNet().cuda().to(memory_format=torch.channels_last)
-    models = [copy.deepcopy(base) for _ in range(n)]
-    opts = [hvd.DistributedOptimizer(_make(hvd, kind, m.parameters()), named_parameters=m.named_parameters(),
-                                     shard_optimizer_state=True, process_set=_FakeSet(n, r), bucket_cap_mb=0.01,
-                                     backward_passes_per_step=k) for r, m in enumerate(models)]
-    team.opts = opts
-    assert len(opts[0]._buckets) > 1
+    base = ConvNet().cuda().to(memory_format=torch.channels_last)
+    models, opts = sharded_team(hvd, team, base, lambda m: make_optimizer(hvd, kind, m.parameters()), min_buckets=2,
+                                backward_passes_per_step=k)
     scalers = [hvd.ShardedGradScaler('cuda', init_scale=256.0) for _ in range(n)]
     fns = [lambda x, y, m=m: torch.nn.functional.cross_entropy(m(x), y) / k for m in models]
     norms = [[] for _ in range(n)]
@@ -349,7 +306,7 @@ def _sharded_run(hvd, team, kind, k, graphed, steps=3):
         orig = o.clip_grad_norm_
         o.clip_grad_norm_ = lambda *a, orig=orig, r=r, **kw: norms[r].append(orig(*a, **kw).clone()) or norms[r][-1]
     if graphed:
-        gsteps = [hvd.GraphedStep(fns[r], opts[r], _batch(0, 0, r, torch.float32), max_grad_norm=0.05, scaler=scalers[r])
+        gsteps = [hvd.GraphedStep(fns[r], opts[r], micro_batch(0, 0, r, torch.float32), max_grad_norm=0.05, scaler=scalers[r])
                   for r in range(n)]
         assert all(g.captured and g.comm_in_graph for g in gsteps), gsteps[0].fallback_reason
         for r, o in enumerate(opts):  # the captured reduce-scatters run once every rank replayed its last graph
@@ -359,13 +316,13 @@ def _sharded_run(hvd, team, kind, k, graphed, steps=3):
         if graphed:
             for j in range(k - 1):
                 for r in range(n):
-                    gsteps[r](*_batch(step, j, r, torch.float32))
-            team.run(lambda r: gsteps[r](*_batch(step, k - 1, r, torch.float32)))
+                    gsteps[r](*micro_batch(step, j, r, torch.float32))
+            team.run(lambda r: gsteps[r](*micro_batch(step, k - 1, r, torch.float32)))
         else:
             for r in range(n):
                 opts[r].zero_grad()
                 for j in range(k):
-                    scalers[r].scale(fns[r](*_batch(step, j, r, torch.float32))).backward()
+                    scalers[r].scale(fns[r](*micro_batch(step, j, r, torch.float32))).backward()
             team.flush()
 
             def update(r):
@@ -377,9 +334,9 @@ def _sharded_run(hvd, team, kind, k, graphed, steps=3):
                 scalers[r].update()
             team.run(update)
         for r in range(1, n):
-            assert _same(norms[r][-1], norms[0][-1]), 'the norm differs between ranks'
+            assert same(norms[r][-1], norms[0][-1]), 'the norm differs between ranks'
             for a, b in zip(models[r].parameters(), models[0].parameters()):
-                assert _same(a.detach(), b.detach()), 'ranks differ'
+                assert same(a.detach(), b.detach()), 'ranks differ'
     return models[0], norms[0]
 
 
@@ -389,15 +346,14 @@ def test_sharded_graphed_clip_and_scaler_on_simulated_ranks(hvd, gteam, kind, k)
     a, na = _sharded_run(hvd, gteam, kind, k, graphed=False)
     b, nb = _sharded_run(hvd, gteam, kind, k, graphed=True)
     assert len(na) == len(nb) == 3 and all(float(x) > 0.05 for x in na)
-    assert all(_same(x, y) for x, y in zip(na, nb))
+    assert all(same(x, y) for x, y in zip(na, nb))
     for p, q in zip(a.parameters(), b.parameters()):
-        assert _same(p.detach(), q.detach())
+        assert same(p.detach(), q.detach())
 
 
 # ---- across real ranks ---------------------------------------------------------------------------------------------------
-@pytest.mark.skipif(torch.cuda.device_count() < 2 if torch.cuda.is_available() else True, reason="needs >= 2 GPUs")
+@pytest.mark.skipif(ngpu() < 2, reason="needs >= 2 GPUs")
 def test_graphed_clip_across_ranks(native_built):
-    from conftest import run_parallel
-    n = 2 if torch.cuda.device_count() < 4 else 4
+    n = 2 if ngpu() < 4 else 4
     rc, out = run_parallel("graphed_clip_worker.py", np=n, timeout=420)
     assert "GRAPHED CLIP OK" in out, out[-4000:]

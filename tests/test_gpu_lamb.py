@@ -11,16 +11,12 @@ import pytest
 import torch
 
 from conftest import run_parallel
-from test_gpu_sharded_clip import _FakeSet, _SimTeam
+from optim_cases import (LOW, LOW_IDS, PAIR_IDS, PAIRS, SIZES, Slot, cat, f32, hvd, mlp, mlp_loss, ngpu,  # noqa: F401
+                         same, two_phase, ulp)
+from sim_ranks import FakeSet, NormConvNet, batch, reduced_grads, ref_step, sharded_team, step_all, team  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-PAIRS = [(torch.float32, torch.float32), (torch.float32, torch.bfloat16), (torch.bfloat16, torch.bfloat16),
-         (torch.float16, torch.float16)]
-PAIR_IDS = ['f32', 'f32-bf16g', 'bf16', 'fp16']
-LOW = [torch.bfloat16, torch.float16]
-LOW_IDS = ['bf16', 'fp16']
-SIZES = [1, 3, 4095, 4096, 4097, (1 << 20) + 3]
 HP = [dict(lr=1e-2, beta1=0.9, beta2=0.999, eps=1e-6, weight_decay=0.01),
       dict(lr=2e-3, beta1=0.8, beta2=0.99, eps=1e-3, weight_decay=0.1, bias_correction=False),
       dict(lr=1e-2, beta1=0.9, beta2=0.999, eps=1e-6, weight_decay=0.0, adapt=False, grad_scale=0.5),
@@ -28,52 +24,6 @@ HP = [dict(lr=1e-2, beta1=0.9, beta2=0.999, eps=1e-6, weight_decay=0.01),
 # Depth of the fp32 sums of squares in the kernel: 16 fmas per thread, a 5-level shuffle tree, 8 warps in order (the
 # per-CTA partials are then added in fp64).  A sum of k non-negative fp32 terms has a relative error below k * 2^-24.
 NORM_RTOL = (16 + 5 + 8) * 2.0 ** -24
-
-
-def _ngpu():
-    return torch.cuda.device_count() if torch.cuda.is_available() else 0
-
-
-@pytest.fixture(scope="module")
-def hvd():
-    import horovod_b200.torch as hvd
-    hvd.init()
-    torch.cuda.set_device(0)
-    yield hvd
-    hvd.shutdown()
-
-
-def _ops():
-    from horovod_b200 import ops
-    return ops
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int16 if t.element_size() == 2 else torch.int32)
-
-
-def _same(a, b):
-    return a.dtype == b.dtype and a.shape == b.shape and torch.equal(_bits(a), _bits(b))
-
-
-class Slot:
-    """A tensor at element `offset` of a larger buffer; the slack around it must come back unchanged."""
-
-    def __init__(self, shape, dtype, offset, fill, memory_format=torch.contiguous_format, slack=67):
-        numel = int(np.prod(shape))
-        self.buf = torch.randn(offset + numel + slack, device='cuda').to(dtype)
-        strides = torch.empty(shape, memory_format=memory_format).stride() if len(shape) == 4 else torch.empty(shape).stride()
-        self.t = self.buf.as_strided(shape, strides, offset)
-        self.t.copy_(fill)
-        self.lo, self.hi = offset, offset + numel
-        self.slack = self._slack().clone()
-
-    def _slack(self):
-        b = _bits(self.buf)
-        return torch.cat([b[:self.lo], b[self.hi:]])
-
-    def intact(self):
-        return torch.equal(self._slack(), self.slack)
 
 
 def _case(shape, pdt, gdt, seed, offsets=(0, 0, 0), memory_format=torch.contiguous_format, master=False):
@@ -89,47 +39,32 @@ def _case(shape, pdt, gdt, seed, offsets=(0, 0, 0), memory_format=torch.contiguo
     return c
 
 
-def _f32(x):
-    return float(np.float32(x))
-
-
 def _ref(cases, lr, beta1, beta2, eps, weight_decay, step, bias_correction=True, adapt=True, grad_scale=1.0):
     """fp64 LAMB from the values the kernel reads (parameter and gradient in their dtypes, fp32 moments) and the
     hyper-parameters as the kernel holds them (fp32).  'scale_*' bound the magnitudes that fp32 rounding errors are
     relative to."""
     out = []
-    b1, b2, lr, eps, wd = _f32(beta1), _f32(beta2), _f32(lr), _f32(eps), _f32(weight_decay)
+    b1, b2, lr, eps, wd = f32(beta1), f32(beta2), f32(lr), f32(eps), f32(weight_decay)
     # as the binding forms them (and fused Adam's): 1 - (beta^step rounded to fp32), in fp32
     c1, c2 = (float(np.float32(1) - np.float32(beta1 ** step)), float(np.float32(1) - np.float32(beta2 ** step))) \
         if bias_correction else (1.0, 1.0)
     for c in cases:
-        w, g = c['p'].t.double(), c['g'].t.double() * _f32(grad_scale)
+        w, g = c['p'].t.double(), c['g'].t.double() * f32(grad_scale)
         mo, vo = c['m'].t.double(), c['v'].t.double()
-        m = b1 * mo + _f32(1 - b1) * g
-        v = b2 * vo + _f32(1 - b2) * g * g
+        m = b1 * mo + f32(1 - b1) * g
+        v = b2 * vo + f32(1 - b2) * g * g
         adam = (m / c1) / ((v / c2).sqrt() + eps)
         u = adam + wd * w
         wn, un = float(w.norm()), float(u.norm())
         r = wn / un if adapt and wn > 0 and un > 0 else 1.0
-        scale_m = (b1 * mo).abs() + (_f32(1 - b1) * g).abs()  # >= |m|: m's rounding errors are relative to this
+        scale_m = (b1 * mo).abs() + (f32(1 - b1) * g).abs()  # >= |m|: m's rounding errors are relative to this
         scale_u = (scale_m / c1) / ((v / c2).sqrt() + eps) + (wd * w).abs()
         out.append({'w': w - lr * r * u, 'm': m, 'v': v, 'scale_m': scale_m, 'scale_u': lr * r * scale_u})
     return out
 
 
-def _ulp(x, dtype):
-    """The spacing of `dtype` at |x| (fp64 tensor), subnormals included."""
-    mant, emin = {torch.bfloat16: (7, -126), torch.float16: (10, -14), torch.float32: (23, -126)}[dtype]
-    e = torch.floor(torch.log2(x.abs().clamp(min=2.0 ** emin))).clamp(min=emin)
-    return torch.pow(2.0, e - mant)
-
-
-def _cat(ts):
-    return torch.cat([t.reshape(-1) for t in ts])
-
-
 def _run_and_check(cases, hp, step):
-    ops = _ops()
+    from horovod_b200 import ops
     pdt = cases[0]['p'].t.dtype
     hp = dict(hp)
     want = _ref(cases, step=step, **hp)
@@ -137,23 +72,23 @@ def _run_and_check(cases, hp, step):
     ops.fused_lamb_step([c['p'].t for c in cases], [c['g'].t for c in cases], [c['m'].t for c in cases],
                         [c['v'].t for c in cases], step=step, **hp)
     torch.cuda.synchronize()
-    e = {k: _cat([x[k] for x in want]) for k in want[0]}
-    got = {k: _cat([c[k].t.double() for c in cases]) for k in ('p', 'm', 'v')}
+    e = {k: cat([x[k] for x in want]) for k in want[0]}
+    got = {k: cat([c[k].t.double() for c in cases]) for k in ('p', 'm', 'v')}
     # the moments: two or three fp32 roundings of non-cancelling terms (v) or of terms bounded by scale_m (m)
     assert bool(((got['m'] - e['m']).abs() <= 4 * 2.0 ** -24 * e['scale_m']).all())
     assert bool(((got['v'] - e['v']).abs() <= 4 * 2.0 ** -24 * e['v']).all())
     err = (got['p'] - e['w']).abs()
     # the fp32 result: r is off by at most NORM_RTOL (plus the norms' share of u's own error), u by a few fp32 roundings
     # of its terms, and the result is rounded once
-    tol = e['scale_u'] * (NORM_RTOL + 32 * 2.0 ** -24) + _ulp(e['w'], torch.float32)
+    tol = e['scale_u'] * (NORM_RTOL + 32 * 2.0 ** -24) + ulp(e['w'], torch.float32)
     if pdt != torch.float32:
         # then rounded to nearest in the parameter dtype: one ulp of it (the fp32 bound only matters where w - lr r u
         # cancels to far below |w|)
-        tol = tol + _ulp(e['w'], pdt)
+        tol = tol + ulp(e['w'], pdt)
     bad = err > tol
     assert not bool(bad.any()), (int(bad.sum()), float((err - tol).max()))
     for i, c in enumerate(cases):
-        assert _same(c['g'].t, g_before[i]), (i, 'grad written')
+        assert same(c['g'].t, g_before[i]), (i, 'grad written')
         for k, s in c.items():
             assert s.intact(), (i, 'wrote outside ' + k)
 
@@ -181,19 +116,6 @@ def test_kernel_unaligned_views(hvd, pair, offsets):
     _run_and_check(cases, HP[0], 3)
 
 
-def _two_phase(cases, master, slots=None, out=None, gsd=None, **hp):
-    """lamb_norms then lamb_apply over `cases`; returns the norms buffer."""
-    ops = _ops()
-    lists = [[c[k].t for c in cases] for k in ('p', 'g', 'm', 'v')]
-    ws = [c['w'].t for c in cases] if master else None
-    out = torch.zeros(2 * len(cases), device='cuda') if out is None else out
-    ops.lamb_norms(*lists, hp['beta1'], hp['beta2'], hp['eps'], hp['weight_decay'], hp['step'], out, slots=slots,
-                   grad_scale_dev=gsd, master_params=ws)
-    ops.lamb_apply(*lists, hp['lr'], hp['beta1'], hp['beta2'], hp['eps'], hp['weight_decay'], hp['step'], out, slots=slots,
-                   master_params=ws)
-    return out
-
-
 @pytest.mark.parametrize("pdt", LOW, ids=LOW_IDS)
 def test_master_kernels_equal_fp32_kernels(hvd, pdt):
     """Masters, moments and norms bit-identical to the fp32-parameter kernel started from the masters; parameters the
@@ -207,8 +129,8 @@ def test_master_kernels_equal_fp32_kernels(hvd, pdt):
         c['p'].t.reshape(-1)[::2] = 0.125  # an outside write: these elements restart from the parameter
     start = []
     for c in cases:
-        same = c['w'].t.to(pdt).view(torch.int16) == c['p'].t.view(torch.int16)
-        start.append(torch.where(same, c['w'].t, c['p'].t.float()))
+        kept = c['w'].t.to(pdt).view(torch.int16) == c['p'].t.view(torch.int16)
+        start.append(torch.where(kept, c['w'].t, c['p'].t.float()))
     ref = [{'p': Slot(s.shape, torch.float32, 0, s, torch.channels_last if s.dim() == 4 else torch.contiguous_format),
             'g': Slot(s.shape, torch.bfloat16 if pdt == torch.bfloat16 else torch.float32, 0, c['g'].t,
                       torch.channels_last if s.dim() == 4 else torch.contiguous_format),
@@ -216,21 +138,21 @@ def test_master_kernels_equal_fp32_kernels(hvd, pdt):
             'v': Slot(s.shape, torch.float32, 0, c['v'].t, torch.channels_last if s.dim() == 4 else torch.contiguous_format)}
            for c, s in zip(cases, start)]
     g_before = [c['g'].t.clone() for c in cases]
-    norms = _two_phase(cases, True, gsd=gsd, **hp)
-    ref_norms = _two_phase(ref, False, gsd=gsd, **hp)
+    norms = two_phase('lamb', cases, True, gsd=gsd, **hp)
+    ref_norms = two_phase('lamb', ref, False, gsd=gsd, **hp)
     torch.cuda.synchronize()
-    assert _same(norms, ref_norms)
+    assert same(norms, ref_norms)
     for i, (c, r) in enumerate(zip(cases, ref)):
-        assert _same(c['w'].t, r['p'].t), (i, 'master')
-        assert _same(c['p'].t, r['p'].t.to(pdt)), (i, 'param is not the rounded master')
-        assert _same(c['m'].t, r['m'].t) and _same(c['v'].t, r['v'].t), (i, 'moments')
-        assert _same(c['g'].t, g_before[i])
+        assert same(c['w'].t, r['p'].t), (i, 'master')
+        assert same(c['p'].t, r['p'].t.to(pdt)), (i, 'param is not the rounded master')
+        assert same(c['m'].t, r['m'].t) and same(c['v'].t, r['v'].t), (i, 'moments')
+        assert same(c['g'].t, g_before[i])
         for k, s in c.items():
             assert s.intact(), (i, 'wrote outside ' + k)
 
 
 def test_deterministic_no_host_sync_and_fixed_launch_count(hvd):
-    ops = _ops()
+    from horovod_b200 import ops
     for n in (5, 200):
         cases = [_case(((1 << 20) + 3 if i == 0 else 1000 + i,), torch.float32, torch.float32, seed=i) for i in range(n)]
         snap = [{k: s.t.clone() for k, s in c.items()} for c in cases]
@@ -251,7 +173,7 @@ def test_deterministic_no_host_sync_and_fixed_launch_count(hvd):
             assert ops.kernel_launches() - before == 3, 'moments + partials, norms, update: independent of the tensor count'
             torch.cuda.synchronize()
             results.append([c[k].t.clone() for c in cases for k in ('p', 'm', 'v')])
-        assert all(_same(a, b) for a, b in zip(*results))
+        assert all(same(a, b) for a, b in zip(*results))
 
 
 @pytest.mark.parametrize("pair", PAIRS, ids=PAIR_IDS)
@@ -259,7 +181,7 @@ def test_grad_scale_dev(hvd, pair):
     """A device factor of 1 is bit-identical to none; a factor k equals gradients scaled by k (k = 4: exact in every
     gradient dtype, fp16 subnormals included, where 1/4 would not be)."""
     pdt, gdt = pair
-    ops = _ops()
+    from horovod_b200 import ops
 
     def run(gscale=1.0, **kw):
         cases = [_case((n,), pdt, gdt, seed=i) for i, n in enumerate([1, 4097, 1 << 16])]
@@ -273,13 +195,13 @@ def test_grad_scale_dev(hvd, pair):
     plain, one = run(), run(grad_scale_dev=torch.ones(1, device='cuda'))
     scaled, dev = run(gscale=4.0), run(grad_scale_dev=torch.tensor([4.0], device='cuda'))
     host = run(grad_scale=4.0)
-    assert all(_same(a, b) for a, b in zip(plain, one))
-    assert all(_same(a, b) and _same(a, c) for a, b, c in zip(scaled, dev, host))
-    assert not all(_same(a, b) for a, b in zip(plain, scaled))
+    assert all(same(a, b) for a, b in zip(plain, one))
+    assert all(same(a, b) and same(a, c) for a, b, c in zip(scaled, dev, host))
+    assert not all(same(a, b) for a, b in zip(plain, scaled))
 
 
 def test_rejects_bad_arguments(hvd):
-    ops = _ops()
+    from horovod_b200 import ops
     z = lambda n=64, dt=torch.float32: torch.zeros(n, device='cuda', dtype=dt)  # noqa: E731
     pb, gb = z(dt=torch.bfloat16), z(dt=torch.bfloat16)
     hp = (1e-3, 0.9, 0.999, 1e-6, 0.01)
@@ -315,18 +237,6 @@ def test_rejects_bad_arguments(hvd):
 
 
 # ---- DistributedOptimizer at world size 1 -------------------------------------------------------------------------------
-def _mlp(dtype, seed=0):
-    torch.manual_seed(seed)
-    return torch.nn.Sequential(torch.nn.Linear(24, 48), torch.nn.GELU(), torch.nn.LayerNorm(48),
-                               torch.nn.Linear(48, 8)).cuda().to(dtype)
-
-
-def _loss(m, step, dtype):
-    g = torch.Generator(device='cuda').manual_seed(step)
-    x = torch.randn(16, 24, device='cuda', generator=g).to(dtype)
-    return m(x).float().square().mean()
-
-
 def _lamb(hvd, m):
     """BERT-style groups: weight decay on the matrices, none (so no trust ratio) on biases and LayerNorm; the always_adapt
     group covers the other branch."""
@@ -341,7 +251,7 @@ def test_fused_optimizer_follows_lamb_step(hvd):
     """fused=True against Lamb.step over 10 steps: broadcast_optimizer_state first, the last Linear frozen for 3 steps
     (its own step count), step(closure) twice."""
     dt = torch.float32
-    m = _mlp(dt)
+    m = mlp(dt)
     twin = copy.deepcopy(m)
     for x in (m, twin):
         x[3].requires_grad_(False)  # before the optimizer is built: it gets no gradient bucket, so no zero gradient
@@ -356,9 +266,9 @@ def test_fused_optimizer_follows_lamb_step(hvd):
                 x[3].requires_grad_(True)
         opt.zero_grad(set_to_none=True)
         ref.zero_grad(set_to_none=True)
-        loss = _loss(m, step, dt)
+        loss = mlp_loss(m, step, dt)
         loss.backward()
-        _loss(twin, step, dt).backward()
+        mlp_loss(twin, step, dt).backward()
         before = hvd.runtime_stats()['kernel_launches']
         if step in (2, 6):
             assert opt.step(lambda: loss) is loss
@@ -380,13 +290,13 @@ def test_checkpoint_round_trip_is_bit_exact(hvd, monkeypatch):
     dt = torch.bfloat16
 
     def fresh():
-        m = _mlp(dt)
+        m = mlp(dt)
         return m, hvd.DistributedOptimizer(_lamb(hvd, m), named_parameters=m.named_parameters(), fused=True)
 
     def train(m, o, steps):
         for s in steps:
             o.zero_grad()
-            _loss(m, s, dt).backward()
+            mlp_loss(m, s, dt).backward()
             o.step()
 
     ma, oa = fresh()
@@ -403,30 +313,30 @@ def test_checkpoint_round_trip_is_bit_exact(hvd, monkeypatch):
     assert all(oc.state[p]['exp_avg'].dtype == torch.float32 for p in mc.parameters())  # not cast to bf16
     train(mc, oc, range(3, 6))
     for (name, a), c in zip(ma.named_parameters(), mc.parameters()):
-        assert _same(a.detach(), c.detach()), name
+        assert same(a.detach(), c.detach()), name
         for key in ('exp_avg', 'exp_avg_sq'):
-            assert _same(oa.state[a][key], oc.state[c][key]), (name, key)
+            assert same(oa.state[a][key], oc.state[c][key]), (name, key)
 
 
 def test_bf16_master_weights_follow_fp32_twin(hvd):
     """A bf16 model with master_weights=True and an fp32 twin on the fused fp32 kernel, fed the same gradients: the
     masters equal the twin's parameters bit for bit, the parameters are the rounded masters."""
     dt = torch.bfloat16
-    m = _mlp(dt)
+    m = mlp(dt)
     twin = copy.deepcopy(m).float()
     opt = hvd.DistributedOptimizer(_lamb(hvd, m), named_parameters=m.named_parameters(), master_weights=True)
     topt = hvd.DistributedOptimizer(_lamb(hvd, twin), named_parameters=twin.named_parameters(), fused=True)
     for step in range(6):
         opt.zero_grad(set_to_none=True)
         topt.zero_grad(set_to_none=True)
-        _loss(m, step, dt).backward()
+        mlp_loss(m, step, dt).backward()
         for q, p in zip(twin.parameters(), m.parameters()):
             q.grad = p.grad.float()
         opt.step()
         topt.step()
         for (name, p), q in zip(m.named_parameters(), twin.parameters()):
-            assert _same(opt.state[p]['master_param'], q.detach()), (name, step)
-            assert _same(p.detach(), q.detach().to(dt)), (name, step)
+            assert same(opt.state[p]['master_param'], q.detach()), (name, step)
+            assert same(p.detach(), q.detach().to(dt)), (name, step)
 
 
 def test_unfusable_plan_falls_back_or_raises(hvd):
@@ -449,125 +359,10 @@ def test_unfusable_plan_falls_back_or_raises(hvd):
 
 
 # ---- sharded (ZeRO-1) on 4 simulated ranks -----------------------------------------------------------------------------
-@pytest.fixture
-def team(hvd, monkeypatch):
-    from horovod_b200.torch import mpi_ops
-    t = _SimTeam(4)
-    monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-    monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-    monkeypatch.setattr(mpi_ops, 'cross_size', lambda: 1)
-    monkeypatch.setattr(mpi_ops, 'captured_reducescatter_', t.reducescatter)
-    monkeypatch.setattr(mpi_ops, 'captured_allgather_', t.allgather)
-    monkeypatch.setattr(mpi_ops, 'captured_allreduce_', t.allreduce)
-    t.opts = []
-
-    def state_allgather(tensor, name, process_set):
-        _, _, bi, key = name.split('.', 3)
-        return torch.cat([o._buckets[int(bi)]['state'][key] for o in t.opts])
-    monkeypatch.setattr(mpi_ops, 'allgather', state_allgather)
-    return t
-
-
-class _ConvNet(torch.nn.Module):
-    def __init__(self):
-        super().__init__()
-        self.conv = torch.nn.Conv2d(3, 8, 3)
-        self.fc = torch.nn.Linear(8 * 6 * 6, 10)
-        self.norm = torch.nn.LayerNorm(10)
-        self.head = torch.nn.Linear(10, 10)
-
-    def forward(self, x):
-        return self.head(self.norm(self.fc(torch.relu(self.conv(x)).flatten(1))))
-
-
-def _batch(step, r, dt):
-    g = torch.Generator(device='cuda').manual_seed(100 * step + r)
-    return torch.randn(5, 3, 8, 8, device='cuda', generator=g).to(dt), torch.randint(0, 10, (5,), device='cuda', generator=g)
-
-
 def _make(hvd, m):
     decay = [m.conv.weight, m.fc.weight, m.head.weight]
     return hvd.Lamb([{'params': decay, 'weight_decay': 0.05}, {'params': [p for p in m.parameters() if all(p is not q for q in decay)]}],
                     lr=1e-2, eps=1e-6)
-
-
-def _sharded_team(hvd, team, base, dt, master):
-    n = team.n
-    models = [copy.deepcopy(base) for _ in range(n)]
-    opts = [hvd.DistributedOptimizer(_make(hvd, m), named_parameters=m.named_parameters(), shard_optimizer_state=True,
-                                     master_weights=master, process_set=_FakeSet(n, r), bucket_cap_mb=0.01 * dt.itemsize / 4)
-            for r, m in enumerate(models)]
-    team.opts = opts
-    # at least one parameter is cut between two ranks' shards, so its norms must cross ranks
-    straddle = 0
-    for b in opts[0]._buckets:
-        for _, off, numel in b['members']:
-            straddle += off // b['shard'] != (off + numel - 1) // b['shard']
-    assert straddle > 0
-    return models, opts
-
-
-def _reduced_grads(opts, params):
-    from horovod_b200.torch.grad_buckets import full_from_shards
-    out = {}
-    for bi, b in enumerate(opts[0]._buckets):
-        full = torch.cat([o._buckets[bi]['gshard'] for o in opts])
-        for p, g in zip(b['params'], full_from_shards(b, [full], [p.shape for p in b['params']], [p.stride() for p in b['params']])):
-            out[p] = g
-    return [out[p] for p in params]
-
-
-def _step_all(team, models, opts, step, dt, clip=None):
-    n = team.n
-    for r in range(n):
-        opts[r].zero_grad()
-        x, y = _batch(step, r, dt)
-        torch.nn.functional.cross_entropy(models[r](x), y).backward()
-    coef = None
-    if clip is not None:
-        team.run(lambda r: opts[r].clip_grad_norm_(clip))
-        coef = opts[0]._clip_coef.clone()
-    else:
-        for o in opts:
-            o.synchronize()
-        team.flush()
-    grads = _reduced_grads(opts, list(models[0].parameters()))
-    mark = len(team.log)
-
-    def step_rank(r):
-        with opts[r].skip_synchronize():
-            opts[r].step()
-    team.run(step_rank)  # in lockstep: lamb_apply must see the allreduced norms
-    assert team.count('ar', mark) == n, 'one norms allreduce per rank and step'
-    for r in range(1, n):
-        for a, b in zip(models[r].parameters(), models[0].parameters()):
-            assert _same(a.detach(), b.detach()), 'ranks differ after the allgather'
-    return grads, coef
-
-
-def _ref_step(ref, ref_opt, grads, coef=None):
-    ref_opt.zero_grad()
-    for p, g in zip(ref.parameters(), grads):
-        p.grad = g.clone()
-    if coef is None:
-        ref_opt.step()
-        return
-    # the clip coefficient reaches the sharded update on the device; the reference gets it the same way
-    from horovod_b200.torch.optimizer import _fused_plan
-    from horovod_b200 import ops
-    with torch.no_grad():
-        for group, ps, gs in _fused_plan(ref_opt):
-            st = [ref_opt.state[p] for p in ps]
-            for s, p in zip(st, ps):
-                if 'exp_avg' not in s:
-                    s['step'] = torch.tensor(0.0)
-                    s['exp_avg'] = torch.zeros_like(p, dtype=torch.float32)
-                    s['exp_avg_sq'] = torch.zeros_like(p, dtype=torch.float32)
-                s['step'] += 1
-            b1, b2 = group['betas']
-            ops.fused_lamb_step(ps, gs, [s['exp_avg'] for s in st], [s['exp_avg_sq'] for s in st], group['lr'], b1, b2,
-                                group['eps'], group['weight_decay'], int(st[0]['step']), group['bias_correction'],
-                                ref_opt.adapts(group), grad_scale_dev=coef.reshape(1))
 
 
 @pytest.mark.parametrize("dt,master", [(torch.float32, False), (torch.bfloat16, True)], ids=['fp32', 'bf16-masters'])
@@ -575,8 +370,8 @@ def test_sharded_lamb_on_simulated_ranks(hvd, team, dt, master):
     """Sharded LAMB against unsharded fused LAMB on the reduced gradients over 5 steps, then a sharded -> unsharded and an
     unsharded -> sharded checkpoint that both continue like the reference."""
     torch.manual_seed(0)
-    base = _ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
-    models, opts = _sharded_team(hvd, team, base, dt, master)
+    base = NormConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
+    models, opts = sharded_team(hvd, team, base, lambda m: _make(hvd, m), dt, straddle=True, master_weights=master)
     ref = copy.deepcopy(base)
     ref_opt = hvd.DistributedOptimizer(_make(hvd, ref), named_parameters=ref.named_parameters(), fused=True,
                                        master_weights=master, zero_copy=False)
@@ -587,8 +382,8 @@ def test_sharded_lamb_on_simulated_ranks(hvd, team, dt, master):
             torch.testing.assert_close(a.float(), b.float(), **tol, msg=lambda s: '%s %s: %s' % (what, name, s))
 
     for step in range(5):
-        grads, _ = _step_all(team, models, opts, step, dt)
-        _ref_step(ref, ref_opt, grads)
+        grads, _ = step_all(team, models, opts, step, dt)
+        ref_step(ref, ref_opt, grads)
         check(models, 'step %d' % step)
     sd = opts[0].state_dict()
     assert all(set(st) >= {'exp_avg', 'exp_avg_sq', 'step'} and (('master_param' in st) == master) for st in sd['state'].values())
@@ -598,13 +393,14 @@ def test_sharded_lamb_on_simulated_ranks(hvd, team, dt, master):
                                       master_weights=master, zero_copy=False)
     un_opt.load_state_dict(copy.deepcopy(sd))
     # unsharded -> sharded
-    models2, opts2 = _sharded_team(hvd, team, copy.deepcopy(ref), dt, master)
+    models2, opts2 = sharded_team(hvd, team, copy.deepcopy(ref), lambda m: _make(hvd, m), dt, straddle=True,
+                                  master_weights=master)
     usd = ref_opt.state_dict()
     for o in opts2:
         o.load_state_dict(usd)
-    grads, _ = _step_all(team, models2, opts2, 5, dt)
-    _ref_step(ref, ref_opt, grads)
-    _ref_step(un, un_opt, grads)
+    grads, _ = step_all(team, models2, opts2, 5, dt)
+    ref_step(ref, ref_opt, grads)
+    ref_step(un, un_opt, grads)
     check(models2, 'unsharded -> sharded')
     for (name, a), b in zip(un.named_parameters(), models2[0].parameters()):
         torch.testing.assert_close(a.float(), b.float(), **tol, msg=lambda s: 'sharded -> unsharded %s: %s' % (name, s))
@@ -614,14 +410,14 @@ def test_sharded_lamb_with_clipping(hvd, team):
     """opt.clip_grad_norm_ on the simulated ranks: its coefficient reaches LAMB's first phase through grad_scale_dev."""
     dt = torch.float32
     torch.manual_seed(0)
-    base = _ConvNet().cuda().to(memory_format=torch.channels_last)
-    models, opts = _sharded_team(hvd, team, base, dt, False)
+    base = NormConvNet().cuda().to(memory_format=torch.channels_last)
+    models, opts = sharded_team(hvd, team, base, lambda m: _make(hvd, m), dt, straddle=True)
     ref = copy.deepcopy(base)
     ref_opt = hvd.DistributedOptimizer(_make(hvd, ref), named_parameters=ref.named_parameters(), fused=True, zero_copy=False)
     for step in range(4):
-        grads, coef = _step_all(team, models, opts, step, dt, clip=0.05)
+        grads, coef = step_all(team, models, opts, step, dt, clip=0.05)
         assert float(coef) < 1.0
-        _ref_step(ref, ref_opt, grads, coef)
+        ref_step(ref, ref_opt, grads, coef, kind='lamb')
         for (name, a), b in zip(models[0].named_parameters(), ref.parameters()):
             torch.testing.assert_close(a, b, rtol=1e-5, atol=1e-6, msg=lambda s: 'step %d %s: %s' % (step, name, s))
 
@@ -631,8 +427,8 @@ def test_sharded_lamb_with_grad_scaler(hvd, team):
     every rank skip alike."""
     n, dt = team.n, torch.float16
     torch.manual_seed(0)
-    base = _ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
-    models, opts = _sharded_team(hvd, team, base, dt, True)
+    base = NormConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
+    models, opts = sharded_team(hvd, team, base, lambda m: _make(hvd, m), dt, straddle=True, master_weights=True)
     scalers = [hvd.ShardedGradScaler('cuda', init_scale=256.0) for _ in range(n)]
     ref = copy.deepcopy(base)
     ref_opt = hvd.DistributedOptimizer(_make(hvd, ref), named_parameters=ref.named_parameters(), master_weights=True,
@@ -640,18 +436,18 @@ def test_sharded_lamb_with_grad_scaler(hvd, team):
     for step in range(4):
         for r in range(n):
             opts[r].zero_grad()
-            x, y = _batch(step, r, dt)
+            x, y = batch(step, r, dt)
             scalers[r].scale(torch.nn.functional.cross_entropy(models[r](x), y)).backward()
         if step == 1:
             opts[0]._buckets[0]['gflat'][0] = math.inf
         before = [s.get_scale() for s in scalers]
         team.run(lambda r: scalers[r].unscale_(opts[r]))
-        grads = _reduced_grads(opts, list(models[0].parameters()))
+        grads = reduced_grads(opts, list(models[0].parameters()))
         team.run(lambda r: (scalers[r].step(opts[r]), scalers[r].update()))
         if step == 1:
             assert all(s.get_scale() == before[0] / 2 for s in scalers)
         else:
-            _ref_step(ref, ref_opt, grads)
+            ref_step(ref, ref_opt, grads)
         for r in range(n):
             for (name, a), b in zip(models[r].named_parameters(), ref.parameters()):
                 torch.testing.assert_close(a.float(), b.float(), rtol=1e-2, atol=1e-3, msg=lambda s: '%s: %s' % (name, s))
@@ -660,17 +456,17 @@ def test_sharded_lamb_with_grad_scaler(hvd, team):
 def test_trust_norms_buffer_only_for_lamb(hvd, team):
     """The sharded optimizer allocates the padded norms buffer for Lamb only."""
     torch.manual_seed(0)
-    base = _ConvNet().cuda()
-    models, opts = _sharded_team(hvd, team, base, torch.float32, False)
+    base = NormConvNet().cuda()
+    models, opts = sharded_team(hvd, team, base, lambda m: _make(hvd, m), torch.float32, straddle=True)
     assert opts[0]._trust_norms is not None and opts[0]._trust_norms.numel() % (32 * team.n) == 0
     m = copy.deepcopy(base)
     o = hvd.DistributedOptimizer(torch.optim.AdamW(m.parameters()), named_parameters=m.named_parameters(),
-                                 shard_optimizer_state=True, process_set=_FakeSet(team.n, 0))
+                                 shard_optimizer_state=True, process_set=FakeSet(team.n, 0))
     assert o._trust_norms is None
 
 
-@pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
+@pytest.mark.skipif(ngpu() < 2, reason="needs >= 2 GPUs")
 def test_sharded_lamb_across_ranks(native_built):
-    n = 2 if _ngpu() < 4 else 4
+    n = 2 if ngpu() < 4 else 4
     rc, out = run_parallel("lamb_worker.py", np=n, timeout=420)
     assert "LAMB OK" in out, out[-4000:]

@@ -20,13 +20,11 @@ import pytest
 import torch
 
 from conftest import run_parallel
-from test_gpu_sharded_clip import _FakeSet, _SimTeam
+from optim_cases import COUNTS, LOW, LOW_IDS, Slot, adam_ref_kernel, bits, hvd, ngpu, same  # noqa: F401  (hvd: fixture)
+from sim_ranks import batch, reduced_grads, ref_step, sharded_team, team  # noqa: F401  (team: fixture)
 
 pytestmark = pytest.mark.gpu
 
-LOW = [torch.bfloat16, torch.float16]
-LOW_IDS = ['bf16', 'fp16']
-COUNTS = [1, 3, 4, 5, 4095, 4096, 4097, 3 * 4096 + 1, (1 << 20) + 3]
 # (param, grad, state) storage offsets in elements; the master and the state share the last one
 OFFSETS = [(0, 0, 0), (1, 0, 0), (0, 1, 0), (0, 0, 1), (2, 0, 0), (0, 2, 2), (3, 3, 3), (0, 3, 0), (3, 0, 2)]
 SGD_HP = [dict(lr=0.05, momentum=0.9, dampening=0.5, weight_decay=1e-2, grad_scale=0.25),
@@ -36,54 +34,7 @@ ADAM_HP = [dict(lr=1e-2, weight_decay=1e-2, adamw=True), dict(lr=1e-2, weight_de
            dict(lr=1e-3, weight_decay=0.0, adamw=True, beta1=0.8, beta2=0.99, grad_scale=0.5)]
 
 
-def _ngpu():
-    return torch.cuda.device_count() if torch.cuda.is_available() else 0
-
-
-@pytest.fixture(scope="module")
-def hvd():
-    import horovod_b200.torch as hvd
-    hvd.init()
-    torch.cuda.set_device(0)
-    yield hvd
-    hvd.shutdown()
-
-
-def _ops():
-    from horovod_b200 import ops
-    return ops
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int16 if t.element_size() == 2 else torch.int32)
-
-
-def _same(a, b):
-    """Bit-identical (NaN-safe, -0 != +0)."""
-    return a.dtype == b.dtype and a.shape == b.shape and torch.equal(_bits(a), _bits(b))
-
-
 # ---- the kernels against the fp32-parameter kernels ------------------------------------------------------------------
-class Slot:
-    """A tensor placed at element `offset` of a larger buffer of random bits; the slack must survive the kernel."""
-
-    def __init__(self, shape, dtype, offset, fill, memory_format=torch.contiguous_format, slack=67):
-        numel = int(np.prod(shape))
-        self.buf = torch.randn(offset + numel + slack, device='cuda').to(dtype)
-        strides = torch.empty(shape, memory_format=memory_format).stride() if len(shape) == 4 else torch.empty(shape).stride()
-        self.t = self.buf.as_strided(shape, strides, offset)
-        self.t.copy_(fill)
-        self.lo, self.hi = offset, offset + numel
-        self.slack = self._slack().clone()
-
-    def _slack(self):
-        b = _bits(self.buf)
-        return torch.cat([b[:self.lo], b[self.hi:]])
-
-    def intact(self):
-        return torch.equal(self._slack(), self.slack)
-
-
 def _case(shape, pdt, seed, offsets=(0, 0, 0), memory_format=torch.contiguous_format, sgd=False):
     """Master-mode slots (param pdt, grad pdt, fp32 master and state) with p == round(master): no reconcile."""
     g = torch.Generator(device='cuda').manual_seed(seed)
@@ -109,7 +60,7 @@ def _ref_grad(g):
 def _kernel_vs_fp32(cases, pdt, sgd, expect_master=None, **hp):
     """One master launch over `cases` and one fp32-parameter launch over copies; masters, states and parameters must be
     bit-identical. expect_master: the masters the update starts from (default: the current ones)."""
-    ops = _ops()
+    from horovod_b200 import ops
     start = expect_master or [c['w'].t.clone() for c in cases]
     ref_p = [s.clone() for s in start]
     ref_g = [_ref_grad(c['g'].t).clone() for c in cases]
@@ -129,11 +80,11 @@ def _kernel_vs_fp32(cases, pdt, sgd, expect_master=None, **hp):
         ops.fused_adam_step(ref_p, ref_g, ref_s['m'], ref_s['v'], grad_scale_dev=gsd, **hp)
     torch.cuda.synchronize()
     for i, c in enumerate(cases):
-        assert _same(c['w'].t, ref_p[i]), (i, 'master')
-        assert _same(c['p'].t, ref_p[i].to(pdt)), (i, 'param is not the rounded master')
+        assert same(c['w'].t, ref_p[i]), (i, 'master')
+        assert same(c['p'].t, ref_p[i].to(pdt)), (i, 'param is not the rounded master')
         for k in keys:
-            assert _same(c[k].t, ref_s[k][i]), (i, k)
-        assert _same(c['g'].t, before_g[i]), (i, 'grad written')
+            assert same(c[k].t, ref_s[k][i]), (i, k)
+        assert same(c['g'].t, before_g[i]), (i, 'grad written')
         for k, s in c.items():
             assert s.intact(), (i, 'wrote outside ' + k)
 
@@ -199,7 +150,7 @@ def test_reconcile_restarts_exactly_the_overwritten_elements(hvd, pdt, kind):
         else:
             idx = torch.randperm(p.numel(), device='cuda', generator=g)[:p.numel() // 7]
         new = (p[idx].float() + 4.0).to(pdt)  # |p| < 1: every element changes
-        assert not (_bits(new) == _bits(p[idx])).any()
+        assert not (bits(new) == bits(p[idx])).any()
         p[idx] = new
         e = w.clone()
         e[idx] = new.float()
@@ -247,7 +198,7 @@ def test_reconcile_after_load_state_dict_and_broadcast_parameters(hvd):
     # a reloaded element that happens to equal its old rounded master is indistinguishable from an untouched one: by the
     # rule it keeps the master (for random weights a handful of the 1152 elements)
     w, new = masters[m[0].weight], m[0].weight.detach()
-    masters[m[0].weight] = torch.where(_bits(w.to(dt)) == _bits(new), w, new.float())
+    masters[m[0].weight] = torch.where(bits(w.to(dt)) == bits(new), w, new.float())
     masters[m[3].weight][0, :5] = 0.5
     # oracle: an fp32 twin starting from those masters, the same gradients and state, the fp32 kernel
     twin = copy.deepcopy(m).float()
@@ -268,8 +219,8 @@ def test_reconcile_after_load_state_dict_and_broadcast_parameters(hvd):
     topt.step()
     torch.cuda.synchronize()
     for (name, p), q in zip(m.named_parameters(), twin.parameters()):
-        assert _same(opt.state[p]['master_param'], q.detach()), name
-        assert _same(p.detach(), q.detach().to(dt)), name
+        assert same(opt.state[p]['master_param'], q.detach()), name
+        assert same(p.detach(), q.detach().to(dt)), name
 
 
 # ---- the capability ----------------------------------------------------------------------------------------------------
@@ -292,16 +243,15 @@ def test_bf16_update_below_half_an_ulp(hvd):
     for _ in range(50):
         ref = ref - torch.tensor(lr, dtype=torch.float32)
     assert float(ref[0]) < 0.96
-    assert _same(out[True][1], ref) and _same(out[True][0], ref.to(torch.bfloat16))
+    assert same(out[True][1], ref) and same(out[True][0], ref.to(torch.bfloat16))
 
 
 def test_bf16_adamw_masters_track_fp32_adamw(hvd):
     """A small bf16 model, 20 AdamW steps on fixed gradients. Every step, the masters and moments agree with the float64
-    model of the fused kernel (test_gpu_fused_optimizer's reference, itself checked against torch.optim) within 1e-6 of
+    model of the fused kernel (adam_ref_kernel, which test_gpu_fused_optimizer checks against torch.optim) within 1e-6 of
     its error scale. Over the 20 steps the masters follow torch's fp32 AdamW on the same gradients, up to the kernel's
     fp32 hyper-parameters (torch forms the betas' powers and bias corrections in float64): within 1e-6 of |p0| plus 1e-4
     of lr per step, while the bf16 parameters without masters would lose most of these updates."""
-    from test_gpu_fused_optimizer import adam_ref_kernel
     dt, lr, wd, steps = torch.bfloat16, 1e-3, 0.05, 20
     m = _mlp(dt)
     ref = [torch.nn.Parameter(p.detach().float().clone()) for p in m.parameters()]
@@ -335,7 +285,7 @@ def test_bf16_adamw_masters_track_fp32_adamw(hvd):
                 assert bool((err <= 1e-6 * scale).all()), (name, step, what, float((err / scale).max()))
             err = (w - q.detach()).abs()
             assert bool((err <= step * (1e-6 * a0 + 1e-4 * lr)).all()), (name, step, float(err.max()))
-            assert _same(p.detach(), w.to(dt)), name
+            assert same(p.detach(), w.to(dt)), name
 
 
 # ---- the optimizer at world size 1 -------------------------------------------------------------------------------------
@@ -366,8 +316,8 @@ def _twin_steps(hvd, make, dtype, steps, frozen_until=0, closure_at=()):
         torch.cuda.synchronize()
         for (name, p), q in zip(m.named_parameters(), twin.parameters()):
             if p.requires_grad and p in opt.state:
-                assert _same(opt.state[p]['master_param'], q.detach()), (name, step)
-            assert _same(p.detach(), q.detach().to(dtype)), (name, step)
+                assert same(opt.state[p]['master_param'], q.detach()), (name, step)
+            assert same(p.detach(), q.detach().to(dtype)), (name, step)
     return m, opt, twin, topt
 
 
@@ -399,6 +349,7 @@ def test_optimizer_follows_fp32_twin(hvd, pdt, kind):
 def test_sgd_parameter_joining_later_starts_its_momentum(hvd, pdt):
     """SGD with momentum and masters: a Linear frozen for 3 steps gets a fresh fp32 momentum buffer (the first-step rule)
     while the others continue theirs, in the fused update: against the master kernel run by hand."""
+    from horovod_b200 import ops
     m = _mlp(pdt)
     m[3].requires_grad_(False)
     opt = hvd.DistributedOptimizer(_sgd(m), named_parameters=m.named_parameters(), master_weights=True)
@@ -415,10 +366,10 @@ def test_sgd_parameter_joining_later_starts_its_momentum(hvd, pdt):
         if step == 3:
             ps = [x.clone() for x in p0]
             ws, bufs = [x.float() for x in p0], [torch.zeros_like(x, dtype=torch.float32) for x in p0]
-            _ops().fused_sgd_step(ps, g0, bufs, 0.05, 0.9, weight_decay=1e-3, first_step=True, master_params=ws)
+            ops.fused_sgd_step(ps, g0, bufs, 0.05, 0.9, weight_decay=1e-3, first_step=True, master_params=ws)
             for p, q, w, b in zip(late, ps, ws, bufs):
-                assert _same(p.detach(), q) and _same(opt.state[p]['master_param'], w)
-                assert _same(opt.state[p]['momentum_buffer'], b)
+                assert same(p.detach(), q) and same(opt.state[p]['master_param'], w)
+                assert same(opt.state[p]['momentum_buffer'], b)
 
 
 def test_graphed_step_equals_eager(hvd, monkeypatch):
@@ -446,8 +397,8 @@ def test_graphed_step_equals_eager(hvd, monkeypatch):
         runs.append((m, opt))
     (a, oa), (b, ob) = runs
     for (name, p), q in zip(a.named_parameters(), b.parameters()):
-        assert _same(p.detach(), q.detach()), name
-        assert _same(oa.state[p]['master_param'], ob.state[q]['master_param']), name
+        assert same(p.detach(), q.detach()), name
+        assert same(oa.state[p]['master_param'], ob.state[q]['master_param']), name
 
 
 @pytest.mark.parametrize("kind", ["adamw", "sgd"])
@@ -484,10 +435,10 @@ def test_checkpoint_round_trip_is_bit_exact(hvd, monkeypatch, kind):
             assert oc.state[p]['momentum_buffer'].dtype == torch.float32
     train(mc, oc, range(3, 6))
     for (name, a), c in zip(ma.named_parameters(), mc.parameters()):
-        assert _same(a.detach(), c.detach()), name
+        assert same(a.detach(), c.detach()), name
         for key, t in oa.state[a].items():
             if torch.is_tensor(t) and t.dim() > 0:
-                assert _same(t, oc.state[c][key]), (name, key)
+                assert same(t, oc.state[c][key]), (name, key)
 
 
 def test_checkpoint_without_masters_loads(hvd):
@@ -515,7 +466,7 @@ def test_checkpoint_without_masters_loads(hvd):
     o2.step()
     t2.step()
     for (name, p), q in zip(m2.named_parameters(), twin.parameters()):
-        assert _same(o2.state[p]['master_param'], q.detach()), name
+        assert same(o2.state[p]['master_param'], q.detach()), name
 
 
 def test_rejections(hvd):
@@ -541,7 +492,7 @@ def test_rejections(hvd):
 
 
 def test_kernel_rejects_bad_master_arguments(hvd):
-    ops = _ops()
+    from horovod_b200 import ops
     z = lambda n=64, dt=torch.float32: torch.zeros(n, device='cuda', dtype=dt)  # noqa: E731
     pb, gb = z(dt=torch.bfloat16), z(dt=torch.bfloat16)
 
@@ -567,26 +518,6 @@ def test_kernel_rejects_bad_master_arguments(hvd):
 
 
 # ---- sharded (ZeRO-1) on 4 simulated ranks -----------------------------------------------------------------------------
-@pytest.fixture
-def team(hvd, monkeypatch):
-    from horovod_b200.torch import mpi_ops
-    t = _SimTeam(4)
-    monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-    monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-    monkeypatch.setattr(mpi_ops, 'cross_size', lambda: 1)
-    monkeypatch.setattr(mpi_ops, 'captured_reducescatter_', t.reducescatter)
-    monkeypatch.setattr(mpi_ops, 'captured_allgather_', t.allgather)
-    monkeypatch.setattr(mpi_ops, 'captured_allreduce_', t.allreduce)
-    t.opts = []
-
-    def state_allgather(tensor, name, process_set):
-        # state_dict()'s gather of one state key of one bucket: the shards of every simulated rank in rank order
-        _, _, bi, key = name.split('.', 3)
-        return torch.cat([o._buckets[int(bi)]['state'][key] for o in t.opts])
-    monkeypatch.setattr(mpi_ops, 'allgather', state_allgather)
-    return t
-
-
 class _ConvNet(torch.nn.Module):
     def __init__(self):
         super().__init__()
@@ -596,11 +527,6 @@ class _ConvNet(torch.nn.Module):
 
     def forward(self, x):
         return self.head(self.fc(torch.relu(self.conv(x)).flatten(1)))
-
-
-def _batch(step, r, dt):
-    g = torch.Generator(device='cuda').manual_seed(100 * step + r)
-    return torch.randn(5, 3, 8, 8, device='cuda', generator=g).to(dt), torch.randint(0, 10, (5,), device='cuda', generator=g)
 
 
 def _make(kind, m):
@@ -614,13 +540,8 @@ def _make(kind, m):
 
 
 def _sharded_team(hvd, team, base, kind, dt):
-    n = team.n
-    models = [copy.deepcopy(base) for _ in range(n)]
-    opts = [hvd.DistributedOptimizer(_make(kind, m), named_parameters=m.named_parameters(), shard_optimizer_state=True,
-                                     master_weights=True, process_set=_FakeSet(n, r), bucket_cap_mb=0.01 * dt.itemsize / 4)
-            for r, m in enumerate(models)]
-    assert len(opts[0]._buckets) > 2 and all('master_param' in b['state'] for b in opts[0]._buckets)
-    team.opts = opts
+    models, opts = sharded_team(hvd, team, base, lambda m: _make(kind, m), dt, min_buckets=3, master_weights=True)
+    assert all('master_param' in b['state'] for b in opts[0]._buckets)
     return models, opts
 
 
@@ -630,26 +551,15 @@ def _reference(hvd, kind, model):
                                     zero_copy=False)
 
 
-def _reduced_grads(opts, params):
-    """Every parameter's reduced gradient, assembled from the owners' gradient shards (what the sharded update reads)."""
-    from horovod_b200.torch.grad_buckets import full_from_shards
-    out = {}
-    for bi, b in enumerate(opts[0]._buckets):
-        full = torch.cat([o._buckets[bi]['gshard'] for o in opts])
-        for p, g in zip(b['params'], full_from_shards(b, [full], [p.shape for p in b['params']], [p.stride() for p in b['params']])):
-            out[p] = g
-    return [out[p] for p in params]
-
-
 def _check_against(models, opts, ref, ref_opt, what):
     sd = opts[0].state_dict()
     for r in range(len(models)):
         for (name, a), b in zip(models[r].named_parameters(), ref.parameters()):
-            assert _same(a.detach(), b.detach()), (what, name, r)
+            assert same(a.detach(), b.detach()), (what, name, r)
     for i, (name, b) in enumerate(ref.named_parameters()):
         for key, t in ref_opt.state[b].items():
             if torch.is_tensor(t) and t.dim() > 0:
-                assert _same(sd['state'][i][key].cuda(), t), (what, name, key)
+                assert same(sd['state'][i][key].cuda(), t), (what, name, key)
     return sd
 
 
@@ -668,26 +578,20 @@ def test_sharded_masters_on_simulated_ranks(hvd, team, dt, kind):
     def step_all(models, opts, step):
         for r in range(n):
             opts[r].zero_grad()
-            x, y = _batch(step, r, dt)
+            x, y = batch(step, r, dt)
             torch.nn.functional.cross_entropy(models[r](x), y).backward()
         for o in opts:
             o.synchronize()
         team.flush()
-        grads = _reduced_grads(opts, list(models[0].parameters()))
+        grads = reduced_grads(opts, list(models[0].parameters()))
         for o in opts:
             with o.skip_synchronize():
                 o.step()
         team.flush()
         return grads
 
-    def ref_step(grads):
-        ref_opt.zero_grad()
-        for p, g in zip(ref.parameters(), grads):
-            p.grad = g.clone()
-        ref_opt.step()
-
     for step in range(4):
-        ref_step(step_all(models, opts, step))
+        ref_step(ref, ref_opt, step_all(models, opts, step))
         sd = _check_against(models, opts, ref, ref_opt, 'step %d' % step)
     if kind == 'sgd':
         # the plain-SGD group's bucket holds masters only; they are saved
@@ -704,14 +608,14 @@ def test_sharded_masters_on_simulated_ranks(hvd, team, dt, kind):
     for o in opts2:
         o.load_state_dict(usd)
     grads = step_all(models2, opts2, 4)
-    ref_step(grads)
+    ref_step(ref, ref_opt, grads)
     for p, g in zip(ref2.parameters(), grads):
         p.grad = g.clone()
     ref2_opt.step()
     _check_against(models2, opts2, ref, ref_opt, 'after unsharded -> sharded')
     for (name, a), b in zip(ref2.named_parameters(), ref.parameters()):
-        assert _same(a.detach(), b.detach()), name
-        assert _same(ref2_opt.state[a]['master_param'], ref_opt.state[b]['master_param']), name
+        assert same(a.detach(), b.detach()), name
+        assert same(ref2_opt.state[a]['master_param'], ref_opt.state[b]['master_param']), name
 
 
 def test_sharded_masters_with_grad_scaler_and_clipping(hvd, team):
@@ -728,13 +632,13 @@ def test_sharded_masters_with_grad_scaler_and_clipping(hvd, team):
     for step in range(5):
         for r in range(n):
             opts[r].zero_grad()
-            x, y = _batch(step, r, dt)
+            x, y = batch(step, r, dt)
             scalers[r].scale(torch.nn.functional.cross_entropy(models[r](x), y)).backward()
         if step == 2:
             opts[0]._buckets[0]['gflat'][0] = math.inf
         before = [s.get_scale() for s in scalers]
         norms = team.run(lambda r: (scalers[r].unscale_(opts[r]), opts[r].clip_grad_norm_(0.5))[1])
-        grads = _reduced_grads(opts, list(models[0].parameters()))  # unscaled in place by unscale_
+        grads = reduced_grads(opts, list(models[0].parameters()))  # unscaled in place by unscale_
         coef = opts[0]._clip_coef.clone()
         team.run(lambda r: (scalers[r].step(opts[r]), scalers[r].update()))
         if step == 2:
@@ -801,8 +705,8 @@ def test_master_kernels_under_compute_sanitizer_memcheck():
     assert p.returncode == 0 and 'MASTER SANITIZER OK' in out and 'ERROR SUMMARY: 0 errors' in out, out[-5000:]
 
 
-@pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
+@pytest.mark.skipif(ngpu() < 2, reason="needs >= 2 GPUs")
 def test_master_weights_across_ranks(native_built):
-    n = 2 if _ngpu() < 4 else 4
+    n = 2 if ngpu() < 4 else 4
     rc, out = run_parallel("master_weights_worker.py", np=n, timeout=420)
     assert "MASTER WEIGHTS OK" in out, out[-4000:]

@@ -5,21 +5,10 @@ import pytest
 import torch
 
 from conftest import run_parallel
+from optim_cases import hvd, ngpu  # noqa: F401  (hvd: fixture)
+from sim_ranks import ConvNetWithUnused, batch, sharded_team, team  # noqa: F401  (team: fixture)
 
 pytestmark = pytest.mark.gpu
-
-
-def _ngpu():
-    return torch.cuda.device_count() if torch.cuda.is_available() else 0
-
-
-@pytest.fixture(scope="module")
-def hvd():
-    import horovod_b200.torch as hvd
-    hvd.init()
-    torch.cuda.set_device(0)
-    yield hvd
-    hvd.shutdown()
 
 
 # shard element counts: a multiple of 8 (16 B in every dtype) but not of the 4 KiB row or the 32 KiB chunk
@@ -164,101 +153,30 @@ def test_world_size_1_returns_the_existing_optimizer(hvd):
         torch.testing.assert_close(a, b, rtol=1e-5, atol=1e-6)
 
 
-class _FakeSet:
-    """Process set of one simulated rank."""
-    process_set_id = 0
-
-    def __init__(self, n, r):
-        self.n, self.r = n, r
-
-    def size(self):
-        return self.n
-
-    def rank(self):
-        return self.r
-
-    def included(self):
-        return True
-
-
-class _SimTeam:
-    """N simulated ranks of the sharded optimizer in one process: every rank's captured collectives are queued and, once
-    all ranks issued them, run by the real kernels as one simulated launch over the N ranks' buffers."""
-
-    def __init__(self, n):
-        from horovod_b200.torch import mpi_ops
-        self.n, self.queues, self.mpi_ops = n, [[] for _ in range(n)], mpi_ops
-
-    def reducescatter(self, tensor, op, prescale_factor, postscale_factor, process_set, max_ctas=0):
-        scale = prescale_factor * postscale_factor / (self.n if op == self.mpi_ops.Average else 1)
-        self.queues[process_set.r].append(('rs', tensor, scale))
-
-    def allgather(self, tensor, process_set, max_ctas=0):
-        self.queues[process_set.r].append(('ag', tensor, 1.0))
-
-    def flush(self):
-        from horovod_b200.ops import sim
-        torch.cuda.synchronize()
-        assert len({len(q) for q in self.queues}) == 1, 'ranks issued different numbers of collectives'
-        for calls in zip(*self.queues):
-            assert len({(c[0], c[1].numel(), c[1].dtype, c[2]) for c in calls}) == 1, 'ranks issued different collectives'
-            if calls[0][0] == 'rs':
-                sim.inplace_reducescatter([c[1] for c in calls], op=sim.SUM, scale=calls[0][2])
-            else:
-                sim.inplace_allgather([c[1] for c in calls])
-        torch.cuda.synchronize()
-        self.queues = [[] for _ in range(self.n)]
-
-
-class _ConvNet(torch.nn.Module):
-    def __init__(self):
-        super().__init__()
-        self.conv = torch.nn.Conv2d(3, 8, 3)
-        self.fc = torch.nn.Linear(8 * 6 * 6, 10)
-        self.unused = torch.nn.Linear(4, 10)  # only in the forward when asked
-
-    def forward(self, x, use_all=True):
-        y = self.fc(torch.relu(self.conv(x)).flatten(1))
-        return y + self.unused(x[:, 0, 0, :4]) if use_all else y
-
-
 @pytest.mark.parametrize("kind", ["adamw", "sgd", "adamw-fp16"])
-def test_sharded_optimizer_on_simulated_ranks(hvd, monkeypatch, kind):
+def test_sharded_optimizer_on_simulated_ranks(hvd, team, kind):
     """The sharded DistributedOptimizer itself (buckets, hooks, launch order, missing gradients, fused shard update,
     synchronize() followed by step()) on 4 simulated ranks, against plain torch on averaged gradients. The fp16 model
     is compared with an fp32 reference model, so only to fp16 accuracy; the ranks must still agree bit for bit."""
     import copy
     import warnings
-    from horovod_b200.torch import mpi_ops
     from horovod_b200.torch.sharded_optimizer import _ShardedDistributedOptimizer
-    n = 4
-    team = _SimTeam(n)
-    monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-    monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-    monkeypatch.setattr(mpi_ops, 'cross_size', lambda: 1)
-    monkeypatch.setattr(mpi_ops, 'captured_reducescatter_', team.reducescatter)
-    monkeypatch.setattr(mpi_ops, 'captured_allgather_', team.allgather)
+    n = team.n
     dt = torch.float16 if kind == 'adamw-fp16' else torch.float32
     tol = dict(rtol=1e-4, atol=1e-5) if dt == torch.float32 else dict(rtol=2e-2, atol=2e-3)
     torch.manual_seed(0)
-    base = _ConvNet().cuda().to(dtype=dt, memory_format=torch.channels_last)
+    base = ConvNetWithUnused().cuda().to(dtype=dt, memory_format=torch.channels_last)
 
     def make(m):
         if kind.startswith('adamw'):
             return torch.optim.AdamW(m.parameters(), lr=1e-2, weight_decay=0.05)
         return torch.optim.SGD(m.parameters(), lr=0.05, momentum=0.9, nesterov=True, weight_decay=1e-4)
 
-    models = [copy.deepcopy(base) for _ in range(n)]
-    opts = [hvd.DistributedOptimizer(make(m), named_parameters=m.named_parameters(), shard_optimizer_state=True,
-                                     process_set=_FakeSet(n, r), bucket_cap_mb=0.01 * dt.itemsize / 4) for r, m in enumerate(models)]
-    assert all(isinstance(o, _ShardedDistributedOptimizer) for o in opts) and len(opts[0]._buckets) > 2
+    models, opts = sharded_team(hvd, team, base, make, dt, min_buckets=3)
+    assert all(isinstance(o, _ShardedDistributedOptimizer) for o in opts)
     assert models[0].conv.weight.is_contiguous(memory_format=torch.channels_last)
     ref = copy.deepcopy(base).float()
     ref_opt = make(ref)
-
-    def batch(step, r):
-        g = torch.Generator(device='cuda').manual_seed(100 * step + r)
-        return torch.randn(5, 3, 8, 8, device='cuda', generator=g), torch.randint(0, 10, (5,), device='cuda', generator=g)
 
     for step in range(6):
         use = lambda r: not (step == 2 or (step == 4 and r == 0))  # noqa: E731  unused on every rank / on rank 0 only
@@ -301,8 +219,8 @@ def test_sharded_optimizer_on_simulated_ranks(hvd, monkeypatch, kind):
     assert models[0].conv.weight.is_contiguous(memory_format=torch.channels_last)
 
 
-@pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
+@pytest.mark.skipif(ngpu() < 2, reason="needs >= 2 GPUs")
 def test_sharded_optimizer_across_ranks(native_built):
-    n = 2 if _ngpu() < 4 else (4 if _ngpu() < 8 else 8)
+    n = 2 if ngpu() < 4 else (4 if ngpu() < 8 else 8)
     rc, out = run_parallel("sharded_optimizer_worker.py", np=n, timeout=420)
     assert "SHARDED OK" in out, out[-4000:]

@@ -4,31 +4,18 @@ on 4 simulated ranks (csrc/common/sim_api.cc) against plain torch on averaged gr
 ranks."""
 import copy
 import math
-import threading
 import warnings
 
 import pytest
 import torch
 
 from conftest import run_parallel
+from optim_cases import SIZES, hvd, ngpu  # noqa: F401  (hvd: fixture)
+from sim_ranks import ConvNetWithUnused, batch, reduced_grads, sharded_team, team  # noqa: F401  (team: fixture)
 
 pytestmark = pytest.mark.gpu
 
 DTYPES = [torch.float32, torch.bfloat16, torch.float16]
-SIZES = [1, 3, 4095, 4096, 4097, (1 << 20) + 3]
-
-
-def _ngpu():
-    return torch.cuda.device_count() if torch.cuda.is_available() else 0
-
-
-@pytest.fixture(scope="module")
-def hvd():
-    import horovod_b200.torch as hvd
-    hvd.init()
-    torch.cuda.set_device(0)
-    yield hvd
-    hvd.shutdown()
 
 
 # ---- the statistics kernel ---------------------------------------------------------------------------------------------
@@ -180,153 +167,6 @@ def test_fused_update_rejects_bad_grad_scale_dev(hvd):
 
 
 # ---- simulated ranks ------------------------------------------------------------------------------------------------------
-class _FakeSet:
-    """Process set of one simulated rank."""
-    process_set_id = 0
-
-    def __init__(self, n, r):
-        self.n, self.r = n, r
-
-    def size(self):
-        return self.n
-
-    def rank(self):
-        return self.r
-
-    def included(self):
-        return True
-
-
-class _SimTeam:
-    """N simulated ranks of the sharded optimizer in one process.  Every rank's captured collectives are queued and run by
-    the real kernels as one simulated launch over the N ranks' buffers: by flush(), or, while run() drives the ranks in
-    one thread each, as soon as every rank issued its next collective (a barrier, as the kernels' flags are on real
-    GPUs), so that what a rank does after a collective sees its result.  `log` keeps (kind, rank) of every call."""
-
-    def __init__(self, n):
-        from horovod_b200.torch import mpi_ops
-        self.n, self.queues, self.mpi_ops, self.log = n, [[] for _ in range(n)], mpi_ops, []
-        self.lockstep = False
-        self.sim_launches = 0
-        self._barrier = threading.Barrier(n, action=self.flush)
-
-    def _issue(self, r, call):
-        self.queues[r].append(call)
-        self.log.append((call[0], r))
-        if self.lockstep:
-            self._barrier.wait(timeout=120)
-
-    def reducescatter(self, tensor, op, prescale_factor, postscale_factor, process_set, max_ctas=0):
-        scale = prescale_factor * postscale_factor / (self.n if op == self.mpi_ops.Average else 1)
-        self._issue(process_set.r, ('rs', tensor, scale))
-
-    def allgather(self, tensor, process_set, max_ctas=0):
-        self._issue(process_set.r, ('ag', tensor, 1.0))
-
-    def allreduce(self, tensor, op=1, prescale_factor=1.0, postscale_factor=1.0, process_set=None, max_ctas=0):
-        assert prescale_factor == postscale_factor == 1.0 and op in (self.mpi_ops.Sum, self.mpi_ops.Max)
-        self._issue(process_set.r, ('ar', tensor, op))
-        return tensor
-
-    def flush(self):
-        from horovod_b200.ops import sim, kernel_launches
-        torch.cuda.synchronize()
-        before = kernel_launches()
-        assert len({len(q) for q in self.queues}) == 1, 'ranks issued different numbers of collectives'
-        for calls in zip(*self.queues):
-            assert len({(c[0], c[1].numel(), c[1].dtype, c[2]) for c in calls}) == 1, 'ranks issued different collectives'
-            ts = [c[1] for c in calls]
-            if calls[0][0] == 'rs':
-                sim.inplace_reducescatter(ts, op=sim.SUM, scale=calls[0][2])
-            elif calls[0][0] == 'ag':
-                sim.inplace_allgather(ts)
-            else:
-                sim.inplace_allreduce(ts, op=sim.SUM if calls[0][2] == self.mpi_ops.Sum else sim.MAX)
-        torch.cuda.synchronize()
-        self.sim_launches += kernel_launches() - before
-        self.queues = [[] for _ in range(self.n)]
-
-    def run(self, fn):
-        """fn(rank) on every rank at once, one thread per rank; returns the results in rank order."""
-        self.flush()
-        self.lockstep = True
-        res, errs = [None] * self.n, []
-
-        def body(r):
-            try:
-                res[r] = fn(r)
-            except BaseException as e:  # noqa: B036  re-raised below
-                errs.append(e)
-                self._barrier.abort()
-        ths = [threading.Thread(target=body, args=(r,)) for r in range(self.n)]
-        for t in ths:
-            t.start()
-        for t in ths:
-            t.join()
-        self.lockstep = False
-        self._barrier.reset()
-        if errs:
-            raise errs[0]
-        torch.cuda.synchronize()
-        return res
-
-    def count(self, kind, since):
-        return sum(1 for k, _ in self.log[since:] if k == kind)
-
-
-@pytest.fixture
-def team(hvd, monkeypatch):
-    from horovod_b200.torch import mpi_ops
-    t = _SimTeam(4)
-    monkeypatch.setattr(mpi_ops, 'symm_empty', lambda numel, dtype, device, process_set: torch.empty(numel, dtype=dtype, device=device))
-    monkeypatch.setattr(mpi_ops, 'symm_available', lambda process_set: True)
-    monkeypatch.setattr(mpi_ops, 'cross_size', lambda: 1)
-    monkeypatch.setattr(mpi_ops, 'captured_reducescatter_', t.reducescatter)
-    monkeypatch.setattr(mpi_ops, 'captured_allgather_', t.allgather)
-    monkeypatch.setattr(mpi_ops, 'captured_allreduce_', t.allreduce)
-    return t
-
-
-class _ConvNet(torch.nn.Module):
-    def __init__(self):
-        super().__init__()
-        self.conv = torch.nn.Conv2d(3, 8, 3)
-        self.fc = torch.nn.Linear(8 * 6 * 6, 10)
-        self.unused = torch.nn.Linear(4, 10)  # only in the forward when asked
-
-    def forward(self, x, use_all=True):
-        y = self.fc(torch.relu(self.conv(x)).flatten(1))
-        return y + self.unused(x[:, 0, 0, :4]) if use_all else y
-
-
-def _batch(step, r):
-    g = torch.Generator(device='cuda').manual_seed(100 * step + r)
-    return torch.randn(5, 3, 8, 8, device='cuda', generator=g), torch.randint(0, 10, (5,), device='cuda', generator=g)
-
-
-def _sharded(hvd, team, base, make, dt):
-    n = team.n
-    models = [copy.deepcopy(base).to(dtype=dt, memory_format=torch.channels_last) for _ in range(n)]
-    opts = [hvd.DistributedOptimizer(make(m), named_parameters=m.named_parameters(), shard_optimizer_state=True,
-                                     process_set=_FakeSet(n, r), bucket_cap_mb=0.01 * dt.itemsize / 4) for r, m in enumerate(models)]
-    assert len(opts[0]._buckets) > 2
-    return models, opts
-
-
-def _reduced_grads(opts, model_params):
-    """The averaged gradient of every parameter, assembled from the ranks' owned shards (what the sharded update sees)."""
-    from horovod_b200.torch.grad_buckets import full_from_shards, shard_range
-    out = {}
-    for bi, b in enumerate(opts[0]._buckets):
-        shards = []
-        for r, o in enumerate(opts):
-            lo, hi = shard_range(o._buckets[bi], r)
-            shards.append(o._buckets[bi]['gflat'][lo:hi])
-        for p, full in zip(b['params'], full_from_shards(b, shards, [p.shape for p in b['params']])):
-            out[p] = full.float()
-    return [out[p] for p in model_params]
-
-
 @pytest.mark.parametrize("kind", ["adamw", "sgd"])
 @pytest.mark.parametrize("dt", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("norm_type", [2.0, math.inf])
@@ -335,7 +175,7 @@ def test_clip_grad_norm_on_simulated_ranks(hvd, team, kind, dt, norm_type):
     clip active on even steps only; in step 2 no rank uses one layer, so clip_grad_norm_ itself reduces those buckets."""
     n = team.n
     torch.manual_seed(0)
-    base = _ConvNet().cuda()
+    base = ConvNetWithUnused().cuda()
 
     def make(m):
         if kind == 'adamw':
@@ -344,7 +184,8 @@ def test_clip_grad_norm_on_simulated_ranks(hvd, team, kind, dt, norm_type):
             return torch.optim.AdamW(m.parameters(), lr=1e-2, eps=1e-3, weight_decay=0.05)
         return torch.optim.SGD(m.parameters(), lr=0.05, momentum=0.9, nesterov=True, weight_decay=1e-4)
 
-    models, opts = _sharded(hvd, team, base, make, dt)
+    models, opts = sharded_team(hvd, team, copy.deepcopy(base).to(dtype=dt, memory_format=torch.channels_last), make, dt,
+                                min_buckets=3)
     ref = copy.deepcopy(base).to(memory_format=torch.channels_last)
     ref_opt = make(ref)
     tol = dict(rtol=1e-4, atol=1e-5) if dt == torch.float32 else dict(rtol=5e-2, atol=1e-2)
@@ -352,7 +193,7 @@ def test_clip_grad_norm_on_simulated_ranks(hvd, team, kind, dt, norm_type):
         use = step != 2
         grads = [torch.zeros_like(p) for p in ref.parameters()]
         for r in range(n):
-            x, y = _batch(step, r)
+            x, y = batch(step, r)
             ref.zero_grad()
             torch.nn.functional.cross_entropy(ref(x, use), y).backward()
             for g, p in zip(grads, ref.parameters()):
@@ -367,7 +208,7 @@ def test_clip_grad_norm_on_simulated_ranks(hvd, team, kind, dt, norm_type):
 
         for r in range(n):
             opts[r].zero_grad()
-            x, y = _batch(step, r)
+            x, y = batch(step, r)
             torch.nn.functional.cross_entropy(models[r](x.to(dt), use), y).backward()
         if step == 1:
             with pytest.raises(AssertionError):
@@ -379,7 +220,7 @@ def test_clip_grad_norm_on_simulated_ranks(hvd, team, kind, dt, norm_type):
             assert team.count('ar', mark) == n and team.count('ag', mark) == 0
             # step 2: the buckets from the unused layer's on were not launched by hooks, clip_grad_norm_ reduces them
             assert (team.count('rs', mark) > 0) == (step == 2)
-            reduced = _reduced_grads(opts, list(models[0].parameters()))
+            reduced = [g.float() for g in reduced_grads(opts, list(models[0].parameters()))]
             mark = len(team.log)
             team.run(lambda r: opts[r].step())
             assert team.count('rs', mark) == 0, 'step() reduced a second time'
@@ -400,13 +241,14 @@ def test_clip_grad_norm_on_simulated_ranks(hvd, team, kind, dt, norm_type):
 
 def test_clip_grad_norm_rejections(hvd, team):
     torch.manual_seed(0)
-    base = _ConvNet().cuda()
-    models, opts = _sharded(hvd, team, base, lambda m: torch.optim.AdamW(m.parameters(), lr=1e-2), torch.float32)
+    base = ConvNetWithUnused().cuda()
+    models, opts = sharded_team(hvd, team, copy.deepcopy(base).to(memory_format=torch.channels_last),
+                                lambda m: torch.optim.AdamW(m.parameters(), lr=1e-2), min_buckets=3)
     for bad in (1.0, 0.0, 3.0, -math.inf):
         with pytest.raises(ValueError):
             opts[0].clip_grad_norm_(1.0, norm_type=bad)
     for r in range(team.n):
-        x, y = _batch(0, r)
+        x, y = batch(0, r)
         torch.nn.functional.cross_entropy(models[r](x), y).backward()
     with pytest.raises(AssertionError):
         opts[0].zero_grad()  # between backward and clip: the reduce-scatters may still read the gradients
@@ -422,12 +264,13 @@ def test_sharded_grad_scaler_on_simulated_ranks(hvd, team):
     from horovod_b200.torch.grad_buckets import shard_range, shard_slices
     n = team.n
     torch.manual_seed(0)
-    base = _ConvNet().cuda()
+    base = ConvNetWithUnused().cuda()
 
     def make(m):
         return torch.optim.AdamW(m.parameters(), lr=1e-2, eps=1e-3, weight_decay=0.05)  # eps: see the clip test
 
-    models, opts = _sharded(hvd, team, base, make, torch.float16)
+    models, opts = sharded_team(hvd, team, copy.deepcopy(base).to(dtype=torch.float16, memory_format=torch.channels_last),
+                                make, torch.float16, min_buckets=3)
     scalers = [hvd.ShardedGradScaler('cuda', init_scale=256.0) for _ in range(n)]
     ref = copy.deepcopy(base).to(memory_format=torch.channels_last)
     ref_opt = make(ref)
@@ -441,7 +284,7 @@ def test_sharded_grad_scaler_on_simulated_ranks(hvd, team):
     for step in range(6):
         grads = [torch.zeros_like(p) for p in ref.parameters()]
         for r in range(n):
-            x, y = _batch(step, r)
+            x, y = batch(step, r)
             ref.zero_grad()
             ref_scaler.scale(torch.nn.functional.cross_entropy(ref(x), y)).backward()
             for g, p in zip(grads, ref.parameters()):
@@ -458,7 +301,7 @@ def test_sharded_grad_scaler_on_simulated_ranks(hvd, team):
 
         for r in range(n):
             opts[r].zero_grad()
-            x, y = _batch(step, r)
+            x, y = batch(step, r)
             scalers[r].scale(torch.nn.functional.cross_entropy(models[r](x.half()), y)).backward()
         if step == 2:
             opts[0]._buckets[0]['gflat'][pos] = math.inf  # rank 0's local gradient; the reduce-scatter is still queued
@@ -514,8 +357,8 @@ def test_sharded_grad_scaler_defers_to_torch_for_other_optimizers(hvd):
     assert all(torch.equal(a, b) for a, b in zip(runs[0][0], runs[1][0]))
 
 
-@pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
+@pytest.mark.skipif(ngpu() < 2, reason="needs >= 2 GPUs")
 def test_sharded_clip_across_ranks(native_built):
-    n = 2 if _ngpu() < 4 else 4
+    n = 2 if ngpu() < 4 else 4
     rc, out = run_parallel("sharded_clip_worker.py", np=n, timeout=420)
     assert "SHARDED CLIP OK" in out, out[-4000:]
