@@ -65,13 +65,29 @@ template <typename P> __device__ __forceinline__ void reconcile4(float* pv, cons
     if (__float_as_uint(to_f<P>(from_f<P>(wv[k]))) == __float_as_uint(pv[k])) pv[k] = wv[k];
 }
 
+// Exponential moving average epilogue (kEma): after the update, e = fmaf(w, x - e, e) with w = 1 - decay, where x is
+// the fp32 master (kMaster) or the value stored into the parameter, rounded to P.  With `start` set the EMA begins now:
+// e = x, and the old e is not read (zero is a valid EMA, so no value of e can mean "absent").  pv holds the updated
+// fp32 value.  The EMA has its own alignment flag, so it works on unaligned views like the other state.
+template <typename P, bool kMaster>
+__device__ __forceinline__ void ema4(float* e, int64_t i, int64_t n, bool ea, const float* pv, float w, int start) {
+  float ev[kOptVec];
+  if (!start) load4<float>(e, i, n, ea, ev);
+#pragma unroll
+  for (int k = 0; k < kOptVec; ++k) {
+    const float x = kMaster ? pv[k] : to_f<P>(from_f<P>(pv[k]));
+    ev[k] = start ? x : fmaf(w, x - ev[k], ev[k]);
+  }
+  store4<float>(e, i, n, ea, ev);
+}
+
 // `grad_scale_dev` (nullptr: 1) is a factor that lives on the device, e.g. a clip coefficient computed by earlier kernels:
 // it reaches the update without a host synchronisation.  Multiplying by 1.f is exact, so nullptr changes no result.
 // Momentum is stored in the parameter dtype, or in fp32 with a master.
-template <typename P, typename G, bool kMaster>
+template <typename P, typename G, bool kMaster, bool kEma>
 __global__ void __launch_bounds__(kOptThreads)
 fused_sgd_kernel(const OptTensor* __restrict__ table, float lr, float momentum, float dampening, float wd, int nesterov,
-                 float grad_scale, const float* __restrict__ grad_scale_dev, int first_step) {
+                 float grad_scale, const float* __restrict__ grad_scale_dev, int first_step, float ema_w, int ema_start) {
   using M = std::conditional_t<kMaster, float, P>;
   const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
@@ -86,6 +102,8 @@ fused_sgd_kernel(const OptTensor* __restrict__ table, float lr, float momentum, 
   const bool pa = is_aligned<P>(p) && (kMaster || !mbuf || is_aligned<M>(mbuf)), ga = is_aligned<G>(g);
   const bool wa = kMaster && is_aligned<float>(w) && (!mbuf || is_aligned<M>(mbuf));
   const bool ma = kMaster ? wa : pa;
+  float* e = kEma ? reinterpret_cast<float*>(t.ema) : nullptr;
+  const bool ea = kEma && is_aligned<float>(e);
 #pragma unroll
   for (int it = 0; it < kOptIters; ++it) {
     const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
@@ -113,13 +131,14 @@ fused_sgd_kernel(const OptTensor* __restrict__ table, float lr, float momentum, 
     if constexpr (kMaster) store4<float>(w, i, n, wa, pv);
     store4<P>(p, i, n, pa, pv);
     if (mbuf) store4<M>(mbuf, i, n, ma, mv);
+    if constexpr (kEma) ema4<P, kMaster>(e, i, n, ea, pv, ema_w, ema_start);
   }
 }
 
-template <typename P, typename G, bool kMaster>
+template <typename P, typename G, bool kMaster, bool kEma>
 __global__ void __launch_bounds__(kOptThreads)
 fused_adam_kernel(const OptTensor* __restrict__ table, float lr, float b1, float b2, float eps, float wd, float c1, float c2,
-                  float grad_scale, const float* __restrict__ grad_scale_dev, int adamw) {
+                  float grad_scale, const float* __restrict__ grad_scale_dev, int adamw, float ema_w, int ema_start) {
   const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
@@ -133,6 +152,8 @@ fused_adam_kernel(const OptTensor* __restrict__ table, float lr, float b1, float
   const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g),
              sa = is_aligned<float>(m) && is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
   const float rsc2 = rsqrtf(c2), step = lr / c1;
+  float* e = kEma ? reinterpret_cast<float*>(t.ema) : nullptr;
+  const bool ea = kEma && is_aligned<float>(e);
 #pragma unroll
   for (int it = 0; it < kOptIters; ++it) {
     const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
@@ -160,6 +181,7 @@ fused_adam_kernel(const OptTensor* __restrict__ table, float lr, float b1, float
     store4<P>(p, i, n, pa, pv);
     store4<float>(m, i, n, sa, mv);
     store4<float>(v, i, n, sa, vv);
+    if constexpr (kEma) ema4<P, kMaster>(e, i, n, ea, pv, ema_w, ema_start);
   }
 }
 
@@ -262,10 +284,10 @@ lamb_finalize_kernel(const OptTensor* __restrict__ table, const float2* __restri
   }
 }
 
-template <typename P, bool kMaster>
+template <typename P, bool kMaster, bool kEma>
 __global__ void __launch_bounds__(kOptThreads)
 fused_lamb_apply_kernel(const OptTensor* __restrict__ table, float lr, float eps, float wd, float c1, float c2, int adapt,
-                        const float* __restrict__ norms) {
+                        const float* __restrict__ norms, float ema_w, int ema_start) {
   const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
@@ -281,6 +303,8 @@ fused_lamb_apply_kernel(const OptTensor* __restrict__ table, float lr, float eps
   const float* v = reinterpret_cast<const float*>(t.state1);
   float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
   const bool pa = is_aligned<P>(p), sa = is_aligned<float>(m) && is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
+  float* e = kEma ? reinterpret_cast<float*>(t.ema) : nullptr;
+  const bool ea = kEma && is_aligned<float>(e);
 #pragma unroll
   for (int it = 0; it < kOptIters; ++it) {
     const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
@@ -298,6 +322,7 @@ fused_lamb_apply_kernel(const OptTensor* __restrict__ table, float lr, float eps
     for (int k = 0; k < kOptVec; ++k) pv[k] = fmaf(-step, lamb_u(mv[k], vv[k], pv[k], c1, c2, eps, wd), pv[k]);
     if constexpr (kMaster) store4<float>(w, i, n, sa, pv);
     store4<P>(p, i, n, pa, pv);
+    if constexpr (kEma) ema4<P, kMaster>(e, i, n, ea, pv, ema_w, ema_start);
   }
 }
 
@@ -356,10 +381,11 @@ fused_lars_norms_kernel(const OptTensor* __restrict__ table, float grad_scale, c
   }
 }
 
-template <typename P, typename G, bool kMaster>
+template <typename P, typename G, bool kMaster, bool kEma>
 __global__ void __launch_bounds__(kOptThreads)
 fused_lars_apply_kernel(const OptTensor* __restrict__ table, float lr, float momentum, float wd, float tc, float eps,
-                        int adapt, float grad_scale, const float* __restrict__ grad_scale_dev, const float* __restrict__ norms) {
+                        int adapt, float grad_scale, const float* __restrict__ grad_scale_dev, const float* __restrict__ norms,
+                        float ema_w, int ema_start) {
   const OptTensor t = table[blockIdx.y];
   const int64_t n = t.count;
   const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
@@ -376,6 +402,8 @@ fused_lars_apply_kernel(const OptTensor* __restrict__ table, float lr, float mom
   float* v = reinterpret_cast<float*>(t.state0);
   float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
   const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g), sa = is_aligned<float>(v) && (!kMaster || is_aligned<float>(w));
+  float* e = kEma ? reinterpret_cast<float*>(t.ema) : nullptr;
+  const bool ea = kEma && is_aligned<float>(e);
 #pragma unroll
   for (int it = 0; it < kOptIters; ++it) {
     const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
@@ -398,6 +426,7 @@ fused_lars_apply_kernel(const OptTensor* __restrict__ table, float lr, float mom
     if constexpr (kMaster) store4<float>(w, i, n, sa, pv);
     store4<P>(p, i, n, pa, pv);
     store4<float>(v, i, n, sa, vv);
+    if constexpr (kEma) ema4<P, kMaster>(e, i, n, ea, pv, ema_w, ema_start);
   }
 }
 
@@ -547,7 +576,8 @@ grad_accumulate_kernel(const AccTable table, int mode) {
 }
 
 // The (param, grad, master) instantiations of the optimizer kernels: launch(OptTypes<P, G, kMaster>()) for a pair that
-// has one, then the launch is counted and checked; cudaErrorInvalidValue without launching for any other pair.
+// has one, then the launch is counted and checked; cudaErrorInvalidValue without launching for any other pair.  The
+// updates that keep an EMA pick their kEma instantiation inside `launch`, so EMA off runs the kernels it always ran.
 template <typename P_, typename G_, bool kMaster_> struct OptTypes {
   using P = P_;
   using G = G_;
@@ -587,24 +617,33 @@ int64_t NormPartials(int64_t count) { return (count + kOptPerBlock - 1) / kOptPe
 
 cudaError_t LaunchFusedSgd(const OptTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
                            float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
-                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev, bool master) {
+                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev, bool master, const OptEma& ema) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
   return DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
     using T = decltype(t);
-    fused_sgd_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
-        table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step);
+    if (ema.on)
+      fused_sgd_kernel<typename T::P, typename T::G, T::kMaster, true><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step, ema.weight, ema.start);
+    else
+      fused_sgd_kernel<typename T::P, typename T::G, T::kMaster, false><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, lr, momentum, dampening, weight_decay, nesterov, grad_scale, grad_scale_dev, first_step, 0.f, 0);
   });
 }
 
 cudaError_t LaunchFusedAdamW(const OptTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
                              float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale, int adamw,
                              int param_dtype, int grad_dtype, cudaStream_t stream, const float* grad_scale_dev,
-                             bool master) {
+                             bool master, const OptEma& ema) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
   return DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
     using T = decltype(t);
-    fused_adam_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
-        table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw);
+    if (ema.on)
+      fused_adam_kernel<typename T::P, typename T::G, T::kMaster, true><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw, ema.weight,
+          ema.start);
+    else
+      fused_adam_kernel<typename T::P, typename T::G, T::kMaster, false><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, lr, beta1, beta2, eps, weight_decay, bias_c1, bias_c2, grad_scale, grad_scale_dev, adamw, 0.f, 0);
   });
 }
 
@@ -622,13 +661,17 @@ cudaError_t LaunchLambNorms(const OptTensor* table, int n, int64_t max_count, fl
 
 cudaError_t LaunchLambApply(const OptTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
                             float bias_c1, float bias_c2, int adapt, const float* norms, int param_dtype, bool master,
-                            cudaStream_t stream) {
+                            cudaStream_t stream, const OptEma& ema) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
   // the gradient is not read: dispatch on the parameter dtype alone
   return DispatchOpt(param_dtype, param_dtype, master, [&](auto t) {
     using T = decltype(t);
-    fused_lamb_apply_kernel<typename T::P, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
-        table, lr, eps, weight_decay, bias_c1, bias_c2, adapt, norms);
+    if (ema.on)
+      fused_lamb_apply_kernel<typename T::P, T::kMaster, true><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, lr, eps, weight_decay, bias_c1, bias_c2, adapt, norms, ema.weight, ema.start);
+    else
+      fused_lamb_apply_kernel<typename T::P, T::kMaster, false><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, lr, eps, weight_decay, bias_c1, bias_c2, adapt, norms, 0.f, 0);
   });
 }
 
@@ -645,12 +688,18 @@ cudaError_t LaunchLarsNorms(const OptTensor* table, int n, int64_t max_count, fl
 
 cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, float lr, float momentum, float weight_decay,
                             float trust_coefficient, float eps, int adapt, float grad_scale, const float* grad_scale_dev,
-                            const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream) {
+                            const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream,
+                            const OptEma& ema) {
   if (n <= 0 || max_count <= 0) return cudaSuccess;
   return DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
     using T = decltype(t);
-    fused_lars_apply_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
-        table, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, grad_scale_dev, norms);
+    if (ema.on)
+      fused_lars_apply_kernel<typename T::P, typename T::G, T::kMaster, true><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, grad_scale_dev, norms, ema.weight,
+          ema.start);
+    else
+      fused_lars_apply_kernel<typename T::P, typename T::G, T::kMaster, false><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, grad_scale_dev, norms, 0.f, 0);
   });
 }
 

@@ -163,19 +163,26 @@ int AdasumNumLaunches(int nranks);
 //   state0         SGD and LARS: the momentum buffer (SGD: nullptr without momentum); Adam and LAMB: exp_avg
 //   state1         Adam and LAMB: exp_avg_sq; SGD and LARS do not read it
 //   partial, slot  LAMB and LARS only: the entry's first stage-1 partial and its norm slot (see LaunchLambNorms)
+//   ema            with `ema.on`: the fp32 exponential moving average of the parameter (see OptEma); otherwise not read
 // Every state is fp32, except SGD momentum without `master`, which has the parameter dtype.  The (param, grad) dtypes are
 // fp32 / fp32, fp32 / bf16, bf16 / bf16 and fp16 / fp16; with `master` bf16 / bf16 and fp16 / fp16 only.  Any other
 // combination returns cudaErrorInvalidValue before anything is launched.  The gradient factor is
 // grad_scale * *grad_scale_dev (nullptr: grad_scale alone, bit for bit).
 struct OptTensor { void* param; const void* grad; void* master; void* state0; void* state1; int64_t count;
-                   int64_t partial; int64_t slot; };
+                   int64_t partial; int64_t slot; void* ema; };
+// The EMA epilogue of the SGD, Adam, LAMB-apply and LARS-apply launches: with `on`, every entry's `ema` becomes
+// fmaf(weight, x - ema, ema) after the update (weight = 1 - decay), x being the fp32 master with `master`, else the value
+// stored into the parameter; with `start` as well, ema = x (the EMA begins with this update).  Off: the kernels without
+// the epilogue run, and `ema` is not read.
+struct OptEma { bool on = false; float weight = 0.f; int start = 0; };
 cudaError_t LaunchFusedSgd(const OptTensor* table, int n, int64_t max_count, float lr, float momentum, float dampening,
                            float weight_decay, int nesterov, float grad_scale, int first_step, int param_dtype,
-                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev = nullptr, bool master = false);
+                           int grad_dtype, cudaStream_t stream, const float* grad_scale_dev = nullptr, bool master = false,
+                           const OptEma& ema = OptEma());
 cudaError_t LaunchFusedAdamW(const OptTensor* table, int n, int64_t max_count, float lr, float beta1, float beta2,
                              float eps, float weight_decay, float bias_c1, float bias_c2, float grad_scale,
                              int adamw, int param_dtype, int grad_dtype, cudaStream_t stream,
-                             const float* grad_scale_dev = nullptr, bool master = false);
+                             const float* grad_scale_dev = nullptr, bool master = false, const OptEma& ema = OptEma());
 // Fused LAMB in two phases (see optim_kernels.cu), so that the norms can be allreduced in between.  Entry i covers
 // `count` elements of a parameter whose whole-tensor norms live in norms[2 * slot] (sum w^2) and norms[2 * slot + 1]
 // (sum u^2); its stage-1 CTA partials start at `partial`, the running sum of NormPartials(count) over the entries before
@@ -189,7 +196,7 @@ cudaError_t LaunchLambNorms(const OptTensor* table, int n, int64_t max_count, fl
                             float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
 cudaError_t LaunchLambApply(const OptTensor* table, int n, int64_t max_count, float lr, float eps, float weight_decay,
                             float bias_c1, float bias_c2, int adapt, const float* norms, int param_dtype, bool master,
-                            cudaStream_t stream);
+                            cudaStream_t stream, const OptEma& ema = OptEma());
 // Fused LARS on LAMB's table and norms layout: norms[2 * slot] = sum w^2, norms[2 * slot + 1] = sum g^2 of the scaled
 // gradient.  LaunchLarsNorms: two launches, nothing but `partial` and `norms` written.  LaunchLarsApply:
 // v = momentum * v + lr * r * (g + wd * w), w -= v (one launch; reads the gradient again, scaled by
@@ -198,7 +205,8 @@ cudaError_t LaunchLarsNorms(const OptTensor* table, int n, int64_t max_count, fl
                             float* partial, float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
 cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, float lr, float momentum, float weight_decay,
                             float trust_coefficient, float eps, int adapt, float grad_scale, const float* grad_scale_dev,
-                            const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream);
+                            const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream,
+                            const OptEma& ema = OptEma());
 // Gradient statistics of flat gradient shards in one pass (see optim_kernels.cu): optional in-place scaling by
 // *inv_scale, then out[0] += sum of squares (norm_inf: out[0] = max(out[0], max |g|)) and out[1] = max(out[1], non-finite).
 // Entries are non-empty and in order; tile_begin is the sum of GradShardStatsTiles(count) of the entries before, `tiles`

@@ -549,7 +549,18 @@ struct OptPlan {
   int param_dtype = 0, grad_dtype = 0;
   bool master = false;
   const float* grad_scale_dev = nullptr;
+  kern::OptEma ema;
 };
+
+// The EMA of one optimizer call (optional, empty list: none): one fp32 tensor per param with its sizes, strides and
+// device, updated after the parameter with weight = 1 - decay; `start` begins every one of them at the updated value.
+struct EmaArgs {
+  const std::vector<at::Tensor>& list;
+  double weight;
+  bool start;
+};
+const std::vector<at::Tensor> kNoTensors;
+const EmaArgs kNoEma{kNoTensors, 0.0, false};
 
 // Checks every argument of one optimizer call and builds its table; nothing is staged or launched here.  Entry i is
 // params[i] with grads[i], masters[i] and each state list's element in its field.  `norms` (LAMB and LARS; nullptr:
@@ -558,13 +569,15 @@ struct OptPlan {
 OptPlan PlanOpt(const char* op, const std::vector<at::Tensor>& params, const std::vector<at::Tensor>& grads,
                 const std::vector<OptState>& states, const std::vector<at::Tensor>& masters,
                 const c10::optional<at::Tensor>& grad_scale_dev, const at::Tensor* norms = nullptr,
-                const std::vector<int64_t>& slots = {}) {
+                const std::vector<int64_t>& slots = {}, const EmaArgs& ema = kNoEma) {
   bool sizes = params.size() == grads.size();
   for (const auto& st : states) sizes = sizes && st.list.size() == params.size();
   TORCH_CHECK(sizes, op, ": list sizes differ");
   TORCH_CHECK(masters.empty() || masters.size() == params.size(), op, ": ", masters.size(), " master params for ",
               params.size(), " params");
   TORCH_CHECK(slots.empty() || slots.size() == params.size(), op, ": ", slots.size(), " slots for ", params.size(), " params");
+  TORCH_CHECK(ema.list.empty() || ema.list.size() == params.size(), op, ": ", ema.list.size(), " ema params for ",
+              params.size(), " params");
   OptPlan plan;
   if (params.empty()) return plan;
   for (size_t i = 0; i < params.size(); ++i) {
@@ -572,6 +585,8 @@ OptPlan PlanOpt(const char* op, const std::vector<at::Tensor>& params, const std
     CheckOptimizerPeer(op, "grads", i, params[i], grads[i], grads[0].scalar_type());
   }
   plan.master = CheckMasters(op, params, grads, masters);
+  for (size_t i = 0; i < ema.list.size(); ++i) CheckOptimizerPeer(op, "ema_params", i, params[i], ema.list[i], at::kFloat);
+  plan.ema = kern::OptEma{!ema.list.empty(), (float)ema.weight, ema.start ? 1 : 0};
   for (const auto& st : states)
     for (size_t i = 0; i < params.size(); ++i)
       CheckOptimizerPeer(op, st.name, i, params[i], st.list[i],
@@ -596,6 +611,7 @@ OptPlan PlanOpt(const char* op, const std::vector<at::Tensor>& params, const std
     kern::OptTensor t{};
     t.param = params[i].data_ptr(); t.grad = grads[i].data_ptr();
     t.master = plan.master ? masters[i].data_ptr() : nullptr;
+    t.ema = plan.ema.on ? ema.list[i].data_ptr() : nullptr;
     for (const auto& st : states) t.*st.field = st.list[i].data_ptr();
     t.count = params[i].numel();
     if (norms != nullptr) {
@@ -636,31 +652,34 @@ float BiasCorrection(const char* op, double beta, int64_t step) {
 
 void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momenta, double lr,
                   double momentum, double dampening, double weight_decay, bool nesterov, double grad_scale, bool first_step,
-                  c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
+                  c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters, std::vector<at::Tensor> emas,
+                  double ema_weight, bool ema_start) {
   const bool has_mom = momentum != 0.0;
   // without momentum the buffers are not read: none, or a list of the params' length
   TORCH_CHECK(has_mom || momenta.empty() || momenta.size() == params.size(),
               "fused_sgd: ", momenta.size(), " momentum buffers for ", params.size(), " params");
   std::vector<OptState> states;
   if (has_mom) states.push_back({"momentum_buffers", momenta, &kern::OptTensor::state0, true});
-  const OptPlan plan = PlanOpt("fused_sgd", params, grads, states, masters, grad_scale_dev);
+  const OptPlan plan = PlanOpt("fused_sgd", params, grads, states, masters, grad_scale_dev, nullptr, {},
+                               EmaArgs{emas, ema_weight, ema_start});
   RunPlan("fused_sgd", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
     return kern::LaunchFusedSgd(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)momentum, (float)dampening,
                                 (float)weight_decay, nesterov ? 1 : 0, (float)grad_scale, first_step ? 1 : 0,
-                                plan.param_dtype, plan.grad_dtype, s, plan.grad_scale_dev, plan.master);
+                                plan.param_dtype, plan.grad_dtype, s, plan.grad_scale_dev, plan.master, plan.ema);
   });
 }
 
 void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
                    std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
                    int64_t step, double grad_scale, bool adamw, c10::optional<at::Tensor> grad_scale_dev,
-                   std::vector<at::Tensor> masters) {
+                   std::vector<at::Tensor> masters, std::vector<at::Tensor> emas, double ema_weight, bool ema_start) {
   const float c1 = BiasCorrection("fused_adam", beta1, step), c2 = BiasCorrection("fused_adam", beta2, step);
-  const OptPlan plan = PlanOpt("fused_adam", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev);
+  const OptPlan plan = PlanOpt("fused_adam", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev,
+                               nullptr, {}, EmaArgs{emas, ema_weight, ema_start});
   RunPlan("fused_adam", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
     return kern::LaunchFusedAdamW(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)beta1, (float)beta2,
                                   (float)eps, (float)weight_decay, c1, c2, (float)grad_scale, adamw ? 1 : 0,
-                                  plan.param_dtype, plan.grad_dtype, s, plan.grad_scale_dev, plan.master);
+                                  plan.param_dtype, plan.grad_dtype, s, plan.grad_scale_dev, plan.master, plan.ema);
   });
 }
 
@@ -690,7 +709,8 @@ cudaError_t LambNormsPhase(const OptPlan& plan, const kern::OptTensor* dt, const
 cudaError_t LambApplyPhase(const OptPlan& plan, const kern::OptTensor* dt, const LambArgs& a, double lr, bool adapt,
                            const at::Tensor& norms, cudaStream_t s) {
   return kern::LaunchLambApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)a.eps, (float)a.weight_decay,
-                               a.c1, a.c2, adapt ? 1 : 0, norms.data_ptr<float>(), plan.param_dtype, plan.master, s);
+                               a.c1, a.c2, adapt ? 1 : 0, norms.data_ptr<float>(), plan.param_dtype, plan.master, s,
+                               plan.ema);
 }
 
 // Phase 1: moments, then the squared norms of every entry ADDED into norms[2 * slot], norms[2 * slot + 1].
@@ -710,10 +730,10 @@ void LambNorms(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
 void LambApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
                std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
                int64_t step, bool bias_correction, bool adapt, std::vector<at::Tensor> masters, at::Tensor norms,
-               std::vector<int64_t> slots) {
+               std::vector<int64_t> slots, std::vector<at::Tensor> emas, double ema_weight, bool ema_start) {
   const LambArgs a = LambHyper("lamb_apply", beta1, beta2, eps, weight_decay, step, bias_correction);
   const OptPlan plan = PlanOpt("lamb_apply", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, c10::nullopt,
-                               &norms, slots);
+                               &norms, slots, EmaArgs{emas, ema_weight, ema_start});
   RunPlan("lamb_apply", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
     return LambApplyPhase(plan, dt, a, lr, adapt, norms, s);
   });
@@ -729,11 +749,12 @@ at::Tensor FreshNorms(const char* op, const std::vector<at::Tensor>& params) {
 void FusedLambStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
                    std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
                    int64_t step, bool bias_correction, bool adapt, double grad_scale,
-                   c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
+                   c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters, std::vector<at::Tensor> emas,
+                   double ema_weight, bool ema_start) {
   at::Tensor norms = FreshNorms("fused_lamb", params);
   const LambArgs a = LambHyper("fused_lamb", beta1, beta2, eps, weight_decay, step, bias_correction);
   const OptPlan plan = PlanOpt("fused_lamb", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev,
-                               &norms);
+                               &norms, {}, EmaArgs{emas, ema_weight, ema_start});
   RunPlan("fused_lamb", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
     const cudaError_t e = LambNormsPhase(plan, dt, a, grad_scale, norms, s);
     return e != cudaSuccess ? e : LambApplyPhase(plan, dt, a, lr, adapt, norms, s);
@@ -758,7 +779,7 @@ cudaError_t LarsApplyPhase(const OptPlan& plan, const kern::OptTensor* dt, doubl
                            cudaStream_t s) {
   return kern::LaunchLarsApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)momentum, (float)weight_decay,
                                (float)trust_coefficient, (float)eps, adapt ? 1 : 0, (float)grad_scale, plan.grad_scale_dev,
-                               norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype, plan.master, s);
+                               norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype, plan.master, s, plan.ema);
 }
 
 // LARS phase 1: the squared norms of every entry's parameter and scaled gradient ADDED into norms[2 * slot],
@@ -778,9 +799,10 @@ void LarsNorms(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
 void LarsApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momentum_buffers,
                double lr, double momentum, double weight_decay, double trust_coefficient, double eps, bool adapt,
                double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters,
-               at::Tensor norms, std::vector<int64_t> slots) {
+               at::Tensor norms, std::vector<int64_t> slots, std::vector<at::Tensor> emas, double ema_weight,
+               bool ema_start) {
   const OptPlan plan = PlanOpt("lars_apply", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &norms,
-                               slots);
+                               slots, EmaArgs{emas, ema_weight, ema_start});
   RunPlan("lars_apply", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
     return LarsApplyPhase(plan, dt, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, norms, s);
   });
@@ -789,9 +811,11 @@ void LarsApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
 // Both LARS phases: three launches, one staged table.
 void FusedLarsStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momentum_buffers,
                    double lr, double momentum, double weight_decay, double trust_coefficient, double eps, bool adapt,
-                   double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters) {
+                   double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters,
+                   std::vector<at::Tensor> emas, double ema_weight, bool ema_start) {
   at::Tensor norms = FreshNorms("fused_lars", params);
-  const OptPlan plan = PlanOpt("fused_lars", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &norms);
+  const OptPlan plan = PlanOpt("fused_lars", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &norms,
+                               {}, EmaArgs{emas, ema_weight, ema_start});
   RunPlan("fused_lars", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
     const cudaError_t e = LarsNormsPhase(plan, dt, grad_scale, norms, s);
     return e != cudaSuccess ? e : LarsApplyPhase(plan, dt, lr, momentum, weight_decay, trust_coefficient, eps, adapt,
@@ -1125,30 +1149,36 @@ PYBIND11_MODULE(_hvd_torch, m) {
         py::arg("channel") = kern::kGraphChannel);
   m.def("fused_sgd_step", &FusedSgdStep, py::arg("params"), py::arg("grads"), py::arg("momenta"), py::arg("lr"),
         py::arg("momentum"), py::arg("dampening"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("grad_scale"),
-        py::arg("first_step"), py::arg("grad_scale_dev") = py::none(), py::arg("master_params") = std::vector<at::Tensor>());
+        py::arg("first_step"), py::arg("grad_scale_dev") = py::none(), py::arg("master_params") = std::vector<at::Tensor>(),
+        py::arg("ema_params") = std::vector<at::Tensor>(), py::arg("ema_weight") = 0.0, py::arg("ema_start") = false);
   m.def("fused_adam_step", &FusedAdamStep, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
         py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
         py::arg("grad_scale"), py::arg("adamw"), py::arg("grad_scale_dev") = py::none(),
-        py::arg("master_params") = std::vector<at::Tensor>());
+        py::arg("master_params") = std::vector<at::Tensor>(),
+        py::arg("ema_params") = std::vector<at::Tensor>(), py::arg("ema_weight") = 0.0, py::arg("ema_start") = false);
   m.def("fused_lamb_step", &FusedLambStep, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
         py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
         py::arg("bias_correction"), py::arg("adapt"), py::arg("grad_scale"), py::arg("grad_scale_dev") = py::none(),
-        py::arg("master_params") = std::vector<at::Tensor>());
+        py::arg("master_params") = std::vector<at::Tensor>(),
+        py::arg("ema_params") = std::vector<at::Tensor>(), py::arg("ema_weight") = 0.0, py::arg("ema_start") = false);
   m.def("lamb_norms", &LambNorms, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
         py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
         py::arg("bias_correction"), py::arg("grad_scale"), py::arg("grad_scale_dev"), py::arg("master_params"),
         py::arg("out"), py::arg("slots"));
   m.def("lamb_apply", &LambApply, py::arg("params"), py::arg("grads"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
         py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("step"),
-        py::arg("bias_correction"), py::arg("adapt"), py::arg("master_params"), py::arg("norms"), py::arg("slots"));
+        py::arg("bias_correction"), py::arg("adapt"), py::arg("master_params"), py::arg("norms"), py::arg("slots"),
+        py::arg("ema_params") = std::vector<at::Tensor>(), py::arg("ema_weight") = 0.0, py::arg("ema_start") = false);
   m.def("fused_lars_step", &FusedLarsStep, py::arg("params"), py::arg("grads"), py::arg("momentum_buffers"), py::arg("lr"),
         py::arg("momentum"), py::arg("weight_decay"), py::arg("trust_coefficient"), py::arg("eps"), py::arg("adapt"),
-        py::arg("grad_scale"), py::arg("grad_scale_dev") = py::none(), py::arg("master_params") = std::vector<at::Tensor>());
+        py::arg("grad_scale"), py::arg("grad_scale_dev") = py::none(), py::arg("master_params") = std::vector<at::Tensor>(),
+        py::arg("ema_params") = std::vector<at::Tensor>(), py::arg("ema_weight") = 0.0, py::arg("ema_start") = false);
   m.def("lars_norms", &LarsNorms, py::arg("params"), py::arg("grads"), py::arg("momentum_buffers"), py::arg("grad_scale"),
         py::arg("grad_scale_dev"), py::arg("master_params"), py::arg("out"), py::arg("slots"));
   m.def("lars_apply", &LarsApply, py::arg("params"), py::arg("grads"), py::arg("momentum_buffers"), py::arg("lr"),
         py::arg("momentum"), py::arg("weight_decay"), py::arg("trust_coefficient"), py::arg("eps"), py::arg("adapt"),
-        py::arg("grad_scale"), py::arg("grad_scale_dev"), py::arg("master_params"), py::arg("norms"), py::arg("slots"));
+        py::arg("grad_scale"), py::arg("grad_scale_dev"), py::arg("master_params"), py::arg("norms"), py::arg("slots"),
+        py::arg("ema_params") = std::vector<at::Tensor>(), py::arg("ema_weight") = 0.0, py::arg("ema_start") = false);
   m.def("grad_shard_stats", &GradShardStats, py::arg("grads"), py::arg("out"), py::arg("inv_scale") = py::none(),
         py::arg("norm_inf") = false);
   m.def("grad_accumulate", &GradAccumulate, py::arg("grads"), py::arg("accs"), py::arg("mode"));

@@ -22,8 +22,18 @@ def _native():
     return n()
 
 
+def _ema(ema_params, ema_decay, ema_start):
+    """The native EMA arguments: (fp32 EMA tensors, weight 1 - decay, start).  No EMA: ([], 0.0, False)."""
+    if not ema_params:
+        return [], 0.0, False
+    if ema_decay is None or not 0.0 <= float(ema_decay) <= 1.0:
+        raise ValueError('ema_decay must be in [0, 1] with ema_params, got %r' % (ema_decay,))
+    return list(ema_params), 1.0 - float(ema_decay), bool(ema_start)
+
+
 def fused_sgd_step(params, grads, momentum_buffers, lr, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False,
-                   grad_scale=1.0, first_step=False, grad_scale_dev=None, master_params=None):
+                   grad_scale=1.0, first_step=False, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
+                   ema_start=False):
     """One launch for the whole parameter list (fp32 / bf16 / fp16 parameters, fp32 or matching gradients).
     `grad_scale_dev`: an optional 1-element fp32 tensor on the parameters' device; the gradients are multiplied by
     grad_scale * grad_scale_dev[0], read by the kernel, so no host synchronisation is needed.
@@ -31,25 +41,31 @@ def fused_sgd_step(params, grads, momentum_buffers, lr, momentum=0.0, dampening=
     `master_params`: optional fp32 master copies of bf16 / fp16 parameters (gradients of the parameters' dtype), one per
     parameter with its sizes and strides; momentum buffers are then fp32 too. The update runs on the master and the
     parameter receives it rounded to nearest-even. Where a parameter no longer equals its rounded master (it was
-    written from outside, or the master is zero-filled), the master first restarts from the parameter."""
+    written from outside, or the master is zero-filled), the master first restarts from the parameter.
+
+    `ema_params`: optional fp32 exponential moving averages, one per parameter with its sizes and strides, updated in the
+    same launch after the parameter: e = fmaf(1 - ema_decay, x - e, e) in fp32, with x the updated master if there is
+    one, else the value stored into the parameter.  `ema_start=True` begins them: e = x, without reading e."""
     return _native().fused_sgd_step(list(params), list(grads), list(momentum_buffers), float(lr), float(momentum), float(dampening),
                                     float(weight_decay), bool(nesterov), float(grad_scale), bool(first_step), grad_scale_dev,
-                                    list(master_params or []))
+                                    list(master_params or []), *_ema(ema_params, ema_decay, ema_start))
 
 
 def fused_adam_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, step=1,
-                    grad_scale=1.0, adamw=True, grad_scale_dev=None, master_params=None):
+                    grad_scale=1.0, adamw=True, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
+                    ema_start=False):
     """One launch of Adam / AdamW for the whole parameter list (fp32 / bf16 / fp16 parameters, fp32 or matching
     gradients, fp32 state with the parameters' sizes and strides; `step` is the 1-based step count). Mismatched
-    lists, dtypes, sizes, strides or devices raise RuntimeError before anything is launched. `grad_scale_dev` and
-    `master_params` as in fused_sgd_step."""
+    lists, dtypes, sizes, strides or devices raise RuntimeError before anything is launched. `grad_scale_dev`,
+    `master_params` and the EMA arguments as in fused_sgd_step."""
     return _native().fused_adam_step(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1), float(beta2),
                                      float(eps), float(weight_decay), int(step), float(grad_scale), bool(adamw), grad_scale_dev,
-                                     list(master_params or []))
+                                     list(master_params or []), *_ema(ema_params, ema_decay, ema_start))
 
 
 def fused_lamb_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1, beta2, eps, weight_decay, step, bias_correction=True,
-                    adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None):
+                    adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
+                    ema_start=False):
     """One LAMB step for the whole parameter list in three launches (moments and per-CTA norm partials, the per-tensor
     norms, the update), with the argument rules of fused_adam_step. For each parameter w (1-based `step`):
 
@@ -57,10 +73,12 @@ def fused_lamb_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1, beta2, eps,
         u = (m / c1) / (sqrt(v / c2) + eps) + weight_decay * w      (c1 = 1 - b1^step, c2 = 1 - b2^step; 1 without bias_correction)
         w -= lr * r * u,   r = ||w|| / ||u|| if adapt and both norms are > 0, else 1
 
+    The EMA arguments are those of fused_sgd_step; the update launch writes the EMA.
     Deterministic: the same input gives the same bits on every call. Nothing is synchronised with the host."""
     return _native().fused_lamb_step(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1),
                                      float(beta2), float(eps), float(weight_decay), int(step), bool(bias_correction),
-                                     bool(adapt), float(grad_scale), grad_scale_dev, list(master_params or []))
+                                     bool(adapt), float(grad_scale), grad_scale_dev, list(master_params or []),
+                                     *_ema(ema_params, ema_decay, ema_start))
 
 
 def lamb_norms(params, grads, exp_avgs, exp_avg_sqs, beta1, beta2, eps, weight_decay, step, out, slots=None,
@@ -77,19 +95,21 @@ def lamb_norms(params, grads, exp_avgs, exp_avg_sqs, beta1, beta2, eps, weight_d
 
 
 def lamb_apply(params, grads, exp_avgs, exp_avg_sqs, lr, beta1, beta2, eps, weight_decay, step, norms, slots=None,
-               bias_correction=True, adapt=True, master_params=None):
+               bias_correction=True, adapt=True, master_params=None, ema_params=None, ema_decay=None, ema_start=False):
     """Second phase: w -= lr * r * u, with u recomputed from the moments of lamb_norms and r from the whole-tensor sums of
     squares in `norms` (e.g. after adding up every rank's pieces). `grads` are checked as in lamb_norms but not read.
-    One launch."""
+    One launch, which also updates the EMA (arguments as in fused_sgd_step)."""
     n = len(params)
     return _native().lamb_apply(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1),
                                 float(beta2), float(eps), float(weight_decay), int(step), bool(bias_correction),
                                 bool(adapt), list(master_params or []), norms,
-                                list(range(n)) if slots is None else [int(s) for s in slots])
+                                list(range(n)) if slots is None else [int(s) for s in slots],
+                                *_ema(ema_params, ema_decay, ema_start))
 
 
 def fused_lars_step(params, grads, momentum_buffers, lr, momentum=0.9, weight_decay=0.0, trust_coefficient=0.001, eps=0.0,
-                    adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None):
+                    adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
+                    ema_start=False):
     """One LARS step for the whole parameter list in three launches (per-CTA norm partials, the per-tensor norms, the
     update), with the argument rules of fused_adam_step; the momentum buffers are fp32. For each parameter w:
 
@@ -97,10 +117,12 @@ def fused_lars_step(params, grads, momentum_buffers, lr, momentum=0.9, weight_de
         r = trust_coefficient * ||w|| / (||g|| + weight_decay * ||w|| + eps) if adapt and both norms are > 0, else 1
         v = momentum * v + lr * r * d;  w -= v
 
+    The EMA arguments are those of fused_sgd_step; the update launch writes the EMA.
     Deterministic: the same input gives the same bits on every call. Nothing is synchronised with the host."""
     return _native().fused_lars_step(list(params), list(grads), list(momentum_buffers), float(lr), float(momentum),
                                      float(weight_decay), float(trust_coefficient), float(eps), bool(adapt),
-                                     float(grad_scale), grad_scale_dev, list(master_params or []))
+                                     float(grad_scale), grad_scale_dev, list(master_params or []),
+                                     *_ema(ema_params, ema_decay, ema_start))
 
 
 def lars_norms(params, grads, momentum_buffers, out, slots=None, grad_scale=1.0, grad_scale_dev=None, master_params=None):
@@ -113,15 +135,17 @@ def lars_norms(params, grads, momentum_buffers, out, slots=None, grad_scale=1.0,
 
 
 def lars_apply(params, grads, momentum_buffers, lr, momentum, weight_decay, trust_coefficient, eps, norms, slots=None,
-               adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None):
+               adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
+               ema_start=False):
     """Second phase: the momentum and parameter update of fused_lars_step, with r from the whole-tensor sums of squares
     in `norms` (e.g. after adding up every rank's pieces). Reads the gradient again: pass the grad_scale /
-    grad_scale_dev of lars_norms. One launch."""
+    grad_scale_dev of lars_norms. One launch, which also updates the EMA (arguments as in fused_sgd_step)."""
     n = len(params)
     return _native().lars_apply(list(params), list(grads), list(momentum_buffers), float(lr), float(momentum),
                                 float(weight_decay), float(trust_coefficient), float(eps), bool(adapt), float(grad_scale),
                                 grad_scale_dev, list(master_params or []), norms,
-                                list(range(n)) if slots is None else [int(s) for s in slots])
+                                list(range(n)) if slots is None else [int(s) for s in slots],
+                                *_ema(ema_params, ema_decay, ema_start))
 
 
 def grad_shard_stats(tensors, out, inv_scale=None, norm_type=2.0):

@@ -9,6 +9,7 @@ tensor), and `fused=True` replaces the wrapped SGD/Adam(W) math by one
 multi-tensor sm_90a kernel (csrc/kernels/optim_kernels.cu).
 """
 import math
+import numbers
 import os
 import warnings
 from contextlib import contextmanager
@@ -34,7 +35,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
                  fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None, master_weights=False,
-                 grad_accumulation_dtype=None):
+                 grad_accumulation_dtype=None, ema_decay=None):
         super(self.__class__, self).__init__(params)
         self._compression = compression
         # fp32 accumulators of bf16 / fp16 gradients over the backward passes of one step (allocated on first use, not
@@ -45,7 +46,10 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         # fp32 master copies of bf16 / fp16 parameters, kept as optimizer state ('master_param') and updated by the fused
         # kernels only: master_weights implies fused, and step() never hands those parameters to torch's own update
         self._master_weights = bool(master_weights)
-        fused = fused or self._master_weights
+        # fp32 exponential moving average of every trainable parameter, kept as optimizer state ('ema_param') and written
+        # by the fused update kernels only: ema_decay implies fused, like master_weights
+        self._ema = init_ema(self, ema_decay)
+        fused = fused or self._master_weights or self._ema
         # opt-in: fp32 gradient buckets travel as bf16 / fp16 (a registered shadow bucket of half the bytes is what the
         # zero-copy kernel reduces; the switch accumulates in fp32).  Not validated on hardware yet (docs/roadmap.md B3).
         if bucket_wire_dtype is None:
@@ -107,27 +111,34 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     # -- reference API ----------------------------------------------------------
     def load_state_dict(self, *args, **kwargs):
+        if self._ema_active:
+            raise RuntimeError('load_state_dict() inside ema_parameters(): the block restores the parameters on exit')
         self._handles = {}
         self._synchronized = False
         self._should_synchronize = True
         for p in self._allreduce_delay:
             self._allreduce_delay[p] = self.backward_passes_per_step
         self._reset_folds()
+        decays = [g.get('ema_decay') for g in self.param_groups]
         super(self.__class__, self).load_state_dict(*args, **kwargs)
+        for g, d in zip(self.param_groups, decays):
+            if d is not None:
+                g.setdefault('ema_decay', d)  # a checkpoint taken without an EMA does not switch it off
         if self._fused and _optimizer_kind(self):
             self._keep_fp32_moments(args[0] if args else kwargs['state_dict'])
 
     def _keep_fp32_moments(self, state_dict):
         """torch casts every loaded floating state tensor to its parameter's dtype. The fused kernels keep fp32 state for
-        bf16 / fp16 parameters (_state_dtype), and with master weights the fp32 master copy, so take the checkpoint's
-        fp32 values back: a checkpoint round-trips exactly instead of losing their low bits."""
+        bf16 / fp16 parameters (_state_dtype), and with master weights the fp32 master copy, and with ema_decay the fp32
+        EMA, so take the checkpoint's fp32 values back: a checkpoint round-trips exactly instead of losing their low
+        bits."""
         kind = _optimizer_kind(self)
         saved = [i for g in state_dict['param_groups'] for i in g['params']]
         params = [p for g in self.param_groups for p in g['params']]
         for pid, p in zip(saved, params):
             st = state_dict['state'].get(pid, {})
             keys = _STATE_KEYS[kind] if _state_dtype(kind, p.dtype, self._master_weights) == torch.float32 else ()
-            for key in keys + (('master_param',) if self._master_weights else ()):
+            for key in keys + (('master_param',) if self._master_weights else ()) + (('ema_param',) if self._ema else ()):
                 t = st.get(key)
                 if torch.is_tensor(t) and t.dtype == torch.float32 and p.dtype != torch.float32 and key in self.state[p]:
                     self.state[p][key] = _state_like(p, t, torch.float32)
@@ -564,6 +575,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         return super(self.__class__, self).step(closure)
 
     def step(self, closure=None):
+        check_not_in_ema(self)
         if self._should_synchronize and not self._reduced:
             if self._synchronized:
                 warnings.warn("optimizer.step() called without optimizer.skip_synchronize() context after "
@@ -573,13 +585,14 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self.synchronize(_defer_shadow_copy=self._fused and closure is None)
         coef = self._clip_coef
         self._drop_iteration_state()
-        if self._master_weights or (self._fused and closure is None):
-            # the masters live in the fused kernels only: evaluate the closure, then the fused update (or an error)
+        if self._master_weights or self._ema or (self._fused and closure is None):
+            # the masters and the EMA live in the fused kernels only: evaluate the closure, then the fused update (or an
+            # error)
             loss = None
             if closure is not None:
                 with torch.enable_grad():
                     loss = closure()
-            if _fused_step(self, coef):  # always True with masters: it raises when the update cannot be fused
+            if _fused_step(self, coef):  # always True with masters or EMA: it raises when the update cannot be fused
                 for bucket in self._buckets:
                     bucket['shadow_fresh'] = False
                 return loss
@@ -587,6 +600,33 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         if coef is not None:  # clip_grad_norm_ expected the fused update, which could not run
             torch._foreach_mul_(self._grads_to_clip(), coef)
         return super(self.__class__, self).step(closure)
+
+    @contextmanager
+    def ema_parameters(self):
+        """Evaluates with the EMA (optimizer built with ema_decay): inside the block every parameter that has an EMA holds
+        it, rounded to the parameter's dtype and written in place (storage and addresses stay, so a captured
+        hvd.GraphedStep remains valid; model.state_dict() taken inside is the EMA model, sharing the parameters' storage,
+        so save or clone it inside).  On exit the parameters get their exact previous values back; masters, moments and
+        the EMA are not touched.  Parameters the optimizer has not updated yet have no EMA and keep their values, and
+        buffers such as BatchNorm running statistics are never averaged.  step() inside the block raises RuntimeError.
+        The stash costs one copy of the parameters in their own dtype."""
+        if not self._ema:
+            raise RuntimeError('ema_parameters() needs an optimizer built with ema_decay')
+        check_not_in_ema(self)
+        pairs = [(p, self.state[p]['ema_param']) for g in self.param_groups for p in g['params']
+                 if 'ema_param' in self.state.get(p, {})]
+        with torch.no_grad():
+            stash = [p.detach().clone() for p, _ in pairs]
+            for p, e in pairs:
+                p.detach().copy_(e)
+        self._ema_active = True
+        try:
+            yield
+        finally:
+            self._ema_active = False
+            with torch.no_grad():
+                for (p, _), s in zip(pairs, stash):
+                    p.detach().copy_(s)
 
     def zero_grad(self, *args, **kwargs):
         if self._handles:
@@ -633,40 +673,77 @@ def _state_dtype(kind, dtype, master):
     return dtype if kind == 'sgd' and not master else torch.float32
 
 
+def check_ema_decay(decay):
+    """ema_decay is None (no EMA) or a number d with 0 <= d <= 1, the range torch's get_ema_multi_avg_fn accepts."""
+    if decay is not None and not (isinstance(decay, numbers.Real) and not isinstance(decay, bool) and 0.0 <= decay <= 1.0):
+        raise ValueError('ema_decay must be None or a number in [0, 1], got %r' % (decay,))
+
+
+def init_ema(opt, ema_decay):
+    """Constructor part of ema_decay, shared by the unsharded and the sharded optimizer: the decay goes into every param
+    group as group['ema_decay'], read at every step like 'lr'.  Returns whether the EMA is on."""
+    check_ema_decay(ema_decay)
+    opt._ema_active = False  # inside ema_parameters()
+    if ema_decay is None:
+        return False
+    opt.defaults['ema_decay'] = float(ema_decay)  # add_param_group() takes it from here
+    for g in opt.param_groups:
+        g['ema_decay'] = float(ema_decay)
+    return True
+
+
+def check_not_in_ema(opt):
+    if opt._ema_active:
+        raise RuntimeError('optimizer.step() inside ema_parameters(): the parameters hold the EMA there, and the update '
+                           'would start from it')
+
+
+def ema_weight(group):
+    """The kernels' EMA weight 1 - d for the group's current decay d, checked (a schedule may have changed it)."""
+    d = group['ema_decay']
+    if torch.is_tensor(d):
+        d = d.item()
+    check_ema_decay(d)
+    return 1.0 - float(d)
+
+
 def _fused_update(opt, kind, group, ps, grads, states, masters, step=0, first_step=False, coef=None, phase=None,
-                  norms=None, slots=None):
+                  norms=None, slots=None, emas=(), ema_start=False):
     """The native fused update of `kind` for params `ps` of `group` (hyper-parameters read now, so LR schedulers work),
     with one list per state key and fp32 masters ([]: none).  coef: a device factor on the gradient (clip coefficient).
-    LAMB / LARS: both phases (phase None), or phase 'norms' / 'apply' on `norms` / `slots` to allreduce in between."""
+    LAMB / LARS: both phases (phase None), or phase 'norms' / 'apply' on `norms` / `slots` to allreduce in between.
+    emas: the fp32 EMA of every param (empty: none), written by the update launch with group['ema_decay'], and begun
+    there with ema_start."""
     native = mpi_ops._native()
     lr, wd = float(group['lr']), float(group.get('weight_decay', 0.0))
+    ema = (list(emas), ema_weight(group), bool(ema_start)) if emas else ([], 0.0, False)
     if kind == 'sgd':
         native.fused_sgd_step(ps, grads, states[0] if states else [], lr, float(group.get('momentum', 0.0)),
                               float(group.get('dampening', 0.0)), wd, bool(group.get('nesterov', False)), 1.0,
-                              first_step, coef, masters)
+                              first_step, coef, masters, *ema)
     elif kind == 'adam':
         b1, b2 = group['betas']
         adamw = isinstance(opt, torch.optim.AdamW) or bool(group.get('decoupled_weight_decay', False))
         native.fused_adam_step(ps, grads, *states, lr, float(b1), float(b2), float(group['eps']), wd, step, 1.0, adamw,
-                               coef, masters)
+                               coef, masters, *ema)
     elif kind == 'lamb':
         b1, b2 = group['betas']
         hp = (float(b1), float(b2), float(group['eps']), wd, step, bool(group['bias_correction']))
         if phase is None:
-            native.fused_lamb_step(ps, grads, *states, lr, *hp, Lamb.adapts(group), 1.0, coef, masters)
+            native.fused_lamb_step(ps, grads, *states, lr, *hp, Lamb.adapts(group), 1.0, coef, masters, *ema)
         elif phase == 'norms':
             native.lamb_norms(ps, grads, *states, *hp, 1.0, coef, masters, norms, slots)
         else:
-            native.lamb_apply(ps, grads, *states, lr, *hp, Lamb.adapts(group), masters, norms, slots)
+            native.lamb_apply(ps, grads, *states, lr, *hp, Lamb.adapts(group), masters, norms, slots, *ema)
     else:
         hp = (lr, float(group['momentum']), wd, float(group['trust_coefficient']), float(group['eps']), Lars.adapts(group),
               1.0, coef, masters)
         if phase is None:
-            native.fused_lars_step(ps, grads, *states, *hp)
+            native.fused_lars_step(ps, grads, *states, *hp, *ema)
         elif phase == 'norms':
             native.lars_norms(ps, grads, *states, 1.0, coef, masters, norms, slots)
         else:
-            native.lars_apply(ps, grads, *states, *hp, norms, slots)
+            native.lars_apply(ps, grads, *states, *hp, norms, slots, *ema)
 
 
 def _fused_plan(opt, why=None):
@@ -720,6 +797,18 @@ def _master_param(opt, p):
     return w
 
 
+def _ema_param(opt, p):
+    """p's fp32 EMA with p's strides and whether it starts now (it does not exist yet: the update writes it whole)."""
+    st = opt.state[p]
+    e = st.get('ema_param')
+    if e is None:
+        st['ema_param'] = torch.empty_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
+        return st['ema_param'], True
+    if e.dtype != torch.float32 or e.stride() != p.stride() or e.device != p.device:
+        e = st['ema_param'] = _state_like(p, e, torch.float32)
+    return e, False
+
+
 def _param_state(opt, kind, p, keys, master):
     """p's state `keys` for the fused kernel and whether it starts now: zeros, or in the kernel's dtype and p's strides
     (torch's step and load_state_dict leave p's dtype or a checkpoint's layout).  The step count becomes a tensor."""
@@ -743,16 +832,24 @@ def _param_state(opt, kind, p, keys, master):
 def _fused_step(opt, coef=None):
     """One multi-tensor kernel for the whole model when the wrapped optimizer is SGD or Adam/AdamW on CUDA, three for
     Lamb and Lars (their trust ratios need whole-tensor norms before the update). With master weights a plan that cannot
-    be fused raises RuntimeError instead of returning False.  coef: the clip coefficient on the device, or None."""
+    be fused raises RuntimeError instead of returning False, and so does one with an EMA.  coef: the clip coefficient on the
+    device, or None."""
     use_master = getattr(opt, '_master_weights', False)
+    use_ema = getattr(opt, '_ema', False)
     why = []
     plan = _fused_plan(opt, why)
     if plan is None:
         if use_master:
             raise RuntimeError('master_weights: the fused optimizer update cannot run (%s), and torch\'s own update would '
                                'bypass the fp32 master weights' % (why[0] if why else 'not eligible'))
+        if use_ema:
+            raise RuntimeError('ema_decay: the fused optimizer update cannot run (%s), and torch\'s own update would not '
+                               'update the EMA' % (why[0] if why else 'not eligible'))
         return False
     kind = _optimizer_kind(opt)
+    for group, _, _ in plan:
+        if use_ema and group.get('ema_decay') is not None:
+            ema_weight(group)  # a scheduled decay out of range raises before any state is created
     with torch.no_grad():
         for group, ps, grads in plan:
             master = use_master and ps[0].dtype != torch.float32
@@ -760,9 +857,12 @@ def _fused_step(opt, coef=None):
             keys = _state_keys(kind, group)
             per_param, fresh = zip(*[_param_state(opt, kind, p, keys, master) for p in ps])
             states = [[st[k] for st in per_param] for k in range(len(keys))]
-            # one launch per (step count, momentum start), normally one: Adam's and LAMB's bias corrections follow each
-            # parameter's own count (a parameter without a gradient does not advance, a checkpoint may mix counts); with
-            # masters an SGD parameter that joins later starts its momentum while the others continue
+            emas, ema_new = zip(*[_ema_param(opt, p) for p in ps]) if use_ema and group.get('ema_decay') is not None \
+                else ([], [False] * len(ps))
+            # one launch per (step count, momentum start, EMA start), normally one: Adam's and LAMB's bias corrections
+            # follow each parameter's own count (a parameter without a gradient does not advance, a checkpoint may mix
+            # counts); with masters an SGD parameter that joins later starts its momentum while the others continue, and
+            # so does the EMA of a parameter whose first gradient comes later
             counts = [0] * len(ps)
             if kind in _COUNTS_STEPS:
                 steps = [opt.state[p]['step'] for p in ps]
@@ -775,12 +875,12 @@ def _fused_step(opt, coef=None):
                         t.add_(1)
                 counts = torch.stack(cpu_steps).tolist() if len(cpu_steps) == len(steps) else [t.item() for t in steps]
             parts = {}
-            for i, (c, f) in enumerate(zip(counts, fresh)):
-                parts.setdefault((int(c), kind == 'sgd' and f), []).append(i)
-            for (step, first), idx in parts.items():
+            for i, (c, f, e) in enumerate(zip(counts, fresh, ema_new)):
+                parts.setdefault((int(c), kind == 'sgd' and f, e), []).append(i)
+            for (step, first, ema_start), idx in parts.items():
                 pick = lambda xs: [xs[i] for i in idx] if xs else xs  # noqa: E731
                 _fused_update(opt, kind, group, pick(ps), pick(grads), [pick(s) for s in states], pick(masters),
-                              step=step, first_step=first, coef=coef)
+                              step=step, first_step=first, coef=coef, emas=pick(emas), ema_start=ema_start)
     return True
 
 
@@ -948,7 +1048,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none, backward_passes_per_step=1,
                          op=Average, gradient_predivide_factor=1.0, num_groups=0, groups=None, sparse_as_dense=False,
                          process_set=global_process_set, fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None,
-                         shard_optimizer_state=False, master_weights=False, grad_accumulation_dtype=None):
+                         shard_optimizer_state=False, master_weights=False, grad_accumulation_dtype=None, ema_decay=None):
     """Wraps `optimizer` so gradients are combined across ranks before the parameter update.
 
     Arguments follow the reference (horovod/torch/optimizer.py:516-608). `fused=True` (new) runs the SGD /
@@ -973,19 +1073,33 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     accumulator and zeroed, and after the last pass it holds the sum rounded once, which is what is reduced and applied.
     Between passes p.grad holds the current pass's gradient only.  fp32 gradients and backward_passes_per_step == 1 are
     unaffected.  The accumulators (one flat buffer per zero-copy bucket, else one per parameter) are allocated on first
-    use and are not optimizer state: checkpoints are taken between steps.  Not with op=Adasum (ValueError)."""
+    use and are not optimizer state: checkpoints are taken between steps.  Not with op=Adasum (ValueError).
+
+    `ema_decay=d` (new; default None) keeps an fp32 exponential moving average of every trainable parameter as optimizer
+    state ('ema_param', sharded like the moments with shard_optimizer_state), written by the same fused kernel launch
+    that updates the parameter: e = x at a parameter's first update, then e = fmaf(w, x - e, e) in fp32 with
+    w = float32(1 - d), where x is the fp32 master with master_weights, else the value stored into the parameter.  The
+    EMA advances only in a step that updates the parameter (not in a step the GradScaler skips, nor for a parameter
+    without a gradient in an unsharded step); a clipped step advances it toward the clipped update.  d is stored as
+    group['ema_decay'] and read at every step like 'lr', so a schedule (warm-up) may change it; 0 <= d <= 1, else
+    ValueError.  `with optimizer.ema_parameters(): ...` evaluates the EMA model.  Buffers (BatchNorm running statistics)
+    are not averaged.  Implies fused=True; SGD / Adam / AdamW / Lamb / Lars only, without maximize, amsgrad or op=Adasum
+    (ValueError); a step whose update cannot be fused raises RuntimeError."""
     check_grad_accumulation_dtype(grad_accumulation_dtype)
+    check_ema_decay(ema_decay)
     if grad_accumulation_dtype is not None and op == Adasum:
         raise ValueError('grad_accumulation_dtype is not supported with op=Adasum')
-    if master_weights:
+    for what, on in (('master_weights', master_weights), ('ema_decay', ema_decay is not None)):
+        if not on:
+            continue
         if op == Adasum:
-            raise ValueError('master_weights is not supported with op=Adasum')
+            raise ValueError('%s is not supported with op=Adasum' % what)
         if _optimizer_kind(optimizer) is None:
-            raise ValueError('master_weights supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
-                             % type(optimizer).__name__)
+            raise ValueError('%s supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
+                             % (what, type(optimizer).__name__))
         for g in optimizer.param_groups:
             if g.get('maximize', False) or g.get('amsgrad', False):
-                raise ValueError('master_weights does not support maximize=True or amsgrad=True')
+                raise ValueError('%s does not support maximize=True or amsgrad=True' % what)
         fused = True
     if gradient_predivide_factor != 1.0:
         if rocm_built_safe():
@@ -1004,12 +1118,12 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
         cls = type(optimizer.__class__.__name__, (_ShardedDistributedOptimizer, optimizer.__class__), {})
         return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,
                    gradient_predivide_factor, groups, sparse_as_dense, process_set, bucket_cap_mb, master_weights,
-                   grad_accumulation_dtype)
+                   grad_accumulation_dtype, ema_decay)
     if op != Adasum or size() == 1:
         cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedOptimizer.__dict__))
         return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,
                    gradient_predivide_factor, groups, sparse_as_dense, process_set, fused, zero_copy, bucket_cap_mb, bucket_wire_dtype,
-                   master_weights, grad_accumulation_dtype)
+                   master_weights, grad_accumulation_dtype, ema_decay)
     if process_set != global_process_set:
         raise NotImplementedError("Adasum does not support non-global process sets yet.")
     cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedAdasumOptimizer.__dict__))

@@ -22,6 +22,13 @@ verdict, and the clip coefficient reaches the update on the device.
 With `master_weights=True` every bf16 / fp16 bucket also keeps an fp32 master copy of its owned shard ('master_param'),
 which the fused kernel updates and rounds into the parameter shard before the allgather.
 
+With `ema_decay=d` every bucket keeps an fp32 exponential moving average of its owned shard ('ema_param', 1/N of the
+parameters per rank, plus padding), written by the same fused launch that updates the shard (the apply phase for
+LAMB / LARS), and a flag saying whether it has begun; every member of a bucket begins at the bucket's first update.
+state_dict() gathers it per parameter like the moments.  `ema_parameters()` is COLLECTIVE: each rank writes its rounded
+EMA shard into its parameter shard and the parameter buckets are allgathered, on entry and again, with the stashed
+own shards, on exit.
+
 With `backward_passes_per_step=k > 1` and `grad_accumulation_dtype=torch.float32` every bf16 / fp16 gradient bucket has an
 fp32 accumulator of its full size: when a bucket has received a backward pass's gradients it is folded into the
 accumulator and zeroed (grad_accumulate_ 'first' / 'add'), and after the k-th pass the sum rounded once is written back
@@ -30,6 +37,7 @@ accumulator and zeroed (grad_accumulate_ 'first' / 'add'), and after the k-th pa
 import math
 import os
 import warnings
+from contextlib import contextmanager
 
 import torch
 
@@ -41,7 +49,8 @@ from horovod_b200.torch.grad_buckets import (ALIGN, adopt_grad, adopt_missing_gr
                                              fold_last, full_from_shards, grad_bucket, mark_fold_last, reset_folds,
                                              scales, shard_from_full, shard_layout, shard_range, shard_slices)
 from horovod_b200.torch.mpi_ops import Average, Sum
-from horovod_b200.torch.optimizer import _COUNTS_STEPS, _STATE_KEYS, _fused_update, _optimizer_kind, _state_dtype, _state_keys
+from horovod_b200.torch.optimizer import (_COUNTS_STEPS, _STATE_KEYS, _fused_update, _optimizer_kind, _state_dtype, _state_keys,
+                                          check_not_in_ema, init_ema)
 
 
 class _ShardedDistributedOptimizer(torch.optim.Optimizer):
@@ -52,7 +61,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
 
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
-                 bucket_cap_mb=32, master_weights=False, grad_accumulation_dtype=None):
+                 bucket_cap_mb=32, master_weights=False, grad_accumulation_dtype=None, ema_decay=None):
         super().__init__(params)
         kind = _optimizer_kind(self)
         if kind is None:
@@ -75,6 +84,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             raise ValueError('shard_optimizer_state needs registered symmetric memory (P2P backend, one host, not elastic)')
 
         self._kind = kind
+        self._ema = init_ema(self, ema_decay)
         # fp32 accumulators of the bf16 / fp16 gradient buckets over the backward passes of one step (b['acc'], plain
         # device memory allocated on first use, not optimizer state)
         self._acc_fp32 = check_grad_accumulation_dtype(grad_accumulation_dtype)
@@ -119,7 +129,11 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 if master:
                     # fp32 master copy of the owned shard of a bf16 / fp16 bucket: optimizer state, sharded like the moments
                     b['state']['master_param'] = b['pshard'].float()
+                if self.param_groups[b['group']].get('ema_decay') is not None:
+                    # fp32 EMA of the owned shard: written whole by the bucket's first update ('ema_started')
+                    b['state']['ema_param'] = torch.zeros(b['shard'], dtype=torch.float32, device=device)
                 b['stepped'] = False
+                b['ema_started'] = False
         # cross-rank gradient statistics: [sum of squares or max |g|, non-finite] in registered memory, padded so that the
         # in-place allreduce can split it across the ranks
         self._stats = mpi_ops.symm_empty(ALIGN // 4 * self._nranks, dtype=torch.float32, device=device,
@@ -290,25 +304,28 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         device, or None."""
         by_group = {}
         for b in self._buckets:
-            by_group.setdefault((b['group'], b['dtype']), []).append(b)
+            by_group.setdefault((b['group'], b['dtype'], b['ema_started']), []).append(b)
         with torch.no_grad():
             if self._kind in ('lamb', 'lars'):
                 self._update_shards_trust(by_group, coef)
                 return
-            for (gi, _), bs in by_group.items():
+            for (gi, _, ema_started), bs in by_group.items():
                 group = self.param_groups[gi]
                 keys = _state_keys(self._kind, group)
-                # every bucket of a (group, dtype) has a master or none has
+                # every bucket of a (group, dtype) has a master or none has, and an EMA or none has
                 masters = [b['state']['master_param'] for b in bs] if 'master_param' in bs[0]['state'] else []
+                emas = [b['state']['ema_param'] for b in bs] if 'ema_param' in bs[0]['state'] else []
                 if self._kind in _COUNTS_STEPS:
                     for b in bs:
                         b['step'] += 1
                 _fused_update(self, self._kind, group, [b['pshard'] for b in bs], [b['gshard'] for b in bs],
                               [[b['state'][key] for b in bs] for key in keys], masters, step=bs[0]['step'],
-                              first_step=bool(keys) and not bs[0]['mom_init'], coef=coef)
+                              first_step=bool(keys) and not bs[0]['mom_init'], coef=coef, emas=emas,
+                              ema_start=not ema_started)
                 for b in bs:
                     b['mom_init'] = b['mom_init'] or (self._kind == 'sgd' and bool(keys))
                     b['stepped'] = True
+                    b['ema_started'] = bool(emas)
 
     def _update_shards_trust(self, by_group, coef):
         """The trust ratios of LAMB and LARS need the norms of whole parameters, which the shards cut at arbitrary
@@ -318,12 +335,13 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         The clip coefficient reaches the phases that read the gradient.  Padding is not touched."""
         keys = _STATE_KEYS[self._kind]
         calls = []
-        for (gi, _), bs in by_group.items():
-            lists, masters, slots = tuple([] for _ in range(2 + len(keys))), [], []
+        for (gi, _, ema_started), bs in by_group.items():
+            lists, masters, slots, emas = tuple([] for _ in range(2 + len(keys))), [], [], []
             for b in bs:
                 st = b['state']
                 b['step'] += 1
                 b['stepped'] = True
+                b['ema_started'] = 'ema_param' in st
                 if self._kind == 'lars':
                     b['mom_init'] = True  # LARS momentum: state_dict() gathers it from now on
                 for k, plo, phi, slo in shard_slices(b, self._rank):
@@ -332,17 +350,19 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                         out.append(t[cut])
                     if 'master_param' in st:
                         masters.append(st['master_param'][cut])
+                    if 'ema_param' in st:
+                        emas.append(st['ema_param'][cut])
                     slots.append(self._slot[b['params'][k]])
-            calls.append((self.param_groups[gi], bs[0]['step'], lists, masters, slots))
+            calls.append((self.param_groups[gi], bs[0]['step'], lists, masters, slots, emas, not ema_started))
         norms = self._trust_norms
         norms.zero_()
-        for group, step, lists, masters, slots in calls:
+        for group, step, lists, masters, slots, _, _ in calls:
             _fused_update(self, self._kind, group, lists[0], lists[1], list(lists[2:]), masters, step=step, coef=coef,
                           phase='norms', norms=norms, slots=slots)
         mpi_ops.captured_allreduce_(norms, op=Sum, process_set=self.process_set)
-        for group, step, lists, masters, slots in calls:
+        for group, step, lists, masters, slots, emas, ema_start in calls:
             _fused_update(self, self._kind, group, lists[0], lists[1], list(lists[2:]), masters, step=step, coef=coef,
-                          phase='apply', norms=norms, slots=slots)
+                          phase='apply', norms=norms, slots=slots, emas=emas, ema_start=ema_start)
 
     def _allgather_params(self):
         comm = self._comm
@@ -353,6 +373,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         torch.cuda.current_stream().wait_stream(comm)
 
     def step(self, closure=None):
+        check_not_in_ema(self)
         loss = None
         if closure is not None:
             with torch.enable_grad():
@@ -370,6 +391,33 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._update_shards(coef)
         self._allgather_params()
         return loss
+
+    @contextmanager
+    def ema_parameters(self):
+        """COLLECTIVE: every rank must enter and leave the block together.  Evaluates with the EMA, as the unsharded
+        optimizer's ema_parameters() does: each rank stashes its own parameter shards, writes its EMA shards rounded to
+        the parameter dtype into them and allgathers the parameter buckets, so every rank holds the whole EMA model in
+        the parameters' own storage.  On exit the stashed shards are written back and allgathered again, which restores
+        every parameter bit for bit.  Buckets whose EMA has not begun keep their values.  step() inside raises
+        RuntimeError."""
+        if not self._ema:
+            raise RuntimeError('ema_parameters() needs an optimizer built with ema_decay')
+        check_not_in_ema(self)
+        bs = [b for b in self._buckets if b['ema_started']]
+        with torch.no_grad():
+            stash = [b['pshard'].clone() for b in bs]
+            for b in bs:
+                b['pshard'].copy_(b['state']['ema_param'])
+            self._allgather_params()
+        self._ema_active = True
+        try:
+            yield
+        finally:
+            self._ema_active = False
+            with torch.no_grad():
+                for b, s in zip(bs, stash):
+                    b['pshard'].copy_(s)
+                self._allgather_params()
 
     def zero_grad(self, set_to_none=True):
         """Zeroes the gradient buckets in place: p.grad stays a view of registered memory (set_to_none is ignored)."""
@@ -420,16 +468,20 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         index = {id(p): i for i, p in enumerate(p for g in self.param_groups for p in g['params'])}
         state = {}
         for b in self._buckets:
-            if not b['state'] or ((b['step'] == 0) if self._kind in _COUNTS_STEPS else
-                                  not (b['mom_init'] or ('master_param' in b['state'] and b['stepped']))):
-                continue  # no state yet (the same on every rank); an SGD / LARS bucket may still hold masters only
+            # which state has begun (the same on every rank); an SGD / LARS bucket may hold masters or an EMA only
+            started = ((b['step'] > 0) if self._kind in _COUNTS_STEPS else
+                       (b['mom_init'] or ('master_param' in b['state'] and b['stepped'])))
+            keys = [key for key in b['state'] if (b['ema_started'] if key == 'ema_param' else started)]
+            if not keys:
+                continue
             gathered = {}
-            for key, shard in b['state'].items():
+            for key in keys:
+                shard = b['state'][key]
                 full = mpi_ops.allgather(shard, name='sharded_opt.state.%d.%s' % (b['index'], key), process_set=self.process_set)
                 gathered[key] = full_from_shards(b, [full], [p.shape for p in b['params']], [p.stride() for p in b['params']])
             for k, p in enumerate(b['params']):
                 st = {key: vals[k].detach().cpu().clone() for key, vals in gathered.items()}
-                if self._kind in _COUNTS_STEPS:
+                if self._kind in _COUNTS_STEPS and started:
                     st['step'] = torch.tensor(float(b['step']))
                 state[index[id(p)]] = st
         sd['state'] = state
@@ -438,6 +490,8 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
     def load_state_dict(self, state_dict):
         """Accepts the format of state_dict() from a sharded or an unsharded optimizer and keeps this rank's slice only.
         Does not communicate."""
+        if self._ema_active:
+            raise RuntimeError('load_state_dict() inside ema_parameters(): the block restores the parameters on exit')
         groups = state_dict['param_groups']
         if len(groups) != len(self.param_groups) or any(len(a['params']) != len(b['params']) for a, b in zip(groups, self.param_groups)):
             raise ValueError('loaded state dict does not match the optimizer\'s parameter groups')
@@ -455,6 +509,12 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 per = [saved_state.get(ids[p], saved_state.get(str(ids[p]), {})) for p in b['params']]
                 for key, shard in b['state'].items():
                     full = [st.get(key) for st in per]
+                    if key == 'ema_param':
+                        # the bucket's EMA begins once for all members: members without a saved EMA (an unsharded
+                        # optimizer had no gradient for them yet) continue from their parameter's current value
+                        b['ema_started'] = any(t is not None for t in full)
+                        if b['ema_started']:
+                            full = [p.detach().float() if t is None else t for t, p in zip(full, b['params'])]
                     shard.copy_(shard_from_full(b, self._rank, [None if t is None else t.detach() for t in full],
                                                 [p.stride() for p in b['params']], dtype=shard.dtype, device='cpu'))
                     if key == 'momentum_buffer':
@@ -474,10 +534,11 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         already hold the same step counts (a fresh start, or load_state_dict() on every rank): if they differ, e.g. after
         loading a checkpoint on the root only, every rank raises ValueError instead of resuming with zero moments."""
         from horovod_b200.torch.functions import allgather_object, broadcast_object
-        mine = {'steps': [b['step'] for b in self._buckets], 'mom_init': [b['mom_init'] for b in self._buckets]}
+        mine = {'steps': [b['step'] for b in self._buckets], 'mom_init': [b['mom_init'] for b in self._buckets],
+                'ema_started': [b['ema_started'] for b in self._buckets]}
         meta = dict(mine, param_groups=[{k: v for k, v in g.items() if k != 'params'} for g in self.param_groups])
         meta = broadcast_object(meta, root_rank, 'sharded_opt.meta', self.process_set)
-        same = mine == {'steps': meta['steps'], 'mom_init': meta['mom_init']}
+        same = mine == {k: meta[k] for k in mine}
         if not all(allgather_object(same, 'sharded_opt.same', self.process_set)):
             raise ValueError('broadcast_optimizer_state: the sharded optimizer state differs between ranks (was the '
                              'checkpoint loaded on the root rank only?); call load_state_dict() on every rank')
