@@ -12,6 +12,7 @@ except ImportError:  # pragma: no cover
 
 from horovod_b200.common.process_sets import global_process_set
 from horovod_b200.torch.mpi_ops import (allgather, broadcast_, broadcast_async_, rank, size, synchronize)
+from horovod_b200.torch.optimizer import _DistributedAdasumOptimizer, _DistributedOptimizerBase
 
 
 def broadcast_parameters(params, root_rank, process_set=global_process_set):
@@ -95,8 +96,10 @@ def broadcast_optimizer_state(optimizer, root_rank, model=None, process_set=glob
                     created.append(p)
         # a zero-grad step must not move the weights: snapshot and restore
         saved = [[p.data.clone() for p in g['params']] for g in optimizer.param_groups]
-        if hasattr(optimizer, '_hvd_super_step'):  # a DistributedOptimizer: the wrapped optimizer's own step
+        if isinstance(optimizer, _DistributedOptimizerBase):  # the wrapped optimizer's own step, without a reduction
             optimizer._hvd_super_step()
+        elif isinstance(optimizer, _DistributedAdasumOptimizer):
+            super(_DistributedAdasumOptimizer, optimizer).step()
         else:
             optimizer.step()
         for g, ps in zip(optimizer.param_groups, saved):

@@ -4,15 +4,12 @@ bucket) and the sharded path (sharded_optimizer.py, ZeRO-1: one reduce-scatter p
 A bucket is a plain dict.  shard_layout() gives its layout ('group', 'dtype', 'members', 'numel', 'shard');
 grad_bucket() adds a flat gradient buffer of registered memory ('gflat') of which every member's p.grad is a view
 ('params', 'views'), and the fp32 accumulation state ('acc', 'arrived', 'folds', 'fold_last').  Each optimizer adds the
-keys of its own launch policy.  The functions here take the optimizer (for its op, scale and accumulation settings)
-and its buckets; neither optimizer derives from anything defined here.
+keys of its own launch policy.  The functions here work on a bucket alone; what also reads the optimizer's settings
+(its op, scales and accumulation) is a method of _DistributedOptimizerBase in optimizer.py.
 """
-from contextlib import contextmanager
-
 import torch
 
 from horovod_b200.torch import mpi_ops
-from horovod_b200.torch.mpi_ops import Average
 
 ALIGN = 128  # bytes: every parameter and every shard starts at a multiple of this
 
@@ -168,35 +165,10 @@ def fold(grads, accs, mode):
         ops.grad_accumulate_(grads, accs, mode)
 
 
-def accumulates(opt, grad):
-    """True when `grad` (a bucket's 'gflat' or a parameter's gradient) is summed over the backward passes in fp32."""
-    return (opt._acc_fp32 and opt.backward_passes_per_step > 1 and grad is not None and grad.is_cuda
-            and not grad.is_sparse and grad.dtype in (torch.bfloat16, torch.float16))
-
-
 def bucket_acc(bucket):
     if bucket['acc'] is None:  # plain device memory: the accumulator never travels
         bucket['acc'] = torch.empty(bucket['numel'], dtype=torch.float32, device=bucket['gflat'].device)
     return bucket['acc']
-
-
-def bucket_accumulators(opt, with_buckets=True):
-    """(16-bit gradients, fp32 accumulators) of every accumulating bucket of `opt`, allocated now if needed."""
-    bs = [b for b in opt._buckets if with_buckets and accumulates(opt, b['gflat'])]
-    return [b['gflat'] for b in bs], [bucket_acc(b) for b in bs]
-
-
-def fold_arrived(opt, bucket, more):
-    """The hook of one of the bucket's gradients.  Once the bucket has this backward pass's gradients and `more` passes
-    of the step are to come, they are folded into the fp32 accumulator and zeroed ('first', then 'add')."""
-    if not accumulates(opt, bucket['gflat']):
-        return
-    bucket['arrived'] += 1
-    if bucket['arrived'] == len(bucket['params']):
-        bucket['arrived'] = 0
-        if more:
-            fold([bucket['gflat']], [bucket_acc(bucket)], 'add' if bucket['folds'] else 'first')
-            bucket['folds'] += 1
 
 
 def fold_last(bucket, capturing):
@@ -208,18 +180,12 @@ def fold_last(bucket, capturing):
         bucket['folds'] = 0
 
 
-def mark_fold_last(opt, capturing):
-    """hvd.GraphedStep begins (capturing) or ends the capture of a step's last graph."""
-    for b in opt._buckets:
-        b['fold_last'] = capturing and accumulates(opt, b['gflat'])
-
-
 def reset_folds(buckets):
     for b in buckets:
         b['arrived'] = b['folds'] = 0
 
 
-# ---- arguments and API shared by both optimizers --------------------------------------------------------------------------
+# ---- arguments shared by the optimizers -----------------------------------------------------------------------------------
 def find_duplicates(lst):
     seen = set()
     dups = set()
@@ -254,21 +220,3 @@ def check_named_parameters(opt, named_parameters):
                          'object ids: %s' % ', '.join(str(id) for id in unnamed_param_ids))
     return named_parameters
 
-
-def scales(opt):
-    """(prescale, postscale) of a gradient reduction: op=Average splits the averaging into pre- and post-division
-    around the sum (reference optimizer.py:197-204)."""
-    if opt.op == Average:
-        return 1.0 / opt.gradient_predivide_factor, opt.gradient_predivide_factor
-    return 1.0, 1.0
-
-
-@contextmanager
-def skip_synchronize(opt):
-    """Use after an explicit optimizer.synchronize() (e.g. gradient clipping) so that step() does not synchronize
-    again."""
-    opt._should_synchronize = False
-    try:
-        yield
-    finally:
-        opt._should_synchronize = True

@@ -53,6 +53,9 @@ import warnings
 
 import torch
 
+from horovod_b200.torch.mpi_ops import Adasum
+from horovod_b200.torch.optimizer import _DistributedAdasumOptimizer, _DistributedOptimizerBase
+
 
 class GraphedStep:
     """Training step whose forward + backward are one CUDA graph replay; `step(*inputs)` returns the (static) loss tensor.
@@ -77,7 +80,7 @@ class GraphedStep:
             self.fallback_reason = 'disabled'
         elif not (torch.cuda.is_available() and all(t.is_cuda for t in example_inputs)):
             self.fallback_reason = 'inputs are not CUDA tensors'
-        elif not hasattr(optimizer, '_graph_mode'):
+        elif not isinstance(optimizer, (_DistributedOptimizerBase, _DistributedAdasumOptimizer)):
             self.fallback_reason = 'optimizer is not an hvd.DistributedOptimizer'
         else:
             try:
@@ -92,11 +95,11 @@ class GraphedStep:
             raise ValueError('hvd.GraphedStep: norm_type must be 2 or inf, got %r' % (norm_type,))
         if max_grad_norm is None and scaler is None:
             return
-        from horovod_b200.torch.mpi_ops import Adasum
-        if getattr(optimizer, 'op', None) == Adasum or hasattr(optimizer, '_whole_model_step'):
+        if isinstance(optimizer, _DistributedAdasumOptimizer) or (isinstance(optimizer, _DistributedOptimizerBase)
+                                                                   and optimizer.op == Adasum):
             raise ValueError('hvd.GraphedStep: max_grad_norm and scaler are not supported with op=Adasum, whose optimizer '
                              'reduces parameter deltas, not gradients')
-        if not (hasattr(optimizer, 'clip_grad_norm_') and hasattr(optimizer, '_drop_iteration_state')):
+        if not isinstance(optimizer, _DistributedOptimizerBase):
             raise ValueError('hvd.GraphedStep: max_grad_norm and scaler need an hvd.DistributedOptimizer')
         if scaler is not None and not all(p.is_cuda for g in optimizer.param_groups for p in g['params']):
             raise ValueError('hvd.GraphedStep: scaler needs an optimizer of CUDA parameters')
@@ -114,6 +117,7 @@ class GraphedStep:
 
     def _capture(self, warmup_iters):
         opt = self.optimizer
+        reduces = isinstance(opt, _DistributedOptimizerBase)  # the Adasum optimizer reduces in step() only
         opt._graph_mode = True
         self.static_inputs = tuple(t.detach().clone(memory_format=torch.preserve_format) for t in self.static_inputs)
         side = torch.cuda.Stream()
@@ -134,12 +138,12 @@ class GraphedStep:
             with torch.cuda.graph(self.graph):
                 # multi-GPU: the gradient buckets' allreduce kernels become nodes of this graph (forked onto a side stream
                 # as soon as a bucket's last gradient is recorded, joined before the capture ends)
-                self.comm_in_graph = bool(getattr(opt, '_begin_graph_capture', lambda: False)())
+                self.comm_in_graph = reduces and opt._begin_graph_capture()
                 self.static_loss = self._fwd_bwd()
                 if self.comm_in_graph:
                     opt._end_graph_capture()
         finally:
-            if hasattr(opt, '_graph_capture'):
+            if reduces:
                 opt._graph_capture = None
         torch.cuda.synchronize()
         self.captured = True
@@ -148,8 +152,8 @@ class GraphedStep:
         """k > 1: the first, middle (k >= 3) and last micro-steps as graphs of one memory pool.  Only the last one
         records the gradient collectives (as the one graph of k == 1 does) and the fp32 accumulation's 'last' folds."""
         opt = self.optimizer
-        fold = getattr(opt, '_graph_fold', None)
-        if fold is not None:
+        reduces = isinstance(opt, _DistributedOptimizerBase)
+        if reduces:
             opt._prepare_accumulators()
         pool = torch.cuda.graph_pool_handle()
         phases = ('first', 'add', 'last') if self.k >= 3 else ('first', 'last')
@@ -158,14 +162,14 @@ class GraphedStep:
             graph = torch.cuda.CUDAGraph()
             try:
                 with torch.cuda.graph(graph, pool=pool):
-                    comm = phase == 'last' and bool(getattr(opt, '_begin_graph_capture', lambda: False)())
+                    comm = phase == 'last' and reduces and opt._begin_graph_capture()
                     loss = self._fwd_bwd(zero_grad=phase == 'first')
-                    if fold is not None:
-                        fold(phase, with_buckets=not comm)  # with comm, each bucket's fold precedes its collective
+                    if reduces:  # with comm, each bucket's fold precedes its collective
+                        opt._graph_fold(phase, with_buckets=not comm)
                     if comm:
                         opt._end_graph_capture()
             finally:
-                if hasattr(opt, '_graph_capture'):
+                if reduces:
                     opt._graph_capture = None
             self.graphs[phase], self.static_losses[phase] = graph, loss
             self.comm_in_graph = self.comm_in_graph or comm
@@ -190,7 +194,7 @@ class GraphedStep:
         self.captured, self.graph, self.comm_in_graph = False, None, False
         self.graphs = self.static_losses = None
         self.optimizer._graph_mode = False
-        if hasattr(self.optimizer, '_graph_comm_captured'):
+        if isinstance(self.optimizer, _DistributedOptimizerBase):
             self.optimizer._graph_comm_captured = False
         self.fallback_reason = '%s: %s' % (type(exc).__name__, str(exc).splitlines()[0] if str(exc) else '')
         try:

@@ -19,36 +19,274 @@ import torch
 from horovod_b200.common.exceptions import HorovodInternalError
 from horovod_b200.common.process_sets import global_process_set
 from horovod_b200.common.util import split_list
-from horovod_b200.torch import grad_buckets, mpi_ops
+from horovod_b200.torch import mpi_ops
 from horovod_b200.torch.compression import Compression
-from horovod_b200.torch.grad_buckets import (accumulates, adopt_grad, adopt_missing_grads, bucket_accumulators,
-                                             check_grad_accumulation_dtype, check_named_parameters, find_duplicates,
-                                             fold, fold_arrived, fold_last, grad_bucket, mark_fold_last, reset_folds,
-                                             scales, shard_layout)
+from horovod_b200.torch.grad_buckets import (adopt_grad, adopt_missing_grads, bucket_acc, check_grad_accumulation_dtype,
+                                             check_named_parameters, find_duplicates, fold, fold_last, grad_bucket,
+                                             reset_folds, shard_layout)
 from horovod_b200.torch.lamb import Lamb
 from horovod_b200.torch.lars import Lars
 from horovod_b200.torch.mpi_ops import (Adasum, Average, Sum, allreduce_async_, grouped_allreduce_async_, rank, size,
                                         synchronize)
 
 
-class _DistributedOptimizer(torch.optim.Optimizer):
+class _DistributedOptimizerBase(torch.optim.Optimizer):
+    """What the two optimizers that reduce gradients share: the unsharded _DistributedOptimizer and the sharded (ZeRO-1)
+    _ShardedDistributedOptimizer.  hvd.DistributedOptimizer() builds a class that derives from one of them and from the
+    wrapped optimizer's class, so super() in this class reaches the wrapped optimizer.
+
+    A subclass sets `_buckets` (its gradient buckets) and `_delay` (parameter -> backward passes of the step still to
+    come), and supplies
+      _reduce_pending()      reduce the gradients that are still pending (for clip_grad_norm_),
+      _grad_norm(norm_type)  (norm of the reduced gradients or None without any, the gradients clip_grad_norm_ scales in
+                             place or None when the fused update applies the coefficient),
+      _ema_pairs()           [(parameter or owned shard, its fp32 EMA)] of every EMA that has begun,
+      _new_graph_capture()   the state of a hvd.GraphedStep capture ({'comm': side stream, ...}), or None when the
+                             reductions cannot be captured,
+      _launch_remaining()    while capturing: launch the reductions that no hook launched."""
+
+    _norm_type_error = 'clip_grad_norm_ supports norm_type 2 and inf, got %r'
+
+    def __init__(self, params, process_set, op, gradient_predivide_factor, backward_passes_per_step,
+                 grad_accumulation_dtype, ema_decay):
+        super().__init__(params)
+        self.process_set = process_set
+        self.op = op
+        self.gradient_predivide_factor = gradient_predivide_factor
+        self.backward_passes_per_step = backward_passes_per_step
+        # fp32 accumulators of bf16 / fp16 gradients over the backward passes of one step (allocated on first use, not
+        # optimizer state)
+        self._acc_fp32 = check_grad_accumulation_dtype(grad_accumulation_dtype)
+        # fp32 exponential moving average of every trainable parameter, kept as optimizer state ('ema_param') and written
+        # by the fused update kernels only: ema_decay implies fused, like master_weights.  The decay goes into every param
+        # group as group['ema_decay'], read at every step like 'lr'.
+        check_ema_decay(ema_decay)
+        self._ema = ema_decay is not None
+        self._ema_active = False  # inside ema_parameters()
+        if self._ema:
+            self.defaults['ema_decay'] = float(ema_decay)  # add_param_group() takes it from here
+            for g in self.param_groups:
+                g['ema_decay'] = float(ema_decay)
+        self._graph_mode = False  # set by hvd.GraphedStep: backward runs as a CUDA graph replay, hooks do not fire
+        self._graph_capture = None  # while hvd.GraphedStep captures: _new_graph_capture()
+        self._graph_comm_captured = False  # the captured graph contains the gradient reductions (nothing left for step())
+        self._should_synchronize = True  # False inside skip_synchronize()
+        self._synchronized = False  # set by a user's synchronize()
+        self._reduced = False       # set by clip_grad_norm_ / ShardedGradScaler: step() does not reduce again, silently
+        self._clip_coef = None      # 0-dim fp32 device tensor from clip_grad_norm_, applied by the next fused step()
+        self._stats_cache = None    # [sum of squares, non-finite] of the unscaled gradients from hvd.ShardedGradScaler
+
+    # ---- one iteration ---------------------------------------------------------------------------------------------------
+    @contextmanager
+    def skip_synchronize(self):
+        """Use after an explicit optimizer.synchronize() (e.g. gradient clipping) so that step() does not synchronize
+        again."""
+        self._should_synchronize = False
+        try:
+            yield
+        finally:
+            self._should_synchronize = True
+
+    def _drop_iteration_state(self):
+        self._synchronized = self._reduced = False
+        self._clip_coef = self._stats_cache = None
+
+    def _start_afresh(self):
+        """A new backward pass or zero_grad() after an iteration whose step() was skipped (e.g. GradScaler found inf)
+        leaves nothing of that iteration behind."""
+        if self._reduced or self._clip_coef is not None:
+            self._drop_iteration_state()
+
+    def _count_backward_pass(self, p):
+        """The top of p's gradient hook in eager mode: counts one of the step's backward passes and returns how many are
+        still to come (0: p's gradient is complete)."""
+        self._start_afresh()
+        if self._delay[p] <= 0:
+            raise AssertionError('Gradients were computed more than backward_passes_per_step times before call to step(). '
+                                 'Increase backward_passes_per_step to accumulate gradients locally.')
+        self._delay[p] -= 1
+        return self._delay[p]
+
+    def set_backward_passes_per_step(self, passes):
+        self.backward_passes_per_step = passes
+        self._delay = dict.fromkeys(self._delay, passes)
+        self._reset_folds()
+
+    def _scales(self):
+        """(prescale, postscale) of a gradient reduction: op=Average splits the averaging into pre- and post-division
+        around the sum (reference optimizer.py:197-204)."""
+        if self.op == Average:
+            return 1.0 / self.gradient_predivide_factor, self.gradient_predivide_factor
+        return 1.0, 1.0
+
+    def _hvd_super_step(self, closure=None):
+        """The wrapped optimizer's own step(), without any reduction."""
+        return super().step(closure)
+
+    # ---- gradient accumulation in fp32 (grad_accumulation_dtype=torch.float32) -------------------------------------------
+    def _accumulates(self, grad):
+        """True when `grad` (a bucket's 'gflat' or a parameter's gradient) is summed over the backward passes in fp32."""
+        return (self._acc_fp32 and self.backward_passes_per_step > 1 and grad is not None and grad.is_cuda
+                and not grad.is_sparse and grad.dtype in (torch.bfloat16, torch.float16))
+
+    def _fold_arrived(self, bucket, more):
+        """The hook of one of the bucket's gradients.  Once the bucket has this backward pass's gradients and `more`
+        passes of the step are to come, they are folded into the fp32 accumulator and zeroed ('first', then 'add')."""
+        if not self._accumulates(bucket['gflat']):
+            return
+        bucket['arrived'] += 1
+        if bucket['arrived'] == len(bucket['params']):
+            bucket['arrived'] = 0
+            if more:
+                fold([bucket['gflat']], [bucket_acc(bucket)], 'add' if bucket['folds'] else 'first')
+                bucket['folds'] += 1
+
+    def _reset_folds(self):
+        reset_folds(self._buckets)
+
+    def _accumulator_pairs(self, with_buckets=True):
+        """(16-bit gradients, fp32 accumulators) of every accumulating bucket, allocated now if needed."""
+        bs = [b for b in self._buckets if with_buckets and self._accumulates(b['gflat'])]
+        return [b['gflat'] for b in bs], [bucket_acc(b) for b in bs]
+
+    def _prepare_accumulators(self):
+        """hvd.GraphedStep, before capture: the accumulators must exist outside the graphs' memory pool."""
+        self._accumulator_pairs()
+
+    def _graph_fold(self, mode, with_buckets=True):
+        """hvd.GraphedStep, while capturing: one fold of every accumulator after the captured backward pass."""
+        fold(*self._accumulator_pairs(with_buckets), mode)
+
+    def _mark_fold_last(self, capturing):
+        """hvd.GraphedStep begins (capturing) or ends the capture of a step's last graph."""
+        for b in self._buckets:
+            b['fold_last'] = capturing and self._accumulates(b['gflat'])
+
+    # ---- gradient reductions as CUDA-graph nodes (hvd.GraphedStep) -------------------------------------------------------
+    def _begin_graph_capture(self):
+        """Called by hvd.GraphedStep right after stream capture began (on the capturing stream): the gradient reductions
+        become nodes of the graph, unless HVD_GRAPH_COMM=0 or the subclass cannot capture them.  Returns whether they do."""
+        self._graph_comm_captured = False
+        if os.environ.get('HVD_GRAPH_COMM', '1') == '0':
+            return False
+        self._graph_capture = self._new_graph_capture()
+        if self._graph_capture is None:
+            return False
+        self._mark_fold_last(True)  # with backward_passes_per_step > 1 this is the step's last graph
+        return True
+
+    def _end_graph_capture(self):
+        """Before stream capture ends: the reductions no hook launched are launched now, then the capturing stream joins
+        the communication stream."""
+        cap = self._graph_capture
+        if cap is None:
+            return
+        self._launch_remaining()
+        torch.cuda.current_stream().wait_stream(cap['comm'])
+        self._graph_capture = None
+        self._mark_fold_last(False)
+        self._graph_comm_captured = True
+
+    # ---- global-norm gradient clipping -----------------------------------------------------------------------------------
+    def _reduce_once(self):
+        """Reduces what is still pending unless this iteration's gradients are reduced already; the following step()
+        neither reduces again nor warns."""
+        if not (self._synchronized or self._reduced):
+            self._reduce_pending()
+            self._reduced = True
+
+    def clip_grad_norm_(self, max_norm, norm_type=2.0, error_if_nonfinite=False):
+        """Global-norm gradient clipping, the counterpart of torch.nn.utils.clip_grad_norm_(model.parameters(), ...):
+        call it after backward (and after GradScaler.unscale_ or ShardedGradScaler.unscale_, if used) and before step().
+
+        Reduces the gradients that are still pending, as synchronize() does (the following step() neither reduces again
+        nor warns), and returns the norm of the reduced gradients as a 0-dim fp32 tensor on their device, with the same
+        bits on every rank.  On CUDA the norm is one statistics kernel per gradient dtype, without a host
+        synchronisation; with sharded optimizer state it is computed from the ranks' owned shards with one scalar
+        allreduce.  When step() runs the fused update (always with sharded state), the clip coefficient
+        min(max_norm / (norm + 1e-6), 1) stays on the device and scales the gradient inside that update, and p.grad is
+        not rescaled; otherwise p.grad is scaled in place, as torch does.  norm_type is 2 or inf; sparse gradients raise
+        ValueError.  error_if_nonfinite=True synchronises with the host, as torch's does."""
+        norm_type = float(norm_type)
+        if norm_type not in (2.0, math.inf):
+            raise ValueError(self._norm_type_error % norm_type)
+        self._reduce_once()
+        total, grads = self._grad_norm(norm_type)
+        if total is None:
+            return torch.zeros((), dtype=torch.float32)
+        if self._clip_coef is not None:
+            total = total * self._clip_coef  # clipping twice: the norm of the gradient as the first clip left it
+        if error_if_nonfinite and bool(torch.logical_or(total.isnan(), total.isinf())):
+            raise RuntimeError('The total norm of order %s for gradients from `parameters` is non-finite, so it cannot be '
+                               'clipped. To disable this error and scale the gradients by the non-finite norm anyway, set '
+                               '`error_if_nonfinite=False`' % norm_type)
+        coef = torch.clamp(max_norm / (total + 1e-6), max=1.0)
+        if grads is None:
+            self._clip_coef = coef if self._clip_coef is None else self._clip_coef * coef
+        else:
+            torch._foreach_mul_(grads, coef)
+        return total
+
+    # ---- the weight EMA (ema_decay) --------------------------------------------------------------------------------------
+    def _check_not_in_ema(self, loading=False):
+        if not self._ema_active:
+            return
+        if loading:
+            raise RuntimeError('load_state_dict() inside ema_parameters(): the block restores the parameters on exit')
+        raise RuntimeError('optimizer.step() inside ema_parameters(): the parameters hold the EMA there, and the update '
+                           'would start from it')
+
+    def _params_written(self):
+        """ema_parameters() wrote the tensors of _ema_pairs(); whole parameters need nothing more."""
+
+    @contextmanager
+    def ema_parameters(self):
+        """Evaluates with the EMA (optimizer built with ema_decay): inside the block every parameter that has an EMA holds
+        it, rounded to the parameter's dtype and written in place (storage and addresses stay, so a captured
+        hvd.GraphedStep remains valid; model.state_dict() taken inside is the EMA model, sharing the parameters' storage,
+        so save or clone it inside).  On exit the parameters get their exact previous values back; masters, moments and
+        the EMA are not touched.  Parameters the optimizer has not updated yet have no EMA and keep their values, and
+        buffers such as BatchNorm running statistics are never averaged.  step() inside the block raises RuntimeError.
+        The stash costs one copy of the parameters in their own dtype.
+
+        With sharded optimizer state the block is COLLECTIVE: every rank must enter and leave it together.  Each rank
+        stashes its own parameter shards, writes its EMA shards into them and allgathers the parameter buckets, so every
+        rank holds the whole EMA model; on exit the stashed shards are written back and allgathered again.  Buckets whose
+        EMA has not begun keep their values."""
+        if not self._ema:
+            raise RuntimeError('ema_parameters() needs an optimizer built with ema_decay')
+        self._check_not_in_ema()
+        pairs = self._ema_pairs()
+        with torch.no_grad():
+            stash = [t.clone() for t, _ in pairs]
+            for t, e in pairs:
+                t.copy_(e)
+            self._params_written()
+        self._ema_active = True
+        try:
+            yield
+        finally:
+            self._ema_active = False
+            with torch.no_grad():
+                for (t, _), s in zip(pairs, stash):
+                    t.copy_(s)
+                self._params_written()
+
+
+class _DistributedOptimizer(_DistributedOptimizerBase):
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
                  fused=False, zero_copy=None, bucket_cap_mb=32, bucket_wire_dtype=None, master_weights=False,
                  grad_accumulation_dtype=None, ema_decay=None):
-        super(self.__class__, self).__init__(params)
+        super().__init__(params, process_set, op, gradient_predivide_factor, backward_passes_per_step,
+                         grad_accumulation_dtype, ema_decay)
         self._compression = compression
-        # fp32 accumulators of bf16 / fp16 gradients over the backward passes of one step (allocated on first use, not
-        # optimizer state): bucket -> bucket['acc'], parameter outside the buckets -> self._param_accs[p]
-        self._acc_fp32 = check_grad_accumulation_dtype(grad_accumulation_dtype)
+        # fp32 accumulators of the parameters outside the buckets (the buckets' are bucket['acc'])
         self._param_accs = {}
         self._acc_open = set()  # parameters outside the buckets folded this step whose 'last' fold is still to come
         # fp32 master copies of bf16 / fp16 parameters, kept as optimizer state ('master_param') and updated by the fused
         # kernels only: master_weights implies fused, and step() never hands those parameters to torch's own update
         self._master_weights = bool(master_weights)
-        # fp32 exponential moving average of every trainable parameter, kept as optimizer state ('ema_param') and written
-        # by the fused update kernels only: ema_decay implies fused, like master_weights
-        self._ema = init_ema(self, ema_decay)
         fused = fused or self._master_weights or self._ema
         # opt-in: fp32 gradient buckets travel as bf16 / fp16 (a registered shadow bucket of half the bytes is what the
         # zero-copy kernel reduces; the switch accumulates in fp32).  Not validated on hardware yet (docs/roadmap.md B3).
@@ -58,24 +296,13 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
         named_parameters = check_named_parameters(self, named_parameters)
         self._parameter_names = {v: k for k, v in sorted(named_parameters)}
-        self.backward_passes_per_step = backward_passes_per_step
-        self._allreduce_delay = {v: self.backward_passes_per_step for _, v in sorted(named_parameters)}
-        self.op = op
-        self.gradient_predivide_factor = gradient_predivide_factor
+        self._delay = {v: self.backward_passes_per_step for _, v in sorted(named_parameters)}
         self.sparse_as_dense = sparse_as_dense
-        self.process_set = process_set
         self._fused = fused
-        self._graph_mode = False  # set by hvd.GraphedStep: backward runs as a CUDA graph replay, hooks do not fire
-        self._graph_capture = None      # while hvd.GraphedStep captures: {'comm': side stream, 'ctas': n, 'launched': set()}
-        self._graph_comm_captured = False  # the captured graph contains the gradient allreduces (nothing left for step())
 
         self._handles = {}
         self._grad_accs = []
         self._requires_update = set()
-        self._synchronized = False
-        self._should_synchronize = True
-        self._reduced = False    # set by clip_grad_norm_: step() does not reduce again, silently
-        self._clip_coef = None   # 0-dim fp32 device tensor from clip_grad_norm_, applied by the next fused step()
 
         self._num_groups = None
         self._groups = None
@@ -110,22 +337,20 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._register_hooks()
 
     # -- reference API ----------------------------------------------------------
-    def load_state_dict(self, *args, **kwargs):
-        if self._ema_active:
-            raise RuntimeError('load_state_dict() inside ema_parameters(): the block restores the parameters on exit')
+    def load_state_dict(self, state_dict):
+        self._check_not_in_ema(loading=True)
         self._handles = {}
         self._synchronized = False
         self._should_synchronize = True
-        for p in self._allreduce_delay:
-            self._allreduce_delay[p] = self.backward_passes_per_step
+        self._delay = dict.fromkeys(self._delay, self.backward_passes_per_step)
         self._reset_folds()
         decays = [g.get('ema_decay') for g in self.param_groups]
-        super(self.__class__, self).load_state_dict(*args, **kwargs)
+        super().load_state_dict(state_dict)
         for g, d in zip(self.param_groups, decays):
             if d is not None:
                 g.setdefault('ema_decay', d)  # a checkpoint taken without an EMA does not switch it off
         if self._fused and _optimizer_kind(self):
-            self._keep_fp32_moments(args[0] if args else kwargs['state_dict'])
+            self._keep_fp32_moments(state_dict)
 
     def _keep_fp32_moments(self, state_dict):
         """torch casts every loaded floating state tensor to its parameter's dtype. The fused kernels keep fp32 state for
@@ -146,12 +371,6 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     @staticmethod
     def find_duplicates(lst):
         return find_duplicates(lst)
-
-    def set_backward_passes_per_step(self, passes):
-        self.backward_passes_per_step = passes
-        for p in self._allreduce_delay:
-            self._allreduce_delay[p] = self.backward_passes_per_step
-        self._reset_folds()
 
     def _register_hooks(self):
         if self._groups is not None:
@@ -224,7 +443,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         captures, as a captured_allreduce_ node forked onto the side stream (so it overlaps the rest of backward)."""
         cap = self._graph_capture
         fold_last(bucket, cap is not None)  # on the caller's stream, so it precedes the allreduce
-        prescale_factor, postscale_factor = scales(self)
+        prescale_factor, postscale_factor = self._scales()
         if cap is not None:
             cap['comm'].wait_stream(torch.cuda.current_stream())  # fork: everything recorded so far (this bucket's gradients) precedes it
         with torch.cuda.stream(cap['comm'] if cap is not None else None):
@@ -256,7 +475,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             else:
                 return mpi_ops.sparse_allreduce_async(tensor, name=name, op=self.op, process_set=self.process_set), None
         tensor_compressed, ctx = self._compression.compress(tensor)
-        prescale_factor, postscale_factor = scales(self)
+        prescale_factor, postscale_factor = self._scales()
         handle = allreduce_async_(tensor_compressed, name=name, op=self.op, prescale_factor=prescale_factor,
                                   postscale_factor=postscale_factor, process_set=self.process_set)
         return handle, ctx
@@ -267,7 +486,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             if p.grad is None:
                 p.grad = torch.zeros_like(p.data)
         tensors_compressed, ctxs = zip(*[self._compression.compress(p.grad) for p in ps])
-        prescale_factor, postscale_factor = scales(self)
+        prescale_factor, postscale_factor = self._scales()
         handle = grouped_allreduce_async_(list(tensors_compressed), name=name, op=self.op, prescale_factor=prescale_factor,
                                           postscale_factor=postscale_factor, process_set=self.process_set)
         return handle, ctxs
@@ -287,34 +506,25 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 if self._graph_capture is not None:
                     self._graph_hook(p)
                 return
-            if self._reduced or self._clip_coef is not None:
-                # a new backward after an iteration whose step() was skipped (e.g. GradScaler found inf): start afresh
-                self._drop_iteration_state()
-            if p in self._handles and self._handles[p][0] is not None:
-                if self._allreduce_delay[p] <= 0:
-                    raise AssertionError(
-                        "Gradients were computed more than backward_passes_per_step times before call to step(). "
-                        "Increase backward_passes_per_step to accumulate gradients locally.")
             assert not p.grad.requires_grad
-            assert self._allreduce_delay[p] > 0
+            more = self._count_backward_pass(p)
             handle, ctx = None, None
-            self._allreduce_delay[p] -= 1
             bucket = self._p_to_bucket.get(p)
             if bucket is not None:
                 adopt_grad(p, bucket['views'][p], densify=True)
                 self._handles[p] = ('bucket', None)
-                fold_arrived(self, bucket, self._allreduce_delay[p] > 0)
-                if self._allreduce_delay[p] == 0:
+                self._fold_arrived(bucket, more > 0)
+                if more == 0:
                     bucket['pending'] -= 1
                     if bucket['pending'] == 0:
                         self._launch_bucket(bucket)
                 return
-            if accumulates(self, p.grad):
-                if self._allreduce_delay[p] > 0:
+            if self._accumulates(p.grad):
+                if more > 0:
                     self._fold_param(p, 'add' if p in self._acc_open else 'first')
                 elif p in self._acc_open:
                     self._fold_param(p, 'last')
-            if self._allreduce_delay[p] == 0:
+            if more == 0:
                 if self._groups is not None:
                     group = self._p_to_group[p]
                     self._group_counts[id(group)] += 1
@@ -326,7 +536,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._handles[p] = (handle, ctx)
         return hook
 
-    # ---- gradient accumulation in fp32 of the parameters outside the buckets (grad_buckets.py has the buckets') ----------
+    # ---- gradient accumulation in fp32 of the parameters outside the buckets (the base class has the buckets') -----------
     def _param_acc(self, p):
         acc = self._param_accs.get(p)
         if acc is None or acc.shape != p.grad.shape or acc.stride() != p.grad.stride():
@@ -350,54 +560,37 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     def _reset_folds(self):
         self._acc_open.clear()
-        reset_folds(self._buckets)
+        super()._reset_folds()
 
     def _accumulator_pairs(self, with_buckets=True):
         """(16-bit gradients, fp32 accumulators) of every accumulating bucket and parameter, allocated now if needed."""
-        grads, accs = bucket_accumulators(self, with_buckets)
+        grads, accs = super()._accumulator_pairs(with_buckets)
         for group in self.param_groups:
             for p in group['params']:
-                if p.requires_grad and p not in self._p_to_bucket and accumulates(self, p.grad):
+                if p.requires_grad and p not in self._p_to_bucket and self._accumulates(p.grad):
                     grads.append(p.grad)
                     accs.append(self._param_acc(p))
         return grads, accs
 
-    def _prepare_accumulators(self):
-        """hvd.GraphedStep, before capture: the accumulators must exist outside the graphs' memory pool."""
-        self._accumulator_pairs()
-
-    def _graph_fold(self, mode, with_buckets=True):
-        """hvd.GraphedStep, while capturing: one fold of every accumulator after the captured backward pass."""
-        fold(*self._accumulator_pairs(with_buckets), mode)
-
     # ---- gradient allreduce as CUDA-graph nodes (hvd.GraphedStep) --------------------------------------------------------
-    def _graph_capturable(self):
-        """The whole gradient reduction can live inside the captured step: every trainable parameter sits in a registered
-        zero-copy bucket and the reduction is one the in-place kernel implements.  With backward_passes_per_step > 1 the
-        reduction is part of the step's last graph only.  Depends on the model and the constructor arguments only, so
-        every rank answers the same."""
+    def _new_graph_capture(self):
+        """The whole gradient reduction can live inside the captured step when every trainable parameter sits in a
+        registered zero-copy bucket and the reduction is one the in-place kernel implements.  With
+        backward_passes_per_step > 1 the reduction is part of the step's last graph only.  Whether it can depends on the
+        model and the constructor arguments only, so every rank answers the same."""
         if not (self._zero_copy and self._buckets and self.op in (Average, Sum)):
-            return False
+            return None
         if not self.process_set.included() or self.process_set.size() <= 1:
-            return False
-        if os.environ.get('HVD_GRAPH_COMM', '1') == '0':
-            return False
-        return all(p in self._p_to_bucket for p in self._requires_update)
-
-    def _begin_graph_capture(self):
-        """Called by hvd.GraphedStep right after stream capture began (on the capturing stream)."""
-        self._graph_comm_captured = False
-        if not self._graph_capturable():
-            return False
+            return None
+        if not all(p in self._p_to_bucket for p in self._requires_update):
+            return None
         lo_pri, hi_pri = torch.cuda.Stream.priority_range() if hasattr(torch.cuda.Stream, 'priority_range') else (0, -1)
-        self._graph_capture = {'comm': torch.cuda.Stream(priority=hi_pri), 'launched': set(),
-                               # few CTAs while backward still needs the SMs, all of them for the tail bucket(s) that nothing overlaps any more
-                               # (without NVLS — teams of 2 — the P2P two-shot kernel needs more CTAs to keep up with backward)
-                               'ctas': int(os.environ.get('HVD_GRAPH_COMM_CTAS', '16' if '+mc' in mpi_ops.gpu_backend_info() and self.process_set.size() >= 4 else '32')),
-                               'tail_ctas': int(os.environ.get('HVD_GRAPH_COMM_TAIL_CTAS', '128')), 'tail': False,
-                               'pending': {id(b): len(b['params']) for b in self._buckets}}
-        mark_fold_last(self, True)  # the step's last graph of an fp32 accumulation
-        return True
+        return {'comm': torch.cuda.Stream(priority=hi_pri), 'launched': set(),
+                # few CTAs while backward still needs the SMs, all of them for the tail bucket(s) that nothing overlaps any more
+                # (without NVLS — teams of 2 — the P2P two-shot kernel needs more CTAs to keep up with backward)
+                'ctas': int(os.environ.get('HVD_GRAPH_COMM_CTAS', '16' if '+mc' in mpi_ops.gpu_backend_info() and self.process_set.size() >= 4 else '32')),
+                'tail_ctas': int(os.environ.get('HVD_GRAPH_COMM_TAIL_CTAS', '128')), 'tail': False,
+                'pending': {id(b): len(b['params']) for b in self._buckets}}
 
     def _graph_hook(self, p):
         bucket = self._p_to_bucket.get(p)
@@ -408,20 +601,13 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         if cap['pending'][id(bucket)] == 0:
             self._launch_bucket(bucket)
 
-    def _end_graph_capture(self):
-        """Before stream capture ends: buckets whose last hook never fired (parameters unused by the step) are reduced
-        now, then the capturing stream joins the communication stream."""
+    def _launch_remaining(self):
+        """Buckets whose last hook never fired (parameters unused by the step) are reduced now."""
         cap = self._graph_capture
-        if cap is None:
-            return
         cap['tail'] = True
         for bucket in self._buckets:
             if id(bucket) not in cap['launched']:
                 self._launch_bucket(bucket)
-        torch.cuda.current_stream().wait_stream(cap['comm'])
-        self._graph_capture = None
-        mark_fold_last(self, False)
-        self._graph_comm_captured = True
 
     def _restore_shadows(self):
         """Reduced values of wire-dtype shadow buckets -> the fp32 gradients that p.grad points at."""
@@ -469,7 +655,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 if bucket.get('shadow') is not None:
                     bucket['shadow_fresh'] = True
                 for p in bucket['params']:
-                    self._allreduce_delay[p] = self.backward_passes_per_step
+                    self._delay[p] = self.backward_passes_per_step
                     self._handles.pop(p, None)
         if self._zero_copy and not _defer_shadow_copy:
             self._restore_shadows()  # callers of synchronize() (gradient clipping, ...) read p.grad
@@ -496,12 +682,12 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 group, ctxs = self._group_handles[handle]
                 outputs = synchronize(handle)
                 for gp, out, c in zip(group, outputs, ctxs):
-                    self._allreduce_delay[gp] = self.backward_passes_per_step
+                    self._delay[gp] = self.backward_passes_per_step
                     if out is not gp.grad:
                         gp.grad.set_(self._compression.decompress(out, c))
                 continue
             output = synchronize(handle)
-            self._allreduce_delay[p] = self.backward_passes_per_step
+            self._delay[p] = self.backward_passes_per_step
             if p.grad.is_sparse:
                 aggregated = self._compression.decompress(output, ctx)
                 if not aggregated.is_sparse:
@@ -513,11 +699,8 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._group_handles.clear()
         self._synchronized = True
 
-    skip_synchronize = grad_buckets.skip_synchronize
-
-    def _drop_iteration_state(self):
-        self._synchronized = self._reduced = False
-        self._clip_coef = None
+    def _reduce_pending(self):
+        self.synchronize(_defer_shadow_copy=self._fused)
 
     def _grads_to_clip(self):
         """The gradients the next update reads, with a fresh wire-dtype shadow in place of its fp32 bucket: each zero-copy
@@ -528,29 +711,14 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             raise ValueError('clip_grad_norm_ does not support sparse gradients')
         return grads
 
-    def clip_grad_norm_(self, max_norm, norm_type=2.0, error_if_nonfinite=False):
-        """Global-norm gradient clipping, the counterpart of torch.nn.utils.clip_grad_norm_(model.parameters(), ...):
-        call it after backward (and after GradScaler.unscale_, if used) and before step().
-
-        Reduces the gradients that are still pending, as synchronize() does (the following step() neither reduces again
-        nor warns), and returns the norm of the reduced gradients as a 0-dim fp32 tensor on their device.  All ranks hold
-        the same reduced gradients, so no further collective is needed.  On CUDA the norm is one statistics kernel per
-        gradient dtype, without a host synchronisation.  When step() runs the fused update, the clip coefficient
-        min(max_norm / (norm + 1e-6), 1) stays on the device and scales the gradient inside that update, and p.grad is
-        not rescaled; otherwise p.grad is scaled in place, as torch does.  norm_type is 2 or inf; sparse gradients raise
-        ValueError.  error_if_nonfinite=True synchronises with the host, as torch's does."""
-        norm_type = float(norm_type)
-        if norm_type not in (2.0, math.inf):
-            raise ValueError('clip_grad_norm_ supports norm_type 2 and inf, got %r' % norm_type)
-        if not (self._synchronized or self._reduced):
-            self.synchronize(_defer_shadow_copy=self._fused)
-            self._reduced = True
+    def _grad_norm(self, norm_type):
+        """All ranks hold the same reduced gradients, so no further collective is needed."""
         fused = self._master_weights or (self._fused and _fused_plan(self) is not None)
         if not fused:
             self._restore_shadows()
         grads = self._grads_to_clip()
         if not grads:
-            return torch.zeros((), dtype=torch.float32)
+            return None, None
         if grads[0].is_cuda:
             from horovod_b200 import ops
             stats = torch.zeros(2, dtype=torch.float32, device=grads[0].device)
@@ -558,24 +726,10 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             total = stats[0].sqrt() if norm_type == 2.0 else stats[0].clone()
         else:  # CPU tensors: torch's norm
             total = torch.nn.utils.get_total_norm(grads, norm_type)
-        if self._clip_coef is not None:
-            total = total * self._clip_coef  # clipping twice: the norm of the gradient as the first clip left it
-        if error_if_nonfinite and bool(torch.logical_or(total.isnan(), total.isinf())):
-            raise RuntimeError('The total norm of order %s for gradients from `parameters` is non-finite, so it cannot be '
-                               'clipped. To disable this error and scale the gradients by the non-finite norm anyway, set '
-                               '`error_if_nonfinite=False`' % norm_type)
-        coef = torch.clamp(max_norm / (total + 1e-6), max=1.0)
-        if fused:
-            self._clip_coef = coef if self._clip_coef is None else self._clip_coef * coef
-        else:
-            torch._foreach_mul_(grads, coef)
-        return total
-
-    def _hvd_super_step(self, closure=None):
-        return super(self.__class__, self).step(closure)
+        return total, None if fused else grads
 
     def step(self, closure=None):
-        check_not_in_ema(self)
+        self._check_not_in_ema()
         if self._should_synchronize and not self._reduced:
             if self._synchronized:
                 warnings.warn("optimizer.step() called without optimizer.skip_synchronize() context after "
@@ -599,41 +753,17 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._restore_shadows()
         if coef is not None:  # clip_grad_norm_ expected the fused update, which could not run
             torch._foreach_mul_(self._grads_to_clip(), coef)
-        return super(self.__class__, self).step(closure)
+        return super().step(closure)
 
-    @contextmanager
-    def ema_parameters(self):
-        """Evaluates with the EMA (optimizer built with ema_decay): inside the block every parameter that has an EMA holds
-        it, rounded to the parameter's dtype and written in place (storage and addresses stay, so a captured
-        hvd.GraphedStep remains valid; model.state_dict() taken inside is the EMA model, sharing the parameters' storage,
-        so save or clone it inside).  On exit the parameters get their exact previous values back; masters, moments and
-        the EMA are not touched.  Parameters the optimizer has not updated yet have no EMA and keep their values, and
-        buffers such as BatchNorm running statistics are never averaged.  step() inside the block raises RuntimeError.
-        The stash costs one copy of the parameters in their own dtype."""
-        if not self._ema:
-            raise RuntimeError('ema_parameters() needs an optimizer built with ema_decay')
-        check_not_in_ema(self)
-        pairs = [(p, self.state[p]['ema_param']) for g in self.param_groups for p in g['params']
-                 if 'ema_param' in self.state.get(p, {})]
-        with torch.no_grad():
-            stash = [p.detach().clone() for p, _ in pairs]
-            for p, e in pairs:
-                p.detach().copy_(e)
-        self._ema_active = True
-        try:
-            yield
-        finally:
-            self._ema_active = False
-            with torch.no_grad():
-                for (p, _), s in zip(pairs, stash):
-                    p.detach().copy_(s)
+    def _ema_pairs(self):
+        return [(p.detach(), self.state[p]['ema_param']) for g in self.param_groups for p in g['params']
+                if 'ema_param' in self.state.get(p, {})]
 
     def zero_grad(self, *args, **kwargs):
         if self._handles:
             raise AssertionError("optimizer.zero_grad() was called after loss.backward() but before optimizer.step() or "
                                  "optimizer.synchronize(). This is prohibited as it can cause a race condition.")
-        if self._reduced or self._clip_coef is not None:
-            self._drop_iteration_state()  # an iteration whose step() was skipped leaves no clip coefficient behind
+        self._start_afresh()
         if self._zero_copy:
             # bucketed gradients must stay views of the registered buffers: zero them in place (one memset per bucket)
             for bucket in self._buckets:
@@ -649,7 +779,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         if self._graph_mode:
             kwargs['set_to_none'] = False
             args = ()
-        return super(self.__class__, self).zero_grad(*args, **kwargs)
+        return super().zero_grad(*args, **kwargs)
 
 
 def _optimizer_kind(opt):
@@ -677,25 +807,6 @@ def check_ema_decay(decay):
     """ema_decay is None (no EMA) or a number d with 0 <= d <= 1, the range torch's get_ema_multi_avg_fn accepts."""
     if decay is not None and not (isinstance(decay, numbers.Real) and not isinstance(decay, bool) and 0.0 <= decay <= 1.0):
         raise ValueError('ema_decay must be None or a number in [0, 1], got %r' % (decay,))
-
-
-def init_ema(opt, ema_decay):
-    """Constructor part of ema_decay, shared by the unsharded and the sharded optimizer: the decay goes into every param
-    group as group['ema_decay'], read at every step like 'lr'.  Returns whether the EMA is on."""
-    check_ema_decay(ema_decay)
-    opt._ema_active = False  # inside ema_parameters()
-    if ema_decay is None:
-        return False
-    opt.defaults['ema_decay'] = float(ema_decay)  # add_param_group() takes it from here
-    for g in opt.param_groups:
-        g['ema_decay'] = float(ema_decay)
-    return True
-
-
-def check_not_in_ema(opt):
-    if opt._ema_active:
-        raise RuntimeError('optimizer.step() inside ema_parameters(): the parameters hold the EMA there, and the update '
-                           'would start from it')
 
 
 def ema_weight(group):
@@ -899,23 +1010,12 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
     (reference horovod/torch/optimizer.py:345-513)"""
 
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1):
-        super(self.__class__, self).__init__(params)
+        super().__init__(params)
         self._compression = compression
-        if named_parameters is not None:
-            named_parameters = list(named_parameters)
-        else:
-            named_parameters = [(f'allreduce.noname.{i}.{j}', v)
-                                for i, param_group in enumerate(self.param_groups)
-                                for j, v in enumerate(param_group['params'])]
-        all_param_ids = {id(v) for param_group in self.param_groups for v in param_group['params']}
-        named_param_ids = {id(v) for k, v in named_parameters}
-        unnamed_param_ids = all_param_ids - named_param_ids
-        if len(unnamed_param_ids):
-            raise ValueError('named_parameters was specified, but one or more model parameters were not named. Python '
-                             'object ids: %s' % ', '.join(str(id) for id in unnamed_param_ids))
+        named_parameters = check_named_parameters(self, named_parameters)
         self._parameter_names = {v: k for k, v in sorted(named_parameters)}
         self.backward_passes_per_step = backward_passes_per_step
-        self._allreduce_delay = {v: self.backward_passes_per_step for _, v in sorted(named_parameters)}
+        self._delay = {v: self.backward_passes_per_step for _, v in sorted(named_parameters)}
         self._handles = {}
         self._grad_accs = []
         self._requires_update = set()
@@ -927,8 +1027,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
 
     def set_backward_passes_per_step(self, passes):
         self.backward_passes_per_step = passes
-        for p in self._allreduce_delay:
-            self._allreduce_delay[p] = self.backward_passes_per_step
+        self._delay = dict.fromkeys(self._delay, passes)
 
     def _register_hooks(self):
         for param_group in self.param_groups:
@@ -951,7 +1050,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
                 group['params'] = []
         start = self._starting_models[p]
         start.data.copy_(p)
-        super(self.__class__, self).step()
+        super().step()
         p.data.sub_(start)  # p now holds the local delta
         tensor_compressed, ctx = self._compression.compress(p.data)
         handle = allreduce_async_(tensor_compressed, name=name, op=Adasum)
@@ -964,21 +1063,18 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
             if self._graph_mode:
                 return
             if p in self._handles and self._handles[p][0] is not None:
-                if self._allreduce_delay[p] <= 0:
+                if self._delay[p] <= 0:
                     raise AssertionError(
                         "Gradients were computed more than backward_passes_per_step times before call to step(). "
                         "Increase backward_passes_per_step to accumulate gradients locally.")
             assert not p.grad.requires_grad
-            assert self._allreduce_delay[p] > 0
+            assert self._delay[p] > 0
             handle, ctx = None, None
-            self._allreduce_delay[p] -= 1
-            if self._allreduce_delay[p] == 0:
+            self._delay[p] -= 1
+            if self._delay[p] == 0:
                 handle, ctx = self._allreduce_grad_async(p)
             self._handles[p] = (handle, ctx)
         return hook
-
-    def _hvd_super_step(self, closure=None):
-        return super(self.__class__, self).step(closure)
 
     def _whole_model_step(self):
         """Same math as the per-parameter hooks, issued once for the whole model (graph mode: backward was a CUDA graph
@@ -992,7 +1088,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
         datas = [p.data for p in ps]
         with torch.no_grad():
             torch._foreach_copy_(starts, datas)
-            super(self.__class__, self).step()
+            super().step()
             torch._foreach_sub_(datas, starts)
             handles = []
             for p in ps:
@@ -1021,7 +1117,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
             return loss
         missing_p = self._requires_update - set(self._handles.keys())
         for p in missing_p:
-            self._allreduce_delay[p] = 0
+            self._delay[p] = 0
             handle, ctx = self._allreduce_grad_async(p)
             self._handles[p] = (handle, ctx)
         for p, (handle, ctx) in self._handles.items():
@@ -1034,7 +1130,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
             start = self._starting_models[p]
             start.data.add_(delta.data)
             p.data.copy_(start)
-            self._allreduce_delay[p] = self.backward_passes_per_step
+            self._delay[p] = self.backward_passes_per_step
         self._handles.clear()
         return loss
 
@@ -1042,7 +1138,7 @@ class _DistributedAdasumOptimizer(torch.optim.Optimizer):
         if self._handles:
             raise AssertionError("optimizer.zero_grad() was called after loss.backward() but before optimizer.step() or "
                                  "optimizer.synchronize(). This is prohibited as it can cause a race condition.")
-        return super(self.__class__, self).zero_grad(*args, **kwargs)
+        return super().zero_grad(*args, **kwargs)
 
 
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none, backward_passes_per_step=1,
@@ -1120,13 +1216,13 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
                    gradient_predivide_factor, groups, sparse_as_dense, process_set, bucket_cap_mb, master_weights,
                    grad_accumulation_dtype, ema_decay)
     if op != Adasum or size() == 1:
-        cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedOptimizer.__dict__))
+        cls = type(optimizer.__class__.__name__, (_DistributedOptimizer, optimizer.__class__), {})
         return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, op,
                    gradient_predivide_factor, groups, sparse_as_dense, process_set, fused, zero_copy, bucket_cap_mb, bucket_wire_dtype,
                    master_weights, grad_accumulation_dtype, ema_decay)
     if process_set != global_process_set:
         raise NotImplementedError("Adasum does not support non-global process sets yet.")
-    cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedAdasumOptimizer.__dict__))
+    cls = type(optimizer.__class__.__name__, (_DistributedAdasumOptimizer, optimizer.__class__), {})
     return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step)
 
 

@@ -34,35 +34,34 @@ fp32 accumulator of its full size: when a bucket has received a backward pass's 
 accumulator and zeroed (grad_accumulate_ 'first' / 'add'), and after the k-th pass the sum rounded once is written back
 ('last') right before the bucket's reduce-scatter, on the same stream.
 """
-import math
-import os
 import warnings
-from contextlib import contextmanager
 
 import torch
 
 from horovod_b200.common.process_sets import global_process_set
-from horovod_b200.torch import grad_buckets, mpi_ops
+from horovod_b200.torch import mpi_ops
 from horovod_b200.torch.compression import Compression
-from horovod_b200.torch.grad_buckets import (ALIGN, adopt_grad, adopt_missing_grads, bucket_accumulators,
-                                             check_grad_accumulation_dtype, check_named_parameters, fold, fold_arrived,
-                                             fold_last, full_from_shards, grad_bucket, mark_fold_last, reset_folds,
-                                             scales, shard_from_full, shard_layout, shard_range, shard_slices)
+from horovod_b200.torch.grad_buckets import (ALIGN, adopt_grad, adopt_missing_grads, check_named_parameters, fold_last,
+                                             full_from_shards, grad_bucket, shard_from_full, shard_layout, shard_range,
+                                             shard_slices)
 from horovod_b200.torch.mpi_ops import Average, Sum
-from horovod_b200.torch.optimizer import (_COUNTS_STEPS, _STATE_KEYS, _fused_update, _optimizer_kind, _state_dtype, _state_keys,
-                                          check_not_in_ema, init_ema)
+from horovod_b200.torch.optimizer import (_COUNTS_STEPS, _STATE_KEYS, _DistributedOptimizerBase, _fused_update,
+                                          _optimizer_kind, _state_dtype, _state_keys)
 
 
-class _ShardedDistributedOptimizer(torch.optim.Optimizer):
+class _ShardedDistributedOptimizer(_DistributedOptimizerBase):
     """Wraps SGD / Adam / AdamW / Lamb / Lars so that every rank keeps optimizer state for 1/N of the parameters (ZeRO
     stage 1).
     Built by `hvd.DistributedOptimizer(opt, shard_optimizer_state=True)`; the dynamic class derives from this one and from
     the wrapped optimizer's class."""
 
+    _norm_type_error = 'clip_grad_norm_ with sharded optimizer state supports norm_type 2 and inf, got %r'
+
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, op=Average,
                  gradient_predivide_factor=1.0, groups=None, sparse_as_dense=False, process_set=global_process_set,
                  bucket_cap_mb=32, master_weights=False, grad_accumulation_dtype=None, ema_decay=None):
-        super().__init__(params)
+        super().__init__(params, process_set, op, gradient_predivide_factor, backward_passes_per_step,
+                         grad_accumulation_dtype, ema_decay)
         kind = _optimizer_kind(self)
         if kind is None:
             raise ValueError('shard_optimizer_state supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
@@ -84,23 +83,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             raise ValueError('shard_optimizer_state needs registered symmetric memory (P2P backend, one host, not elastic)')
 
         self._kind = kind
-        self._ema = init_ema(self, ema_decay)
-        # fp32 accumulators of the bf16 / fp16 gradient buckets over the backward passes of one step (b['acc'], plain
-        # device memory allocated on first use, not optimizer state)
-        self._acc_fp32 = check_grad_accumulation_dtype(grad_accumulation_dtype)
-        self.process_set = process_set
-        self.op = op
-        self.gradient_predivide_factor = gradient_predivide_factor
-        self.backward_passes_per_step = backward_passes_per_step
         self._nranks, self._rank = process_set.size(), process_set.rank()
-        self._graph_mode = False        # set by hvd.GraphedStep
-        self._graph_capture = None      # while hvd.GraphedStep captures: {'comm': stream}
-        self._graph_comm_captured = False
-        self._should_synchronize = True
-        self._synchronized = False      # set by a user's synchronize(): step() warns and does not reduce again
-        self._reduced = False           # set by clip_grad_norm_ / ShardedGradScaler: step() does not reduce again, silently
-        self._clip_coef = None          # 0-dim fp32 device tensor from clip_grad_norm_, applied by the next step()
-        self._stats_cache = None        # [sum of squares, non-finite] of the unscaled gradients from ShardedGradScaler
         _, hi_pri = torch.cuda.Stream.priority_range()
         device = trainable[0][0].device if any(trainable) else torch.device('cuda', torch.cuda.current_device())
         self._comm = torch.cuda.Stream(device=device, priority=hi_pri)
@@ -158,16 +141,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._next = 0
         for b in self._buckets:
             b['pending'], b['ready'] = len(b['params']), False
-        reset_folds(self._buckets)
-
-    # ---- gradient accumulation in fp32 (grad_accumulation_dtype=torch.float32) -------------------------------------------
-    def _prepare_accumulators(self):
-        """hvd.GraphedStep, before capture: the accumulators must exist outside the graphs' memory pool."""
-        bucket_accumulators(self)
-
-    def _graph_fold(self, mode, with_buckets=True):
-        """hvd.GraphedStep, while capturing: one fold of every accumulating bucket after the captured backward pass."""
-        fold(*bucket_accumulators(self, with_buckets), mode)
+        self._reset_folds()
 
     def _comm_stream(self):
         return self._graph_capture['comm'] if self._graph_capture is not None else self._comm
@@ -181,7 +155,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
             fold_last(b, self._graph_capture is not None)
             comm = self._comm_stream()
             comm.wait_stream(torch.cuda.current_stream())
-            pre, post = scales(self)
+            pre, post = self._scales()
             with torch.cuda.stream(comm):
                 mpi_ops.captured_reducescatter_(b['gflat'], op=self.op, prescale_factor=pre, postscale_factor=post,
                                                 process_set=self.process_set)
@@ -198,16 +172,10 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 if bucket['pending'] == 0:
                     self._mark_ready(bucket)
                 return
-            if self._reduced or self._synchronized or self._clip_coef is not None or self._stats_cache is not None:
-                # a new backward after an iteration whose step() was skipped (e.g. GradScaler found inf): start afresh
-                self._drop_iteration_state()
-            if self._delay[p] <= 0:
-                raise AssertionError('Gradients were computed more than backward_passes_per_step times before call to step(). '
-                                     'Increase backward_passes_per_step to accumulate gradients locally.')
-            self._delay[p] -= 1
+            more = self._count_backward_pass(p)
             self._seen.add(p)
-            fold_arrived(self, bucket, self._delay[p] > 0)
-            if self._delay[p] == 0:
+            self._fold_arrived(bucket, more > 0)
+            if more == 0:
                 bucket['pending'] -= 1
                 if bucket['pending'] == 0:
                     self._mark_ready(bucket)
@@ -233,21 +201,16 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 self._mark_ready(b)
             torch.cuda.current_stream().wait_stream(self._comm)
         self._reset_launch_order()
-        self._delay = {p: self.backward_passes_per_step for p in self._delay}
+        self._delay = dict.fromkeys(self._delay, self.backward_passes_per_step)
         self._seen.clear()
 
     def _reduce_once(self):
-        """Reduces what is still pending unless this iteration's gradients are reduced already; the following step()
-        neither reduces again nor warns."""
         if self._graph_capture is not None:
             raise RuntimeError('clip_grad_norm_ and ShardedGradScaler work in eager mode only, not inside hvd.GraphedStep')
-        if not (self._synchronized or self._reduced):
-            self._reduce_pending()
-            self._reduced = True
+        super()._reduce_once()
 
-    def _drop_iteration_state(self):
-        self._synchronized = self._reduced = False
-        self._clip_coef = self._stats_cache = None
+    def _start_afresh(self):
+        self._drop_iteration_state()  # also after a synchronize() no step() followed: the new gradients need reducing
 
     def _shard_stats(self, norm_type, inv_scale=None):
         """[sum of squares (norm_type 2) or max |g| (inf), non-finite flag] of the reduced gradients over all ranks'
@@ -268,36 +231,12 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._stats_cache = stats
         return found_inf
 
-    def clip_grad_norm_(self, max_norm, norm_type=2.0, error_if_nonfinite=False):
-        """Global-norm gradient clipping for sharded optimizer state, the counterpart of
-        torch.nn.utils.clip_grad_norm_(model.parameters(), ...): call it after backward (and after
-        ShardedGradScaler.unscale_, if used) and before step().
-
-        Reduces the gradients that are still pending (the following step() does not reduce again), computes the norm of
-        the whole averaged gradient from the ranks' owned shards with one scalar allreduce, and returns it as a 0-dim
-        fp32 CUDA tensor with the same bits on every rank.  The clip coefficient min(max_norm / (norm + 1e-6), 1) stays on
-        the device and is applied by the next step() inside the fused update: unlike torch, p.grad itself is not
-        rescaled.  norm_type is 2 or inf.  error_if_nonfinite=True synchronises with the host, as torch's does."""
-        norm_type = float(norm_type)
-        if norm_type not in (2.0, math.inf):
-            raise ValueError('clip_grad_norm_ with sharded optimizer state supports norm_type 2 and inf, got %r' % norm_type)
-        self._reduce_once()
+    def _grad_norm(self, norm_type):
         if norm_type == 2.0 and self._stats_cache is not None:
             stats = self._stats_cache  # ShardedGradScaler.unscale_ computed them in its pass over the same gradients
         else:
             stats = self._shard_stats(norm_type)
-        total = stats[0].sqrt() if norm_type == 2.0 else stats[0].clone()
-        if self._clip_coef is not None:
-            total = total * self._clip_coef  # clipping twice: the norm of the gradient as the first clip left it
-        if error_if_nonfinite and bool(torch.logical_or(total.isnan(), total.isinf())):
-            raise RuntimeError('The total norm of order %s for gradients from `parameters` is non-finite, so it cannot be '
-                               'clipped. To disable this error and scale the gradients by the non-finite norm anyway, set '
-                               '`error_if_nonfinite=False`' % norm_type)
-        coef = torch.clamp(max_norm / (total + 1e-6), max=1.0)
-        self._clip_coef = coef if self._clip_coef is None else self._clip_coef * coef
-        return total
-
-    skip_synchronize = grad_buckets.skip_synchronize
+        return (stats[0].sqrt() if norm_type == 2.0 else stats[0].clone()), None
 
     def _update_shards(self, coef=None):
         """One fused kernel per param group and dtype over this rank's shards.  coef: the clip coefficient on the
@@ -373,7 +312,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         torch.cuda.current_stream().wait_stream(comm)
 
     def step(self, closure=None):
-        check_not_in_ema(self)
+        self._check_not_in_ema()
         loss = None
         if closure is not None:
             with torch.enable_grad():
@@ -392,32 +331,10 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
         self._allgather_params()
         return loss
 
-    @contextmanager
-    def ema_parameters(self):
-        """COLLECTIVE: every rank must enter and leave the block together.  Evaluates with the EMA, as the unsharded
-        optimizer's ema_parameters() does: each rank stashes its own parameter shards, writes its EMA shards rounded to
-        the parameter dtype into them and allgathers the parameter buckets, so every rank holds the whole EMA model in
-        the parameters' own storage.  On exit the stashed shards are written back and allgathered again, which restores
-        every parameter bit for bit.  Buckets whose EMA has not begun keep their values.  step() inside raises
-        RuntimeError."""
-        if not self._ema:
-            raise RuntimeError('ema_parameters() needs an optimizer built with ema_decay')
-        check_not_in_ema(self)
-        bs = [b for b in self._buckets if b['ema_started']]
-        with torch.no_grad():
-            stash = [b['pshard'].clone() for b in bs]
-            for b in bs:
-                b['pshard'].copy_(b['state']['ema_param'])
-            self._allgather_params()
-        self._ema_active = True
-        try:
-            yield
-        finally:
-            self._ema_active = False
-            with torch.no_grad():
-                for b, s in zip(bs, stash):
-                    b['pshard'].copy_(s)
-                self._allgather_params()
+    _params_written = _allgather_params  # ema_parameters() wrote the owned shards
+
+    def _ema_pairs(self):
+        return [(b['pshard'], b['state']['ema_param']) for b in self._buckets if b['ema_started']]
 
     def zero_grad(self, set_to_none=True):
         """Zeroes the gradient buckets in place: p.grad stays a view of registered memory (set_to_none is ignored)."""
@@ -432,33 +349,16 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 if p.grad is None:
                     p.grad = b['views'][p]
 
-    def set_backward_passes_per_step(self, passes):
-        self.backward_passes_per_step = passes
-        self._delay = {p: passes for p in self._delay}
-        reset_folds(self._buckets)
-
     # ---- hvd.GraphedStep -----------------------------------------------------------------------------------------------
-    def _begin_graph_capture(self):
-        """Called by hvd.GraphedStep right after stream capture began: the reduce-scatters become graph nodes."""
-        self._graph_comm_captured = False
-        if os.environ.get('HVD_GRAPH_COMM', '1') == '0':
-            return False
-        self._graph_capture = {'comm': torch.cuda.Stream(device=self._comm.device, priority=self._comm.priority)}
+    def _new_graph_capture(self):
+        """The reduce-scatters become graph nodes, on a stream like the eager one."""
         self._reset_launch_order()
-        mark_fold_last(self, True)  # with backward_passes_per_step > 1 this is the step's last graph
-        return True
+        return {'comm': torch.cuda.Stream(device=self._comm.device, priority=self._comm.priority)}
 
-    def _end_graph_capture(self):
-        cap = self._graph_capture
-        if cap is None:
-            return
+    def _launch_remaining(self):
         for b in self._buckets[self._next:]:
             self._mark_ready(b)
-        torch.cuda.current_stream().wait_stream(cap['comm'])
-        self._graph_capture = None
         self._reset_launch_order()
-        mark_fold_last(self, False)
-        self._graph_comm_captured = True
 
     # ---- checkpoints ------------------------------------------------------------------------------------------------------
     def state_dict(self):
@@ -490,8 +390,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
     def load_state_dict(self, state_dict):
         """Accepts the format of state_dict() from a sharded or an unsharded optimizer and keeps this rank's slice only.
         Does not communicate."""
-        if self._ema_active:
-            raise RuntimeError('load_state_dict() inside ema_parameters(): the block restores the parameters on exit')
+        self._check_not_in_ema(loading=True)
         groups = state_dict['param_groups']
         if len(groups) != len(self.param_groups) or any(len(a['params']) != len(b['params']) for a, b in zip(groups, self.param_groups)):
             raise ValueError('loaded state dict does not match the optimizer\'s parameter groups')
@@ -525,7 +424,7 @@ class _ShardedDistributedOptimizer(torch.optim.Optimizer):
                 steps = [float(st['step']) for st in per if 'step' in st]
                 b['step'] = int(max(steps)) if steps else 0
         self._reset_launch_order()
-        self._delay = {p: self.backward_passes_per_step for p in self._delay}
+        self._delay = dict.fromkeys(self._delay, self.backward_passes_per_step)
         self._seen.clear()
 
     def _broadcast_state(self, root_rank):
