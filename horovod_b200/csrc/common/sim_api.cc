@@ -4,6 +4,7 @@
 // exactly what runs across NVLink; only the address mapping differs.  Lets the
 // kernels be validated (and run under compute-sanitizer) on one GPU.
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <string>
@@ -349,6 +350,53 @@ int64_t hvd_plan_collective(int kind, int nranks, int ntensors, const int64_t* d
   }
   if (m > max_rows) { CopyMessage("more than max_rows ranges", err, err_len); return -6; }
   return m;
+}
+
+// PlanAllreduce of one rank on the host only (the pointers are never dereferenced): pieces counts[t] / in_ptrs[t] /
+// out_ptrs[t], the wire dtype the engine chose, HVD_ALLREDUCE_VARIANT `variant` and the rest of the AllreducePolicy.  Writes
+// one row of 15 int64 per launch, {reduce, variant, ctas, total_bytes, reduce_lo, reduce_hi, dtype, wire_dtype, op, the bits
+// of prescale and of postscale, InlineDescs, nout, oneshot_nvls, ndesc}, and the launches' descriptors in order, one row
+// {in, out, offset, count} each.  Returns the number of launches, -5 (no plan) with the reason in `err`, or -6 (more than
+// max_launches or max_descs).
+int64_t hvd_plan_allreduce(int nranks, int ntensors, const int64_t* counts, const uint64_t* in_ptrs, const uint64_t* out_ptrs,
+                           int dtype, int wire_dtype, int op, double prescale, double postscale, const char* variant,
+                           int64_t oneshot_max_bytes, int multicast, int64_t nvls_min_bytes, int64_t cap, int comm_ctas,
+                           int64_t large_msg_ctas, int64_t* launch_rows, int64_t max_launches, int64_t* desc_rows, int64_t max_descs,
+                           char* err, int err_len) {
+  std::vector<PlanTensor> ts(ntensors);
+  for (int i = 0; i < ntensors; ++i) {
+    ts[i].in = (const void*)in_ptrs[i]; ts[i].out = (void*)out_ptrs[i]; ts[i].dims = {counts[i]};
+  }
+  ReduceParams rp;
+  rp.dtype = (DataType)dtype; rp.op = (ReduceOp)op; rp.prescale = prescale; rp.postscale = postscale;
+  AllreducePolicy pol;
+  pol.variant = variant;
+  pol.oneshot_max_bytes = oneshot_max_bytes;
+  pol.multicast = multicast != 0;
+  pol.nvls_min_bytes = nvls_min_bytes;
+  pol.large_msg_ctas = large_msg_ctas;
+  Plan plan;
+  Status st = PlanAllreduce(nranks, ts, rp, (DataType)wire_dtype, pol, cap, comm_ctas, &plan);
+  if (!st.ok()) { CopyMessage(st.reason(), err, err_len); return -5; }
+  int64_t nd = 0;
+  for (const PlanLaunch& l : plan) nd += (int64_t)l.table.size();
+  if ((int64_t)plan.size() > max_launches || nd > max_descs) { CopyMessage("more than max_launches or max_descs", err, err_len); return -6; }
+  int64_t* o = launch_rows;
+  int64_t* d = desc_rows;
+  for (const PlanLaunch& l : plan) {
+    const kern::AllreduceArgs& a = l.args;
+    int64_t pre, post;
+    memcpy(&pre, &a.prescale, sizeof pre);
+    memcpy(&post, &a.postscale, sizeof post);
+    const int64_t row[15] = {l.reduce, a.variant, l.ctas, a.total_bytes, a.reduce_lo, a.reduce_hi, a.dtype, a.wire_dtype, a.op, pre, post,
+                             InlineDescs(a), a.nout, a.oneshot_nvls, a.ndesc};
+    o = std::copy(row, row + 15, o);
+    for (const kern::TensorDesc& t : l.table) {
+      const int64_t drow[4] = {(int64_t)(uintptr_t)t.in, (int64_t)(uintptr_t)t.out, t.offset, t.count};
+      d = std::copy(drow, drow + 4, d);
+    }
+  }
+  return (int64_t)plan.size();
 }
 
 // Adasum over N simulated ranks: in_ptrs/out_ptrs [nranks][ntensors]; dtype fp32/fp16/bf16.

@@ -23,6 +23,62 @@ void AddExchange(Plan* plan, std::vector<kern::CopyDesc>& sends, std::vector<ker
 std::string Str(int64_t v) { return std::to_string(v); }
 }  // namespace
 
+// Small messages are latency bound (few CTAs = cheap flag barrier, SMs left to compute); >= 64 MiB of plain tensors are
+// bound by the local pack / unpack phases, which need two CTAs per SM (ncu: 12.5 % warps active at one).
+int CtasFor(int variant, int64_t seg_bytes, int n, int comm_ctas, int64_t large_msg_ctas) {
+  const int64_t per = variant == kern::kOneShot ? 8192 : (int64_t)4096 * n;  // >= 2 rows (one-shot) or one row per rank (two-shot) per CTA
+  // (a one-shot CTA makes four dependent NVLink trips, so a 1 MiB message wants more than 16 CTAs)
+  const int64_t cap_ctas = seg_bytes <= (256 << 10) ? std::min<int64_t>(comm_ctas, 16)
+                         : seg_bytes <= (16 << 20) ? std::min<int64_t>(comm_ctas, 64)
+                         : seg_bytes < (64 << 20) ? comm_ctas : std::max<int64_t>(comm_ctas, large_msg_ctas);
+  return (int)std::max<int64_t>(1, std::min<int64_t>(cap_ctas, (seg_bytes + per - 1) / per));
+}
+
+// Every rank packs the same pieces at the same offsets and reduces the whole segment, so the plan is the same on every
+// rank up to the tensor addresses.  A piece that does not fit the rest of the segment is split across segments.
+Status PlanAllreduce(int n, const std::vector<PlanTensor>& ts, const ReduceParams& rp, DataType wire, const AllreducePolicy& pol,
+                     int64_t cap, int comm_ctas, Plan* plan) {
+  cap = cap / 128 * 128;
+  if (cap < 128) return Status::InvalidArgument("allreduce: a symmetric buffer of " + Str(cap) + " bytes cannot hold 128 bytes");
+  const int64_t esz = (int64_t)DataTypeSize(rp.dtype), wsz = (int64_t)DataTypeSize(wire);
+  const bool multimem = pol.multicast && MultimemReduces(wire, rp.op);
+  PlanLaunch l;  // the segment being filled
+  int64_t seg_bytes = 0;
+  auto flush = [&]() {
+    if (l.table.empty()) return;
+    kern::AllreduceArgs& a = l.args;
+    a.ndesc = (int)l.table.size();
+    a.total_bytes = seg_bytes;
+    a.reduce_lo = 0; a.reduce_hi = seg_bytes;
+    a.prescale = rp.prescale; a.postscale = rp.postscale;
+    a.op = (int)rp.op; a.dtype = (int)rp.dtype; a.wire_dtype = (int)wire;
+    if (pol.variant == "oneshot") a.variant = kern::kOneShot;
+    else if (pol.variant == "twoshot") a.variant = kern::kTwoShot;
+    else if (pol.variant == "nvls" && multimem) a.variant = kern::kNvls;
+    else if (seg_bytes <= pol.oneshot_max_bytes) a.variant = kern::kOneShot;
+    // in-switch reduction pays off from 4 GPUs (measured: slower than two-shot at N=2)
+    else if (multimem && n >= 4 && seg_bytes >= pol.nvls_min_bytes) a.variant = kern::kNvls;
+    else a.variant = kern::kTwoShot;
+    l.reduce = true;
+    l.ctas = CtasFor(a.variant, seg_bytes, n, comm_ctas, pol.large_msg_ctas);
+    plan->push_back(std::move(l));
+    l = PlanLaunch();
+    seg_bytes = 0;
+  };
+  for (const PlanTensor& t : ts) {
+    const int64_t count = t.dims[0];
+    for (int64_t done = 0; done < count;) {
+      if (cap - seg_bytes < 128) flush();
+      const int64_t take = std::min(count - done, (cap - seg_bytes) / wsz);
+      l.table.push_back({(const char*)t.in + done * esz, (char*)t.out + done * esz, seg_bytes, take});
+      seg_bytes += Align128(take * wsz);
+      done += take;
+    }
+  }
+  flush();
+  return Status::OK();
+}
+
 // The fused buffer is laid out destination-rank major — region q holds block q of EVERY tensor of the (fused) response —
 // so each rank reduces one contiguous range straight into its output tensors: one launch per segment that fits the
 // buffer.  A tensor whose blocks do not fit is split into element windows [w0, w0 + len) of every block.

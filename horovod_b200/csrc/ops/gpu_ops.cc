@@ -202,6 +202,31 @@ Status BuildPieces(Entries& es, const Response& r, int device, cudaStream_t s, s
   return Status::OK();
 }
 
+// The pieces' packed layout in a fusion buffer, each at the next 128-byte boundary; returns the buffer's bytes.
+int64_t PackDescs(const std::vector<Piece>& pieces, int64_t esz, std::vector<kern::TensorDesc>* descs) {
+  int64_t total = 0;
+  for (auto& p : pieces) {
+    descs->push_back({p.in, p.out, total, p.count});
+    total += Align128(p.count * esz);
+  }
+  return total;
+}
+
+// Arguments of the zero-copy kernel over every rank's copy of a tensor, ptr[p] + off as mapped into this process, without
+// multicast; false when the kernel cannot apply the scale factors to `op` (it scales sums only).
+bool FillInplaceArgs(int n, void* const* ptr, int64_t off, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
+                     double postscale, int max_ctas, kern::InplaceArgs* ia) {
+  if (op != ReduceOp::SUM && op != ReduceOp::AVERAGE && !(prescale == 1.0 && postscale == 1.0)) return false;
+  *ia = kern::InplaceArgs {};
+  for (int p = 0; p < n; ++p) ia->ptr[p] = (char*)ptr[p] + off;
+  ia->bytes = bytes;
+  ia->scale = prescale * postscale;
+  ia->op = (int)op;
+  ia->dtype = (int)dtype;
+  ia->ctas = (int)std::max<int64_t>(1, std::min<int64_t>(max_ctas, (bytes + 4096ll * n - 1) / (4096ll * n)));
+  return true;
+}
+
 }  // namespace
 
 std::shared_ptr<SymmTeam> GpuOps::EnsureTeam(ProcessSet& ps, int device) {
@@ -243,12 +268,6 @@ std::shared_ptr<SymmTeam> GpuOps::EnsureTeam(ProcessSet& ps, int device) {
   // (same decision on every rank: a team exists everywhere or nowhere, the flags come from the shared environment)
   if (ps.team && ps.id == 0 && env_.calibrate && env_.variant == "auto") Calibrate(ps, *ps.team, device);
   return ps.team;
-}
-
-namespace {
-Status RunExchange(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, std::vector<kern::CopyDesc>& sends,
-                   std::vector<kern::CopyDesc>& recvs, int max_ctas, int64_t grid_bytes);
-Status LaunchPlan(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, const Plan& plan, const char* what);
 }
 
 bool GpuOps::EnsureHierarchy(ProcessSet& ps, int device) {
@@ -307,12 +326,7 @@ Status GpuOps::HierarchicalAllreduce(ProcessSet& ps, Entries& es, const Response
   Status st = BuildPieces(es, r, device, s, &pieces);
   if (!st.ok()) return st;
   std::vector<kern::TensorDesc> descs;
-  int64_t total = 0;
-  for (auto& p : pieces) {
-    kern::TensorDesc d; d.in = p.in; d.out = p.out; d.offset = total; d.count = p.count;
-    descs.push_back(d);
-    total += Align128(p.count * esz);
-  }
+  const int64_t total = PackDescs(pieces, esz, &descs);
   if (total == 0) return Status::OK();
   const int64_t B = Align128((total + L - 1) / L);  // shard bytes per local GPU
   char* F = (char*)ctx.TempAlloc(device, (size_t)(B * L), true, s);
@@ -323,26 +337,14 @@ Status GpuOps::HierarchicalAllreduce(ProcessSet& ps, Entries& es, const Response
   if (env_.timeline && env_.timeline->Initialized()) env_.timeline->ActivityStartAll(es, HVD_ACT_HIER_ALLREDUCE);
   HVD_CUDA(kern::LaunchPackUnpack(F, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.prescale, 0, 132, s));
   // ---- 1. intra-host reduce-scatter: local GPU q ends up with block q of the host-local reduction ----
-  const int64_t cap = (int64_t)team.buffer_bytes();
-  const int64_t win = std::min<int64_t>(B, cap / L / 128 * 128);
-  for (int64_t w0 = 0; w0 < B; w0 += win) {
-    const int64_t cnt = std::min(win, B - w0) / esz;
-    std::vector<kern::TensorDesc> table(L + 1);
-    for (int q = 0; q < L; ++q) { table[q].in = F + q * B + w0; table[q].out = nullptr; table[q].offset = q * win; table[q].count = cnt; }
-    table[L].in = nullptr; table[L].out = S + w0; table[L].offset = li * win; table[L].count = cnt;
-    const auto* dt = (const kern::TensorDesc*)ctx.Stage(device, table.data(), table.size() * sizeof(kern::TensorDesc), s);
-    if (!dt) return Status::UnknownError("descriptor table too large");
-    kern::AllreduceArgs a {};
-    a.ndesc = L; a.descs = dt; a.out_descs = dt + L; a.nout = 1;
-    a.total_bytes = (int64_t)L * win;
-    a.reduce_lo = li * win; a.reduce_hi = li * win + Align128(cnt * esz);
-    a.prescale = 1.0; a.postscale = 1.0;
-    a.op = (int)r.reduce_op; a.dtype = (int)r.dtype; a.wire_dtype = (int)r.dtype;
-    a.variant = kern::kOneShot;
-    a.ctas = (int)std::max<int64_t>(1, std::min<int64_t>(env_.params->comm_ctas, (a.total_bytes + 16383) / 16384));
-    cudaError_t ce = kern::LaunchAllreduce(team.Params(team.NextSlot()), a, s);
-    if (ce != cudaSuccess) return Status::UnknownError(std::string("hierarchical reduce-scatter launch failed: ") + cudaGetErrorString(ce));
-  }
+  PlanTensor fused;
+  fused.in = F; fused.out = S; fused.dims = {L * B / esz};
+  ReduceParams rp;
+  rp.dtype = r.dtype; rp.op = r.reduce_op;
+  Plan plan;
+  st = PlanReducescatter(li, L, {fused}, rp, (int64_t)team.buffer_bytes(), env_.params->comm_ctas, &plan);
+  if (st.ok()) st = LaunchPlan(team, device, s, plan, "hierarchical reduce-scatter");
+  if (!st.ok()) return st;
   // ---- 2. cross-host allreduce of the shard (pinned staging; the CPU transport is the inter-node fabric here) ----
   char* host = (char*)ctx.PinnedHost(device, (size_t)B);
   if (!host) return Status::UnknownError("out of pinned host memory for the hierarchical shard");
@@ -352,18 +354,12 @@ Status GpuOps::HierarchicalAllreduce(ProcessSet& ps, Entries& es, const Response
   cpu::Allreduce(ps.cross_transport.get(), host, B / esz, r.dtype, r.reduce_op);
   HVD_CUDA(cudaMemcpyAsync(S, host, (size_t)B, cudaMemcpyHostToDevice, s));
   // ---- 3. intra-host allgather of the shards back into the fusion buffer ----
-  const int64_t gcap = cap / 16 * 16;
-  for (int64_t w0 = 0; w0 < B; w0 += gcap) {
-    const int64_t b = std::min(gcap, B - w0);
-    std::vector<kern::CopyDesc> sends, recvs;
-    sends.push_back({S + w0, nullptr, 0, b, li, 0});
-    for (int k = 0; k < L; ++k) {
-      int p = (li + k) % L;
-      recvs.push_back({nullptr, F + p * B + w0, 0, b, p, 0});
-    }
-    st = RunExchange(team, ctx, device, s, sends, recvs, env_.params->comm_ctas, b);
-    if (!st.ok()) return st;
-  }
+  PlanTensor shard;
+  shard.in = S; shard.out = F; shard.dims.assign(L, B);
+  plan.clear();
+  st = PlanAllgather(li, L, {shard}, 1, (int64_t)team.buffer_bytes(), env_.params->comm_ctas, &plan);
+  if (st.ok()) st = LaunchPlan(team, device, s, plan, "hierarchical allgather");
+  if (!st.ok()) return st;
   HVD_CUDA(kern::LaunchPackUnpack(F, dtab, (int)descs.size(), total, (int)r.dtype, (int)r.dtype, r.postscale, 1, 132, s));
   return Status::OK();
 }
@@ -377,20 +373,11 @@ bool GpuOps::BuildInplaceArgs(SymmTeam& team, const void* ptr, int64_t bytes, Da
   int64_t off = 0;
   if (bytes <= 0 || (bytes & 15) || !team.FindRegion(ptr, (size_t)bytes, &view, &off) || (off & 15)) return false;
   if (expect_off >= 0 && expect_off != off) return false;
-  const bool sum_like = op == ReduceOp::SUM || op == ReduceOp::AVERAGE;
-  if (!sum_like && !(prescale == 1.0 && postscale == 1.0)) return false;
-  kern::InplaceArgs ia {};
-  for (int p = 0; p < n; ++p) ia.ptr[p] = (char*)view.ptr[p] + off;
-  ia.mc = view.mc ? (char*)view.mc + off : nullptr;
-  ia.bytes = bytes;
-  ia.scale = prescale * postscale;
-  ia.op = (int)op;
-  ia.dtype = (int)dtype;
+  if (!FillInplaceArgs(n, view.ptr, off, bytes, dtype, op, prescale, postscale, max_ctas, out)) return false;
+  out->mc = view.mc ? (char*)view.mc + off : nullptr;
   // (the crossover of THIS kernel — no pack / unpack around the NVLink phase — is not the packed kernels' nvls_min_bytes)
-  ia.use_multicast = (ia.mc && sum_like && env_.variant != "twoshot" && (n >= 4 || env_.variant == "nvls") && bytes >= env_.zero_copy_nvls_min_bytes &&
-                      (dtype == DataType::FLOAT32 || dtype == DataType::FLOAT16 || dtype == DataType::BFLOAT16)) ? 1 : 0;
-  ia.ctas = (int)std::max<int64_t>(1, std::min<int64_t>(max_ctas, (bytes + 4096ll * n - 1) / (4096ll * n)));
-  *out = ia;
+  out->use_multicast = (out->mc && MultimemReduces(dtype, op) && env_.variant != "twoshot" && (n >= 4 || env_.variant == "nvls") &&
+                        bytes >= env_.zero_copy_nvls_min_bytes) ? 1 : 0;
   return true;
 }
 
@@ -401,69 +388,43 @@ bool GpuOps::BuildInplaceArgs(SymmTeam& team, const void* ptr, int64_t bytes, Da
 // Nothing like it exists in the reference (its cycle loop negotiates every tensor every step, controller.cc:209-252).
 Status GpuOps::CapturedAllreduce(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                                  double postscale, int max_ctas, cudaStream_t stream, int channel) {
-  std::shared_ptr<SymmTeam> team;
-  { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
-  if (!team) return Status::PreconditionError("captured allreduce: the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
-  if (team->abort_state() != 0) return Status::Aborted("captured allreduce: the team was aborted");
-  kern::InplaceArgs ia {};
-  if (max_ctas <= 0) max_ctas = env_.params->comm_ctas;
-  if (!BuildInplaceArgs(*team, ptr, bytes, dtype, op, prescale, postscale, -1, std::min(max_ctas, kern::kMaxCtas), &ia))
-    return Status::InvalidArgument("captured allreduce: tensor is not (entirely) inside registered symmetric memory, is not 16 B "
-                                   "aligned, or combines MIN/MAX/PRODUCT with scale factors");
-  cudaError_t ce = kern::LaunchInplaceAllreduce(team->Params(0, channel), ia, stream);
-  if (ce != cudaSuccess) return Status::UnknownError(std::string("captured allreduce launch failed: ") + cudaGetErrorString(ce));
-  return Status::OK();
+  return LaunchCaptured(ps, "allreduce", kern::LaunchInplaceAllreduce, ptr, bytes, dtype, op, prescale, postscale, max_ctas, stream,
+                        channel);
 }
 
 // The two halves of a sharded optimizer step, launched exactly like CapturedAllreduce (caller's stream, graph channel, no
 // negotiation).  Rank r owns the contiguous slice [r*S, (r+1)*S), S = bytes / n, of the registered range.
 Status GpuOps::CapturedReducescatter(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                                      double postscale, int max_ctas, cudaStream_t stream) {
-  std::shared_ptr<SymmTeam> team;
-  { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
-  if (!team) return Status::PreconditionError("captured reducescatter: the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
-  if (team->abort_state() != 0) return Status::Aborted("captured reducescatter: the team was aborted");
-  if (bytes % (16 * (int64_t)team->nranks()) != 0)
-    return Status::InvalidArgument("captured reducescatter: the byte size must be a multiple of 16 * the process set size");
-  kern::InplaceArgs ia {};
-  if (max_ctas <= 0) max_ctas = env_.params->comm_ctas;
-  if (!BuildInplaceArgs(*team, ptr, bytes, dtype, op, prescale, postscale, -1, std::min(max_ctas, kern::kMaxCtas), &ia))
-    return Status::InvalidArgument("captured reducescatter: tensor is not (entirely) inside registered symmetric memory, is not 16 B "
-                                   "aligned, or combines MIN/MAX/PRODUCT with scale factors");
-  cudaError_t ce = kern::LaunchInplaceReducescatter(team->Params(0, kern::kGraphChannel), ia, stream);
-  if (ce != cudaSuccess) return Status::UnknownError(std::string("captured reducescatter launch failed: ") + cudaGetErrorString(ce));
-  return Status::OK();
+  return LaunchCaptured(ps, "reducescatter", kern::LaunchInplaceReducescatter, ptr, bytes, dtype, op, prescale, postscale, max_ctas,
+                        stream, kern::kGraphChannel);
 }
 
 Status GpuOps::CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int max_ctas, cudaStream_t stream, int channel) {
-  std::shared_ptr<SymmTeam> team;
-  { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
-  if (!team) return Status::PreconditionError("captured allgather: the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
-  if (team->abort_state() != 0) return Status::Aborted("captured allgather: the team was aborted");
-  if (bytes % (16 * (int64_t)team->nranks()) != 0)
-    return Status::InvalidArgument("captured allgather: the byte size must be a multiple of 16 * the process set size");
-  kern::InplaceArgs ia {};
-  if (max_ctas <= 0) max_ctas = env_.params->comm_ctas;
   // a byte copy: described as an fp32 SUM so that the multicast store follows the same policy as the reductions
-  if (!BuildInplaceArgs(*team, ptr, bytes, DataType::FLOAT32, ReduceOp::SUM, 1.0, 1.0, -1, std::min(max_ctas, kern::kMaxCtas), &ia))
-    return Status::InvalidArgument("captured allgather: tensor is not (entirely) inside registered symmetric memory or is not 16 B aligned");
-  cudaError_t ce = kern::LaunchInplaceAllgather(team->Params(0, channel), ia, stream);
-  if (ce != cudaSuccess) return Status::UnknownError(std::string("captured allgather launch failed: ") + cudaGetErrorString(ce));
-  return Status::OK();
+  return LaunchCaptured(ps, "allgather", kern::LaunchInplaceAllgather, ptr, bytes, DataType::FLOAT32, ReduceOp::SUM, 1.0, 1.0, max_ctas,
+                        stream, channel);
 }
 
-// CTAs of a fused allreduce launch.  Small messages are latency bound (few CTAs = cheap flag barrier, SMs left to compute);
-// >= 64 MiB of plain tensors are bound by the local pack / unpack phases, which need two CTAs per SM (ncu: 12.5 % warps
-// active at one).
-int GpuOps::CtasFor(int variant, int64_t seg_bytes, int n) const {
-  const TunableParams& tp = *env_.params;
-  const int64_t per = variant == kern::kOneShot ? 8192 : (int64_t)4096 * n;  // >= 2 rows (one-shot) or one row per rank (two-shot) per CTA
-  const int64_t big_ctas = env_.large_msg_ctas;
-  // (a one-shot CTA makes four dependent NVLink trips, so a 1 MiB message wants more than 16 CTAs)
-  const int64_t cap_ctas = seg_bytes <= (256 << 10) ? std::min<int64_t>(tp.comm_ctas, 16)
-                         : seg_bytes <= (16 << 20) ? std::min<int64_t>(tp.comm_ctas, 64)
-                         : seg_bytes < (64 << 20) ? tp.comm_ctas : std::max<int64_t>(tp.comm_ctas, big_ctas);
-  return (int)std::max<int64_t>(1, std::min<int64_t>(cap_ctas, (seg_bytes + per - 1) / per));
+Status GpuOps::LaunchCaptured(ProcessSet& ps, const char* what, InplaceLaunch launch, void* ptr, int64_t bytes, DataType dtype,
+                              ReduceOp op, double prescale, double postscale, int max_ctas, cudaStream_t stream, int channel) {
+  const std::string name = std::string("captured ") + what;
+  std::shared_ptr<SymmTeam> team;
+  { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
+  if (!team) return Status::PreconditionError(name + ": the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
+  if (team->abort_state() != 0) return Status::Aborted(name + ": the team was aborted");
+  // reducescatter and allgather split the range into one contiguous shard per rank
+  if (launch != kern::LaunchInplaceAllreduce && bytes % (16 * (int64_t)team->nranks()) != 0)
+    return Status::InvalidArgument(name + ": the byte size must be a multiple of 16 * the process set size");
+  kern::InplaceArgs ia {};
+  if (max_ctas <= 0) max_ctas = env_.params->comm_ctas;
+  if (!BuildInplaceArgs(*team, ptr, bytes, dtype, op, prescale, postscale, -1, std::min(max_ctas, kern::kMaxCtas), &ia))
+    return Status::InvalidArgument(name + (launch == kern::LaunchInplaceAllgather
+        ? ": tensor is not (entirely) inside registered symmetric memory or is not 16 B aligned"
+        : ": tensor is not (entirely) inside registered symmetric memory, is not 16 B aligned, or combines MIN/MAX/PRODUCT with scale factors"));
+  cudaError_t ce = launch(team->Params(0, channel), ia, stream);
+  if (ce != cudaSuccess) return Status::UnknownError(name + " launch failed: " + cudaGetErrorString(ce));
+  return Status::OK();
 }
 
 // Measures, on THIS box and team, where the allreduce variants cross over (SURVEY 5.8: "variant picked per message size
@@ -516,7 +477,7 @@ void GpuOps::Calibrate(ProcessSet& ps, SymmTeam& team, int device) {
         a.total_bytes = bytes; a.reduce_lo = 0; a.reduce_hi = bytes;
         a.prescale = 1.0; a.postscale = 1.0; a.op = (int)ReduceOp::SUM; a.dtype = (int)DataType::FLOAT32; a.wire_dtype = (int)DataType::FLOAT32;
         a.variant = variants[vi];
-        a.ctas = CtasFor(a.variant, bytes, n);
+        a.ctas = CtasFor(a.variant, bytes, n, env_.params->comm_ctas, env_.large_msg_ctas);
         const int warm = 2, iters = 6;
         bool ok = true;
         for (int it = 0; it < warm + iters && ok; ++it) {
@@ -633,9 +594,7 @@ Status GpuOps::Allreduce(ProcessSet& ps, Entries& es, const Response& r, int dev
       // ---- plain tensor, in place, IPC-registrable on every rank (negotiated symm_key == -2): zero-copy P2P two-shot on
       //      the peers' mappings of each other's ordinary allocations ----
       if (r.symm_key == -2 && pieces.size() == 1 && es[0] && pieces[0].in == pieces[0].out && env_.variant != "oneshot") {
-        const bool sum_like = r.reduce_op == ReduceOp::SUM || r.reduce_op == ReduceOp::AVERAGE;
-        const bool nvls_better = sum_like && team->has_multicast() && n > env_.ipc_max_ranks &&
-                                 (r.dtype == DataType::FLOAT32 || r.dtype == DataType::FLOAT16 || r.dtype == DataType::BFLOAT16);
+        const bool nvls_better = MultimemReduces(r.dtype, r.reduce_op) && team->has_multicast() && n > env_.ipc_max_ranks;
         if (!nvls_better) {
           if (!ps.ipc) ps.ipc = std::make_shared<IpcRegistry>();
           const int64_t bytes = pieces[0].count * (int64_t)esz;
@@ -644,12 +603,9 @@ Status GpuOps::Allreduce(ProcessSet& ps, Entries& es, const Response& r, int dev
           const IpcRegistry::Entry* ent = r.from_cache ? ps.ipc->Find(es[0]->name)
                                                        : &ps.ipc->Exchange(ps.transport.get(), es[0]->name, pieces[0].in, (size_t)bytes);
           if (ent && ent->my_ptr != pieces[0].in) ent = nullptr;
-          if (ent && ent->usable && (sum_like || (r.prescale == 1.0 && r.postscale == 1.0))) {
-            kern::InplaceArgs ia {};
-            for (int p = 0; p < n; ++p) ia.ptr[p] = ent->ptr[p];
-            ia.mc = nullptr; ia.bytes = bytes; ia.scale = r.prescale * r.postscale; ia.op = (int)r.reduce_op; ia.dtype = (int)r.dtype;
-            ia.use_multicast = 0;
-            ia.ctas = (int)std::max<int64_t>(1, std::min<int64_t>(env_.params->comm_ctas, (bytes + 4096ll * n - 1) / (4096ll * n)));
+          kern::InplaceArgs ia {};
+          if (ent && ent->usable &&
+              FillInplaceArgs(n, ent->ptr, 0, bytes, r.dtype, r.reduce_op, r.prescale, r.postscale, env_.params->comm_ctas, &ia)) {
             kern::CommParams cp = team->Params(team->NextSlot());
             if (env_.timeline && env_.timeline->Initialized()) env_.timeline->ActivityStartAll(es, HVD_ACT_P2P_ALLREDUCE_TWOSHOT);
             cudaError_t ce = kern::LaunchInplaceAllreduce(cp, ia, s);
@@ -667,70 +623,22 @@ Status GpuOps::Allreduce(ProcessSet& ps, Entries& es, const Response& r, int dev
       if (r.dtype == DataType::FLOAT32 && (env_.wire_dtype == DataType::BFLOAT16 || env_.wire_dtype == DataType::FLOAT16) &&
           (r.reduce_op == ReduceOp::SUM || r.reduce_op == ReduceOp::AVERAGE))
         wire = env_.wire_dtype;
-      const int64_t wsz = (int64_t)DataTypeSize(wire);
       // the tail of each buffer slot (reserved when the team was created) belongs to the latency lane
       const int64_t lat_area = (int64_t)team->reserved_tail();
-      int64_t cap = (int64_t)team->buffer_bytes() / 128 * 128;
       if (lat_lane && lat_area < env_.latency_lane_bytes) lat_lane = false;  // tiny buffers: no reserved tail (same on every rank)
-      if (lat_lane) cap = lat_area / 128 * 128;
-      const TunableParams& tp = *env_.params;
-      // split into segments that fit the symmetric buffer
-      std::vector<kern::TensorDesc> descs;
-      int64_t seg_bytes = 0;
-      auto flush = [&]() -> Status {
-        if (descs.empty()) return Status::OK();
-        kern::AllreduceArgs a {};
-        a.ndesc = (int)descs.size();
-        a.total_bytes = seg_bytes;
-        a.reduce_lo = 0; a.reduce_hi = seg_bytes;
-        a.prescale = r.prescale; a.postscale = r.postscale;
-        a.op = (int)r.reduce_op; a.dtype = (int)r.dtype; a.wire_dtype = (int)wire;
-        // variant by message size (thresholds are autotuned)
-        int variant = kern::kTwoShot;
-        const bool nvls_ok = team->has_multicast() && (r.reduce_op == ReduceOp::SUM || r.reduce_op == ReduceOp::AVERAGE) &&
-                             (wire == DataType::FLOAT32 || wire == DataType::FLOAT16 || wire == DataType::BFLOAT16);
-        if (env_.variant == "oneshot") variant = kern::kOneShot;
-        else if (env_.variant == "twoshot") variant = kern::kTwoShot;
-        else if (env_.variant == "nvls" && nvls_ok) variant = kern::kNvls;
-        else {
-          if (seg_bytes <= tp.oneshot_max_bytes) variant = kern::kOneShot;
-          else if (nvls_ok && n >= 4 && seg_bytes >= tp.nvls_min_bytes) variant = kern::kNvls;  // in-switch reduction pays off from 4 GPUs (measured: slower than two-shot at N=2)
-        }
-        a.variant = variant;
-        a.ctas = CtasFor(variant, seg_bytes, n);
-        if (a.ndesc <= kern::kInlineDescs) {
-          memcpy(a.inline_descs, descs.data(), descs.size() * sizeof(kern::TensorDesc));
-          a.descs = nullptr;
-        } else {
-          a.descs = (const kern::TensorDesc*)ctx.Stage(device, descs.data(), descs.size() * sizeof(kern::TensorDesc), s);
-          if (!a.descs) return Status::UnknownError("descriptor table too large");
-        }
-        kern::CommParams cp = lat_lane ? team->Params(team->NextLatencySlot(), kern::kLatencyChannel, (int64_t)team->buffer_bytes())
-                                       : team->Params(team->NextSlot());
-        if (env_.timeline && env_.timeline->Initialized())
-          env_.timeline->ActivityStartAll(es, variant == kern::kOneShot ? HVD_ACT_P2P_ALLREDUCE_ONESHOT
-                                              : variant == kern::kNvls ? HVD_ACT_P2P_ALLREDUCE_NVLS : HVD_ACT_P2P_ALLREDUCE_TWOSHOT);
-        cudaError_t ce = kern::LaunchAllreduce(cp, a, s);
-        if (ce != cudaSuccess) return Status::UnknownError(std::string("allreduce kernel launch failed: ") + cudaGetErrorString(ce));
-        descs.clear();
-        seg_bytes = 0;
-        return Status::OK();
-      };
-      for (auto& p : pieces) {
-        int64_t done_el = 0;
-        while (done_el < p.count || (p.count == 0 && done_el == 0)) {
-          if (p.count == 0) break;
-          int64_t space = cap - seg_bytes;
-          if (space < 128) { st = flush(); if (!st.ok()) return st; space = cap; }
-          int64_t take = std::min<int64_t>(p.count - done_el, space / wsz);
-          kern::TensorDesc d;
-          d.in = p.in + done_el * esz; d.out = p.out + done_el * esz; d.offset = seg_bytes; d.count = take;
-          descs.push_back(d);
-          seg_bytes += Align128(take * wsz);
-          done_el += take;
-        }
-      }
-      st = flush();
+      std::vector<PlanTensor> ts(pieces.size());
+      for (size_t i = 0; i < pieces.size(); ++i) { ts[i].in = pieces[i].in; ts[i].out = pieces[i].out; ts[i].dims = {pieces[i].count}; }
+      ReduceParams rp;
+      rp.dtype = r.dtype; rp.op = r.reduce_op; rp.prescale = r.prescale; rp.postscale = r.postscale;
+      AllreducePolicy pol;
+      pol.variant = env_.variant;
+      pol.oneshot_max_bytes = env_.params->oneshot_max_bytes;
+      pol.multicast = team->has_multicast();
+      pol.nvls_min_bytes = env_.params->nvls_min_bytes;
+      pol.large_msg_ctas = env_.large_msg_ctas;
+      Plan plan;
+      st = PlanAllreduce(n, ts, rp, wire, pol, lat_lane ? lat_area : (int64_t)team->buffer_bytes(), env_.params->comm_ctas, &plan);
+      if (st.ok()) st = LaunchPlan(*team, device, s, plan, "allreduce", &es, lat_lane);
       if (!st.ok()) return st;
     }
   }
@@ -764,12 +672,7 @@ Status GpuOps::NcclAllreduce(ProcessSet& ps, Entries& es, const Response& r, int
   }
   // fused: scaled pack -> ncclAllReduce in place on the fusion buffer -> scaled unpack
   std::vector<kern::TensorDesc> descs;
-  int64_t total = 0;
-  for (auto& p : pieces) {
-    kern::TensorDesc d; d.in = p.in; d.out = p.out; d.offset = total; d.count = p.count;
-    descs.push_back(d);
-    total += Align128(p.count * (int64_t)esz);
-  }
+  const int64_t total = PackDescs(pieces, (int64_t)esz, &descs);
   char* fusion = (char*)ctx.TempAlloc(device, (size_t)total, false, s);
   if (!fusion) return Status::UnknownError("out of device memory for the NCCL fusion buffer");
   const auto* dtab = (const kern::TensorDesc*)ctx.Stage(device, descs.data(), descs.size() * sizeof(kern::TensorDesc), s);
@@ -864,13 +767,12 @@ Status GpuOps::Reducescatter(ProcessSet& ps, Entries& es, const Response& r, int
   }
   ReduceParams rp;
   rp.dtype = r.dtype; rp.op = r.reduce_op; rp.prescale = r.prescale; rp.postscale = r.postscale;
-  const bool sum_like = r.reduce_op == ReduceOp::SUM || r.reduce_op == ReduceOp::AVERAGE;
-  const bool float_wire = r.dtype == DataType::FLOAT32 || r.dtype == DataType::FLOAT16 || r.dtype == DataType::BFLOAT16;
-  rp.nvls = team->has_multicast() && sum_like && float_wire && n >= 4 && env_.variant != "oneshot" && env_.variant != "twoshot";
+  rp.nvls = team->has_multicast() && MultimemReduces(r.dtype, r.reduce_op) && n >= 4 && env_.variant != "oneshot" &&
+            env_.variant != "twoshot";
   rp.nvls_min_bytes = env_.params->nvls_min_bytes;
   Plan plan;
   Status st = PlanReducescatter(me, n, ts, rp, (int64_t)team->buffer_bytes(), (int)env_.params->comm_ctas, &plan);
-  if (st.ok()) st = LaunchPlan(*team, ctx, device, s, plan, "reducescatter");
+  if (st.ok()) st = LaunchPlan(*team, device, s, plan, "reducescatter");
   if (!st.ok()) return st;
   ctx.TempFreeAll(device, s);
   return FinishEvent(device, s, es.size(), done);
@@ -897,32 +799,37 @@ Status StageAndLaunchExchange(SymmTeam& team, GpuContext& ctx, int device, cudaS
   return Status::OK();
 }
 
-// `grid_bytes` sizes the grid and MUST be the same number on every rank (CTA b rendezvouses with CTA b of its peers).
-Status RunExchange(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, std::vector<kern::CopyDesc>& sends,
-                   std::vector<kern::CopyDesc>& recvs, int max_ctas, int64_t grid_bytes) {
-  return StageAndLaunchExchange(team, ctx, device, s, sends, recvs,
-                                (int)std::max<int64_t>(1, std::min<int64_t>(max_ctas, (grid_bytes + 32767) / 32768)));
-}
+}  // namespace
 
-// Stages and launches every entry of a plan (collective_plan.h) in order, each on the team's next buffer slot.
-Status LaunchPlan(SymmTeam& team, GpuContext& ctx, int device, cudaStream_t s, const Plan& plan, const char* what) {
+Status GpuOps::LaunchPlan(SymmTeam& team, int device, cudaStream_t s, const Plan& plan, const char* what, Entries* es,
+                          bool latency_lane) {
+  GpuContext& ctx = GpuContext::Get();
   for (const PlanLaunch& l : plan) {
     if (!l.reduce) {
       Status st = StageAndLaunchExchange(team, ctx, device, s, l.sends, l.recvs, l.ctas);
       if (!st.ok()) return st;
       continue;
     }
-    const auto* dt = (const kern::TensorDesc*)ctx.Stage(device, l.table.data(), l.table.size() * sizeof(kern::TensorDesc), s);
-    if (!dt) return Status::UnknownError("descriptor table too large");
     kern::AllreduceArgs a = l.args;
-    a.descs = dt; a.out_descs = dt + a.ndesc; a.ctas = l.ctas;
-    kern::CommParams cp = team.Params(team.NextSlot());
+    a.ctas = l.ctas;
+    if (InlineDescs(a)) {
+      memcpy(a.inline_descs, l.table.data(), l.table.size() * sizeof(kern::TensorDesc));  // no staging: small responses are latency bound
+    } else {
+      const auto* dt = (const kern::TensorDesc*)ctx.Stage(device, l.table.data(), l.table.size() * sizeof(kern::TensorDesc), s);
+      if (!dt) return Status::UnknownError("descriptor table too large");
+      a.descs = dt;
+      a.out_descs = a.nout ? dt + a.ndesc : nullptr;
+    }
+    kern::CommParams cp = latency_lane ? team.Params(team.NextLatencySlot(), kern::kLatencyChannel, (int64_t)team.buffer_bytes())
+                                       : team.Params(team.NextSlot());
+    if (es && env_.timeline && env_.timeline->Initialized())
+      env_.timeline->ActivityStartAll(*es, a.variant == kern::kOneShot ? HVD_ACT_P2P_ALLREDUCE_ONESHOT
+                                           : a.variant == kern::kNvls ? HVD_ACT_P2P_ALLREDUCE_NVLS : HVD_ACT_P2P_ALLREDUCE_TWOSHOT);
     cudaError_t ce = kern::LaunchAllreduce(cp, a, s);
     if (ce != cudaSuccess) return Status::UnknownError(std::string(what) + " kernel launch failed: " + cudaGetErrorString(ce));
   }
   return Status::OK();
 }
-}  // namespace
 
 // A fused allgather response (several tensors, per-rank first dims in r.tensor_sizes) is ONE exchange launch: every rank
 // packs its blocks of all tensors back to back into its symmetric buffer and pulls every peer's blocks straight into the
@@ -982,7 +889,7 @@ Status GpuOps::Allgather(ProcessSet& ps, Entries& es, const Response& r, int dev
   }
   Plan plan;
   Status st = PlanAllgather(me, n, ts, esz, (int64_t)team->buffer_bytes(), (int)env_.params->comm_ctas, &plan);
-  if (st.ok()) st = LaunchPlan(*team, ctx, device, s, plan, "allgather");
+  if (st.ok()) st = LaunchPlan(*team, device, s, plan, "allgather");
   if (!st.ok()) return st;
   return FinishEvent(device, s, es.size(), done);
 }
@@ -1022,7 +929,7 @@ Status GpuOps::Broadcast(ProcessSet& ps, Entries& es, const Response& r, int dev
   }
   Plan plan;
   Status st = PlanBroadcast(me, n, root, ts, use_mc, (int64_t)team->buffer_bytes(), (int)env_.params->comm_ctas, &plan);
-  if (st.ok()) st = LaunchPlan(*team, ctx, device, s, plan, "broadcast");
+  if (st.ok()) st = LaunchPlan(*team, device, s, plan, "broadcast");
   if (!st.ok()) return st;
   return FinishEvent(device, s, es.size(), done);
 }
@@ -1073,7 +980,7 @@ Status GpuOps::Alltoall(ProcessSet& ps, Entries& es, const Response& r, int devi
     t.in = e->input; t.out = e->output; t.row = row; t.dims = all;
     Plan plan;
     Status st = PlanAlltoall(me, n, {t}, esz, (int64_t)team->buffer_bytes(), (int)env_.params->comm_ctas, &plan);
-    if (st.ok()) st = LaunchPlan(*team, ctx, device, s, plan, "alltoall");
+    if (st.ok()) st = LaunchPlan(*team, device, s, plan, "alltoall");
     if (!st.ok()) return st;
   }
   return FinishEvent(device, s, es.size(), done);

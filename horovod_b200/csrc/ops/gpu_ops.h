@@ -21,6 +21,7 @@
 #include "../common/timeline.h"
 #include "../kernels/p2p_kernels.h"
 #include "../symm/symm_memory.h"
+#include "collective_plan.h"
 
 namespace hvd {
 
@@ -138,7 +139,15 @@ class GpuOps {
   Status AdasumP2P(ProcessSet& ps, SymmTeam& team, Entries& es, const Response& r, const std::vector<int64_t>& counts,
                    int device, cudaStream_t s);
   void Calibrate(ProcessSet& ps, SymmTeam& team, int device);
-  int CtasFor(int variant, int64_t seg_bytes, int n) const;
+  // Stages and launches every entry of a plan (collective_plan.h) in order, each on the team's next buffer slot, or on
+  // its next latency-lane slot.  `es`: the entries of an allreduce, whose timelines record each launch's kernel.
+  Status LaunchPlan(SymmTeam& team, int device, cudaStream_t s, const Plan& plan, const char* what, Entries* es = nullptr,
+                    bool latency_lane = false);
+  // What the captured collectives share: the set's team, the zero-copy arguments of the registered range and the launch
+  // on the caller's stream.  `launch` is kern::LaunchInplaceAllreduce, LaunchInplaceReducescatter or LaunchInplaceAllgather.
+  using InplaceLaunch = cudaError_t (*)(const kern::CommParams&, const kern::InplaceArgs&, cudaStream_t);
+  Status LaunchCaptured(ProcessSet& ps, const char* what, InplaceLaunch launch, void* ptr, int64_t bytes, DataType dtype, ReduceOp op,
+                        double prescale, double postscale, int max_ctas, cudaStream_t stream, int channel);
   GpuOpEnv env_;
   uint64_t team_counter_ = 0;
   std::atomic<uint64_t> ipc_launches_{0};

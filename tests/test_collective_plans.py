@@ -1,5 +1,5 @@
-"""Launch plans of reducescatter, allgather(v), broadcast and alltoall(v) (csrc/ops/collective_plan.{h,cc}) on the host,
-no GPU needed.
+"""Launch plans of allreduce, reducescatter, allgather(v), broadcast and alltoall(v) (csrc/ops/collective_plan.{h,cc}) on
+the host, no GPU needed.
 
 `hvd_plan_collective` plans every rank of a simulated team with fake tensor addresses (never dereferenced), runs the
 cross-rank agreement check (`CheckPlans`: same launches and grids on every rank, buffer bounds and alignment, every
@@ -7,8 +7,13 @@ receive inside a send of its peer, the reducescatter region layout, exact covera
 byte range the plans move.  This file decodes those ranges and compares them with where the bytes must come from,
 computed here independently of the planner: the row split of reducescatter (the first dim0 % n ranks get one extra row),
 allgather displacements, alltoall send / receive displacements, and the broadcast root.
+
+`hvd_plan_allreduce` returns one rank's allreduce plan, which must match tests/golden/allreduce_plans.json field for field:
+the launches the engine made before the plan was a host function.
 """
 import ctypes
+import json
+import os
 
 import numpy as np
 import pytest
@@ -30,6 +35,11 @@ def lib():
                                           ctypes.c_int, u64p, u64p, ctypes.c_int64, ctypes.c_int, ctypes.POINTER(ctypes.c_int),
                                           i64p, ctypes.c_int64, ctypes.c_char_p, ctypes.c_int]
         L.hvd_plan_collective.restype = ctypes.c_int64
+        L.hvd_plan_allreduce.argtypes = [ctypes.c_int, ctypes.c_int, i64p, u64p, u64p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                         ctypes.c_double, ctypes.c_double, ctypes.c_char_p, ctypes.c_int64, ctypes.c_int,
+                                         ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int64, i64p, ctypes.c_int64, i64p,
+                                         ctypes.c_int64, ctypes.c_char_p, ctypes.c_int]
+        L.hvd_plan_allreduce.restype = ctypes.c_int64
         _lib = L
     return _lib
 
@@ -275,3 +285,72 @@ def test_no_plan_for_a_buffer_too_small(kind, n, cap, dims):
 def test_nothing_to_move_is_no_launch():
     for kind, dims in ((RS, [0]), (AG, [[0, 0, 0]]), (BC, [0]), (A2A, [[[0] * 3] * 3])):
         assert verify(Config(kind, 3, dims, [2], 4, 4096, 8, root=0 if kind == BC else -1)) == 0
+
+
+@pytest.mark.parametrize('L', [2, 3, 4, 8])
+def test_hierarchical_windows(L):
+    """The two intra-host halves of the hierarchical allreduce: the reducescatter of the fusion buffer (L blocks of B bytes,
+    B a multiple of 128) into the shard, and the allgather of the shard back into every block, in windows of the buffer."""
+    for esz in (2, 4):
+        for B in (128, 128 * 37, 3 * 4096 + 5 * 128):
+            for cap in (128 * L, 4096, 3 * 4096, 1 << 20):
+                region = cap // L // 128 * 128
+                assert verify(Config(RS, L, [L * B // esz], [1], esz, cap, 128)) == -(-B // region)
+                window = cap // 16 * 16
+                assert verify(Config(AG, L, [[B] * L], [1], 1, cap, 128)) == -(-B // window)
+
+
+# --- allreduce ---------------------------------------------------------------------------------------------------------
+LAUNCH_FIELDS = ('reduce', 'variant', 'ctas', 'total_bytes', 'reduce_lo', 'reduce_hi', 'dtype', 'wire_dtype', 'op', 'prescale',
+                 'postscale', 'inline', 'nout', 'oneshot_nvls', 'ndesc')
+
+
+def plan_allreduce(c, max_launches=1024, max_descs=4096):
+    """One rank's allreduce plan for a golden case's inputs, as one dict per launch with the golden's fields."""
+    T = len(c['counts'])
+    launches = np.zeros((max_launches, len(LAUNCH_FIELDS)), dtype=np.int64)
+    descs = np.zeros((max_descs, 4), dtype=np.int64)
+    err = ctypes.create_string_buffer(512)
+    m = lib().hvd_plan_allreduce(
+        c['n'], T, (ctypes.c_int64 * T)(*c['counts']), (ctypes.c_uint64 * T)(*c['ins']), (ctypes.c_uint64 * T)(*c['outs']),
+        c['dtype'], c['wire'], c['op'], c['prescale'], c['postscale'], c['variant'].encode(), c['oneshot_max_bytes'],
+        c['multicast'], c['nvls_min_bytes'], c['cap'], c['comm_ctas'], c['large_msg_ctas'],
+        launches.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), max_launches,
+        descs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), max_descs, err, 512)
+    assert m >= 0, (m, err.value.decode())
+    out, d = [], 0
+    for row in launches[:m]:
+        f = dict(zip(LAUNCH_FIELDS, (int(v) for v in row)))
+        f['prescale'], f['postscale'] = (float(v) for v in row[9:11].view(np.float64))
+        f['descs'] = descs[d:d + f['ndesc']].tolist()
+        d += f['ndesc']
+        out.append(f)
+    return out
+
+
+def test_allreduce_plans_match_the_golden():
+    """Segments, variant, grid, arguments, inline or staged descriptors and every descriptor of each launch, over n = 2 / 4 / 8,
+    fp32 / bf16 / fp16 / int32 and an fp32 -> bf16 wire, SUM / AVERAGE / MIN, every HVD_ALLREDUCE_VARIANT, with and without
+    multicast, both sides of both crossovers, the four CtasFor bands, buffers that split pieces, zero-count pieces and more
+    pieces than kInlineDescs."""
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'allreduce_plans.json')) as f:
+        golden = json.load(f)
+    assert len(golden['cases']) > 100
+    for case in golden['cases']:
+        c = dict(zip(golden['inputs'], case))
+        launches = [dict(zip(golden['launch'], l)) for l in case[len(golden['inputs'])]]
+        got = plan_allreduce(c)
+        what = {k: v for k, v in c.items() if k not in ('ins', 'outs')}
+        assert len(got) == len(launches), (what, len(got), len(launches))
+        for k, (g, want) in enumerate(zip(got, launches)):
+            assert g['reduce'] == 1 and g['ndesc'] == len(want['descs']), (what, k, g)
+            for field, v in want.items():
+                assert g[field] == v, (what, k, field, g[field], v)
+
+
+def test_allreduce_needs_128_bytes_of_buffer():
+    c = dict(n=2, counts=[64], ins=[1 << 32], outs=[1 << 33], dtype=7, wire=7, op=SUM, prescale=1.0, postscale=1.0, variant='auto',
+             oneshot_max_bytes=0, multicast=0, nvls_min_bytes=0, cap=127, comm_ctas=8, large_msg_ctas=8)
+    with pytest.raises(AssertionError, match='-5.*bytes'):
+        plan_allreduce(c)
+    assert len(plan_allreduce(dict(c, cap=128))) == 2
