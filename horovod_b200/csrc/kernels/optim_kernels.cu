@@ -7,6 +7,8 @@
 // update instead of a separate elementwise pass.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <algorithm>
+#include <cstring>
 #include <type_traits>
 #include "p2p_kernels.h"
 
@@ -430,6 +432,240 @@ fused_lars_apply_kernel(const OptTensor* __restrict__ table, float lr, float mom
   }
 }
 
+// Adafactor (Shazeer & Stern 2018) as torch.optim.Adafactor computes it, for g the scaled gradient at step t:
+//   beta_w = t^beta2_decay, rho = min(lr, 1 / sqrt(t)), alpha = max(eps2, ||w|| / sqrt(n)) * rho (w before decay)
+//   factored [.., R, C]: row_var = lerp(row_var, mean_c g^2, beta_w), col_var = lerp(col_var, mean_r g^2, beta_w),
+//                        v = row_var * col_var / max(mean_r row_var, eps1)
+//   dim <= 1:            variance = lerp(variance, g^2, beta_w), v = variance
+//   u = g * rsqrt(max(v, eps1^2)), denom = max(1, ||u|| / (sqrt(n) * d)), w = w * (1 - lr * wd) - (alpha / denom) * u
+// Five launches and no state between them: adafactor_stats_kernel (z = 0: one warp per row sums g^2 over the row and
+// lerps row_var; z = 1: one thread per (column, chunk of kAfRowChunk rows) writes a column partial),
+// adafactor_factors_kernel (z = 0: one thread per column adds its partials in fp64 in chunk order and lerps col_var;
+// z = 1: one CTA per matrix of the batch takes the mean of row_var in fp64), adafactor_norms_kernel (per-CTA
+// (sum w^2, sum u^2) partials in LAMB's layout; lerps and stores the variance of dim <= 1 entries), lamb_finalize_kernel,
+// and adafactor_apply_kernel, which recomputes u with the same code.  Every sum has a fixed order: deterministic.
+constexpr int kAfRowChunk = 64;
+
+__device__ __forceinline__ float af_lerp(float a, float b, float w) {  // at::native::lerp's two-sided formula
+  return fabsf(w) < 0.5f ? a + w * (b - a) : b - (b - a) * (1.f - w);
+}
+
+__device__ __forceinline__ unsigned af_batch(const AdafactorGeom& gm) { return (unsigned)gm.size[0] * gm.size[1] * gm.size[2]; }
+
+// storage offset of matrix b of the batch (row-major over the leading dims)
+__device__ __forceinline__ unsigned af_batch_offset(const AdafactorGeom& gm, unsigned b) {
+  unsigned off = 0;
+#pragma unroll
+  for (int d = 2; d >= 0; --d) {
+    off += (b % (unsigned)gm.size[d]) * (unsigned)gm.stride[d];
+    b /= (unsigned)gm.size[d];
+  }
+  return off;
+}
+
+// v of the factored element at storage offset o: a dense layout's strides are a mixed radix, so coordinate
+// d = (o / stride[d]) % size[d]
+__device__ __forceinline__ float af_vhat(const AdafactorGeom& gm, const float* __restrict__ rmean, unsigned o, float eps1) {
+  const unsigned c = (o / (unsigned)gm.stride[4]) % (unsigned)gm.size[4], r = (o / (unsigned)gm.stride[3]) % (unsigned)gm.size[3];
+  unsigned b = 0;
+#pragma unroll
+  for (int d = 0; d < 3; ++d) b = b * (unsigned)gm.size[d] + (o / (unsigned)gm.stride[d]) % (unsigned)gm.size[d];
+  const float rv = gm.row_var[(size_t)b * gm.size[3] + r], cv = gm.col_var[(size_t)b * gm.size[4] + c];
+  return rv * cv / fmaxf(rmean[gm.batch_off + b], eps1);
+}
+
+// u for 4 elements from the scaled gradient dv and, for dim <= 1 entries, the (lerped) variance vv; 0 past the end
+__device__ __forceinline__ void af_u4(const AdafactorGeom& gm, const float* __restrict__ rmean, int64_t i, int64_t n,
+                                      const float* dv, const float* vv, float eps1, float eps1_sq, float* uv) {
+#pragma unroll
+  for (int k = 0; k < kOptVec; ++k) {
+    uv[k] = 0.f;
+    if (i + k < n) {
+      const float v = gm.row_var ? af_vhat(gm, rmean, (unsigned)(i + k), eps1) : vv[k];
+      uv[k] = dv[k] * rsqrtf(fmaxf(v, eps1_sq));
+    }
+  }
+}
+
+template <typename G>
+__global__ void __launch_bounds__(kOptThreads)
+adafactor_stats_kernel(const OptTensor* __restrict__ table, const AdafactorGeom* __restrict__ geom, float beta_w,
+                       float grad_scale, const float* __restrict__ grad_scale_dev, float* __restrict__ colpart) {
+  const AdafactorGeom& gm = geom[blockIdx.y];
+  if (gm.row_var == nullptr) return;
+  const G* g = reinterpret_cast<const G*>(table[blockIdx.y].grad);
+  const unsigned R = gm.size[3], C = gm.size[4], B = af_batch(gm);
+  if (blockIdx.z == 0) {
+    const unsigned row = blockIdx.x * (kOptThreads / 32) + threadIdx.x / 32, lane = threadIdx.x % 32;
+    if (row >= B * R) return;  // uniform per warp
+    grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
+    const G* gr = g + af_batch_offset(gm, row / R) + (size_t)(row % R) * gm.stride[3];
+    float s = 0.f;
+    for (unsigned c = lane; c < C; c += 32) {
+      const float x = to_f<G>(gr[(size_t)c * gm.stride[4]]) * grad_scale;
+      s = fmaf(x, x, s);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) gm.row_var[row] = af_lerp(gm.row_var[row], s / (float)C, beta_w);
+  } else {
+    const unsigned chunks = (R + kAfRowChunk - 1) / kAfRowChunk, j = blockIdx.x * kOptThreads + threadIdx.x;
+    if (j >= B * C * chunks) return;
+    grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
+    const unsigned c = j % C, bk = j / C, b = bk % B, k = bk / B, r1 = min(R, (k + 1) * kAfRowChunk);
+    const G* gc = g + af_batch_offset(gm, b) + (size_t)c * gm.stride[4];
+    float s = 0.f;
+    for (unsigned r = k * kAfRowChunk; r < r1; ++r) {
+      const float x = to_f<G>(gc[(size_t)r * gm.stride[3]]) * grad_scale;
+      s = fmaf(x, x, s);
+    }
+    colpart[gm.col_off + j] = s;  // [chunk][b][c]: adjacent threads, adjacent columns
+  }
+}
+
+__global__ void __launch_bounds__(kOptThreads)
+adafactor_factors_kernel(const AdafactorGeom* __restrict__ geom, float beta_w, const float* __restrict__ colpart,
+                         float* __restrict__ rmean) {
+  __shared__ double red[kOptThreads];
+  const AdafactorGeom& gm = geom[blockIdx.y];
+  if (gm.row_var == nullptr) return;
+  const unsigned R = gm.size[3], C = gm.size[4], B = af_batch(gm);
+  if (blockIdx.z == 0) {
+    const unsigned j = blockIdx.x * kOptThreads + threadIdx.x;  // b * C + c
+    if (j >= B * C) return;
+    const unsigned chunks = (R + kAfRowChunk - 1) / kAfRowChunk;
+    double s = 0.0;
+    for (unsigned k = 0; k < chunks; ++k) s += (double)colpart[gm.col_off + (size_t)k * B * C + j];
+    gm.col_var[j] = af_lerp(gm.col_var[j], (float)(s / R), beta_w);
+  } else {
+    const unsigned b = blockIdx.x;
+    if (b >= B) return;  // uniform per CTA
+    double s = 0.0;
+    for (unsigned r = threadIdx.x; r < R; r += kOptThreads) s += (double)gm.row_var[(size_t)b * R + r];
+    red[threadIdx.x] = s;
+    __syncthreads();
+#pragma unroll
+    for (int h = kOptThreads / 2; h > 0; h >>= 1) {
+      if (threadIdx.x < h) red[threadIdx.x] += red[threadIdx.x + h];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) rmean[gm.batch_off + b] = (float)(red[0] / R);
+  }
+}
+
+template <typename P, typename G, bool kMaster>
+__global__ void __launch_bounds__(kOptThreads)
+adafactor_norms_kernel(const OptTensor* __restrict__ table, const AdafactorGeom* __restrict__ geom, float beta_w,
+                       float eps1, float eps1_sq, float grad_scale, const float* __restrict__ grad_scale_dev,
+                       const float* __restrict__ rmean, float2* __restrict__ partial) {
+  __shared__ float2 red[kOptThreads / 32];
+  const OptTensor t = table[blockIdx.y];
+  const AdafactorGeom& gm = geom[blockIdx.y];
+  const int64_t n = t.count;
+  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  if (base >= n) return;
+  grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
+  const P* p = reinterpret_cast<const P*>(t.param);
+  const G* g = reinterpret_cast<const G*>(t.grad);
+  float* var = reinterpret_cast<float*>(t.state0);
+  const float* w = kMaster ? reinterpret_cast<const float*>(t.master) : nullptr;
+  const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g), va = is_aligned<float>(var), wa = kMaster && is_aligned<float>(w);
+  float sw = 0.f, su = 0.f;
+#pragma unroll
+  for (int it = 0; it < kOptIters; ++it) {
+    const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
+    if (i >= n) break;
+    float pv[kOptVec], dv[kOptVec], vv[kOptVec] = {0.f, 0.f, 0.f, 0.f}, uv[kOptVec];
+    load4<P>(p, i, n, pa, pv);
+    load4<G>(g, i, n, ga, dv);
+    if constexpr (kMaster) {
+      float wv[kOptVec];
+      load4<float>(w, i, n, wa, wv);
+      reconcile4<P>(pv, wv);
+    }
+#pragma unroll
+    for (int k = 0; k < kOptVec; ++k) dv[k] *= grad_scale;
+    if (!gm.row_var) {
+      load4<float>(var, i, n, va, vv);
+#pragma unroll
+      for (int k = 0; k < kOptVec; ++k) vv[k] = af_lerp(vv[k], dv[k] * dv[k], beta_w);
+      store4<float>(var, i, n, va, vv);
+    }
+    af_u4(gm, rmean, i, n, dv, vv, eps1, eps1_sq, uv);
+#pragma unroll
+    for (int k = 0; k < kOptVec; ++k) {  // past the end w reads as 0 and u is 0
+      sw = fmaf(pv[k], pv[k], sw);
+      su = fmaf(uv[k], uv[k], su);
+    }
+  }
+  // CTA partial: the tree of fused_lamb_norms_kernel
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    sw += __shfl_xor_sync(0xffffffffu, sw, o);
+    su += __shfl_xor_sync(0xffffffffu, su, o);
+  }
+  if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = make_float2(sw, su);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float2 a = red[0];
+    for (int k = 1; k < kOptThreads / 32; ++k) { a.x += red[k].x; a.y += red[k].y; }
+    partial[t.partial + blockIdx.x] = a;
+  }
+}
+
+template <typename P, typename G, bool kMaster, bool kEma>
+__global__ void __launch_bounds__(kOptThreads)
+adafactor_apply_kernel(const OptTensor* __restrict__ table, const AdafactorGeom* __restrict__ geom, AdafactorHyper h,
+                       float grad_scale, const float* __restrict__ grad_scale_dev, const float* __restrict__ rmean,
+                       const float* __restrict__ norms, float ema_w, int ema_start) {
+  const OptTensor t = table[blockIdx.y];
+  const AdafactorGeom& gm = geom[blockIdx.y];
+  const int64_t n = t.count;
+  const int64_t base = (int64_t)blockIdx.x * kOptPerBlock;
+  if (base >= n) return;
+  grad_scale *= grad_scale_dev ? *grad_scale_dev : 1.f;
+  const float rn = sqrtf((float)n);
+  const float alpha = fmaxf(h.eps2, sqrtf(norms[2 * t.slot]) / rn) * h.rho;
+  const float step = alpha / fmaxf(1.f, sqrtf(norms[2 * t.slot + 1]) / (rn * h.d));
+  P* p = reinterpret_cast<P*>(t.param);
+  const G* g = reinterpret_cast<const G*>(t.grad);
+  const float* var = reinterpret_cast<const float*>(t.state0);
+  float* w = kMaster ? reinterpret_cast<float*>(t.master) : nullptr;
+  const bool pa = is_aligned<P>(p), ga = is_aligned<G>(g), va = is_aligned<float>(var), wa = kMaster && is_aligned<float>(w);
+  float* e = kEma ? reinterpret_cast<float*>(t.ema) : nullptr;
+  const bool ea = kEma && is_aligned<float>(e);
+#pragma unroll
+  for (int it = 0; it < kOptIters; ++it) {
+    const int64_t i = base + ((int64_t)it * kOptThreads + threadIdx.x) * kOptVec;
+    if (i >= n) break;
+    float pv[kOptVec], dv[kOptVec], vv[kOptVec] = {0.f, 0.f, 0.f, 0.f}, uv[kOptVec];
+    load4<P>(p, i, n, pa, pv);
+    load4<G>(g, i, n, ga, dv);
+    if constexpr (kMaster) {
+      float wv[kOptVec];
+      load4<float>(w, i, n, wa, wv);
+      reconcile4<P>(pv, wv);  // the same value the norms launch started from: nothing wrote p or the master in between
+    }
+#pragma unroll
+    for (int k = 0; k < kOptVec; ++k) dv[k] *= grad_scale;
+    if (!gm.row_var) load4<float>(var, i, n, va, vv);  // lerped by the norms launch
+    af_u4(gm, rmean, i, n, dv, vv, h.eps1, h.eps1_sq, uv);
+#pragma unroll
+    for (int k = 0; k < kOptVec; ++k) pv[k] = fmaf(-step, uv[k], pv[k] * h.decay);
+    if constexpr (kMaster) store4<float>(w, i, n, wa, pv);
+    store4<P>(p, i, n, pa, pv);
+    if constexpr (kEma) ema4<P, kMaster>(e, i, n, ea, pv, ema_w, ema_start);
+  }
+}
+
+// Host bytes as kernel parameters: a launch captured into a CUDA graph keeps its own copy of them.
+constexpr int kUploadChunk = 4000;
+struct UploadChunk { unsigned char b[kUploadChunk]; };
+
+__global__ void __launch_bounds__(kOptThreads) upload_bytes_kernel(unsigned char* __restrict__ dst, const UploadChunk c, int bytes) {
+  for (int i = threadIdx.x; i < bytes; i += kOptThreads) dst[i] = c.b[i];
+}
+
 // max that keeps a NaN once it has seen one (fmaxf drops it), so an inf-norm of NaN gradients is NaN as in torch
 __device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
 __device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
@@ -701,6 +937,64 @@ cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, fl
       fused_lars_apply_kernel<typename T::P, typename T::G, T::kMaster, false><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
           table, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, grad_scale_dev, norms, 0.f, 0);
   });
+}
+
+int64_t AdafactorRowChunks(int64_t rows) { return (rows + kAfRowChunk - 1) / kAfRowChunk; }
+
+int64_t AdafactorStatsCtas(int64_t batch, int64_t rows, int64_t cols) {
+  const int64_t row_ctas = (batch * rows + kOptThreads / 32 - 1) / (kOptThreads / 32);
+  const int64_t col_ctas = (batch * cols * AdafactorRowChunks(rows) + kOptThreads - 1) / kOptThreads;
+  return std::max(row_ctas, col_ctas);
+}
+
+int64_t AdafactorFactorCtas(int64_t batch, int64_t cols) {
+  return std::max(batch, (batch * cols + kOptThreads - 1) / kOptThreads);
+}
+
+cudaError_t LaunchAdafactor(const OptTensor* table, const AdafactorGeom* geom, int n, int64_t max_count, int64_t stats_ctas,
+                            int64_t factor_ctas, const AdafactorHyper& h, float grad_scale, const float* grad_scale_dev,
+                            float* colpart, float* rmean, float* partial, float* norms, int param_dtype, int grad_dtype,
+                            bool master, cudaStream_t stream, const OptEma& ema) {
+  if (n <= 0 || max_count <= 0) return cudaSuccess;
+  if (stats_ctas < 1 || factor_ctas < 1 || stats_ctas > 0x7fffffff || factor_ctas > 0x7fffffff) return cudaErrorInvalidValue;
+  cudaError_t e = DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    adafactor_stats_kernel<typename T::G><<<dim3((unsigned)stats_ctas, (unsigned)n, 2), kOptThreads, 0, stream>>>(
+        table, geom, h.beta_w, grad_scale, grad_scale_dev, colpart);
+  });
+  if (e != cudaSuccess) return e;
+  adafactor_factors_kernel<<<dim3((unsigned)factor_ctas, (unsigned)n, 2), kOptThreads, 0, stream>>>(geom, h.beta_w, colpart, rmean);
+  CountKernelLaunch();
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  float2* part = reinterpret_cast<float2*>(partial);
+  e = FinalizeNorms(DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    adafactor_norms_kernel<typename T::P, typename T::G, T::kMaster><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+        table, geom, h.beta_w, h.eps1, h.eps1_sq, grad_scale, grad_scale_dev, rmean, part);
+  }), table, n, part, norms, stream);
+  if (e != cudaSuccess) return e;
+  return DispatchOpt(param_dtype, grad_dtype, master, [&](auto t) {
+    using T = decltype(t);
+    if (ema.on)
+      adafactor_apply_kernel<typename T::P, typename T::G, T::kMaster, true><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, geom, h, grad_scale, grad_scale_dev, rmean, norms, ema.weight, ema.start);
+    else
+      adafactor_apply_kernel<typename T::P, typename T::G, T::kMaster, false><<<OptGrid(n, max_count), kOptThreads, 0, stream>>>(
+          table, geom, h, grad_scale, grad_scale_dev, rmean, norms, 0.f, 0);
+  });
+}
+
+cudaError_t LaunchUploadBytes(void* dst, const void* host, size_t bytes, cudaStream_t stream) {
+  for (size_t off = 0; off < bytes; off += kUploadChunk) {
+    UploadChunk c;
+    const int len = (int)std::min<size_t>(kUploadChunk, bytes - off);
+    memcpy(c.b, static_cast<const unsigned char*>(host) + off, (size_t)len);
+    upload_bytes_kernel<<<1, kOptThreads, 0, stream>>>(static_cast<unsigned char*>(dst) + off, c, len);
+    CountKernelLaunch();
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 int64_t GradShardStatsTiles(int64_t count) { return (count + kOptPerBlock - 1) / kOptPerBlock; }

@@ -207,6 +207,37 @@ cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, fl
                             float trust_coefficient, float eps, int adapt, float grad_scale, const float* grad_scale_dev,
                             const float* norms, int param_dtype, int grad_dtype, bool master, cudaStream_t stream,
                             const OptEma& ema = OptEma());
+// Fused Adafactor (torch.optim.Adafactor's update, see optim_kernels.cu) on the OptTensor table plus a parallel geometry
+// table: entry i of both describes one whole parameter.  A parameter of dim <= 1 keeps its fp32 `variance` (its sizes and
+// strides) in OptTensor::state0 and has row_var == nullptr here.  A parameter of dim 2..kAdafactorMaxDims is factored over
+// its last two dims [R, C], the leading dims (up to three, padded with 1 in front) forming a batch of B matrices:
+//   size, stride   the logical sizes [b0, b1, b2, R, C] and the parameter's element strides for them (any dense layout;
+//                  a dim of size 1 carries stride 1).  The parameter has fewer than 2^31 elements.
+//   row_var        fp32 [B, R], col_var fp32 [B, C], both contiguous (torch's [..., R, 1] and [..., 1, C])
+//   col_off        the entry's first column partial (B * C * AdafactorRowChunks(R) of them)
+//   batch_off      the entry's first per-batch mean of row_var (B of them)
+constexpr int kAdafactorMaxDims = 5;
+struct AdafactorGeom { int32_t size[kAdafactorMaxDims]; int32_t stride[kAdafactorMaxDims]; float* row_var; float* col_var;
+                       int64_t col_off; int64_t batch_off; };
+// Per-launch hyper-parameters as the kernels use them: beta_w = 1 - beta2_t = step^beta2_decay, rho = min(lr, step^-0.5),
+// eps1_sq = eps1 * eps1 and decay = 1 - lr * weight_decay, each rounded from double once.
+struct AdafactorHyper { float beta_w, rho, eps1, eps1_sq, eps2, d, decay; };
+int64_t AdafactorRowChunks(int64_t rows);
+// CTAs along x that the stats and factor launches need for a factored entry of B matrices [R, C].
+int64_t AdafactorStatsCtas(int64_t batch, int64_t rows, int64_t cols);
+int64_t AdafactorFactorCtas(int64_t batch, int64_t cols);
+// The whole step in five launches: row sums (row_var lerped) and column partials of g^2; column sums (col_var lerped) and
+// the per-batch means of row_var; per-CTA (sum w^2, sum u^2) partials, which also lerp the variance of dim <= 1 entries;
+// the finalize of those into `norms` (2 floats per entry, zeroed by the caller); the update.  colpart / rmean / partial
+// are scratch of sum B * C * AdafactorRowChunks(R), sum B and 2 * sum NormPartials(count) floats.  `stats_ctas` /
+// `factor_ctas`: the largest AdafactorStatsCtas / AdafactorFactorCtas over the entries (at least 1).
+cudaError_t LaunchAdafactor(const OptTensor* table, const AdafactorGeom* geom, int n, int64_t max_count, int64_t stats_ctas,
+                            int64_t factor_ctas, const AdafactorHyper& h, float grad_scale, const float* grad_scale_dev,
+                            float* colpart, float* rmean, float* partial, float* norms, int param_dtype, int grad_dtype,
+                            bool master, cudaStream_t stream, const OptEma& ema);
+// Copies `bytes` of host memory to device memory `dst` on `stream` through kernel parameters, so that the copy of a
+// launch captured into a CUDA graph is part of the graph (one launch per 4000 bytes).
+cudaError_t LaunchUploadBytes(void* dst, const void* host, size_t bytes, cudaStream_t stream);
 // Gradient statistics of flat gradient shards in one pass (see optim_kernels.cu): optional in-place scaling by
 // *inv_scale, then out[0] += sum of squares (norm_inf: out[0] = max(out[0], max |g|)) and out[1] = max(out[1], non-finite).
 // Entries are non-empty and in order; tile_begin is the sum of GradShardStatsTiles(count) of the entries before, `tiles`

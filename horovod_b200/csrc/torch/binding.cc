@@ -823,6 +823,126 @@ void FusedLarsStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   });
 }
 
+// ---- fused Adafactor: the OptTensor table of PlanOpt (variance of dim <= 1 params in state0, one norm slot per param)
+// plus a geometry table parallel to it for the factored params.  Both tables and all scratch live in tensors of torch's
+// caching allocator on the current stream, and the tables reach the device through kernel parameters, so the call can
+// be captured into a CUDA graph.
+
+// Checks that `f` is params[i]'s row (`dim` = -1) or column (`dim` = -2) factor: fp32, contiguous, on its device, with
+// its sizes except 1 at `dim`.
+void CheckAdafactorFactor(const char* op, const char* what, size_t i, const at::Tensor& param,
+                          const c10::optional<at::Tensor>& f, int64_t dim) {
+  TORCH_CHECK(f.has_value() && f->defined(), op, ": ", what, "[", i, "] is missing for params[", i, "] of dim ", param.dim());
+  TORCH_CHECK(f->device() == param.device(), op, ": ", what, "[", i, "] is on ", f->device(), ", params[", i, "] on ",
+              param.device());
+  TORCH_CHECK(f->scalar_type() == at::kFloat, op, ": ", what, "[", i, "] is ", f->scalar_type(), ", expected Float");
+  std::vector<int64_t> want = param.sizes().vec();
+  want[want.size() + dim] = 1;
+  TORCH_CHECK(f->sizes() == at::IntArrayRef(want), op, ": ", what, "[", i, "] has size ", f->sizes(), ", expected ",
+              at::IntArrayRef(want));
+  TORCH_CHECK(f->is_contiguous(), op, ": ", what, "[", i, "] must be contiguous");
+}
+
+void FusedAdafactorStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads,
+                        std::vector<c10::optional<at::Tensor>> row_vars, std::vector<c10::optional<at::Tensor>> col_vars,
+                        std::vector<c10::optional<at::Tensor>> variances, double lr, double beta2_decay, double eps1,
+                        double eps2, double d, double weight_decay, int64_t step, double grad_scale,
+                        c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters,
+                        std::vector<at::Tensor> emas, double ema_weight, bool ema_start) {
+  const char* op = "fused_adafactor";
+  TORCH_CHECK(row_vars.size() == params.size() && col_vars.size() == params.size() && variances.size() == params.size(),
+              op, ": list sizes differ");
+  TORCH_CHECK(step >= 1, op, ": step must be >= 1, got ", step);
+  TORCH_CHECK(eps1 >= 0.0 && d > 0.0, op, ": eps1 must be >= 0 and d > 0, got eps1 = ", eps1, ", d = ", d);
+  if (params.empty()) return;
+  // not zeroed yet: nothing is launched before every argument is checked
+  at::Tensor norms = at::empty({2 * (int64_t)params.size()}, params[0].options().dtype(at::kFloat));
+  OptPlan plan = PlanOpt(op, params, grads, {}, masters, grad_scale_dev, &norms, {}, EmaArgs{emas, ema_weight, ema_start});
+  for (size_t i = 0; i < params.size(); ++i) {
+    const at::Tensor& p = params[i];
+    TORCH_CHECK(p.dim() <= kern::kAdafactorMaxDims, op, ": params[", i, "] has ", p.dim(), " dims, at most ",
+                kern::kAdafactorMaxDims, " are supported");
+    if (p.dim() >= 2) {
+      CheckAdafactorFactor(op, "row_vars", i, p, row_vars[i], -1);
+      CheckAdafactorFactor(op, "col_vars", i, p, col_vars[i], -2);
+      TORCH_CHECK(!(variances[i].has_value() && variances[i]->defined()), op, ": variances[", i,
+                  "] is given for params[", i, "] of dim ", p.dim(), ", which keeps row / column factors");
+      TORCH_CHECK(p.numel() < ((int64_t)1 << 31), op, ": params[", i, "] has ", p.numel(), " elements, at most 2^31 - 1 ",
+                  "are supported for a factored parameter");
+    } else {
+      TORCH_CHECK(!(row_vars[i].has_value() && row_vars[i]->defined()) && !(col_vars[i].has_value() && col_vars[i]->defined()),
+                  op, ": row_vars[", i, "] / col_vars[", i, "] are given for params[", i, "] of dim ", p.dim(),
+                  ", which keeps a variance");
+      TORCH_CHECK(variances[i].has_value() && variances[i]->defined(), op, ": variances[", i, "] is missing for params[",
+                  i, "] of dim ", p.dim());
+      CheckOptimizerPeer(op, "variances", i, p, *variances[i], at::kFloat);
+    }
+  }
+  // the geometry of every table entry (PlanOpt gives zero-size params no entry) and the scratch offsets
+  std::vector<kern::AdafactorGeom> geom;
+  int64_t colparts = 0, batches = 0, stats_ctas = 1, factor_ctas = 1;
+  for (size_t i = 0, e = 0; i < params.size(); ++i) {
+    const at::Tensor& p = params[i];
+    if (p.numel() == 0) continue;
+    kern::AdafactorGeom g{};
+    for (int k = 0; k < kern::kAdafactorMaxDims; ++k) { g.size[k] = 1; g.stride[k] = 1; }
+    if (p.dim() >= 2) {
+      for (int64_t k = 0; k < p.dim(); ++k) {
+        const int slot = kern::kAdafactorMaxDims - (int)p.dim() + (int)k;
+        g.size[slot] = (int32_t)p.size(k);
+        g.stride[slot] = p.size(k) == 1 ? 1 : (int32_t)p.stride(k);
+      }
+      g.row_var = row_vars[i]->data_ptr<float>();
+      g.col_var = col_vars[i]->data_ptr<float>();
+      const int64_t B = (int64_t)g.size[0] * g.size[1] * g.size[2], R = g.size[3], C = g.size[4];
+      g.col_off = colparts;
+      g.batch_off = batches;
+      colparts += B * C * kern::AdafactorRowChunks(R);
+      batches += B;
+      stats_ctas = std::max(stats_ctas, kern::AdafactorStatsCtas(B, R, C));
+      factor_ctas = std::max(factor_ctas, kern::AdafactorFactorCtas(B, C));
+    } else {
+      plan.table[e].state0 = variances[i]->data_ptr();
+    }
+    geom.push_back(g);
+    ++e;
+  }
+  if (plan.table.empty()) return;
+  TORCH_CHECK(plan.table.size() <= 65535, op, ": at most 65535 non-empty params per call, got ", plan.table.size());
+  kern::AdafactorHyper h;
+  const double t = (double)step;
+  h.beta_w = (float)std::pow(t, beta2_decay);
+  h.rho = (float)std::min(lr, 1.0 / std::sqrt(t));
+  h.eps1 = (float)eps1;
+  h.eps1_sq = (float)(eps1 * eps1);
+  h.eps2 = (float)eps2;
+  h.d = (float)d;
+  h.decay = (float)(1.0 - lr * weight_decay);
+  const size_t tab_bytes = plan.table.size() * sizeof(kern::OptTensor);
+  const size_t geom_at = (tab_bytes + 255) / 256 * 256, bytes = geom_at + geom.size() * sizeof(kern::AdafactorGeom);
+  std::vector<unsigned char> host(bytes);
+  memcpy(host.data(), plan.table.data(), tab_bytes);
+  memcpy(host.data() + geom_at, geom.data(), geom.size() * sizeof(kern::AdafactorGeom));
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t s = c10::cuda::getCurrentCUDAStream(params[0].get_device());
+  at::Tensor tables = at::empty({(int64_t)bytes}, params[0].options().dtype(at::kByte));
+  at::Tensor work = at::empty({colparts + batches + 2 * plan.partials}, norms.options());
+  norms.zero_();
+  float* w = work.data_ptr<float>();
+  cudaError_t e = kern::LaunchUploadBytes(tables.data_ptr(), host.data(), bytes, s);
+  if (e == cudaSuccess) {
+    const auto* dt = reinterpret_cast<const kern::OptTensor*>(tables.data_ptr<uint8_t>());
+    const auto* dg = reinterpret_cast<const kern::AdafactorGeom*>(tables.data_ptr<uint8_t>() + geom_at);
+    // the float2 CTA partials first, where the allocator's alignment holds; then the column partials and batch means
+    float* part = w;
+    float* cols = part + 2 * plan.partials;
+    e = kern::LaunchAdafactor(dt, dg, (int)plan.table.size(), plan.max_count, stats_ctas, factor_ctas, h,
+                              (float)grad_scale, plan.grad_scale_dev, cols, cols + colparts, part,
+                              norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype, plan.master, s, plan.ema);
+  }
+  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+}
+
 // The stats kernel's last-CTA ticket: one zeroed counter per (device, stream), which every launch leaves zeroed again.
 // Launches on one stream run one after the other, so they can share it; launches on different streams may overlap and
 // must not.  Kept for the life of the process (4 bytes per stream that ever ran the kernel).
@@ -1179,6 +1299,10 @@ PYBIND11_MODULE(_hvd_torch, m) {
         py::arg("momentum"), py::arg("weight_decay"), py::arg("trust_coefficient"), py::arg("eps"), py::arg("adapt"),
         py::arg("grad_scale"), py::arg("grad_scale_dev"), py::arg("master_params"), py::arg("norms"), py::arg("slots"),
         py::arg("ema_params") = std::vector<at::Tensor>(), py::arg("ema_weight") = 0.0, py::arg("ema_start") = false);
+  m.def("fused_adafactor_step", &FusedAdafactorStep, py::arg("params"), py::arg("grads"), py::arg("row_vars"),
+        py::arg("col_vars"), py::arg("variances"), py::arg("lr"), py::arg("beta2_decay"), py::arg("eps1"), py::arg("eps2"),
+        py::arg("d"), py::arg("weight_decay"), py::arg("step"), py::arg("grad_scale"), py::arg("grad_scale_dev"),
+        py::arg("master_params"), py::arg("ema_params"), py::arg("ema_weight"), py::arg("ema_start"));
   m.def("grad_shard_stats", &GradShardStats, py::arg("grads"), py::arg("out"), py::arg("inv_scale") = py::none(),
         py::arg("norm_inf") = false);
   m.def("grad_accumulate", &GradAccumulate, py::arg("grads"), py::arg("accs"), py::arg("mode"));

@@ -5,6 +5,7 @@
   (same file);
 * `fused_lars_step`, and its two phases `lars_norms` / `lars_apply` — multi-tensor LARS on LAMB's table and norms
   layout (same file);
+* `fused_adafactor_step` — multi-tensor torch.optim.Adafactor with factored second moments (same file);
 * `grad_shard_stats` — one-pass gradient norm statistics, non-finite check and optional in-place unscale (same file);
 * `grad_accumulate_` — folds bf16 / fp16 gradients into fp32 accumulators for gradient accumulation (same file);
 * `sync_bn_stats`, `sync_bn_combine`, `sync_bn_elemt`, `sync_bn_backward_reduce`, `sync_bn_backward_elemt` — the
@@ -14,6 +15,8 @@
   numerics tests, `bench/kernel_micro.py` and the ncu captures;
 * `kernel_launches()` — how many kernels of this library were launched by this process (bench.py's `gpu_launches`).
 """
+import torch
+
 from horovod_b200.ops import sim  # noqa: F401
 
 
@@ -146,6 +149,37 @@ def lars_apply(params, grads, momentum_buffers, lr, momentum, weight_decay, trus
                                 grad_scale_dev, list(master_params or []), norms,
                                 list(range(n)) if slots is None else [int(s) for s in slots],
                                 *_ema(ema_params, ema_decay, ema_start))
+
+
+def fused_adafactor_step(params, grads, row_vars, col_vars, variances, lr, beta2_decay, eps1, eps2, d, weight_decay, step,
+                         grad_scale=1.0, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
+                         ema_start=False):
+    """One torch.optim.Adafactor step for the whole parameter list in five launches (row sums and column partials of g^2,
+    the factors, per-CTA norm partials, the per-tensor norms, the update), with the argument rules of fused_adam_step.
+    Parameters of dim >= 2 (at most 5) keep fp32 factors over their last two dims, row_vars[i] of shape [..., R, 1] and
+    col_vars[i] of shape [..., 1, C] (contiguous), and None in variances[i]; parameters of dim <= 1 keep an fp32
+    variances[i] with their sizes and strides, and None in the factor lists.  Any dense layout.  For each parameter w
+    (1-based `step` t):
+
+        g = grad * grad_scale [* grad_scale_dev[0]];  beta_w = t^beta2_decay;  rho = min(lr, 1 / sqrt(t))
+        alpha = max(eps2, ||w|| / sqrt(numel)) * rho                     (w before the decay)
+        dim >= 2: row_var = lerp(row_var, mean_c g^2, beta_w);  col_var = lerp(col_var, mean_r g^2, beta_w)
+                  v = row_var * col_var / max(mean_r row_var, eps1)
+        dim <= 1: variance = lerp(variance, g^2, beta_w);  v = variance
+        u = g * rsqrt(max(v, eps1^2));  denom = max(1, ||u|| / (sqrt(numel) * d))
+        w = w * (1 - lr * weight_decay) - (alpha / denom) * u             (one fp32 expression, rounded once)
+
+    `eps1=None` is torch.finfo(params' dtype).eps, as torch resolves it.  `master_params` and the EMA arguments as in
+    fused_sgd_step.  Scratch comes from torch's caching allocator on the current stream; nothing is synchronised with the
+    host, so the call can be captured into a CUDA graph.  Deterministic: the same input gives the same bits on every
+    call, and a parameter's result does not depend on the other parameters of the call."""
+    params = list(params)
+    if eps1 is None:
+        eps1 = torch.finfo(params[0].dtype).eps if params else 0.0
+    return _native().fused_adafactor_step(params, list(grads), list(row_vars), list(col_vars), list(variances), float(lr),
+                                          float(beta2_decay), float(eps1), float(eps2), float(d), float(weight_decay),
+                                          int(step), float(grad_scale), grad_scale_dev, list(master_params or []),
+                                          *_ema(ema_params, ema_decay, ema_start))
 
 
 def grad_shard_stats(tensors, out, inv_scale=None, norm_type=2.0):

@@ -366,7 +366,10 @@ class _DistributedOptimizer(_DistributedOptimizerBase):
             for key in keys + (('master_param',) if self._master_weights else ()) + (('ema_param',) if self._ema else ()):
                 t = st.get(key)
                 if torch.is_tensor(t) and t.dtype == torch.float32 and p.dtype != torch.float32 and key in self.state[p]:
-                    self.state[p][key] = _state_like(p, t, torch.float32)
+                    if key in ('row_var', 'col_var'):  # Adafactor's factors: their own shapes, contiguous
+                        self.state[p][key] = t.to(p.device, torch.float32, copy=True).contiguous()
+                    else:
+                        self.state[p][key] = _state_like(p, t, torch.float32)
 
     @staticmethod
     def find_duplicates(lst):
@@ -783,16 +786,21 @@ class _DistributedOptimizer(_DistributedOptimizerBase):
 
 
 def _optimizer_kind(opt):
-    """Which fused update serves `opt`: 'sgd', 'adam' (Adam and AdamW), 'lamb' (hvd.Lamb), 'lars' (hvd.Lars), or None."""
-    kinds = ((torch.optim.SGD, 'sgd'), ((torch.optim.Adam, torch.optim.AdamW), 'adam'), (Lamb, 'lamb'), (Lars, 'lars'))
+    """Which fused update serves `opt`: 'sgd', 'adam' (Adam and AdamW), 'lamb' (hvd.Lamb), 'lars' (hvd.Lars),
+    'adafactor' (torch.optim.Adafactor), or None."""
+    kinds = ((torch.optim.SGD, 'sgd'), ((torch.optim.Adam, torch.optim.AdamW), 'adam'), (Lamb, 'lamb'), (Lars, 'lars'),
+             (torch.optim.Adafactor, 'adafactor'))
     return next((kind for cls, kind in kinds if isinstance(opt, cls)), None)
 
 
 # The state the fused kernels keep per parameter (per owned shard with sharded state), in the order the kernels take it.
-# Every state tensor is fp32 except SGD momentum without master weights (_state_dtype).  Adam and LAMB also count steps.
+# Every state tensor is fp32 except SGD momentum without master weights (_state_dtype).  Adam, LAMB and Adafactor also
+# count steps.  Adafactor keeps row_var / col_var (torch's factor shapes) for a parameter of dim >= 2, else variance.
 _STATE_KEYS = {'sgd': ('momentum_buffer',), 'adam': ('exp_avg', 'exp_avg_sq'), 'lamb': ('exp_avg', 'exp_avg_sq'),
-               'lars': ('momentum_buffer',)}
-_COUNTS_STEPS = ('adam', 'lamb')
+               'lars': ('momentum_buffer',), 'adafactor': ('row_var', 'col_var', 'variance')}
+_COUNTS_STEPS = ('adam', 'lamb', 'adafactor')
+# the most dims of a parameter the fused Adafactor takes: the two factored dims and three batch dims
+_ADAFACTOR_MAX_DIMS = 5
 
 
 def _state_keys(kind, group):
@@ -846,6 +854,11 @@ def _fused_update(opt, kind, group, ps, grads, states, masters, step=0, first_st
             native.lamb_norms(ps, grads, *states, *hp, 1.0, coef, masters, norms, slots)
         else:
             native.lamb_apply(ps, grads, *states, lr, *hp, Lamb.adapts(group), masters, norms, slots, *ema)
+    elif kind == 'adafactor':
+        eps1, eps2 = group['eps']
+        eps1 = torch.finfo(ps[0].dtype).eps if eps1 is None else float(eps1)  # resolved per launch, as torch does
+        native.fused_adafactor_step(ps, grads, *states, lr, float(group['beta2_decay']), eps1, float(eps2),
+                                    float(group['d']), wd, step, 1.0, coef, masters, *ema)
     else:
         hp = (lr, float(group['momentum']), wd, float(group['trust_coefficient']), float(group['eps']), Lars.adapts(group),
               1.0, coef, masters)
@@ -869,7 +882,8 @@ def _fused_plan(opt, why=None):
     master = getattr(opt, '_master_weights', False)
     kind = _optimizer_kind(opt)
     if kind is None:
-        return no('the optimizer is %s, not SGD, Adam or AdamW, or hvd.Lamb or hvd.Lars' % type(opt).__name__)
+        return no('the optimizer is %s, not SGD, Adam or AdamW, hvd.Lamb or hvd.Lars, or torch.optim.Adafactor'
+                  % type(opt).__name__)
     grad_of = getattr(opt, '_grad_for_update', lambda q: q.grad)
     plan = []
     for group in opt.param_groups:
@@ -880,6 +894,8 @@ def _fused_plan(opt, why=None):
             return no('maximize=True or amsgrad=True')
         if not all(p.is_cuda and not p.grad.is_sparse and mpi_ops._is_dense(p) and p.grad.stride() == p.stride() for p in params):
             return no('a parameter is not a dense CUDA tensor, its gradient is sparse, or its strides differ from the gradient\'s')
+        if kind == 'adafactor' and any(p.dim() > _ADAFACTOR_MAX_DIMS for p in params):
+            return no('a parameter has more than %d dims, the most the fused Adafactor factors' % _ADAFACTOR_MAX_DIMS)
         by_dtype = {}
         for p in params:
             by_dtype.setdefault((p.dtype, grad_of(p).dtype), []).append(p)
@@ -940,6 +956,33 @@ def _param_state(opt, kind, p, keys, master):
     return out, fresh
 
 
+def _adafactor_state(opt, p):
+    """p's Adafactor state for the fused kernel as [row_var], [col_var], [variance] (None where p has none) and whether it
+    starts now: zeros in torch's shapes, or fp32 (torch's own step keeps it in the gradient dtype) with the layout the
+    kernel takes -- contiguous factors, a variance with p's strides."""
+    st = opt.state[p]
+    fresh = st.get('row_var') is None and st.get('variance') is None
+    if p.dim() >= 2:
+        for key, dim in (('row_var', -1), ('col_var', -2)):
+            shape = list(p.shape)
+            shape[dim] = 1
+            t = st.get(key)
+            if t is None:
+                st[key] = torch.zeros(shape, dtype=torch.float32, device=p.device)
+            elif t.dtype != torch.float32 or not t.is_contiguous() or t.device != p.device:
+                if list(t.shape) != shape:
+                    raise RuntimeError('optimizer state %s of shape %s does not fit a parameter of shape %s'
+                                       % (key, tuple(t.shape), tuple(p.shape)))
+                st[key] = t.to(device=p.device, dtype=torch.float32, memory_format=torch.contiguous_format)
+        return [st['row_var'], st['col_var'], None], fresh
+    t = st.get('variance')
+    if t is None:
+        t = st['variance'] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
+    elif t.dtype != torch.float32 or t.stride() != p.stride():
+        t = st['variance'] = _state_like(p, t, torch.float32)
+    return [None, None, t], fresh
+
+
 def _fused_step(opt, coef=None):
     """One multi-tensor kernel for the whole model when the wrapped optimizer is SGD or Adam/AdamW on CUDA, three for
     Lamb and Lars (their trust ratios need whole-tensor norms before the update). With master weights a plan that cannot
@@ -966,7 +1009,13 @@ def _fused_step(opt, coef=None):
             master = use_master and ps[0].dtype != torch.float32
             masters = [_master_param(opt, p) for p in ps] if master else []
             keys = _state_keys(kind, group)
-            per_param, fresh = zip(*[_param_state(opt, kind, p, keys, master) for p in ps])
+            if kind == 'adafactor':
+                per_param, fresh = zip(*[_adafactor_state(opt, p) for p in ps])
+                for p, f in zip(ps, fresh):
+                    step = 0.0 if f else opt.state[p]['step']
+                    opt.state[p]['step'] = step if torch.is_tensor(step) else torch.tensor(float(step))
+            else:
+                per_param, fresh = zip(*[_param_state(opt, kind, p, keys, master) for p in ps])
             states = [[st[k] for st in per_param] for k in range(len(keys))]
             emas, ema_new = zip(*[_ema_param(opt, p) for p in ps]) if use_ema and group.get('ema_decay') is not None \
                 else ([], [False] * len(ps))
@@ -1148,7 +1197,13 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     """Wraps `optimizer` so gradients are combined across ranks before the parameter update.
 
     Arguments follow the reference (horovod/torch/optimizer.py:516-608). `fused=True` (new) runs the SGD /
-    Adam(W) update as one multi-tensor CUDA kernel.
+    Adam(W) update as one multi-tensor CUDA kernel, and hvd.Lamb, hvd.Lars and torch.optim.Adafactor in a few.
+
+    torch.optim.Adafactor (fused): torch's update and state keys (step, row_var [..., R, 1] and col_var [..., 1, C] for
+    a parameter of dim >= 2, at most 5 dims, else variance), so checkpoints load both ways, with three differences: the
+    state is fp32 for every parameter dtype (torch keeps the gradient dtype); for bf16 / fp16 parameters without
+    masters the decay and the update are one fp32 expression rounded once (torch rounds twice); and maximize=True stays
+    on torch's own step.  No host synchronisation and no model-sized temporary.  Not with shard_optimizer_state.
 
     `shard_optimizer_state=True` (new, ZeRO stage 1) keeps the optimizer state of 1/N of the parameters on each of the N
     ranks: gradients are reduce-scattered, each rank updates its shard with the fused kernel and the parameters are
@@ -1160,7 +1215,7 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     ('master_param', sharded like the moments with shard_optimizer_state): the update runs in fp32 on the master and the
     parameter receives it rounded to nearest-even, so updates smaller than half an ulp of the parameter are not lost.
     SGD momentum is then fp32 as well.  fp32 parameters are unaffected.  Implies fused=True; SGD / Adam / AdamW / Lamb /
-    Lars only, without maximize, amsgrad or op=Adasum (ValueError).  A parameter written from outside the optimizer
+    Lars / Adafactor only, without maximize, amsgrad or op=Adasum (ValueError).  A parameter written from outside the optimizer
     (load_state_dict, broadcast_parameters, an in-place edit) is picked up by the next step: where it no longer equals
     its rounded master, the master restarts from it.
 
@@ -1179,7 +1234,7 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     without a gradient in an unsharded step); a clipped step advances it toward the clipped update.  d is stored as
     group['ema_decay'] and read at every step like 'lr', so a schedule (warm-up) may change it; 0 <= d <= 1, else
     ValueError.  `with optimizer.ema_parameters(): ...` evaluates the EMA model.  Buffers (BatchNorm running statistics)
-    are not averaged.  Implies fused=True; SGD / Adam / AdamW / Lamb / Lars only, without maximize, amsgrad or op=Adasum
+    are not averaged.  Implies fused=True; SGD / Adam / AdamW / Lamb / Lars / Adafactor only, without maximize, amsgrad or op=Adasum
     (ValueError); a step whose update cannot be fused raises RuntimeError."""
     check_grad_accumulation_dtype(grad_accumulation_dtype)
     check_ema_decay(ema_decay)
@@ -1191,8 +1246,8 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
         if op == Adasum:
             raise ValueError('%s is not supported with op=Adasum' % what)
         if _optimizer_kind(optimizer) is None:
-            raise ValueError('%s supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
-                             % (what, type(optimizer).__name__))
+            raise ValueError('%s supports SGD, Adam and AdamW, hvd.Lamb and hvd.Lars, and torch.optim.Adafactor, only, '
+                             'not %s' % (what, type(optimizer).__name__))
         for g in optimizer.param_groups:
             if g.get('maximize', False) or g.get('amsgrad', False):
                 raise ValueError('%s does not support maximize=True or amsgrad=True' % what)

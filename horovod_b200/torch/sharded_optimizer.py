@@ -66,6 +66,10 @@ class _ShardedDistributedOptimizer(_DistributedOptimizerBase):
         if kind is None:
             raise ValueError('shard_optimizer_state supports SGD, Adam and AdamW, and hvd.Lamb and hvd.Lars, only, not %s'
                              % type(self).__name__)
+        if kind == 'adafactor':
+            raise ValueError('shard_optimizer_state does not support torch.optim.Adafactor: its factored state is already '
+                             'O(R + C) per matrix, so sharding would save only master weights, and the row / column '
+                             'factors would need an allreduce of partial row and column sums')
         for g in self.param_groups:
             if g.get('maximize', False) or (kind == 'adam' and g.get('amsgrad', False)):
                 raise ValueError('shard_optimizer_state does not support maximize=True or amsgrad=True')
