@@ -625,19 +625,37 @@ OptPlan PlanOpt(const char* op, const std::vector<at::Tensor>& params, const std
   return plan;
 }
 
-// Stages the plan's table once on the params' device and runs launch(device table, current stream) there, which makes
-// one or more kern::Launch* calls and returns the first error.
+// The optimizer kernels select the table entry with blockIdx.y, which CUDA caps at 65535.  A piece of that many entries
+// (72 B each) also fits the 8 MiB staging ring of GpuContext::Stage.
+constexpr size_t kOptMaxEntries = 65535;
+
+// One launch's share of a plan's table: `n` entries staged on the device and the longest of their counts.
+struct OptPiece {
+  const kern::OptTensor* table;
+  int n;
+  int64_t max_count;
+};
+
+// Stages the plan's table on the params' device in pieces of at most kOptMaxEntries entries (one piece, so one launch
+// per phase, when the table fits) and runs launch(piece, current stream) for each, which makes one or more kern::Launch*
+// calls and returns the first error.  Every entry keeps its norm slot and partial offset, so the LAMB / LARS phases run
+// piece by piece unchanged.
 template <typename F>
 void RunPlan(const char* op, const OptPlan& plan, const std::vector<at::Tensor>& params, F&& launch) {
   if (plan.table.empty()) return;
   const int device = (int)params[0].get_device();
   c10::cuda::CUDAGuard guard(params[0].device());
   cudaStream_t s = c10::cuda::getCurrentCUDAStream(device);
-  const auto* dt = (const kern::OptTensor*)GpuContext::Get().Stage(device, plan.table.data(),
-                                                                    plan.table.size() * sizeof(kern::OptTensor), s);
-  TORCH_CHECK(dt != nullptr, op, ": table too large");
-  const cudaError_t e = launch(dt, s);
-  TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+  for (size_t lo = 0; lo < plan.table.size(); lo += kOptMaxEntries) {
+    const size_t n = std::min(kOptMaxEntries, plan.table.size() - lo);
+    int64_t max_count = 0;
+    for (size_t i = lo; i < lo + n; ++i) max_count = std::max(max_count, plan.table[i].count);
+    const auto* dt = (const kern::OptTensor*)GpuContext::Get().Stage(device, plan.table.data() + lo,
+                                                                      n * sizeof(kern::OptTensor), s);
+    TORCH_CHECK(dt != nullptr, op, ": table too large");
+    const cudaError_t e = launch(OptPiece{dt, (int)n, max_count}, s);
+    TORCH_CHECK(e == cudaSuccess, op, " launch failed: ", cudaGetErrorString(e));
+  }
 }
 
 std::vector<OptState> MomentStates(const std::vector<at::Tensor>& exp_avg, const std::vector<at::Tensor>& exp_avg_sq) {
@@ -662,8 +680,8 @@ void FusedSgdStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads,
   if (has_mom) states.push_back({"momentum_buffers", momenta, &kern::OptTensor::state0, true});
   const OptPlan plan = PlanOpt("fused_sgd", params, grads, states, masters, grad_scale_dev, nullptr, {},
                                EmaArgs{emas, ema_weight, ema_start});
-  RunPlan("fused_sgd", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
-    return kern::LaunchFusedSgd(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)momentum, (float)dampening,
+  RunPlan("fused_sgd", plan, params, [&](const OptPiece& pc, cudaStream_t s) {
+    return kern::LaunchFusedSgd(pc.table, pc.n, pc.max_count, (float)lr, (float)momentum, (float)dampening,
                                 (float)weight_decay, nesterov ? 1 : 0, (float)grad_scale, first_step ? 1 : 0,
                                 plan.param_dtype, plan.grad_dtype, s, plan.grad_scale_dev, plan.master, plan.ema);
   });
@@ -676,8 +694,8 @@ void FusedAdamStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   const float c1 = BiasCorrection("fused_adam", beta1, step), c2 = BiasCorrection("fused_adam", beta2, step);
   const OptPlan plan = PlanOpt("fused_adam", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev,
                                nullptr, {}, EmaArgs{emas, ema_weight, ema_start});
-  RunPlan("fused_adam", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
-    return kern::LaunchFusedAdamW(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)beta1, (float)beta2,
+  RunPlan("fused_adam", plan, params, [&](const OptPiece& pc, cudaStream_t s) {
+    return kern::LaunchFusedAdamW(pc.table, pc.n, pc.max_count, (float)lr, (float)beta1, (float)beta2,
                                   (float)eps, (float)weight_decay, c1, c2, (float)grad_scale, adamw ? 1 : 0,
                                   plan.param_dtype, plan.grad_dtype, s, plan.grad_scale_dev, plan.master, plan.ema);
   });
@@ -697,18 +715,18 @@ LambArgs LambHyper(const char* op, double beta1, double beta2, double eps, doubl
   return bias_correction ? LambArgs{beta1, beta2, eps, weight_decay, c1, c2} : LambArgs{beta1, beta2, eps, weight_decay, 1.f, 1.f};
 }
 
-cudaError_t LambNormsPhase(const OptPlan& plan, const kern::OptTensor* dt, const LambArgs& a, double grad_scale,
+cudaError_t LambNormsPhase(const OptPlan& plan, const OptPiece& pc, const LambArgs& a, double grad_scale,
                            at::Tensor& norms, cudaStream_t s) {
   at::Tensor work = NormsScratch(plan, norms);
-  return kern::LaunchLambNorms(dt, (int)plan.table.size(), plan.max_count, (float)a.beta1, (float)a.beta2, (float)a.eps,
+  return kern::LaunchLambNorms(pc.table, pc.n, pc.max_count, (float)a.beta1, (float)a.beta2, (float)a.eps,
                                (float)a.weight_decay, a.c1, a.c2, (float)grad_scale, plan.grad_scale_dev,
                                work.data_ptr<float>(), norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype,
                                plan.master, s);
 }
 
-cudaError_t LambApplyPhase(const OptPlan& plan, const kern::OptTensor* dt, const LambArgs& a, double lr, bool adapt,
+cudaError_t LambApplyPhase(const OptPlan& plan, const OptPiece& pc, const LambArgs& a, double lr, bool adapt,
                            const at::Tensor& norms, cudaStream_t s) {
-  return kern::LaunchLambApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)a.eps, (float)a.weight_decay,
+  return kern::LaunchLambApply(pc.table, pc.n, pc.max_count, (float)lr, (float)a.eps, (float)a.weight_decay,
                                a.c1, a.c2, adapt ? 1 : 0, norms.data_ptr<float>(), plan.param_dtype, plan.master, s,
                                plan.ema);
 }
@@ -721,8 +739,8 @@ void LambNorms(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
   const LambArgs a = LambHyper("lamb_norms", beta1, beta2, eps, weight_decay, step, bias_correction);
   const OptPlan plan = PlanOpt("lamb_norms", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev,
                                &out, slots);
-  RunPlan("lamb_norms", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
-    return LambNormsPhase(plan, dt, a, grad_scale, out, s);
+  RunPlan("lamb_norms", plan, params, [&](const OptPiece& pc, cudaStream_t s) {
+    return LambNormsPhase(plan, pc, a, grad_scale, out, s);
   });
 }
 
@@ -734,8 +752,8 @@ void LambApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
   const LambArgs a = LambHyper("lamb_apply", beta1, beta2, eps, weight_decay, step, bias_correction);
   const OptPlan plan = PlanOpt("lamb_apply", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, c10::nullopt,
                                &norms, slots, EmaArgs{emas, ema_weight, ema_start});
-  RunPlan("lamb_apply", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
-    return LambApplyPhase(plan, dt, a, lr, adapt, norms, s);
+  RunPlan("lamb_apply", plan, params, [&](const OptPiece& pc, cudaStream_t s) {
+    return LambApplyPhase(plan, pc, a, lr, adapt, norms, s);
   });
 }
 
@@ -745,7 +763,7 @@ at::Tensor FreshNorms(const char* op, const std::vector<at::Tensor>& params) {
   return params.empty() ? at::Tensor() : at::zeros({2 * (int64_t)params.size()}, params[0].options().dtype(at::kFloat));
 }
 
-// Both phases: three launches, one staged table.
+// Both phases: three launches per staged piece of the table (one piece up to 65535 entries).
 void FusedLambStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avg,
                    std::vector<at::Tensor> exp_avg_sq, double lr, double beta1, double beta2, double eps, double weight_decay,
                    int64_t step, bool bias_correction, bool adapt, double grad_scale,
@@ -755,9 +773,9 @@ void FusedLambStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   const LambArgs a = LambHyper("fused_lamb", beta1, beta2, eps, weight_decay, step, bias_correction);
   const OptPlan plan = PlanOpt("fused_lamb", params, grads, MomentStates(exp_avg, exp_avg_sq), masters, grad_scale_dev,
                                &norms, {}, EmaArgs{emas, ema_weight, ema_start});
-  RunPlan("fused_lamb", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
-    const cudaError_t e = LambNormsPhase(plan, dt, a, grad_scale, norms, s);
-    return e != cudaSuccess ? e : LambApplyPhase(plan, dt, a, lr, adapt, norms, s);
+  RunPlan("fused_lamb", plan, params, [&](const OptPiece& pc, cudaStream_t s) {
+    const cudaError_t e = LambNormsPhase(plan, pc, a, grad_scale, norms, s);
+    return e != cudaSuccess ? e : LambApplyPhase(plan, pc, a, lr, adapt, norms, s);
   });
 }
 
@@ -766,18 +784,18 @@ std::vector<OptState> LarsStates(const std::vector<at::Tensor>& momentum_buffers
   return {{"momentum_buffers", momentum_buffers, &kern::OptTensor::state0}};
 }
 
-cudaError_t LarsNormsPhase(const OptPlan& plan, const kern::OptTensor* dt, double grad_scale, at::Tensor& norms,
+cudaError_t LarsNormsPhase(const OptPlan& plan, const OptPiece& pc, double grad_scale, at::Tensor& norms,
                            cudaStream_t s) {
   at::Tensor work = NormsScratch(plan, norms);
-  return kern::LaunchLarsNorms(dt, (int)plan.table.size(), plan.max_count, (float)grad_scale, plan.grad_scale_dev,
+  return kern::LaunchLarsNorms(pc.table, pc.n, pc.max_count, (float)grad_scale, plan.grad_scale_dev,
                                work.data_ptr<float>(), norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype,
                                plan.master, s);
 }
 
-cudaError_t LarsApplyPhase(const OptPlan& plan, const kern::OptTensor* dt, double lr, double momentum, double weight_decay,
+cudaError_t LarsApplyPhase(const OptPlan& plan, const OptPiece& pc, double lr, double momentum, double weight_decay,
                            double trust_coefficient, double eps, bool adapt, double grad_scale, const at::Tensor& norms,
                            cudaStream_t s) {
-  return kern::LaunchLarsApply(dt, (int)plan.table.size(), plan.max_count, (float)lr, (float)momentum, (float)weight_decay,
+  return kern::LaunchLarsApply(pc.table, pc.n, pc.max_count, (float)lr, (float)momentum, (float)weight_decay,
                                (float)trust_coefficient, (float)eps, adapt ? 1 : 0, (float)grad_scale, plan.grad_scale_dev,
                                norms.data_ptr<float>(), plan.param_dtype, plan.grad_dtype, plan.master, s, plan.ema);
 }
@@ -789,8 +807,8 @@ void LarsNorms(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
                std::vector<int64_t> slots) {
   const OptPlan plan = PlanOpt("lars_norms", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &out,
                                slots);
-  RunPlan("lars_norms", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
-    return LarsNormsPhase(plan, dt, grad_scale, out, s);
+  RunPlan("lars_norms", plan, params, [&](const OptPiece& pc, cudaStream_t s) {
+    return LarsNormsPhase(plan, pc, grad_scale, out, s);
   });
 }
 
@@ -803,12 +821,12 @@ void LarsApply(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, st
                bool ema_start) {
   const OptPlan plan = PlanOpt("lars_apply", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &norms,
                                slots, EmaArgs{emas, ema_weight, ema_start});
-  RunPlan("lars_apply", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
-    return LarsApplyPhase(plan, dt, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, norms, s);
+  RunPlan("lars_apply", plan, params, [&](const OptPiece& pc, cudaStream_t s) {
+    return LarsApplyPhase(plan, pc, lr, momentum, weight_decay, trust_coefficient, eps, adapt, grad_scale, norms, s);
   });
 }
 
-// Both LARS phases: three launches, one staged table.
+// Both LARS phases: three launches per staged piece of the table (one piece up to 65535 entries).
 void FusedLarsStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> momentum_buffers,
                    double lr, double momentum, double weight_decay, double trust_coefficient, double eps, bool adapt,
                    double grad_scale, c10::optional<at::Tensor> grad_scale_dev, std::vector<at::Tensor> masters,
@@ -816,9 +834,9 @@ void FusedLarsStep(std::vector<at::Tensor> params, std::vector<at::Tensor> grads
   at::Tensor norms = FreshNorms("fused_lars", params);
   const OptPlan plan = PlanOpt("fused_lars", params, grads, LarsStates(momentum_buffers), masters, grad_scale_dev, &norms,
                                {}, EmaArgs{emas, ema_weight, ema_start});
-  RunPlan("fused_lars", plan, params, [&](const kern::OptTensor* dt, cudaStream_t s) {
-    const cudaError_t e = LarsNormsPhase(plan, dt, grad_scale, norms, s);
-    return e != cudaSuccess ? e : LarsApplyPhase(plan, dt, lr, momentum, weight_decay, trust_coefficient, eps, adapt,
+  RunPlan("fused_lars", plan, params, [&](const OptPiece& pc, cudaStream_t s) {
+    const cudaError_t e = LarsNormsPhase(plan, pc, grad_scale, norms, s);
+    return e != cudaSuccess ? e : LarsApplyPhase(plan, pc, lr, momentum, weight_decay, trust_coefficient, eps, adapt,
                                                  grad_scale, norms, s);
   });
 }

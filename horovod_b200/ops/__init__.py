@@ -37,7 +37,7 @@ def _ema(ema_params, ema_decay, ema_start):
 def fused_sgd_step(params, grads, momentum_buffers, lr, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False,
                    grad_scale=1.0, first_step=False, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
                    ema_start=False):
-    """One launch for the whole parameter list (fp32 / bf16 / fp16 parameters, fp32 or matching gradients).
+    """One launch per 65535 non-empty parameters (fp32 / bf16 / fp16 parameters, fp32 or matching gradients).
     `grad_scale_dev`: an optional 1-element fp32 tensor on the parameters' device; the gradients are multiplied by
     grad_scale * grad_scale_dev[0], read by the kernel, so no host synchronisation is needed.
 
@@ -48,7 +48,12 @@ def fused_sgd_step(params, grads, momentum_buffers, lr, momentum=0.0, dampening=
 
     `ema_params`: optional fp32 exponential moving averages, one per parameter with its sizes and strides, updated in the
     same launch after the parameter: e = fmaf(1 - ema_decay, x - e, e) in fp32, with x the updated master if there is
-    one, else the value stored into the parameter.  `ema_start=True` begins them: e = x, without reading e."""
+    one, else the value stored into the parameter.  `ema_start=True` begins them: e = x, without reading e.
+
+    A call with more than 65535 non-empty parameters (the grid limit of one launch) stages its table in pieces through a
+    fixed host-to-device ring, and filling that ring may wait for the stream: such a call can synchronise with the host
+    and cannot be captured into a CUDA graph.  The same holds for fused_adam_step, fused_lamb_step, fused_lars_step and
+    their phases."""
     return _native().fused_sgd_step(list(params), list(grads), list(momentum_buffers), float(lr), float(momentum), float(dampening),
                                     float(weight_decay), bool(nesterov), float(grad_scale), bool(first_step), grad_scale_dev,
                                     list(master_params or []), *_ema(ema_params, ema_decay, ema_start))
@@ -57,7 +62,7 @@ def fused_sgd_step(params, grads, momentum_buffers, lr, momentum=0.0, dampening=
 def fused_adam_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, step=1,
                     grad_scale=1.0, adamw=True, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
                     ema_start=False):
-    """One launch of Adam / AdamW for the whole parameter list (fp32 / bf16 / fp16 parameters, fp32 or matching
+    """One launch of Adam / AdamW per 65535 non-empty parameters (fp32 / bf16 / fp16 parameters, fp32 or matching
     gradients, fp32 state with the parameters' sizes and strides; `step` is the 1-based step count). Mismatched
     lists, dtypes, sizes, strides or devices raise RuntimeError before anything is launched. `grad_scale_dev`,
     `master_params` and the EMA arguments as in fused_sgd_step."""
@@ -69,15 +74,16 @@ def fused_adam_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1=0.9, beta2=0
 def fused_lamb_step(params, grads, exp_avgs, exp_avg_sqs, lr, beta1, beta2, eps, weight_decay, step, bias_correction=True,
                     adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
                     ema_start=False):
-    """One LAMB step for the whole parameter list in three launches (moments and per-CTA norm partials, the per-tensor
-    norms, the update), with the argument rules of fused_adam_step. For each parameter w (1-based `step`):
+    """One LAMB step in three launches per 65535 non-empty parameters (moments and per-CTA norm partials, the
+    per-tensor norms, the update), with the argument rules of fused_adam_step. For each parameter w (1-based `step`):
 
         g = grad * grad_scale [* grad_scale_dev[0]];  m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g^2
         u = (m / c1) / (sqrt(v / c2) + eps) + weight_decay * w      (c1 = 1 - b1^step, c2 = 1 - b2^step; 1 without bias_correction)
         w -= lr * r * u,   r = ||w|| / ||u|| if adapt and both norms are > 0, else 1
 
     The EMA arguments are those of fused_sgd_step; the update launch writes the EMA.
-    Deterministic: the same input gives the same bits on every call. Nothing is synchronised with the host."""
+    Deterministic: the same input gives the same bits on every call. Up to 65535 non-empty parameters nothing is
+    synchronised with the host (see fused_sgd_step)."""
     return _native().fused_lamb_step(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), float(lr), float(beta1),
                                      float(beta2), float(eps), float(weight_decay), int(step), bool(bias_correction),
                                      bool(adapt), float(grad_scale), grad_scale_dev, list(master_params or []),
@@ -113,15 +119,16 @@ def lamb_apply(params, grads, exp_avgs, exp_avg_sqs, lr, beta1, beta2, eps, weig
 def fused_lars_step(params, grads, momentum_buffers, lr, momentum=0.9, weight_decay=0.0, trust_coefficient=0.001, eps=0.0,
                     adapt=True, grad_scale=1.0, grad_scale_dev=None, master_params=None, ema_params=None, ema_decay=None,
                     ema_start=False):
-    """One LARS step for the whole parameter list in three launches (per-CTA norm partials, the per-tensor norms, the
-    update), with the argument rules of fused_adam_step; the momentum buffers are fp32. For each parameter w:
+    """One LARS step in three launches per 65535 non-empty parameters (per-CTA norm partials, the per-tensor norms,
+    the update), with the argument rules of fused_adam_step; the momentum buffers are fp32. For each parameter w:
 
         g = grad * grad_scale [* grad_scale_dev[0]];  d = g + weight_decay * w
         r = trust_coefficient * ||w|| / (||g|| + weight_decay * ||w|| + eps) if adapt and both norms are > 0, else 1
         v = momentum * v + lr * r * d;  w -= v
 
     The EMA arguments are those of fused_sgd_step; the update launch writes the EMA.
-    Deterministic: the same input gives the same bits on every call. Nothing is synchronised with the host."""
+    Deterministic: the same input gives the same bits on every call. Up to 65535 non-empty parameters nothing is
+    synchronised with the host (see fused_sgd_step)."""
     return _native().fused_lars_step(list(params), list(grads), list(momentum_buffers), float(lr), float(momentum),
                                      float(weight_decay), float(trust_coefficient), float(eps), bool(adapt),
                                      float(grad_scale), grad_scale_dev, list(master_params or []),
@@ -172,7 +179,8 @@ def fused_adafactor_step(params, grads, row_vars, col_vars, variances, lr, beta2
     `eps1=None` is torch.finfo(params' dtype).eps, as torch resolves it.  `master_params` and the EMA arguments as in
     fused_sgd_step.  Scratch comes from torch's caching allocator on the current stream; nothing is synchronised with the
     host, so the call can be captured into a CUDA graph.  Deterministic: the same input gives the same bits on every
-    call, and a parameter's result does not depend on the other parameters of the call."""
+    call, and a parameter's result does not depend on the other parameters of the call.  At most 65535 non-empty
+    parameters per call (one launch's grid); more raise RuntimeError before anything is launched."""
     params = list(params)
     if eps1 is None:
         eps1 = torch.finfo(params[0].dtype).eps if params else 0.0
