@@ -1031,6 +1031,22 @@ Status Engine::CapturedAllgather(void* ptr, int64_t bytes, int32_t psid, int max
   return gpu_ops_->CapturedAllgather(*ps, ptr, bytes, max_ctas, (cudaStream_t)stream, channel);
 }
 
+Status Engine::CapturedAlltoall(const void* in, int64_t rows, int64_t row_bytes, const void* splits, int64_t nsplits,
+                                bool splits_int64, void* out, int64_t capacity, int64_t* recv_splits, int* status, int32_t psid,
+                                int max_ctas, void* stream) {
+  std::shared_ptr<ProcessSet> ps;
+  Status st = CheckSet(psid, &ps);
+  if (!st.ok()) return st;
+  if (nsplits != ps->set_size())
+    return Status::InvalidArgument("captured alltoall: splits has " + std::to_string(nsplits) + " entries, the process set " +
+                                   std::to_string(ps->set_size()) + " ranks");
+  // unlike the in-place collectives, a one-rank alltoall still has to move rows: there is no kernel without a team
+  if (ps->set_size() < 2) return Status::PreconditionError("captured alltoall needs a peer-mapped process set of at least 2 ranks");
+  captured_launches_.fetch_add(1, std::memory_order_relaxed);
+  return gpu_ops_->CapturedAlltoall(*ps, in, rows, row_bytes, splits, nsplits, splits_int64, out, capacity, recv_splits, status,
+                                    max_ctas, (cudaStream_t)stream);
+}
+
 Status Engine::StartTimeline(const std::string& file, bool mark_cycles) {
   if (!initialized_.load()) return Status::PreconditionError(NOT_INITIALIZED_ERROR_MSG);
   std::lock_guard<std::mutex> l(tl_mu_);

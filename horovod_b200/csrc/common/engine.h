@@ -89,6 +89,10 @@ class Engine {
   Status CapturedReducescatter(void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale, double postscale,
                                int32_t process_set_id, int max_ctas, void* stream);
   Status CapturedAllgather(void* ptr, int64_t bytes, int32_t process_set_id, int max_ctas, void* stream, int channel = 1);
+  // Alltoall with device-resident splits, same launch contract (see GpuOps::CapturedAlltoall); needs a set of >= 2 ranks.
+  Status CapturedAlltoall(const void* in, int64_t rows, int64_t row_bytes, const void* splits, int64_t nsplits, bool splits_int64,
+                          void* out, int64_t capacity, int64_t* recv_splits, int* status, int32_t process_set_id, int max_ctas,
+                          void* stream);
 
   // ---- timeline ----
   Status StartTimeline(const std::string& file, bool mark_cycles);

@@ -510,6 +510,38 @@ int hvd_sim_inplace_allgather(int nranks, int device, int64_t bytes, const uint6
   return hvd_sim_inplace_sharded(nranks, device, bytes, ptrs, 0, 1, ctas, 1.0, repeats, 0);
 }
 
+// The captured alltoall over N simulated ranks, every rank's arguments indexed by rank: in_ptrs / rows / row_bytes its
+// input, split_ptrs its n splits on the device (int64 with splits_int64, else int32), out_ptrs / capacity its output,
+// recv_ptrs (int64, n) and status_ptrs (int32, 1).  Without `streams` the N kernels run on the harness's streams and the
+// call waits for them (returns 0, a cudaError_t, -1 or -3 as hvd_sim_inplace).  With `streams` (N cudaStream_t) it only
+// launches rank r's kernel on streams[r] and returns, so that a caller can order the launches after device work of its
+// own or capture all N ranks into one CUDA graph; the harness of this rank count must exist by then (one call without
+// `streams`), and must not be reset while such a graph may still run.
+int hvd_sim_captured_alltoall(int nranks, int device, const uint64_t* in_ptrs, const int64_t* rows, const int64_t* row_bytes,
+                              const uint64_t* split_ptrs, int splits_int64, const uint64_t* out_ptrs, const int64_t* capacity,
+                              const uint64_t* recv_ptrs, const uint64_t* status_ptrs, int ctas, const uint64_t* streams) {
+  if (nranks < 2 || nranks > kern::kMaxPeers || cudaSetDevice(device) != cudaSuccess) return -1;
+  Sim* sim = streams ? (g_sims.count(nranks) ? &g_sims[nranks] : nullptr) : GetSim(nranks, device, 1 << 20);
+  if (!sim) return -1;
+  // rejected on every rank or on none: a rank launched alone would wait at its barrier for peers that never come
+  if (ctas < 1 || ctas > kern::kMaxCtas) return (int)cudaErrorInvalidValue;
+  for (int r = 0; r < nranks; ++r)
+    if (rows[r] < 0 || capacity[r] < 0 || row_bytes[r] < 0) return (int)cudaErrorInvalidValue;
+  if (!streams) cudaDeviceSynchronize();
+  for (int r = 0; r < nranks; ++r) {
+    kern::CapturedAlltoallArgs a {};
+    for (int p = 0; p < nranks; ++p) { a.in[p] = (const void*)in_ptrs[p]; a.counts[p] = sim->teams[r]->CountRegion(p); }
+    a.in_offset = 0; a.rows = rows[r]; a.capacity = capacity[r]; a.row_bytes = row_bytes[r];
+    a.splits = (const void*)split_ptrs[r]; a.splits_int64 = splits_int64;
+    a.out = (void*)out_ptrs[r]; a.recv_splits = (int64_t*)recv_ptrs[r]; a.status = (int*)status_ptrs[r];
+    a.ctas = ctas;
+    cudaError_t e = kern::LaunchCapturedAlltoall(sim->teams[r]->Params(0, kern::kAlltoallChannel), a,
+                                                 streams ? (cudaStream_t)streams[r] : sim->streams[r]);
+    if (e != cudaSuccess) return (int)e;
+  }
+  return streams ? 0 : Finish(nranks, cudaDeviceSynchronize());
+}
+
 void hvd_sim_reset() {
   for (auto& kv : g_sims) for (auto st : kv.second.streams) cudaStreamDestroy(st);
   g_sims.clear();

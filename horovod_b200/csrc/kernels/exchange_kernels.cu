@@ -18,25 +18,6 @@ namespace {
 
 constexpr int kXChunk = 32768;  // chunk -> CTA mapping granularity inside the symmetric buffer (one 8-deep trip of the CTA)
 
-__device__ __forceinline__ void copy_bytes_vec(const char* src, char* dst, int64_t n) {
-  // 16 B vectors, 8 in flight per thread (all loads of a trip are issued before the first store: an NVLink round trip is
-  // ~2 us) when both sides are 16 B aligned, bytes otherwise
-  if ((((uintptr_t)src | (uintptr_t)dst) & 15) == 0) {
-    const int64_t nv = n / 16;
-    constexpr int U = 8;
-    for (int64_t i0 = threadIdx.x; i0 < nv; i0 += (int64_t)U * kThreads) {
-      uint4 v[U];
-#pragma unroll
-      for (int j = 0; j < U; ++j) { int64_t i = i0 + (int64_t)j * kThreads; if (i < nv) v[j] = ld_stream(src + i * 16); }
-#pragma unroll
-      for (int j = 0; j < U; ++j) { int64_t i = i0 + (int64_t)j * kThreads; if (i < nv) st_stream(dst + i * 16, v[j]); }
-    }
-    for (int64_t i = nv * 16 + threadIdx.x; i < n; i += kThreads) dst[i] = src[i];
-  } else {
-    for (int64_t i = threadIdx.x; i < n; i += kThreads) dst[i] = src[i];
-  }
-}
-
 // Root side of a multicast broadcast: local source -> multimem.st on the team's multicast mapping, i.e. ONE read of the
 // source and one NVLink egress stream that the switch replicates into every rank's symmetric buffer (a pull-style
 // broadcast makes the root serve N-1 readers).  `src` and `mc` are 16 B aligned; a tail shorter than 16 B is zero-padded

@@ -35,7 +35,15 @@ constexpr int kLatencyChannel = 3;            // the latency lane of small allre
 // hvd.SyncBatchNorm's captured collectives on the compute stream: inside hvd.GraphedStep they run while the gradient
 // buckets' allreduces (kGraphChannel, forked stream) may be resident, so they need flag words and epochs of their own
 constexpr int kSyncBnChannel = 4;
+// hvd.captured_alltoall on the compute stream: like kSyncBnChannel, it may run while the gradient buckets' allreduces are
+// resident on kGraphChannel, so it has flag words and epochs of its own
+constexpr int kAlltoallChannel = 5;
 constexpr int kChannelFlagsOffset = 128 * 1024;  // bytes from the start of the flag region; channel c >= 1 at + (c-1) * kFlagWords * 4
+// The count region of hvd.captured_alltoall, after the last channel's flag words: one row of kA2aRowWords int64 per CTA
+// (see CapturedAlltoallArgs).  Reserved with the flag region when the team is created, so a first call may be captured.
+constexpr int kA2aRowWords = 16;
+constexpr int kCountRegionOffset = kChannelFlagsOffset + (kNumChannels - 1) * kFlagWords * 4;
+constexpr int kCountRegionBytes = kMaxCtas * kA2aRowWords * 8;
 
 // Everything a kernel needs to talk to its peers. Passed by value
 // (__grid_constant__).
@@ -127,6 +135,35 @@ struct ExchangeArgs {
   int ctas;
 };
 cudaError_t LaunchExchange(const CommParams& cp, const ExchangeArgs& args, cudaStream_t stream);
+
+// Alltoall whose split vectors exist only on the device (see alltoall_kernels.cu), one launch on barrier channel
+// kAlltoallChannel.  Rank p sends the first splits_p[0] rows of its input to rank 0, the next splits_p[1] to rank 1, ...;
+// rank q receives them into `out` in sender order.  Every CTA b publishes this rank's row {splits[0 .. n), rows, capacity,
+// row_bytes, in_offset} into row b of its count region, meets CTA b of every peer, reads all n rows and derives the same
+// verdict on every rank: kA2aOk, or the first of the codes below that applies, in which case no row is copied.
+// `recv_splits` (int64, n) receives the column that was sent to this rank in either case; CTA 0 writes it and `status`.
+enum AlltoallStatus : int {
+  kA2aOk = 0,
+  kA2aNegativeSplit = 1,     // some rank's split is negative
+  kA2aSendOverflow = 2,      // some rank's splits sum to more than its input rows
+  kA2aRecvOverflow = 3,      // some rank would receive more rows than its capacity
+  kA2aRowBytesMismatch = 4,  // the ranks' row sizes in bytes differ
+  kA2aAborted = 5,           // a peer did not reach the barrier (team aborted or timed out); nothing else is written
+};
+constexpr int kA2aRows = kMaxPeers, kA2aCapacity = kMaxPeers + 1, kA2aRowBytes = kMaxPeers + 2, kA2aInOffset = kMaxPeers + 3;
+struct CapturedAlltoallArgs {
+  const void* in[kMaxPeers];    // every rank's registered region as mapped into this process
+  int64_t* counts[kMaxPeers];   // every rank's count region (kCountRegionOffset of its flag region) as mapped here
+  int64_t in_offset;            // byte offset of this rank's input rows in its region
+  int64_t rows, capacity, row_bytes;
+  const void* splits;           // this rank's n splits, int32 or int64 (splits_int64)
+  int splits_int64;
+  void* out;                    // capacity * row_bytes bytes
+  int64_t* recv_splits;
+  int* status;
+  int ctas;                     // the same on every rank
+};
+cudaError_t LaunchCapturedAlltoall(const CommParams& cp, const CapturedAlltoallArgs& args, cudaStream_t stream);
 
 // Stand-alone batched pack / unpack / scale (NCCL-baseline path and odd cases).
 // direction 0: tensors -> buffer (prescale), 1: buffer -> tensors (postscale)

@@ -406,6 +406,33 @@ Status GpuOps::CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int m
                         stream, channel);
 }
 
+// The inputs are read in place from every sender's registered region, and each rank publishes the byte offset of its own
+// input with its splits, so only the region (not the offset) has to be the same on every rank.
+Status GpuOps::CapturedAlltoall(ProcessSet& ps, const void* in, int64_t rows, int64_t row_bytes, const void* splits, int64_t nsplits,
+                                bool splits_int64, void* out, int64_t capacity, int64_t* recv_splits, int* status, int max_ctas,
+                                cudaStream_t stream) {
+  const std::string name = "captured alltoall";
+  std::shared_ptr<SymmTeam> team;
+  { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
+  if (!team) return Status::PreconditionError(name + ": the process set has no peer-mapped team (allocate the tensor with hvd.symm_empty first)");
+  if (team->abort_state() != 0) return Status::Aborted(name + ": the team was aborted");
+  const int n = team->nranks();
+  if (nsplits != n) return Status::InvalidArgument(name + ": splits must have one entry per rank of the team");
+  SymmTeam::RegionView view;
+  int64_t off = 0;
+  if (!team->FindRegion(in, (size_t)(rows * row_bytes), &view, &off))
+    return Status::InvalidArgument(name + ": tensor is not (entirely) inside registered symmetric memory");
+  kern::CapturedAlltoallArgs a {};
+  for (int p = 0; p < n; ++p) { a.in[p] = view.ptr[p]; a.counts[p] = team->CountRegion(p); }
+  a.in_offset = off; a.rows = rows; a.capacity = capacity; a.row_bytes = row_bytes;
+  a.splits = splits; a.splits_int64 = splits_int64 ? 1 : 0;
+  a.out = out; a.recv_splits = recv_splits; a.status = status;
+  a.ctas = std::min(max_ctas > 0 ? max_ctas : env_.params->comm_ctas, kern::kMaxCtas);
+  cudaError_t ce = kern::LaunchCapturedAlltoall(team->Params(0, kern::kAlltoallChannel), a, stream);
+  if (ce != cudaSuccess) return Status::UnknownError(name + " launch failed: " + cudaGetErrorString(ce));
+  return Status::OK();
+}
+
 Status GpuOps::LaunchCaptured(ProcessSet& ps, const char* what, InplaceLaunch launch, void* ptr, int64_t bytes, DataType dtype,
                               ReduceOp op, double prescale, double postscale, int max_ctas, cudaStream_t stream, int channel) {
   const std::string name = std::string("captured ") + what;

@@ -119,6 +119,13 @@ class GpuOps {
   Status CapturedReducescatter(ProcessSet& ps, void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                                double postscale, int max_ctas, cudaStream_t stream);
   Status CapturedAllgather(ProcessSet& ps, void* ptr, int64_t bytes, int max_ctas, cudaStream_t stream, int channel);
+  // Alltoall of `rows` rows of `row_bytes` at `in` (inside a registered region) whose splits (n int32 / int64 values) exist
+  // only on the device: ONE kernel on `stream` on barrier channel kern::kAlltoallChannel, same launch contract as the other
+  // captured collectives; every rank passes the same grid (`max_ctas`).  Writes up to `capacity` rows to `out`, the
+  // received splits to `recv_splits` and the verdict (kern::AlltoallStatus) to `status`.
+  Status CapturedAlltoall(ProcessSet& ps, const void* in, int64_t rows, int64_t row_bytes, const void* splits, int64_t nsplits,
+                          bool splits_int64, void* out, int64_t capacity, int64_t* recv_splits, int* status, int max_ctas,
+                          cudaStream_t stream);
   bool BuildInplaceArgs(SymmTeam& team, const void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                         double postscale, int64_t expect_off, int max_ctas, kern::InplaceArgs* out);
 

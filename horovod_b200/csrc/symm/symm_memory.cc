@@ -282,6 +282,7 @@ namespace {
 constexpr size_t kFlagRegionBytes = 256 * 1024;
 static_assert(kern::kFlagWords * 4 + 2 * kern::kAdasumScratchStride <= (long long)kern::kChannelFlagsOffset, "Adasum scratch overlaps the channel flags");
 static_assert(kern::kChannelFlagsOffset + (kern::kNumChannels - 1) * kern::kFlagWords * 4 <= (long long)kFlagRegionBytes, "flag region too small");
+static_assert(kern::kCountRegionOffset + kern::kCountRegionBytes <= (long long)kFlagRegionBytes, "no room for the alltoall count region");
 }
 
 std::shared_ptr<SymmTeam> SymmTeam::Create(Transport* t, int device, size_t buffer_bytes, bool want_mc,

@@ -66,6 +66,8 @@ class SymmTeam {
   // zero-copy (registered-region) kernels may use a channel other than the one that owns the slots.
   // `byte_offset` shifts the data pointers (buffers and multicast alias) into a sub-area of the slot.
   kern::CommParams Params(int which, int channel = 0, int64_t byte_offset = 0) const;
+  // Rank `peer`'s count region of the captured alltoall (kern::kCountRegionOffset of its flag region), as mapped here.
+  int64_t* CountRegion(int peer) const { return (int64_t*)((char*)flags_[peer] + kern::kCountRegionOffset); }
   // Next ping-pong slot (ops alternate so a fast rank never overwrites data a
   // slow peer is still reading).
   int NextSlot() { int s = slot_; slot_ ^= 1; return s; }

@@ -488,6 +488,37 @@ void CapturedAllgather(at::Tensor tensor, int process_set_id, int max_ctas, int 
   ThrowIfError(Engine::Get().CapturedAllgather(tensor.data_ptr(), bytes, process_set_id, max_ctas, (void*)stream, channel));
 }
 
+// Alltoall of the rows (dim 0) of a registered tensor with splits that only the device reads, launched like
+// CapturedAllreduce.  The outputs are allocated on the current stream (from the graph's pool under capture):
+// output [capacity, *row] in the tensor's dtype, recv_splits int64 [n] and status int32 [1] (kern::AlltoallStatus).
+std::tuple<at::Tensor, at::Tensor, at::Tensor> CapturedAlltoall(at::Tensor tensor, at::Tensor splits, int64_t capacity,
+                                                                int process_set_id, int max_ctas) {
+  const char* op = "captured_alltoall";
+  TORCH_CHECK(tensor.is_cuda(), op, ": CUDA tensor expected");
+  TORCH_CHECK(tensor.dim() >= 1, op, ": tensor must have at least one dimension (its rows)");
+  TORCH_CHECK(tensor.is_contiguous(), op, ": tensor must be contiguous");
+  TORCH_CHECK(splits.is_cuda() && splits.device() == tensor.device(), op, ": splits must be on the tensor's device ", tensor.device(),
+              ", got ", splits.device());
+  TORCH_CHECK(splits.scalar_type() == at::kInt || splits.scalar_type() == at::kLong, op, ": splits must be int32 or int64, got ",
+              splits.scalar_type());
+  TORCH_CHECK(splits.dim() == 1 && splits.is_contiguous(), op, ": splits must be a contiguous 1-D tensor, got sizes ", splits.sizes());
+  TORCH_CHECK(capacity >= 0, op, ": capacity must be >= 0, got ", capacity);
+  c10::cuda::CUDAGuard guard(tensor.device());
+  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(tensor.get_device());
+  const int64_t rows = tensor.size(0);
+  const int64_t row_bytes = c10::multiply_integers(tensor.sizes().slice(1)) * (int64_t)tensor.element_size();
+  std::vector<int64_t> out_sizes = tensor.sizes().vec();
+  out_sizes[0] = capacity;
+  at::Tensor out = at::empty(out_sizes, tensor.options());
+  at::Tensor recv = at::empty({splits.numel()}, tensor.options().dtype(at::kLong));
+  at::Tensor status = at::empty({1}, tensor.options().dtype(at::kInt));
+  ThrowIfError(Engine::Get().CapturedAlltoall(tensor.data_ptr(), rows, row_bytes, splits.data_ptr(), splits.numel(),
+                                              splits.scalar_type() == at::kLong, out.data_ptr(), capacity,
+                                              recv.data_ptr<int64_t>(), status.data_ptr<int>(), process_set_id, max_ctas,
+                                              (void*)stream));
+  return {out, recv, status};
+}
+
 // ---- fused optimizer kernels (an extra of this library; see kernels/optim_kernels.cu) --------------
 // The kernels address every tensor of entry i with the element index of params[i] and take one element type per list, so
 // each companion tensor must have the param's sizes and strides, one dtype per list, and live on the param's device.
@@ -1285,6 +1316,8 @@ PYBIND11_MODULE(_hvd_torch, m) {
   m.def("captured_reducescatter_", &CapturedReducescatter);
   m.def("captured_allgather_", &CapturedAllgather, py::arg("tensor"), py::arg("process_set_id"), py::arg("max_ctas"),
         py::arg("channel") = kern::kGraphChannel);
+  m.def("captured_alltoall", &CapturedAlltoall, py::arg("tensor"), py::arg("splits"), py::arg("capacity"),
+        py::arg("process_set_id"), py::arg("max_ctas"));
   m.def("fused_sgd_step", &FusedSgdStep, py::arg("params"), py::arg("grads"), py::arg("momenta"), py::arg("lr"),
         py::arg("momentum"), py::arg("dampening"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("grad_scale"),
         py::arg("first_step"), py::arg("grad_scale_dev") = py::none(), py::arg("master_params") = std::vector<at::Tensor>(),

@@ -44,6 +44,8 @@ def lib():
         L.hvd_sim_broadcast.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, i64p, ctypes.c_int, u64p, u64p, ctypes.c_int64,
                                         ctypes.c_int]
         L.hvd_sim_alltoallv.argtypes = plan + [ctypes.c_int, u64p, u64p, ctypes.c_int64, ctypes.c_int]
+        L.hvd_sim_captured_alltoall.argtypes = [ctypes.c_int, ctypes.c_int, u64p, i64p, i64p, u64p, ctypes.c_int, u64p, i64p, u64p,
+                                                u64p, ctypes.c_int, u64p]
         _lib = L
     return _lib
 
@@ -161,3 +163,24 @@ def alltoallv(ins, outs, splits, cap=1 << 20, ctas=8, device=0):
     flat = [splits[i][p][q] for i in range(t) for p in range(n) for q in range(n)]
     _check(lib().hvd_sim_alltoallv(n, device, t, _i64(flat), _i64(_row(a) for a in ins[0]), DTYPE_CODE[ins[0][0].dtype], _ptrs(ins),
                                    _ptrs(outs), cap, ctas), 'sim alltoallv')
+
+
+def captured_alltoall(ins, splits, outs, recv_splits, status, ctas=8, streams=None, device=0):
+    """The kernel of hvd.captured_alltoall on N simulated ranks, every argument a list indexed by rank: ins[r] [S_r, *row]
+    (contiguous), splits[r] int32 / int64 [N] on the device, outs[r] [capacity_r, *row], recv_splits[r] int64 [N],
+    status[r] int32 [1].  Rows and row bytes come from each rank's own tensors, so ranks may disagree on them.
+
+    streams=None runs the N kernels and waits for them.  With streams (N torch.cuda.Stream) rank r's kernel is only
+    launched on streams[r], after whatever that stream already holds, so a caller can order it after device work of its
+    own or capture all N ranks into one CUDA graph.  That needs one earlier call with streams=None for this N, which
+    creates the simulated team the kernels keep using."""
+    n = len(ins)
+    if len({s.dtype for s in splits}) != 1:
+        raise ValueError('sim captured alltoall: every rank\'s splits need the same dtype')
+    u64 = lambda vals: (ctypes.c_uint64 * n)(*vals)  # noqa: E731
+    rc = lib().hvd_sim_captured_alltoall(
+        n, device, u64(t.data_ptr() for t in ins), _i64(t.shape[0] for t in ins), _i64(_row(t) * t.element_size() for t in ins),
+        u64(s.data_ptr() for s in splits), int(splits[0].dtype == torch.int64), u64(t.data_ptr() for t in outs),
+        _i64(t.shape[0] for t in outs), u64(t.data_ptr() for t in recv_splits), u64(t.data_ptr() for t in status), ctas,
+        None if streams is None else u64(s.cuda_stream for s in streams))
+    _check(rc, 'sim captured alltoall')

@@ -17,7 +17,7 @@ from horovod_b200.torch.mpi_ops import (  # noqa: F401
     alltoall, alltoall_async,
     reducescatter, reducescatter_async, grouped_reducescatter, grouped_reducescatter_async,
     join, barrier, poll, synchronize, symm_empty, symm_available, captured_allreduce_,
-    captured_reducescatter_, captured_allgather_,
+    captured_reducescatter_, captured_allgather_, captured_alltoall,
     Average, Sum, Adasum, Min, Max, Product)
 from horovod_b200.torch.functions import (broadcast_parameters, broadcast_optimizer_state, broadcast_object,  # noqa: F401
                                           allgather_object)

@@ -741,6 +741,41 @@ def captured_allgather_(tensor, process_set=global_process_set, max_ctas=0):
     return tensor
 
 
+# status codes of captured_alltoall (kern::AlltoallStatus)
+ALLTOALL_OK, ALLTOALL_NEGATIVE_SPLIT, ALLTOALL_SEND_OVERFLOW, ALLTOALL_RECV_OVERFLOW, ALLTOALL_ROW_BYTES_MISMATCH, \
+    ALLTOALL_ABORTED = range(6)
+
+
+def captured_alltoall(tensor, splits, capacity, process_set=global_process_set, max_ctas=0):
+    """Alltoall of the rows of `tensor` whose split vector exists only on the device, issued like `captured_allreduce_`:
+    ONE kernel on the current CUDA stream, no handle, no negotiation, no host synchronisation, so it can be captured
+    into a CUDA graph (the dispatch / combine of expert parallelism with router-computed row counts).
+
+    tensor: a contiguous CUDA tensor [S, *row] in registered memory (`hvd.symm_empty`, or a view of one) of any dtype.
+    The first splits[0] rows go to rank 0, the next splits[1] to rank 1, and so on.  The rows are read in place by the
+    receivers: do not overwrite them before the call (stream order takes care of that).
+    splits: int32 or int64 CUDA tensor [N] on the same device, N = process set size; only the device reads it.
+    capacity: rows of the output.
+
+    Returns (output, recv_splits, status), allocated on the current stream: output [capacity, *row] holds the rows from
+    rank 0, then those from rank 1, ...; rows past the total received are not written.  recv_splits: int64 [N], the rows
+    each rank sent here.  status: int32 [1], the same on every rank: 0 on success, else the first of
+    ALLTOALL_NEGATIVE_SPLIT (1), ALLTOALL_SEND_OVERFLOW (2: some rank's splits sum to more than its S),
+    ALLTOALL_RECV_OVERFLOW (3: some rank would receive more than its capacity) and ALLTOALL_ROW_BYTES_MISMATCH (4) that
+    applies; then no rank copies any row, recv_splits still holds what was sent, and the next call works normally.
+    ALLTOALL_ABORTED (5): a peer never arrived (the team was aborted or timed out).
+
+    Contract: every rank of the process set issues the same sequence of captured collectives with the same `max_ctas`
+    (0: the engine's CTA count), and a rank's captured_alltoall calls run in one stream order.  Argument errors the host
+    can see raise HorovodInternalError, as does a process set for which `symm_available` is False."""
+    if not symm_available(process_set):
+        raise HorovodInternalError('captured_alltoall needs a peer-mapped process set of more than one rank (hvd.symm_available)')
+    try:
+        return tuple(_native().captured_alltoall(tensor, splits, int(capacity), process_set.process_set_id, int(max_ctas)))
+    except (RuntimeError, ValueError, TypeError) as e:
+        raise HorovodInternalError(e)
+
+
 def symm_available(process_set=global_process_set):
     """True when the zero-copy path can be used: CUDA, more than one rank, everything on one NVLink domain."""
     return torch.cuda.is_available() and is_initialized() and process_set.size() is not None and process_set.size() > 1 \
