@@ -32,6 +32,11 @@ template <> __device__ __forceinline__ __half from_f<__half>(float v) { return _
 
 template <typename T> struct alignas(sizeof(T) * kOptVec) Vec4 { T v[kOptVec]; };
 
+// max that keeps a NaN once it has seen one (fmaxf drops it), as torch's clamp and max do: an inf-norm of NaN gradients
+// is NaN, and so is an Adafactor v clamped from a NaN
+__device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
+__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
+
 template <typename T> __device__ __forceinline__ void load4(const T* p, int64_t i, int64_t n, bool aligned, float* o) {
   if (aligned && i + kOptVec <= n) {
     Vec4<T> v = *reinterpret_cast<const Vec4<T>*>(p + i);
@@ -362,10 +367,12 @@ fused_lars_norms_kernel(const OptTensor* __restrict__ table, float grad_scale, c
       reconcile4<P>(pv, wv);
     }
 #pragma unroll
-    for (int k = 0; k < kOptVec; ++k) {  // past the end both read as 0
-      const float d = gv[k] * grad_scale;
-      sw = fmaf(pv[k], pv[k], sw);
-      sg = fmaf(d, d, sg);
+    for (int k = 0; k < kOptVec; ++k) {
+      if (i + k < n) {  // past the end g reads as 0, and 0 * grad_scale is NaN for an infinite scale
+        const float d = gv[k] * grad_scale;
+        sw = fmaf(pv[k], pv[k], sw);
+        sg = fmaf(d, d, sg);
+      }
     }
   }
   // CTA partial: the tree of fused_lamb_norms_kernel
@@ -438,6 +445,8 @@ fused_lars_apply_kernel(const OptTensor* __restrict__ table, float lr, float mom
 //                        v = row_var * col_var / max(mean_r row_var, eps1)
 //   dim <= 1:            variance = lerp(variance, g^2, beta_w), v = variance
 //   u = g * rsqrt(max(v, eps1^2)), denom = max(1, ||u|| / (sqrt(n) * d)), w = w * (1 - lr * wd) - (alpha / denom) * u
+// The two clamps of v keep a NaN, as torch's clamp does; alpha's and denom's max drop one, as Python's max(eps2, nan) and
+// max(1, nan) do.
 // Five launches and no state between them: adafactor_stats_kernel (z = 0: one warp per row sums g^2 over the row and
 // lerps row_var; z = 1: one thread per (column, chunk of kAfRowChunk rows) writes a column partial),
 // adafactor_factors_kernel (z = 0: one thread per column adds its partials in fp64 in chunk order and lerps col_var;
@@ -471,7 +480,7 @@ __device__ __forceinline__ float af_vhat(const AdafactorGeom& gm, const float* _
 #pragma unroll
   for (int d = 0; d < 3; ++d) b = b * (unsigned)gm.size[d] + (o / (unsigned)gm.stride[d]) % (unsigned)gm.size[d];
   const float rv = gm.row_var[(size_t)b * gm.size[3] + r], cv = gm.col_var[(size_t)b * gm.size[4] + c];
-  return rv * cv / fmaxf(rmean[gm.batch_off + b], eps1);
+  return rv * cv / nan_max(rmean[gm.batch_off + b], eps1);
 }
 
 // u for 4 elements from the scaled gradient dv and, for dim <= 1 entries, the (lerped) variance vv; 0 past the end
@@ -482,7 +491,7 @@ __device__ __forceinline__ void af_u4(const AdafactorGeom& gm, const float* __re
     uv[k] = 0.f;
     if (i + k < n) {
       const float v = gm.row_var ? af_vhat(gm, rmean, (unsigned)(i + k), eps1) : vv[k];
-      uv[k] = dv[k] * rsqrtf(fmaxf(v, eps1_sq));
+      uv[k] = dv[k] * rsqrtf(nan_max(v, eps1_sq));
     }
   }
 }
@@ -665,10 +674,6 @@ struct UploadChunk { unsigned char b[kUploadChunk]; };
 __global__ void __launch_bounds__(kOptThreads) upload_bytes_kernel(unsigned char* __restrict__ dst, const UploadChunk c, int bytes) {
   for (int i = threadIdx.x; i < bytes; i += kOptThreads) dst[i] = c.b[i];
 }
-
-// max that keeps a NaN once it has seen one (fmaxf drops it), so an inf-norm of NaN gradients is NaN as in torch
-__device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
-__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
 
 // Gradient statistics of a table of flat gradient shards in one read pass: optional in-place scaling by *inv_scale, the
 // sum of squares (norm_inf = 0) or the max |g| (norm_inf = 1) of the scaled values as stored, and a non-finite flag.

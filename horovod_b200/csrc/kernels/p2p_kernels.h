@@ -249,7 +249,8 @@ cudaError_t LaunchLarsApply(const OptTensor* table, int n, int64_t max_count, fl
 // strides) in OptTensor::state0 and has row_var == nullptr here.  A parameter of dim 2..kAdafactorMaxDims is factored over
 // its last two dims [R, C], the leading dims (up to three, padded with 1 in front) forming a batch of B matrices:
 //   size, stride   the logical sizes [b0, b1, b2, R, C] and the parameter's element strides for them (any dense layout;
-//                  a dim of size 1 carries stride 1).  The parameter has fewer than 2^31 elements.
+//                  a dim of size 1 carries stride 1), each below 2^31.  The parameter has fewer than 2^32
+//                  elements: the kernels compute its element offsets in 32-bit unsigned arithmetic.
 //   row_var        fp32 [B, R], col_var fp32 [B, C], both contiguous (torch's [..., R, 1] and [..., 1, C])
 //   col_off        the entry's first column partial (B * C * AdafactorRowChunks(R) of them)
 //   batch_off      the entry's first per-batch mean of row_var (B of them)

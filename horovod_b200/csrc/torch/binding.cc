@@ -904,6 +904,18 @@ void FusedAdafactorStep(std::vector<at::Tensor> params, std::vector<at::Tensor> 
   TORCH_CHECK(step >= 1, op, ": step must be >= 1, got ", step);
   TORCH_CHECK(eps1 >= 0.0 && d > 0.0, op, ": eps1 must be >= 0 and d > 0, got eps1 = ", eps1, ", d = ", d);
   if (params.empty()) return;
+  // the kernels address a parameter's elements with 32-bit unsigned offsets, and the geometry of a factored parameter
+  // holds its sizes and strides as int32
+  for (size_t i = 0; i < params.size(); ++i) {
+    const at::Tensor& p = params[i];
+    TORCH_CHECK(p.numel() < ((int64_t)1 << 32), op, ": params[", i, "] has ", p.numel(),
+                " elements, at most 2^32 - 1 are supported");
+    if (p.dim() < 2) continue;
+    for (int64_t k = 0; k < p.dim(); ++k)
+      TORCH_CHECK(p.size(k) < ((int64_t)1 << 31) && (p.size(k) == 1 || p.stride(k) < ((int64_t)1 << 31)), op,
+                  ": params[", i, "] has size ", p.size(k), " and stride ", p.stride(k), " in dim ", k,
+                  ", at most 2^31 - 1 are supported in each dim of a factored parameter");
+  }
   // not zeroed yet: nothing is launched before every argument is checked
   at::Tensor norms = at::empty({2 * (int64_t)params.size()}, params[0].options().dtype(at::kFloat));
   OptPlan plan = PlanOpt(op, params, grads, {}, masters, grad_scale_dev, &norms, {}, EmaArgs{emas, ema_weight, ema_start});
@@ -916,8 +928,6 @@ void FusedAdafactorStep(std::vector<at::Tensor> params, std::vector<at::Tensor> 
       CheckAdafactorFactor(op, "col_vars", i, p, col_vars[i], -2);
       TORCH_CHECK(!(variances[i].has_value() && variances[i]->defined()), op, ": variances[", i,
                   "] is given for params[", i, "] of dim ", p.dim(), ", which keeps row / column factors");
-      TORCH_CHECK(p.numel() < ((int64_t)1 << 31), op, ": params[", i, "] has ", p.numel(), " elements, at most 2^31 - 1 ",
-                  "are supported for a factored parameter");
     } else {
       TORCH_CHECK(!(row_vars[i].has_value() && row_vars[i]->defined()) && !(col_vars[i].has_value() && col_vars[i]->defined()),
                   op, ": row_vars[", i, "] / col_vars[", i, "] are given for params[", i, "] of dim ", p.dim(),

@@ -176,11 +176,17 @@ def fused_adafactor_step(params, grads, row_vars, col_vars, variances, lr, beta2
         u = g * rsqrt(max(v, eps1^2));  denom = max(1, ||u|| / (sqrt(numel) * d))
         w = w * (1 - lr * weight_decay) - (alpha / denom) * u             (one fp32 expression, rounded once)
 
+    The max of the two clamps of v keeps a NaN (torch's clamp), the max in alpha and denom drops one (Python's max(eps2,
+    nan) and max(1, nan), as torch evaluates them): a NaN gradient element makes its row's and column's v NaN, and with
+    them the mean of row_var and so every v of that matrix, exactly where torch.optim.Adafactor gives NaN.
+
     `eps1=None` is torch.finfo(params' dtype).eps, as torch resolves it.  `master_params` and the EMA arguments as in
     fused_sgd_step.  Scratch comes from torch's caching allocator on the current stream; nothing is synchronised with the
     host, so the call can be captured into a CUDA graph.  Deterministic: the same input gives the same bits on every
     call, and a parameter's result does not depend on the other parameters of the call.  At most 65535 non-empty
-    parameters per call (one launch's grid); more raise RuntimeError before anything is launched."""
+    parameters per call (one launch's grid); each parameter must have fewer than 2^32 elements (the kernels' element
+    offsets are 32-bit), and a factored one sizes and strides below 2^31 in every dim.  A call past any of these limits
+    raises RuntimeError before anything is launched."""
     params = list(params)
     if eps1 is None:
         eps1 = torch.finfo(params[0].dtype).eps if params else 0.0

@@ -107,6 +107,92 @@ def adam_ref_kernel(p, g, m, v, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_dec
                     f32(grad_scale), bias)
 
 
+# ---- the float64 references of the fused LAMB, LARS and Adafactor updates --------------------------------------------
+def lamb_ref(cases, lr, beta1, beta2, eps, weight_decay, step, bias_correction=True, adapt=True, grad_scale=1.0,
+             fp32_moments=False):
+    """fp64 LAMB from the values the kernel reads (parameter and gradient in their dtypes, fp32 moments) and the
+    hyper-parameters as the kernel holds them (fp32).  'scale_*' bound the magnitudes that fp32 rounding errors are
+    relative to.  `fp32_moments`: m, v and v / c2 rounded to fp32 in the kernel's operation order, m = fmaf(b1, m,
+    (1 - b1) g), v = fmaf(b2, v, ((1 - b2) g) g) and sqrt(v / c2), for values that overflow fp32 where float64 would
+    not."""
+    out = []
+    b1, b2, lr, eps, wd = f32(beta1), f32(beta2), f32(lr), f32(eps), f32(weight_decay)
+    # as the binding forms them (and fused Adam's): 1 - (beta^step rounded to fp32), in fp32
+    c1, c2 = (float(np.float32(1) - np.float32(beta1 ** step)), float(np.float32(1) - np.float32(beta2 ** step))) \
+        if bias_correction else (1.0, 1.0)
+    for c in cases:
+        w, g = c['p'].t.double(), c['g'].t.double() * f32(grad_scale)
+        mo, vo = c['m'].t.double(), c['v'].t.double()
+        if fp32_moments:
+            f = lambda x: x.float().double()  # noqa: E731
+            m = f(b1 * mo + f(f32(1 - b1) * g))
+            v = f(b2 * vo + f(f(f32(1 - b2) * g) * g))
+            vc = f(v / c2)
+        else:
+            m = b1 * mo + f32(1 - b1) * g
+            v = b2 * vo + f32(1 - b2) * g * g
+            vc = v / c2
+        adam = (m / c1) / (vc.sqrt() + eps)
+        u = adam + wd * w
+        wn, un = float(w.norm()), float(u.norm())
+        r = wn / un if adapt and wn > 0 and un > 0 else 1.0
+        scale_m = (b1 * mo).abs() + (f32(1 - b1) * g).abs()  # >= |m|: m's rounding errors are relative to this
+        scale_u = (scale_m / c1) / (vc.sqrt() + eps) + (wd * w).abs()
+        out.append({'w': w - lr * r * u, 'm': m, 'v': v, 'scale_m': scale_m, 'scale_u': lr * r * scale_u})
+    return out
+
+
+def lars_ref(cases, lr, momentum, weight_decay, trust_coefficient, eps, adapt=True, grad_scale=1.0, fp32_norms=False):
+    """fp64 LARS from the values the kernel reads (parameter and gradient in their dtypes, fp32 momentum) and the
+    hyper-parameters as the kernel holds them (fp32).  'scale_v' bounds the magnitudes that fp32 rounding errors are
+    relative to.  `fp32_norms`: the sums of squares rounded to fp32, as the kernel stores them, so one past the fp32
+    maximum is inf (||g|| = inf gives r = 0)."""
+    lr, mom, wd, tc, eps = f32(lr), f32(momentum), f32(weight_decay), f32(trust_coefficient), f32(eps)
+    out = []
+    for c in cases:
+        w, g = c['p'].t.double(), c['g'].t.double() * f32(grad_scale)
+        vo = c['v'].t.double()
+        wn, gn = float(w.norm()), float(g.norm())
+        if fp32_norms:
+            wn, gn = (float(torch.tensor(x * x, dtype=torch.float64).float()) ** 0.5 for x in (wn, gn))
+        r = tc * wn / (gn + wd * wn + eps) if adapt and wn > 0 and gn > 0 else 1.0
+        d = g + wd * w
+        v = mom * vo + lr * r * d
+        scale_v = mom * vo.abs() + lr * r * (g.abs() + (wd * w).abs())
+        out.append({'w': w - v, 'v': v, 'scale_v': scale_v})
+    return out
+
+
+def adafactor_ref(c, lr, beta2_decay, eps1, eps2, d, weight_decay, step, grad_scale=1.0, fp32_squares=False):
+    """fp64 Adafactor from the values the kernel reads, with its fp32 hyper-parameters.  Returns the new parameter, its
+    state, and the magnitude |alpha / denom * u| (the update) that the rounding errors are relative to.
+    `fp32_squares`: g^2 rounded to fp32 as the kernel squares the scaled gradient, so a square past the fp32 maximum
+    is inf."""
+    pdt = c['p'].t.dtype
+    eps1 = torch.finfo(pdt).eps if eps1 is None else eps1
+    beta_w, rho = f32(step ** beta2_decay), f32(min(lr, 1 / step ** 0.5))
+    e1, e1sq, e2, dd, decay = f32(eps1), f32(eps1 * eps1), f32(eps2), f32(d), f32(1 - lr * weight_decay)
+    w, g = c['p'].t.double(), c['g'].t.double() * f32(grad_scale)
+    # torch's two-sided lerp, as torch.optim.Adafactor and the kernel use it: lerp(0, inf, 1) is NaN, not inf
+    lerp = lambda a, b: torch.lerp(a, b, beta_w)  # noqa: E731
+    sq = (g * g).float().double() if fp32_squares else g * g
+    out = {}
+    if w.dim() >= 2:
+        r = lerp(c['r'].t.double(), sq.mean(-1, keepdim=True))
+        col = lerp(c['c'].t.double(), sq.mean(-2, keepdim=True))
+        v = r * col / r.mean(-2, keepdim=True).clamp(min=e1)
+        out.update(r=r, c=col)
+    else:
+        v = out['v'] = lerp(c['v'].t.double(), sq)
+    u = g * v.clamp(min=e1sq).rsqrt()
+    n = max(w.numel(), 1)
+    alpha = max(e2, float(w.norm()) / n ** 0.5) * rho
+    denom = max(1.0, float(u.norm()) / (n ** 0.5 * dd))
+    out['p'] = w * decay - alpha / denom * u
+    out['scale'] = (alpha / denom * u).abs()
+    return out
+
+
 # ---- LAMB / LARS kernel cases -------------------------------------------------------------------------------------------
 def two_phase(kind, cases, master, gsd=None, **hp):
     """lamb_norms then lamb_apply (kind 'lamb') or lars_norms then lars_apply ('lars') over `cases`; returns the norms

@@ -9,8 +9,8 @@ import pytest
 import torch
 
 from conftest import run_parallel
-from optim_cases import (LOW, LOW_IDS, PAIR_IDS, PAIRS, SIZES, Slot, cat, f32, hvd, mlp, mlp_loss, ngpu, same,  # noqa: F401
-                         ulp)
+from optim_cases import (LOW, LOW_IDS, PAIR_IDS, PAIRS, SIZES, Slot, adafactor_ref, cat, f32, hvd, mlp,  # noqa: F401
+                         mlp_loss, ngpu, same, ulp)
 
 pytestmark = pytest.mark.gpu
 
@@ -62,32 +62,6 @@ def _run(cases, hp, step, master=False, **kw):
                              master_params=[c['w'].t for c in cases] if master else None, **hp, **kw)
 
 
-def _ref(c, lr, beta2_decay, eps1, eps2, d, weight_decay, step, grad_scale=1.0):
-    """fp64 Adafactor from the values the kernel reads, with its fp32 hyper-parameters.  Returns the new parameter, its
-    state, and the magnitude |alpha / denom * u| (the update) that the rounding errors are relative to."""
-    pdt = c['p'].t.dtype
-    eps1 = torch.finfo(pdt).eps if eps1 is None else eps1
-    beta_w, rho = f32(step ** beta2_decay), f32(min(lr, 1 / step ** 0.5))
-    e1, e1sq, e2, dd, decay = f32(eps1), f32(eps1 * eps1), f32(eps2), f32(d), f32(1 - lr * weight_decay)
-    w, g = c['p'].t.double(), c['g'].t.double() * f32(grad_scale)
-    lerp = lambda a, b: a + beta_w * (b - a)  # noqa: E731
-    out = {}
-    if w.dim() >= 2:
-        r = lerp(c['r'].t.double(), (g * g).mean(-1, keepdim=True))
-        col = lerp(c['c'].t.double(), (g * g).mean(-2, keepdim=True))
-        v = r * col / r.mean(-2, keepdim=True).clamp(min=e1)
-        out.update(r=r, c=col)
-    else:
-        v = out['v'] = lerp(c['v'].t.double(), g * g)
-    u = g * v.clamp(min=e1sq).rsqrt()
-    n = max(w.numel(), 1)
-    alpha = max(e2, float(w.norm()) / n ** 0.5) * rho
-    denom = max(1.0, float(u.norm()) / (n ** 0.5 * dd))
-    out['p'] = w * decay - alpha / denom * u
-    out['scale'] = (alpha / denom * u).abs()
-    return out
-
-
 def _tol_rel(shape):
     """Relative error bound of the update alpha / denom * u.  v: a row sum of C squares in fp32 (C / 32 fmas per lane and a
     5-level tree), a column sum of 64-row chunks in fp32 added in fp64, the row mean in fp64, lerps (3 roundings each),
@@ -102,7 +76,7 @@ def _tol_rel(shape):
 def _check(cases, hp, step, before):
     pdt = cases[0]['p'].t.dtype
     for i, (c, b) in enumerate(zip(cases, before)):
-        want = _ref(b, step=step, **hp)
+        want = adafactor_ref(b, step=step, **hp)
         got = c['p'].t.double()
         tol = want['scale'] * _tol_rel(c['p'].t.shape) + want['p'].abs() * 2 * U + ulp(want['p'], torch.float32)
         if pdt != torch.float32:

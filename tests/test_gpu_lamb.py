@@ -11,8 +11,8 @@ import pytest
 import torch
 
 from conftest import run_parallel
-from optim_cases import (LOW, LOW_IDS, PAIR_IDS, PAIRS, SIZES, Slot, cat, f32, hvd, mlp, mlp_loss, ngpu,  # noqa: F401
-                         same, two_phase, ulp)
+from optim_cases import (LOW, LOW_IDS, PAIR_IDS, PAIRS, SIZES, Slot, cat, f32, hvd, lamb_ref, mlp, mlp_loss,  # noqa: F401
+                         ngpu, same, two_phase, ulp)
 from sim_ranks import FakeSet, NormConvNet, batch, reduced_grads, ref_step, sharded_team, step_all, team  # noqa: F401
 
 pytestmark = pytest.mark.gpu
@@ -39,35 +39,11 @@ def _case(shape, pdt, gdt, seed, offsets=(0, 0, 0), memory_format=torch.contiguo
     return c
 
 
-def _ref(cases, lr, beta1, beta2, eps, weight_decay, step, bias_correction=True, adapt=True, grad_scale=1.0):
-    """fp64 LAMB from the values the kernel reads (parameter and gradient in their dtypes, fp32 moments) and the
-    hyper-parameters as the kernel holds them (fp32).  'scale_*' bound the magnitudes that fp32 rounding errors are
-    relative to."""
-    out = []
-    b1, b2, lr, eps, wd = f32(beta1), f32(beta2), f32(lr), f32(eps), f32(weight_decay)
-    # as the binding forms them (and fused Adam's): 1 - (beta^step rounded to fp32), in fp32
-    c1, c2 = (float(np.float32(1) - np.float32(beta1 ** step)), float(np.float32(1) - np.float32(beta2 ** step))) \
-        if bias_correction else (1.0, 1.0)
-    for c in cases:
-        w, g = c['p'].t.double(), c['g'].t.double() * f32(grad_scale)
-        mo, vo = c['m'].t.double(), c['v'].t.double()
-        m = b1 * mo + f32(1 - b1) * g
-        v = b2 * vo + f32(1 - b2) * g * g
-        adam = (m / c1) / ((v / c2).sqrt() + eps)
-        u = adam + wd * w
-        wn, un = float(w.norm()), float(u.norm())
-        r = wn / un if adapt and wn > 0 and un > 0 else 1.0
-        scale_m = (b1 * mo).abs() + (f32(1 - b1) * g).abs()  # >= |m|: m's rounding errors are relative to this
-        scale_u = (scale_m / c1) / ((v / c2).sqrt() + eps) + (wd * w).abs()
-        out.append({'w': w - lr * r * u, 'm': m, 'v': v, 'scale_m': scale_m, 'scale_u': lr * r * scale_u})
-    return out
-
-
 def _run_and_check(cases, hp, step):
     from horovod_b200 import ops
     pdt = cases[0]['p'].t.dtype
     hp = dict(hp)
-    want = _ref(cases, step=step, **hp)
+    want = lamb_ref(cases, step=step, **hp)
     g_before = [c['g'].t.clone() for c in cases]
     ops.fused_lamb_step([c['p'].t for c in cases], [c['g'].t for c in cases], [c['m'].t for c in cases],
                         [c['v'].t for c in cases], step=step, **hp)

@@ -10,8 +10,8 @@ import pytest
 import torch
 
 from conftest import run_parallel
-from optim_cases import (LOW, LOW_IDS, PAIR_IDS, PAIRS, SIZES, Slot, cat, f32, hvd, mlp, mlp_loss, ngpu,  # noqa: F401
-                         same, two_phase, ulp)
+from optim_cases import (LOW, LOW_IDS, PAIR_IDS, PAIRS, SIZES, Slot, cat, f32, hvd, lars_ref, mlp, mlp_loss,  # noqa: F401
+                         ngpu, same, two_phase, ulp)
 from sim_ranks import FakeSet, NormConvNet, batch, reduced_grads, ref_step, sharded_team, step_all, team  # noqa: F401
 
 pytestmark = pytest.mark.gpu
@@ -44,28 +44,10 @@ def _case(shape, pdt, gdt, seed, offsets=(0, 0, 0), memory_format=torch.contiguo
     return c
 
 
-def _ref(cases, lr, momentum, weight_decay, trust_coefficient, eps, adapt=True, grad_scale=1.0):
-    """fp64 LARS from the values the kernel reads (parameter and gradient in their dtypes, fp32 momentum) and the
-    hyper-parameters as the kernel holds them (fp32).  'scale_v' bounds the magnitudes that fp32 rounding errors are
-    relative to."""
-    lr, mom, wd, tc, eps = f32(lr), f32(momentum), f32(weight_decay), f32(trust_coefficient), f32(eps)
-    out = []
-    for c in cases:
-        w, g = c['p'].t.double(), c['g'].t.double() * f32(grad_scale)
-        vo = c['v'].t.double()
-        wn, gn = float(w.norm()), float(g.norm())
-        r = tc * wn / (gn + wd * wn + eps) if adapt and wn > 0 and gn > 0 else 1.0
-        d = g + wd * w
-        v = mom * vo + lr * r * d
-        scale_v = mom * vo.abs() + lr * r * (g.abs() + (wd * w).abs())
-        out.append({'w': w - v, 'v': v, 'scale_v': scale_v})
-    return out
-
-
 def _run_and_check(cases, hp):
     from horovod_b200 import ops
     pdt = cases[0]['p'].t.dtype
-    want = _ref(cases, **hp)
+    want = lars_ref(cases, **hp)
     g_before = [c['g'].t.clone() for c in cases]
     ops.fused_lars_step([c['p'].t for c in cases], [c['g'].t for c in cases], [c['v'].t for c in cases], **hp)
     torch.cuda.synchronize()
