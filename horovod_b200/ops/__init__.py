@@ -10,6 +10,8 @@
 * `grad_accumulate_` — folds bf16 / fp16 gradients into fp32 accumulators for gradient accumulation (same file);
 * `sync_bn_stats`, `sync_bn_combine`, `sync_bn_elemt`, `sync_bn_backward_reduce`, `sync_bn_backward_elemt` — the
   kernels of hvd.SyncBatchNorm's native path (`csrc/kernels/sync_bn_kernels.cu`);
+* `moe_permute`, `moe_scatter`, `moe_gather`, `moe_regroup`, `moe_regroup_reverse` — the local data movement of
+  hvd.ExpertDispatcher (`csrc/kernels/moe_kernels.cu`);
 * `symm_empty`, `symm_available` — registered symmetric memory for the zero-copy allreduce path;
 * `sim` — the single-GPU simulation harness (N ranks = N concurrently running kernels on one device) used by the
   numerics tests, `bench/kernel_micro.py` and the ncu captures;
@@ -290,6 +292,52 @@ def sync_bn_backward_elemt(grad_output, x, mean, invstd, weight, sums, count):
     """dx = (dy - sum_dy / n - (x - mean) * invstd^2 * sum_dy_xmu / n) * invstd * weight, with the summed `sums` of
     sync_bn_backward_reduce and n = count[0] of sync_bn_combine.  One launch."""
     return _native().sync_bn_backward_elemt(grad_output, x, mean, invstd, weight, sums, count)
+
+
+def moe_permute(x, expert_idx, num_experts, nranks, send, counts, ctas=0):
+    """The dispatch's first step, in three launches: the stable order of the [T, k] assignments by expert (expert
+    ascending, then t * k + j ascending: torch.argsort(expert_idx.flatten(), stable=True)) and the copy of x[t] to the
+    send rows of its k assignments.  x [T, hidden] and send [R >= T * k, hidden]: contiguous, one dtype (fp32 / bf16 /
+    fp16).  expert_idx: int32 / int64 [T, k], 1 <= k <= 16.  counts: int64 [num_experts], receives this rank's count per
+    expert.  Returns (pos, splits): pos int32 [T, k], the send row of each assignment; splits int32 [nranks], the rows
+    for each rank's num_experts / nranks experts.  An id outside [0, num_experts) makes every split -1 and every count
+    0.  Nothing is synchronised with the host; the same input gives the same bits on every call."""
+    return tuple(_native().moe_permute(x, expert_idx, send, counts, int(num_experts), int(nranks), int(ctas)))
+
+
+def moe_scatter(src, pos, dst, gates=None, dot_rows=None, status=None, ctas=0):
+    """dst[pos[t, j]] = src[t] for every t < T and j < k (the bytes as they are), or with `gates` ([T, k], fp32 or src's
+    dtype) round(gates[t, j] * src[t]) computed in fp32.  With `dot_rows` (rows like dst) also returns grad_gates [T, k]
+    in the gates' dtype: grad_gates[t, j] = the fp32 dot of src[t] and dot_rows[pos[t, j]], summed in an order that
+    depends on the row length only.  Positions outside dst's rows are skipped.  A non-zero status[0] (int32 on the
+    device) writes no row and zero gate gradients.  One launch; returns grad_gates or None."""
+    return _native().moe_scatter(src, pos, dst, gates, dot_rows, status, int(ctas))
+
+
+def moe_gather(src, pos, gates=None, status=None, ctas=0):
+    """y[t] = sum over j ascending of gates[t, j] * src[pos[t, j]], in fp32 (each product rounded, then added), rounded
+    once to src's dtype; without gates a plain fp32 sum in j order.  Positions outside src's rows add nothing; a non-zero
+    status[0] gives y = 0.  One launch; returns y [T, hidden]."""
+    return _native().moe_gather(src, pos, gates, status, int(ctas))
+
+
+def moe_regroup(src, counts, status=None, out=None, ctas=0):
+    """Received rows grouped by source rank (rank 0's rows for local experts 0, 1, ..., then rank 1's, ...) to rows
+    grouped by local expert, then source rank, keeping the senders' order.  counts: int64 [nranks, experts_per_rank],
+    counts[p, e] the rows from rank p for local expert e.  Rows of `out` (default: new, like src) past the total are
+    zeroed; all of them when status[0] is non-zero.  out may be src itself with one expert per rank (the order is the
+    same; only the tail is written).  One launch; returns (out, offsets), offsets int32 [experts_per_rank] the end row of
+    each group (torch._grouped_mm's `offs`)."""
+    if out is None:
+        out = torch.empty_like(src)
+    return out, _native().moe_regroup(src, counts, status, out, False, int(ctas))
+
+
+def moe_regroup_reverse(src, counts, out, status=None, ctas=0):
+    """The inverse of moe_regroup: rows grouped by local expert back to source-rank order, into `out` (rows like src;
+    only the rows below the total are written).  One launch; returns the return splits, int32 [nranks]: the rows of
+    each source rank, all zero when status[0] is non-zero."""
+    return _native().moe_regroup(src, counts, status, out, True, int(ctas))
 
 
 def symm_empty(*args, **kwargs):

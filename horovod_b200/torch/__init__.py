@@ -27,4 +27,5 @@ from horovod_b200.torch.optimizer import DistributedOptimizer  # noqa: F401
 from horovod_b200.torch.sharded_optimizer import ShardedGradScaler  # noqa: F401
 from horovod_b200.torch.sync_batch_norm import SyncBatchNorm  # noqa: F401
 from horovod_b200.torch.graph import GraphedStep  # noqa: F401
+from horovod_b200.torch.moe import ExpertDispatcher  # noqa: F401
 from horovod_b200.torch import elastic  # noqa: F401
