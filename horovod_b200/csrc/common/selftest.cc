@@ -567,16 +567,18 @@ void TestEngines(int n, int planes = 0) {   // 0: loopback only, 1: one host's s
       }
       // duplicate name while in flight is rejected locally
       {
-        std::vector<float> big(1 << 16, 1.f);
+        // When the first "dup" has already finished, the second is accepted and stays in flight past this scope (it runs
+        // once the other ranks send a second "dup" or join), so its callback owns the buffer the engine still reads.
+        auto big = std::make_shared<std::vector<float>>(1 << 16, 1.f);
         auto ent = std::make_shared<TensorTableEntry>();
-        ent->name = "dup"; ent->input = big.data(); ent->output = big.data(); ent->dtype = DataType::FLOAT32;
-        ent->shape = TensorShape({(int64_t)big.size()}); ent->reduce_op = ReduceOp::SUM;
+        ent->name = "dup"; ent->input = big->data(); ent->output = big->data(); ent->dtype = DataType::FLOAT32;
+        ent->shape = TensorShape({(int64_t)big->size()}); ent->reduce_op = ReduceOp::SUM;
         std::promise<Status> p;
         ent->callback = [&p](const Completion& c) { p.set_value(c.status); };
         std::vector<std::shared_ptr<TensorTableEntry>> es{ent};
         Status st1 = e.EnqueueAllreduces(es, 0);
         auto ent2 = std::make_shared<TensorTableEntry>(*ent);
-        ent2->callback = [](const Completion&) {};
+        ent2->callback = [big](const Completion&) {};
         std::vector<std::shared_ptr<TensorTableEntry>> es2{ent2};
         Status st2 = e.EnqueueAllreduces(es2, 0);
         p.get_future().get();

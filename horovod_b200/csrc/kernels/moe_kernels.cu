@@ -309,7 +309,8 @@ moe_scatter_kernel(const T* __restrict__ src, int64_t ntok, int k, int64_t h, co
 
 // ---- gather ---------------------------------------------------------------------------------------------------------
 // One warp per token t: y[t] = round(sum_j g_j * src[pos[t * k + j]]) with the sum in fp32, j ascending (g_j = 1 without
-// gates: a plain sum).  Positions outside [0, src_rows) add nothing; a non-zero *status gives y = 0.
+// gates: a plain sum).  Positions outside [0, src_rows) add nothing; a token with none inside, or a non-zero *status,
+// gives y = +0 (the empty sum).
 template <typename T, typename G>
 __global__ void __launch_bounds__(kMoeThreads)
 moe_gather_kernel(const T* __restrict__ src, int64_t src_rows, const int* __restrict__ pos, int k, int64_t ntok, int64_t h,
@@ -326,11 +327,13 @@ moe_gather_kernel(const T* __restrict__ src, int64_t src_rows, const int* __rest
 #pragma unroll
       for (int u = 0; u < kMoeUnroll; ++u)
 #pragma unroll
-        for (int i = 0; i < V; ++i) acc[u][i] = dead ? 0.f : -0.f;  // -0 + x == x for every x: the sum starts at term 0
+        for (int i = 0; i < V; ++i) acc[u][i] = -0.f;  // -0 + x == x for every x: the sum starts at term 0
+      bool any = false;  // whether some j was in range (warp-uniform)
       if (!dead) {
         for (int j = 0; j < k; ++j) {
           const int p = pos[t * k + j];
           if (p < 0 || p >= src_rows) continue;
+          any = true;
           const T* r = src + (int64_t)p * h;
           const bool vr = aligned16(r);
           const float g = gates ? to_f(gates[t * k + j]) : 1.f;
@@ -344,6 +347,11 @@ moe_gather_kernel(const T* __restrict__ src, int64_t src_rows, const int* __rest
             for (int i = 0; i < V; ++i) acc[u][i] = __fadd_rn(acc[u][i], gates ? __fmul_rn(g, v[u][i]) : v[u][i]);
         }
       }
+      if (!any)
+#pragma unroll
+        for (int u = 0; u < kMoeUnroll; ++u)
+#pragma unroll
+          for (int i = 0; i < V; ++i) acc[u][i] = 0.f;
 #pragma unroll
       for (int u = 0; u < kMoeUnroll; ++u)
         if (c0 + 32 * u < nch) st_chunk(yr, c0 + 32 * u, h, vy, acc[u]);

@@ -316,8 +316,8 @@ def moe_scatter(src, pos, dst, gates=None, dot_rows=None, status=None, ctas=0):
 
 def moe_gather(src, pos, gates=None, status=None, ctas=0):
     """y[t] = sum over j ascending of gates[t, j] * src[pos[t, j]], in fp32 (each product rounded, then added), rounded
-    once to src's dtype; without gates a plain fp32 sum in j order.  Positions outside src's rows add nothing; a non-zero
-    status[0] gives y = 0.  One launch; returns y [T, hidden]."""
+    once to src's dtype; without gates a plain fp32 sum in j order.  Positions outside src's rows add nothing (a token
+    with none inside gets +0, the empty sum); a non-zero status[0] gives y = +0.  One launch; returns y [T, hidden]."""
     return _native().moe_gather(src, pos, gates, status, int(ctas))
 
 

@@ -12,6 +12,7 @@
   the operation's own tests.  Gathers from a large tensor go through views of one chunk each (`_take`).
 """
 import gc
+import time
 
 import numpy as np
 import pytest
@@ -549,3 +550,207 @@ def test_large_inplace_reducescatter_allgather_bf16(room):
         assert same(_take(t, idx), reduced), 'allgather at the windows'
     for a, b in _chunks(n):
         assert same(ts[0][a:b], ts[1][a:b]), ('allgather: the ranks differ', a)
+
+
+# ---- expert-parallel dispatch (moe_kernels.cu) and the captured alltoall past 2^31 --------------------------------------
+
+def _peak(what, t0):
+    """Prints the wall time since t0 and the peak device memory of the test, for the record."""
+    torch.cuda.synchronize()
+    print(f'\n{what}: {time.perf_counter() - t0:.1f} s, peak {torch.cuda.max_memory_allocated() / GiB:.1f} GiB')
+
+
+def _seeded_ints(t, seed, high):
+    """Fills a 1-D integer tensor in place with seeded values in [0, high), chunk by chunk."""
+    for k, (a, b) in enumerate(_chunks(t.numel())):
+        g = torch.Generator(device='cuda').manual_seed(1000 * seed + k)
+        t[a:b].copy_(torch.randint(0, high, (b - a,), device='cuda', generator=g, dtype=t.dtype))
+
+
+def test_large_moe_permute_bf16(room):
+    """Needs 30 GiB.  moe_permute at the binding's limit: T k = 2^31 - 16 assignments (k = 16, int32 ids over E = 8
+    experts, n = 4 ranks) of bf16 rows of h = 3 (6 bytes, the element path), so the send buffer passes 2^31 elements
+    and 2^33 bytes.  The counts against bincount in chunks, the splits, and for every chunk and expert that the positions
+    of that expert's assignments, ascending, are exactly base_e, base_e + 1, ... (the stable argsort, checked without a
+    global sort); send[pos[a]] == x[a // k] at the windows.  Prints the call's time: the last route CTA scans the 2^20
+    tiles serially per expert."""
+    from horovod_b200 import ops
+    room(30 * GiB)
+    torch.cuda.reset_peak_memory_stats()
+    t_start = time.perf_counter()
+    k, E, n, h = 16, 8, 4, 3
+    A = B31 - 16
+    T = A // k
+    ids = torch.empty(A, dtype=torch.int32, device='cuda')
+    _seeded_ints(ids, 40, E)
+    x = torch.empty(T * h, dtype=torch.bfloat16, device='cuda')
+    _fill(x, 41)
+    x = x.view(T, h)
+    send = torch.empty(A, h, dtype=torch.bfloat16, device='cuda')
+    counts = torch.full((E,), -5, dtype=torch.int64, device='cuda')
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    pos, splits = ops.moe_permute(x, ids.view(T, k), E, n, send, counts)
+    torch.cuda.synchronize()
+    print(f'\nmoe_permute of {A} assignments: {time.perf_counter() - t0:.2f} s')
+    want = sum(torch.bincount(ids[a:b], minlength=E) for a, b in _chunks(A))
+    assert torch.equal(counts, want), (counts.tolist(), want.tolist())
+    assert splits.tolist() == want.view(n, -1).sum(1).tolist()
+    base = torch.cumsum(want, 0) - want
+    flat = pos.view(-1)
+    seen = [0] * E
+    for a, b in _chunks(A):
+        chunk_ids, chunk_pos = ids[a:b], flat[a:b]
+        for e in range(E):
+            got = chunk_pos[chunk_ids == e].long()
+            start = int(base[e]) + seen[e]
+            assert torch.equal(got, torch.arange(start, start + got.numel(), device='cuda')), ('stable order', a, e)
+            seen[e] += got.numel()
+    assert seen == want.tolist()
+    idx = _windows(A)
+    p = _take(flat, idx).long()
+    for c in range(h):
+        assert same(_take(send, p * h + c), _take(x, (idx // k) * h + c)), ('send rows', c)
+    assert int(p.max()) * h > (1 << 32), 'the windows reach a send row past element 2^32'
+    _peak('test_large_moe_permute_bf16', t_start)
+
+
+def _rows_at(t, rows):
+    """t[rows] for a 2-D tensor of more than 2^31 elements, one row view at a time."""
+    return torch.stack([t[r] for r in rows.tolist()])
+
+
+@pytest.mark.parametrize("h", [1 << 15, (1 << 15) + 3], ids=['vector', 'element'])
+def test_large_moe_scatter_gather_regroup_bf16(room, h):
+    """Needs 30 GiB.  T = 2^16 + 1 bf16 tokens of h = 2^15 (16 B rows, the vector path) or 2^15 + 3 (the element path),
+    k = 2 over 4 experts: x passes 2^31 elements and the send buffer 2^32.  Checked at the tokens whose rows straddle
+    element 2^31, whose send rows lie past element 2^32, the last token and 64 random ones:
+    - moe_permute's copy: send[pos[t, j]] == x[t];
+    - the weighted gather, bit-exact to the fp32 model and within the float64 bound;
+    - the scaled scatter, bit-exact, and its gate-gradient dot within dot_bound;
+    - the regroup with counts [4, 8] at sampled rows against a host-computed row map, and its reverse as the exact
+      inverse, chunk by chunk."""
+    from horovod_b200 import ops
+    from test_gpu_moe_dispatch import dot_bound, ref_gather
+    from test_gpu_moe_edges import check_value, gather64, same_bits
+    room(30 * GiB)
+    torch.cuda.reset_peak_memory_stats()
+    t_start = time.perf_counter()
+    T, k, E = (1 << 16) + 1, 2, 4
+    R = T * k
+    x = torch.empty(T * h, dtype=torch.bfloat16, device='cuda')
+    _fill(x, 50)
+    x = x.view(T, h)
+    ids = torch.randint(0, E, (T, k), device='cuda', generator=torch.Generator(device='cuda').manual_seed(51))
+    send = torch.empty(R, h, dtype=torch.bfloat16, device='cuda')
+    pos, _ = ops.moe_permute(x, ids, E, 1, send, torch.empty(E, dtype=torch.int64, device='cuda'))
+    gates = torch.rand(T, k, device='cuda', generator=torch.Generator(device='cuda').manual_seed(52))
+    y = ops.moe_gather(send, pos, gates)
+    dst = torch.zeros(R, h, dtype=torch.bfloat16, device='cuda')
+    gg = ops.moe_scatter(x, pos, dst, gates, send)
+    torch.cuda.synchronize()
+    far = ((pos.long() + 1) * h > (1 << 32)).any(1).nonzero().flatten()  # a send row reaching past element 2^32
+    assert far.numel() > 0
+    toks = torch.cat([torch.arange(B31 // h - 1, B31 // h + 2, device='cuda'), far, torch.tensor([T - 1], device='cuda'),
+                      torch.randint(0, T, (64,), device='cuda', generator=torch.Generator(device='cuda').manual_seed(53))])
+    toks = toks[toks < T].unique()
+    xt, pt, gt = _rows_at(x, toks), pos[toks], gates[toks]
+    rows = [_rows_at(send, pt[:, j]) for j in range(k)]
+    for j in range(k):
+        assert same(rows[j], xt), ('send rows', j)
+    local = torch.cat(rows)  # the k send rows of each token, as a small src with pos = j * len(toks) + i
+    lpos = torch.stack([torch.arange(len(toks), device='cuda') + j * len(toks) for j in range(k)], 1).to(torch.int32)
+    yt = _rows_at(y, toks)
+    assert same_bits(yt, ref_gather(local, lpos, gt, torch.bfloat16)), 'gather bits'
+    w64, bound = gather64(local, lpos, gt)
+    check_value(yt, w64, bound, 'gather value')
+    for j in range(k):
+        assert same(_rows_at(dst, pt[:, j]), (gt[:, j:j + 1] * xt.float()).to(torch.bfloat16)), ('scatter', j)
+        exact = (xt.double() * rows[j].double()).sum(-1)
+        assert bool(((gg[toks, j].double() - exact).abs() <= dot_bound(xt, rows[j])).all()), ('gate gradient', j)
+    del y, dst, gg
+    gc.collect()
+    torch.cuda.empty_cache()
+    # regroup: 4 source ranks x 8 local experts, 5 rows short of R, some segments empty
+    g = torch.Generator().manual_seed(54)
+    wts = torch.rand(32, generator=g) * (torch.rand(32, generator=g) > 0.25)
+    c = (wts / wts.sum() * (R - 5)).floor().long()
+    c[int(wts.argmax())] += R - 5 - int(c.sum())
+    counts = c.view(4, 8)
+    total = int(counts.sum())
+    out, offsets = ops.moe_regroup(send, counts.cuda())
+    torch.cuda.synchronize()
+    cl = counts.tolist()
+    src_start, at = {}, 0
+    for p in range(4):
+        for e in range(8):
+            src_start[(p, e)], at = at, at + cl[p][e]
+    row_map, ends = [], []
+    for e in range(8):
+        for p in range(4):
+            row_map += range(src_start[(p, e)], src_start[(p, e)] + cl[p][e])
+        ends.append(len(row_map))
+    assert offsets.tolist() == ends
+    sample = torch.cat([torch.arange(0, 16), torch.arange(B31 // h - 2, B31 // h + 3), torch.arange((1 << 32) // h - 2, R),
+                        torch.randint(0, R, (128,), generator=g)]).unique()
+    sample = sample[sample < R]
+    inside = sample[sample < total]
+    assert same(_rows_at(out, inside.cuda()), _rows_at(send, torch.tensor([row_map[r] for r in inside.tolist()]).cuda()))
+    assert not bool(out[total:].view(torch.int16).any()), 'tail not zeroed'
+    back = torch.full_like(send, 3.0)
+    ret = ops.moe_regroup_reverse(out, counts.cuda(), back)
+    torch.cuda.synchronize()
+    assert ret.tolist() == counts.sum(1).tolist()
+    flat_b, flat_s = back.view(-1), send.view(-1)
+    for a, b in _chunks(total * h):
+        assert same(flat_b[a:b], flat_s[a:b]), ('reverse is not the inverse', a)
+    assert bool((back[total:] == 3.0).all()), 'reverse wrote past the total'
+    _peak(f'test_large_moe_scatter_gather_regroup_bf16[{h}]', t_start)
+
+
+def _seeded_bytes(seed, k, length):
+    g = torch.Generator(device='cuda').manual_seed(1000 * seed + k)
+    return torch.randint(0, 256, (length,), dtype=torch.uint8, device='cuda', generator=g)
+
+
+@pytest.mark.parametrize("R,row", [(530000, 4098), (265000, 8192)], ids=['bytes', 'vector'])
+def test_large_captured_alltoall(room, R, row):
+    """Needs 10 GiB.  The captured alltoall on 2 simulated ranks whose inputs are each just over 2^31 bytes: R rows of
+    4098 bytes (unaligned rows, the byte path) or of 8192 bytes (the 16 B vector path), splits [[R - 1000, 1000],
+    [R - 500, 500]], so rank 0's output passes byte 2^32 and both source offsets rank 1 reads are past 2^31.  The output
+    byte for byte against the inputs, chunk by chunk on the device, the guard rows after it untouched, and the inputs
+    unchanged against their seeded fill."""
+    from horovod_b200.ops import sim
+    room(10 * GiB)
+    torch.cuda.reset_peak_memory_stats()
+    t_start = time.perf_counter()
+    assert R * row > B31
+    M = [[R - 1000, 1000], [R - 500, 500]]
+    ins = [torch.empty(R, row, dtype=torch.uint8, device='cuda') for _ in range(2)]
+    for r, t in enumerate(ins):
+        for i, (a, b) in enumerate(_chunks(t.numel())):
+            t.view(-1)[a:b] = _seeded_bytes(60 + r, i, b - a)
+    recv_rows = [M[0][q] + M[1][q] for q in range(2)]
+    outs = [torch.full((recv_rows[q] + 3, row), 0x5A, dtype=torch.uint8, device='cuda') for q in range(2)]
+    assert recv_rows[0] * row > (1 << 32)
+    splits = [torch.tensor(m, dtype=torch.int64, device='cuda') for m in M]
+    recv = [torch.full((2,), -7, dtype=torch.int64, device='cuda') for _ in range(2)]
+    status = [torch.full((1,), -7, dtype=torch.int32, device='cuda') for _ in range(2)]
+    sim.captured_alltoall(ins, splits, outs, recv, status, ctas=8)
+    torch.cuda.synchronize()
+    assert [int(s) for s in status] == [0, 0]
+    assert recv[0].tolist() == [M[0][0], M[1][0]] and recv[1].tolist() == [M[0][1], M[1][1]]
+    # (output q, its first row, sender p, the sender's first row, rows)
+    pieces = [(0, 0, 0, 0, M[0][0]), (0, M[0][0], 1, 0, M[1][0]), (1, 0, 0, M[0][0], M[0][1]),
+              (1, M[0][1], 1, M[1][0], M[1][1])]
+    for q, o0, p, i0, n in pieces:
+        dst, src = outs[q].view(-1)[o0 * row:(o0 + n) * row], ins[p].view(-1)[i0 * row:(i0 + n) * row]
+        for a, b in _chunks(n * row):
+            assert torch.equal(dst[a:b], src[a:b]), ('output', q, p, a)
+    assert (M[0][0] * row > B31) and (M[1][0] * row > B31)
+    for q in range(2):
+        assert bool((outs[q][recv_rows[q]:] == 0x5A).all()), ('guard rows', q)
+    for r, t in enumerate(ins):
+        for i, (a, b) in enumerate(_chunks(t.numel())):
+            assert torch.equal(t.view(-1)[a:b], _seeded_bytes(60 + r, i, b - a)), ('input written', r, a)
+    _peak(f'test_large_captured_alltoall[{row}]', t_start)
