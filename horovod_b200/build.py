@@ -68,7 +68,9 @@ def _run(cmd):
     return r.stdout
 
 
-def _compile(src, stamp, force, verbose):
+def _compile(src, stamp, force, verbose, cxx=None):
+    """Compiles one source into build/obj unless its content stamp is unchanged.  `cxx`: the compiler command for a .cc
+    file without its input and output (default: the runtime's)."""
     rel = os.path.relpath(src, CSRC).replace("/", "__")
     obj = os.path.join(OBJ, rel + ".o")
     stamp = _src_stamp(src, stamp)
@@ -79,6 +81,8 @@ def _compile(src, stamp, force, verbose):
         cmd = [NVCC] + ARCH + ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"] + inc + ["-c", src, "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
+    elif cxx is not None:
+        cmd = cxx + ["-c", src, "-o", obj]
     else:
         # the host reduction / scaling loops of ops/ want the vectoriser (-O3); the rest of the runtime is control flow
         opt = "-O3" if os.sep + "ops" + os.sep in src else "-O2"
@@ -101,7 +105,9 @@ def build_core(force=False, verbose=False):
     with ThreadPoolExecutor(max_workers=max(2, os.cpu_count() or 4)) as ex:
         objs = list(ex.map(lambda s: _compile(s, stamp, force, verbose), cu + cc))
     lib = os.path.join(OUT, "libhvd_core.so")
-    link_stamp = hashlib.sha1("".join(sorted(f for f in os.listdir(OBJ) if ".o." in f)).encode()).hexdigest()[:16]
+    # the stamps of the runtime's objects only (build_torch keeps the binding's torch__*.o next to them)
+    link_stamp = hashlib.sha1("".join(sorted(f for f in os.listdir(OBJ) if ".o." in f and not f.startswith("torch__")))
+                              .encode()).hexdigest()[:16]
     stamp_file = os.path.join(OBJ, "core_link.stamp")
     old = open(stamp_file).read() if os.path.exists(stamp_file) else ""
     if force or not os.path.exists(lib) or old != link_stamp:
@@ -122,12 +128,17 @@ def build_torch(force=False):
     import torch
     from torch.utils import cpp_extension
 
-    src = os.path.join(CSRC, "torch", "binding.cc")
+    tdir = os.path.join(CSRC, "torch")
+    srcs = [os.path.join(tdir, f) for f in sorted(os.listdir(tdir)) if f.endswith(".cc")]
     lib = os.path.join(OUT, "_hvd_torch.so")
-    core = os.path.join(OUT, "libhvd_core.so")
+    os.makedirs(OBJ, exist_ok=True)
     stamp_file = os.path.join(OBJ, "torch_binding.stamp")
     core_stamp = os.path.join(OBJ, "core_link.stamp")
-    stamp = _src_stamp(src, _header_digest()) + "-" + torch.__version__ + "-" + (open(core_stamp).read() if os.path.exists(core_stamp) else "")
+    # the binding's sources are compiled against the torch headers: a torch upgrade rebuilds every object
+    hstamp = _header_digest() + torch.__version__
+    src_stamps = "".join(_src_stamp(s, hstamp) for s in srcs)
+    stamp = hashlib.sha1(src_stamps.encode()).hexdigest()[:16] + "-" + torch.__version__ + "-" + (
+        open(core_stamp).read() if os.path.exists(core_stamp) else "")
     old = open(stamp_file).read() if os.path.exists(stamp_file) else ""
     if not force and os.path.exists(lib) and old == stamp:
         return lib
@@ -135,12 +146,13 @@ def build_torch(force=False):
                                                                "-I" + sysconfig.get_paths()["include"]]
     tlib = os.path.join(os.path.dirname(torch.__file__), "lib")
     abi = int(torch._C._GLIBCXX_USE_CXX11_ABI) if hasattr(torch._C, "_GLIBCXX_USE_CXX11_ABI") else 1
-    cmd = ["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-pthread", "-DTORCH_EXTENSION_NAME=_hvd_torch",
-           "-DTORCH_API_INCLUDE_EXTENSION_H", "-D_GLIBCXX_USE_CXX11_ABI=%d" % abi, "-Wno-deprecated-declarations"] + inc + [
-               src, "-o", lib, "-L" + OUT, "-lhvd_core", "-L" + tlib, "-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch", "-ltorch_python",
-               "-L" + os.path.join(CUDA_HOME, "lib64"), "-lcudart",
-               "-Wl,-rpath,$ORIGIN", "-Wl,-rpath," + tlib]
-    _run(cmd)
+    cxx = ["g++", "-O2", "-std=c++17", "-fPIC", "-pthread", "-DTORCH_EXTENSION_NAME=_hvd_torch",
+           "-DTORCH_API_INCLUDE_EXTENSION_H", "-D_GLIBCXX_USE_CXX11_ABI=%d" % abi, "-Wno-deprecated-declarations"] + inc
+    with ThreadPoolExecutor(max_workers=max(2, os.cpu_count() or 4)) as ex:
+        objs = list(ex.map(lambda s: _compile(s, hstamp, force, False, cxx), srcs))
+    _run(["g++", "-shared", "-pthread"] + objs + [
+        "-o", lib, "-L" + OUT, "-lhvd_core", "-L" + tlib, "-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch", "-ltorch_python",
+        "-L" + os.path.join(CUDA_HOME, "lib64"), "-lcudart", "-Wl,-rpath,$ORIGIN", "-Wl,-rpath," + tlib])
     with open(stamp_file, "w") as f:
         f.write(stamp)
     return lib

@@ -21,6 +21,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <type_traits>
+#include "moe_kernels.h"
 #include "p2p_kernels.h"
 
 namespace hvd {

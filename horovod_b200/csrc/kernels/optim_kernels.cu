@@ -10,6 +10,7 @@
 #include <algorithm>
 #include <cstring>
 #include <type_traits>
+#include "optim_kernels.h"
 #include "p2p_kernels.h"
 
 namespace hvd {

@@ -14,6 +14,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include "p2p_kernels.h"
+#include "sync_bn_kernels.h"
 
 namespace hvd {
 namespace kern {

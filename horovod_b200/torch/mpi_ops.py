@@ -5,7 +5,7 @@ join, barrier, poll/synchronize.
 API parity: horovod/torch/mpi_ops.py.  (The module keeps the reference's
 historical file name so user code that imports `horovod.torch.mpi_ops` ports
 by changing only the package name; nothing here is MPI.)  Native calls go to
-csrc/torch/binding.cc (`_hvd_torch`).  GPU collectives complete through CUDA
+`_hvd_torch`, whose collective entry points are in csrc/torch/binding.cc.  GPU collectives complete through CUDA
 events chained into the caller's stream, so `synchronize()` does not block the
 host on the GPU.
 """
