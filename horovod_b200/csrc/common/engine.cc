@@ -1047,6 +1047,24 @@ Status Engine::CapturedAlltoall(const void* in, int64_t rows, int64_t row_bytes,
                                     max_ctas, (cudaStream_t)stream);
 }
 
+Status Engine::CapturedUlyssesExchange(const void* in, void* out, const int64_t* dims, int64_t elem_bytes, int direction,
+                                       bool head_first, void* staging, int64_t staging_bytes, int* status, int nranks, int32_t psid,
+                                       int max_ctas, void* stream) {
+  std::shared_ptr<ProcessSet> ps;
+  Status st = CheckSet(psid, &ps);
+  if (!st.ok()) return st;
+  if (nranks != ps->set_size())
+    return Status::InvalidArgument("ulysses exchange: the output was sized for " + std::to_string(nranks) + " ranks, the process set has " +
+                                   std::to_string(ps->set_size()));
+  if (ps->set_size() < 2) return Status::PreconditionError("ulysses exchange needs a peer-mapped process set of at least 2 ranks");
+  const bool split_d1 = (direction == kern::kUlySeqToHeads) == head_first;
+  if ((split_d1 ? dims[1] : dims[3]) % nranks != 0)
+    return Status::InvalidArgument("ulysses exchange: the split dim must be a multiple of the process set size");
+  captured_launches_.fetch_add(1, std::memory_order_relaxed);
+  return gpu_ops_->CapturedUlyssesExchange(*ps, in, out, dims, elem_bytes, direction, head_first, staging, staging_bytes, status,
+                                           max_ctas, (cudaStream_t)stream);
+}
+
 Status Engine::StartTimeline(const std::string& file, bool mark_cycles) {
   if (!initialized_.load()) return Status::PreconditionError(NOT_INITIALIZED_ERROR_MSG);
   std::lock_guard<std::mutex> l(tl_mu_);

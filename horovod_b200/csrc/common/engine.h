@@ -93,6 +93,11 @@ class Engine {
   Status CapturedAlltoall(const void* in, int64_t rows, int64_t row_bytes, const void* splits, int64_t nsplits, bool splits_int64,
                           void* out, int64_t capacity, int64_t* recv_splits, int* status, int32_t process_set_id, int max_ctas,
                           void* stream);
+  // Ulysses sequence-parallel exchange, same launch contract (see GpuOps::CapturedUlyssesExchange); `nranks` is the set
+  // size the caller sized the output for, and the split dim (dims[1] or dims[3]) must be a multiple of it.
+  Status CapturedUlyssesExchange(const void* in, void* out, const int64_t* dims, int64_t elem_bytes, int direction, bool head_first,
+                                 void* staging, int64_t staging_bytes, int* status, int nranks, int32_t process_set_id, int max_ctas,
+                                 void* stream);
 
   // ---- timeline ----
   Status StartTimeline(const std::string& file, bool mark_cycles);

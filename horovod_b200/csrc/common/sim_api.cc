@@ -542,6 +542,39 @@ int hvd_sim_captured_alltoall(int nranks, int device, const uint64_t* in_ptrs, c
   return streams ? 0 : Finish(nranks, cudaDeviceSynchronize());
 }
 
+// The Ulysses exchange over N simulated ranks: in_ptrs / out_ptrs / staging_ptrs rank r's input, output and staging
+// buffer (plain device memory, staging_bytes[r] bytes), dims (5 per rank: A, D1, M, D2, R), elem_bytes and status_ptrs
+// (int32, 1) per rank, so that ranks may disagree on the shape.  `streams` as hvd_sim_captured_alltoall.
+int hvd_sim_ulysses_exchange(int nranks, int device, const uint64_t* in_ptrs, const uint64_t* out_ptrs, const uint64_t* staging_ptrs,
+                             const int64_t* staging_bytes, const int64_t* dims, const int64_t* elem_bytes, int direction, int head_first,
+                             const uint64_t* status_ptrs, int ctas, const uint64_t* streams) {
+  if (nranks < 2 || nranks > kern::kMaxPeers || cudaSetDevice(device) != cudaSuccess) return -1;
+  Sim* sim = streams ? (g_sims.count(nranks) ? &g_sims[nranks] : nullptr) : GetSim(nranks, device, 1 << 20);
+  if (!sim) return -1;
+  std::vector<kern::UlyssesArgs> args(nranks);
+  for (int r = 0; r < nranks; ++r) {
+    kern::UlyssesArgs& a = args[r];
+    for (int p = 0; p < nranks; ++p) { a.staging[p] = (const void*)staging_ptrs[p]; a.counts[p] = sim->teams[r]->CountRegion(p); }
+    a.staging_offset = 0; a.staging_bytes = staging_bytes[r];
+    a.in = (const void*)in_ptrs[r]; a.out = (void*)out_ptrs[r];
+    for (int k = 0; k < 5; ++k) a.dims[k] = dims[5 * r + k];
+    a.elem_bytes = elem_bytes[r]; a.direction = direction; a.head_first = head_first; a.status = (int*)status_ptrs[r];
+    a.ctas = ctas;
+  }
+  // rejected on every rank or on none: a rank launched alone would wait at its barrier for peers that never come
+  for (int r = 0; r < nranks; ++r) {
+    kern::UlyssesArgs probe = args[r];
+    if (kern::PlanUlyssesExchange(nranks, &probe) != cudaSuccess) return (int)cudaErrorInvalidValue;
+  }
+  if (!streams) cudaDeviceSynchronize();
+  for (int r = 0; r < nranks; ++r) {
+    cudaError_t e = kern::LaunchUlyssesExchange(sim->teams[r]->Params(0, kern::kAlltoallChannel), args[r],
+                                                streams ? (cudaStream_t)streams[r] : sim->streams[r]);
+    if (e != cudaSuccess) return (int)e;
+  }
+  return streams ? 0 : Finish(nranks, cudaDeviceSynchronize());
+}
+
 void hvd_sim_reset() {
   for (auto& kv : g_sims) for (auto st : kv.second.streams) cudaStreamDestroy(st);
   g_sims.clear();

@@ -165,6 +165,46 @@ struct CapturedAlltoallArgs {
 };
 cudaError_t LaunchCapturedAlltoall(const CommParams& cp, const CapturedAlltoallArgs& args, cudaStream_t stream);
 
+// Ulysses sequence-parallel exchange (hvd.UlyssesExchange, see ulysses_kernels.cu), one launch on barrier channel
+// kAlltoallChannel that shares the count region with the captured alltoall: a process set's captured alltoalls,
+// ExpertDispatcher exchanges and Ulysses exchanges must be issued in one stream order.  The input of every rank is viewed
+// as [A, D1, M, D2, R] elements of elem_bytes, where D1 and D2 are the sequence and head dims in tensor order
+// (head_first: D1 is the head dim).  kUlySeqToHeads splits the head dim into N blocks, block q to rank q, and
+// concatenates the sequence blocks of rank 0, 1, ...; kUlyHeadsToSeq splits the sequence dim and concatenates heads.
+// Every CTA b stages exactly the runs that CTA b of every peer pulls from it, publishes
+// {direction, head_first, A, D1, M, D2, R, elem_bytes, staging_offset} into row b of its count region and meets CTA b
+// of every peer; if the shapes differ, status becomes kA2aRowBytesMismatch on every rank, nothing is pulled and the
+// output is zero-filled.  `status` keeps the first non-zero code: the kernel only writes it while it holds 0.
+enum UlyssesDirection : int { kUlySeqToHeads = 0, kUlyHeadsToSeq = 1 };
+constexpr int kUlyShapeWords = 8;                  // the words of a row that every rank must agree on
+constexpr int kUlyStagingOffset = kUlyShapeWords;  // then the staging offset
+// The (receiver, sender) blocks of one exchange, all alike: runs j = (a * ni + i) * nm + m of run_bytes contiguous
+// bytes, at a * stride[0] + i * stride[1] + m * stride[2] from the block's base.  Block q of the input starts at
+// q * split_off, block p of the output at p * cat_off, block q of the staging buffer (packed runs) at q * block_bytes.
+struct UlyssesGeometry {
+  int64_t ni, nm, nruns, run_bytes, block_bytes, split_off, cat_off;
+  int64_t in_stride[3], out_stride[3], packed_stride[3];
+};
+struct UlyssesArgs {
+  const void* staging[kMaxPeers];  // every rank's registered region as mapped into this process
+  int64_t* counts[kMaxPeers];      // every rank's count region as mapped here
+  int64_t staging_offset;          // byte offset of this rank's staging buffer in its region
+  int64_t staging_bytes;           // its size: at least the input's bytes
+  const void* in;                  // this rank's contiguous input
+  void* out;                       // its output, the same number of bytes
+  int64_t dims[5];                 // A, D1, M, D2, R of the input
+  int64_t elem_bytes;
+  int direction;                   // UlyssesDirection
+  int head_first;
+  int* status;
+  int ctas;                        // the same on every rank
+  UlyssesGeometry geo;             // filled in by the launcher from the fields above and the team size
+};
+// Checks the arguments of an exchange on a team of `nranks` and fills in args->geo: cudaErrorInvalidValue when the split
+// dim is not a multiple of nranks, the input does not fit the staging buffer, or a field is out of range.
+cudaError_t PlanUlyssesExchange(int nranks, UlyssesArgs* args);
+cudaError_t LaunchUlyssesExchange(const CommParams& cp, const UlyssesArgs& args, cudaStream_t stream);
+
 // Stand-alone batched pack / unpack / scale (NCCL-baseline path and odd cases).
 // direction 0: tensors -> buffer (prescale), 1: buffer -> tensors (postscale)
 cudaError_t LaunchPackUnpack(void* buffer, const TensorDesc* descs, int ndesc, int64_t total_bytes, int dtype,

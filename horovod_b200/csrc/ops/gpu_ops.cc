@@ -433,6 +433,33 @@ Status GpuOps::CapturedAlltoall(ProcessSet& ps, const void* in, int64_t rows, in
   return Status::OK();
 }
 
+// Each rank publishes the offset of its own staging buffer, so only the region (not the offset) has to be the same on
+// every rank.
+Status GpuOps::CapturedUlyssesExchange(ProcessSet& ps, const void* in, void* out, const int64_t* dims, int64_t elem_bytes,
+                                       int direction, bool head_first, void* staging, int64_t staging_bytes, int* status,
+                                       int max_ctas, cudaStream_t stream) {
+  const std::string name = "ulysses exchange";
+  std::shared_ptr<SymmTeam> team;
+  { std::lock_guard<std::mutex> l(ps.team_mu); team = ps.team; }
+  if (!team) return Status::PreconditionError(name + ": the process set has no peer-mapped team (allocate the staging buffer with hvd.symm_empty first)");
+  if (team->abort_state() != 0) return Status::Aborted(name + ": the team was aborted");
+  const int n = team->nranks();
+  SymmTeam::RegionView view;
+  int64_t off = 0;
+  if (staging_bytes <= 0 || !team->FindRegion(staging, (size_t)staging_bytes, &view, &off))
+    return Status::InvalidArgument(name + ": the staging buffer is not (entirely) inside registered symmetric memory");
+  kern::UlyssesArgs a {};
+  for (int p = 0; p < n; ++p) { a.staging[p] = view.ptr[p]; a.counts[p] = team->CountRegion(p); }
+  a.staging_offset = off; a.staging_bytes = staging_bytes;
+  a.in = in; a.out = out;
+  for (int k = 0; k < 5; ++k) a.dims[k] = dims[k];
+  a.elem_bytes = elem_bytes; a.direction = direction; a.head_first = head_first ? 1 : 0; a.status = status;
+  a.ctas = std::min(max_ctas > 0 ? max_ctas : env_.params->comm_ctas, kern::kMaxCtas);
+  cudaError_t ce = kern::LaunchUlyssesExchange(team->Params(0, kern::kAlltoallChannel), a, stream);
+  if (ce != cudaSuccess) return Status::UnknownError(name + " launch failed: " + cudaGetErrorString(ce));
+  return Status::OK();
+}
+
 Status GpuOps::LaunchCaptured(ProcessSet& ps, const char* what, InplaceLaunch launch, void* ptr, int64_t bytes, DataType dtype,
                               ReduceOp op, double prescale, double postscale, int max_ctas, cudaStream_t stream, int channel) {
   const std::string name = std::string("captured ") + what;

@@ -126,6 +126,12 @@ class GpuOps {
   Status CapturedAlltoall(ProcessSet& ps, const void* in, int64_t rows, int64_t row_bytes, const void* splits, int64_t nsplits,
                           bool splits_int64, void* out, int64_t capacity, int64_t* recv_splits, int* status, int max_ctas,
                           cudaStream_t stream);
+  // Ulysses exchange of the contiguous input `in` (viewed as dims = [A, D1, M, D2, R] elements of elem_bytes, see
+  // kern::UlyssesArgs) into `out` through this rank's staging buffer [staging, staging + staging_bytes), which must lie
+  // in a registered region: ONE kernel on `stream` on barrier channel kern::kAlltoallChannel, same launch contract as
+  // CapturedAlltoall.  `status` keeps the first non-zero kern::AlltoallStatus.
+  Status CapturedUlyssesExchange(ProcessSet& ps, const void* in, void* out, const int64_t* dims, int64_t elem_bytes, int direction,
+                                 bool head_first, void* staging, int64_t staging_bytes, int* status, int max_ctas, cudaStream_t stream);
   bool BuildInplaceArgs(SymmTeam& team, const void* ptr, int64_t bytes, DataType dtype, ReduceOp op, double prescale,
                         double postscale, int64_t expect_off, int max_ctas, kern::InplaceArgs* out);
 

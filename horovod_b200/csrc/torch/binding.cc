@@ -494,6 +494,46 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> CapturedAlltoall(at::Tensor tenso
   return {out, recv, status};
 }
 
+// Ulysses exchange of a contiguous tensor between sequence shards and head shards (hvd.UlyssesExchange), launched like
+// CapturedAllreduce through this rank's registered staging buffer.  direction 0 (seq -> heads) splits head_dim into
+// nranks blocks and concatenates the ranks' blocks along seq_dim; direction 1 (heads -> seq) splits seq_dim and
+// concatenates along head_dim.  The output is allocated on the current stream; `status` (int32 [1]) keeps the first
+// non-zero kern::AlltoallStatus.
+at::Tensor CapturedUlyssesExchange(at::Tensor tensor, at::Tensor staging, at::Tensor status, int64_t seq_dim, int64_t head_dim,
+                                   int direction, int nranks, int process_set_id, int max_ctas) {
+  const char* op = "ulysses_exchange";
+  TORCH_CHECK(tensor.is_cuda(), op, ": CUDA tensor expected");
+  TORCH_CHECK(tensor.is_contiguous(), op, ": tensor must be contiguous");
+  TORCH_CHECK(direction == kern::kUlySeqToHeads || direction == kern::kUlyHeadsToSeq, op, ": direction must be 0 or 1, got ", direction);
+  TORCH_CHECK(nranks >= 1 && nranks <= kern::kMaxPeers, op, ": nranks must be in [1, ", kern::kMaxPeers, "], got ", nranks);
+  const int64_t nd = tensor.dim();
+  TORCH_CHECK(seq_dim >= 0 && seq_dim < nd && head_dim >= 0 && head_dim < nd && seq_dim != head_dim, op,
+              ": seq_dim and head_dim must be two distinct dims of a ", nd, "-D tensor, got ", seq_dim, " and ", head_dim);
+  const int64_t split = direction == kern::kUlySeqToHeads ? head_dim : seq_dim;
+  TORCH_CHECK(tensor.size(split) % nranks == 0, op, ": dim ", split, " (size ", tensor.size(split), ") must be a multiple of ",
+              nranks);
+  TORCH_CHECK(staging.is_cuda() && staging.device() == tensor.device() && staging.is_contiguous(), op,
+              ": staging must be a contiguous tensor on ", tensor.device());
+  const int64_t bytes = tensor.numel() * (int64_t)tensor.element_size();
+  const int64_t staging_bytes = staging.numel() * (int64_t)staging.element_size();
+  TORCH_CHECK(staging_bytes >= bytes, op, ": the tensor has ", bytes, " bytes, the staging buffer ", staging_bytes);
+  CheckVector(op, "status", status, tensor.device(), {at::kInt}, 1);
+  const OnDevice on(tensor);
+  const int64_t lo = std::min(seq_dim, head_dim), hi = std::max(seq_dim, head_dim);
+  const auto sz = tensor.sizes();
+  const int64_t dims[5] = {c10::multiply_integers(sz.slice(0, lo)), sz[lo], c10::multiply_integers(sz.slice(lo + 1, hi - lo - 1)),
+                           sz[hi], c10::multiply_integers(sz.slice(hi + 1))};
+  std::vector<int64_t> out_sizes = sz.vec();
+  const int64_t concat = split == head_dim ? seq_dim : head_dim;
+  out_sizes[split] /= nranks;
+  out_sizes[concat] *= nranks;
+  at::Tensor out = at::empty(out_sizes, tensor.options());
+  ThrowIfError(Engine::Get().CapturedUlyssesExchange(tensor.data_ptr(), out.data_ptr(), dims, tensor.element_size(), direction,
+                                                     head_dim < seq_dim, staging.data_ptr(), staging_bytes, status.data_ptr<int>(),
+                                                     nranks, process_set_id, max_ctas, (void*)on.stream));
+  return out;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(_hvd_torch, m) {
@@ -520,6 +560,9 @@ PYBIND11_MODULE(_hvd_torch, m) {
         py::arg("channel") = kern::kGraphChannel);
   m.def("captured_alltoall", &CapturedAlltoall, py::arg("tensor"), py::arg("splits"), py::arg("capacity"),
         py::arg("process_set_id"), py::arg("max_ctas"));
+  m.def("captured_ulysses_exchange", &CapturedUlyssesExchange, py::arg("tensor"), py::arg("staging"), py::arg("status"),
+        py::arg("seq_dim"), py::arg("head_dim"), py::arg("direction"), py::arg("nranks"), py::arg("process_set_id"),
+        py::arg("max_ctas"));
   DefOptim(m);
   DefSyncBn(m);
   DefMoe(m);

@@ -11,6 +11,7 @@ for every simulated rank, check that the plans agree and only then launch them. 
 launch may use: small caps force the windowed multi-launch paths.
 """
 import ctypes
+import math
 
 import torch
 
@@ -46,6 +47,8 @@ def lib():
         L.hvd_sim_alltoallv.argtypes = plan + [ctypes.c_int, u64p, u64p, ctypes.c_int64, ctypes.c_int]
         L.hvd_sim_captured_alltoall.argtypes = [ctypes.c_int, ctypes.c_int, u64p, i64p, i64p, u64p, ctypes.c_int, u64p, i64p, u64p,
                                                 u64p, ctypes.c_int, u64p]
+        L.hvd_sim_ulysses_exchange.argtypes = [ctypes.c_int, ctypes.c_int, u64p, u64p, u64p, i64p, i64p, i64p, ctypes.c_int,
+                                               ctypes.c_int, u64p, ctypes.c_int, u64p]
         _lib = L
     return _lib
 
@@ -184,3 +187,33 @@ def captured_alltoall(ins, splits, outs, recv_splits, status, ctas=8, streams=No
         _i64(t.shape[0] for t in outs), u64(t.data_ptr() for t in recv_splits), u64(t.data_ptr() for t in status), ctas,
         None if streams is None else u64(s.cuda_stream for s in streams))
     _check(rc, 'sim captured alltoall')
+
+
+SEQ_TO_HEADS, HEADS_TO_SEQ = 0, 1
+
+
+def ulysses_view(shape, seq_dim, head_dim):
+    """[A, D1, M, D2, R] of a tensor of `shape` whose named dims are seq_dim and head_dim (D1 the first of them)."""
+    lo, hi = min(seq_dim, head_dim), max(seq_dim, head_dim)
+    return [math.prod(shape[:lo]), shape[lo], math.prod(shape[lo + 1:hi]), shape[hi], math.prod(shape[hi + 1:])]
+
+
+def ulysses_exchange(ins, outs, seq_dim, head_dim, direction, status, staging=None, ctas=8, streams=None, device=0):
+    """The kernel of hvd.UlyssesExchange on N simulated ranks, every argument a list indexed by rank: ins[r] contiguous,
+    outs[r] with the same bytes (contiguous), status[r] int32 [1] (keeps the first non-zero code).  direction
+    SEQ_TO_HEADS splits head_dim into N blocks and concatenates the ranks' blocks along seq_dim; HEADS_TO_SEQ splits
+    seq_dim and concatenates along head_dim.  The view [A, D1, M, D2, R] and the element size come from each rank's own
+    input, so ranks may disagree on them.  staging[r]: rank r's staging buffer (any contiguous CUDA tensor of at least
+    the input's bytes); None allocates one per rank for this call, which a captured graph must not rely on.
+
+    streams as in captured_alltoall: with streams, rank r's kernel is only launched on streams[r]."""
+    n = len(ins)
+    if staging is None:
+        staging = [torch.empty(max(t.numel() * t.element_size(), 1), dtype=torch.uint8, device=t.device) for t in ins]
+    u64 = lambda vals: (ctypes.c_uint64 * n)(*vals)  # noqa: E731
+    dims = [d for t in ins for d in ulysses_view(list(t.shape), seq_dim, head_dim)]
+    rc = lib().hvd_sim_ulysses_exchange(
+        n, device, u64(t.data_ptr() for t in ins), u64(t.data_ptr() for t in outs), u64(t.data_ptr() for t in staging),
+        _i64(t.numel() * t.element_size() for t in staging), _i64(dims), _i64(t.element_size() for t in ins), int(direction),
+        int(head_dim < seq_dim), u64(t.data_ptr() for t in status), ctas, None if streams is None else u64(s.cuda_stream for s in streams))
+    _check(rc, 'sim ulysses exchange')
